@@ -133,8 +133,8 @@ int uvx_debug_gemm_stages(int n);
 /* tuning hook of the weight-streaming forms: enable (0 = never, 1 = decode form + single-pass form, 2 = decode form only; -1 =
  * UVX_GEMM_WS env, default 2), `mode` (ignored), upper bound on the persistent grid of every uvx_gemm_bf16 launch (0 = one CTA per SM) */
 int uvx_debug_gemm_ws(int enable, int mode, int grid);
-/* hooks of tuning knobs the Hopper kernel does not have (TMA-store epilogue, phase timestamps, L2 prefetch distance, cluster shape,
- * pipeline isolation): accepted for ABI compatibility, no effect */
+/* hooks of tuning knobs the Hopper kernel does not have (TMA-store epilogue, phase timestamps, L2 prefetch distance, pipeline
+ * isolation): accepted for ABI compatibility, no effect */
 int uvx_debug_gemm_tma_store(int on);
 int uvx_debug_gemm_times(void* dev_buf);
 int uvx_debug_gemm_pf(int pf);
@@ -147,7 +147,11 @@ int uvx_debug_gemm_ws_times(void* dev_buf);
  * head_dim): r = 32q + j -> row 128t + 16q + j (j < 16) or its rotation partner 128t + 64 + 16q + (j - 16).  out: ceil(N/R) * (K/64) * R * 64 bf16 elements.                 */
 int uvx_tile_weight(const void* W, int64_t N, int64_t K, int64_t w_row_stride, int32_t R, int32_t interleave, void* out,
                     uvx_stream_t stream);
+/* tuning hook: thread-block cluster of uvx_gemm_bf16, cm tiles along M x cn along N sharing their A / W boxes by TMA multicast
+ * ((0, 0) = heuristic: clusters for calls of <= 256 rows and one batch unless UVX_GEMM_CLUSTER=0; (1, 1) = none).  An axis whose
+ * tile count it does not divide falls back to 1.  The cluster shape never changes the result bits. */
 int uvx_debug_gemm_cluster(int cm, int cn);
+/* accepted for ABI compatibility, no effect */
 int uvx_debug_gemm_mode(int mode);
 
 /* ---------------------------------------------------------------------------------------------

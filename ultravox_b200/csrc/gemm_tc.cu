@@ -5,7 +5,8 @@
 // Persistent, warp-specialised kernel: grid = min(#units, #SMs), each CTA walks units u = blockIdx.x + i*gridDim.x (a unit is
 // one output tile, or one K range of it under split-K).  A CTA tile is (MT*128) x BN: MT in {1,2} row sub-tiles share one W
 // tile (at M <= 256 - the LLM prefill - every weight byte is fetched from L2/HBM once), BN in {64,128,208,256} (208: ragged
-// last column tile allowed).
+// last column tile allowed).  At M <= 256 CTAs also run in thread-block clusters of cm x cn tiles that split the loads of the
+// A box (along N) and of the W box (along M) and multicast them to their peers (pick_cluster).
 //   warpgroup 0    one thread issues the TMA loads: the A box {64 k, MT*128 rows, 1 batch} and the W box {64 k, BN rows} into
 //                  a deep 128B-swizzled shared-memory ring (mbarrier expect_tx); it runs ahead across unit boundaries.
 //   warpgroups 1-2 consumers: warpgroup c owns rows [64c, 64c+64) of each 128-row sub-tile and issues wgmma m64 x BN x 16
@@ -50,6 +51,7 @@ struct GemmParams {
   int64_t rope_rows_per_seq, rope_pos_offset;
   int rope_cols;
   int stages;              // ring depth
+  int cm, cn;              // thread-block cluster of cm x cn tiles (1 x 1: no cluster); cm divides m_tiles * a_batch, cn n_tiles
 };
 
 static constexpr int kSmemTotal = 227 * 1024;
@@ -125,32 +127,51 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   const int tiles_m_total = p.m_tiles * (int)p.a_batch;
   const int num_kb = (int)((p.K + kBK - 1) / kBK);
-  const int num_units = p.num_tiles * p.splits;
   const int stages = p.stages;
+  // Thread-block cluster of cm x cn tiles (rank r = rm * cn + rn), walked in lockstep: the cluster takes cluster units
+  // (cluster tile, split) and CTA (rm, rn) computes m-tile gm * cm + rm and n-tile gn * cn + rn of cluster tile (gm, gn) with the
+  // split's k range, so every member runs the same k-blocks in the same ring order.  It loads its 1/cn share of the A box and
+  // multicasts it along its row (same m-tile), and its 1/cm share of the W box to its column (same n-tile).  1 x 1 is the plain
+  // persistent walk: unit u = blockIdx.x + i * gridDim.x, tiles consecutive along M.
+  const int csize = p.cm * p.cn;
+  const int rank = csize > 1 ? (int)cluster_ctarank() : 0;
+  const int rm = rank / p.cn, rn = rank % p.cn;
+  const int cluster_tiles_m = tiles_m_total / p.cm;
+  const int num_units = p.num_tiles / csize * p.splits;
+  const int first_unit = blockIdx.x / csize, unit_step = gridDim.x / csize;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 8);  // one arrival per consumer warp
+      mbar_init(&empty_bar[s], 8 * csize);  // one arrival per consumer warp of every CTA of the cluster
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  __syncthreads();
+  // no CTA multicasts into a peer before the peer's barriers are initialised
+  if (csize > 1) cluster_sync();
+  else __syncthreads();
   // set-up above overlapped the previous kernel's tail; its outputs are visible after griddepcontrol.wait
   pdl_wait();
 
   if (wg == 0) {
-    // ---- TMA producer (one thread)
+    // ---- TMA producer (one thread); its warpgroup hands registers to the consumers' accumulators (128 x 40 + 256 x 232
+    // fits the 384 x 168 the CTA was launched with)
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (tid == 0) {
       asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"(&tmW) : "memory");
+      // slices are whole 8-row (1 KB) swizzle atoms; each lands at its own offset of the box in every CTA of the mask
+      const int a_slice = MT * 128 / p.cn, w_slice = BN / p.cm;
+      const uint16_t row_mask = (uint16_t)(((1u << p.cn) - 1u) << (rm * p.cn));
+      uint16_t col_mask = 0;
+      for (int j = 0; j < p.cm; ++j) col_mask |= (uint16_t)(1u << (j * p.cn + rn));
       int s = 0;
       uint32_t ph = 0;
-      for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
-        const int tile = unit / p.splits, split = unit % p.splits;
-        const int tm_idx = tile % tiles_m_total;  // consecutive tiles share the W tile
-        const int tn_idx = tile / tiles_m_total;
+      for (int unit = first_unit; unit < num_units; unit += unit_step) {
+        const int ctile = unit / p.splits, split = unit % p.splits;
+        const int tm_idx = (ctile % cluster_tiles_m) * p.cm + rm;  // consecutive tiles share the W tile
+        const int tn_idx = (ctile / cluster_tiles_m) * p.cn + rn;
         const int b = tm_idx / p.m_tiles;
         const int m0 = (tm_idx % p.m_tiles) * (MT * 128);
         const int kb_begin = split * p.kb_per_split;
@@ -161,25 +182,45 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         for (int kb = kb_begin; kb < kb_end; ++kb) {
           mbar_wait(&empty_bar[s], ph ^ 1u);
           uint8_t* sa = smem + s * L::kStageBytes;
+          // the whole stage lands in every CTA (own slices and the peers'); TMA zero fill counts toward the bytes
           mbar_expect_tx(&full_bar[s], (uint32_t)L::kStageBytes);
-          tma_load_3d(sa, &tmA, kb * kBK, m0, b, &full_bar[s]);
-          tma_load_2d(sa + L::kABytes, &tmW, p.w_tiled ? 0 : kb * kBK, p.w_tiled ? wt_base + kb * BN : tn_idx * BN, &full_bar[s]);
+          uint8_t* da = sa + rn * a_slice * (kBK * 2);
+          if (p.cn > 1) tma_load_3d_mc(da, &tmA, kb * kBK, m0 + rn * a_slice, b, &full_bar[s], row_mask);
+          else tma_load_3d(da, &tmA, kb * kBK, m0, b, &full_bar[s]);
+          uint8_t* dw = sa + L::kABytes + rm * w_slice * (kBK * 2);
+          const int w0 = p.w_tiled ? 0 : kb * kBK;
+          const int w1 = (p.w_tiled ? wt_base + kb * BN : tn_idx * BN) + rm * w_slice;
+          if (p.cm > 1) tma_load_2d_mc(dw, &tmW, w0, w1, &full_bar[s], col_mask);
+          else tma_load_2d(dw, &tmW, w0, w1, &full_bar[s]);
           if (++s == stages) { s = 0; ph ^= 1u; }
         }
       }
     }
+    // no CTA leaves while a peer can still write into its shared memory or arrive on its barriers
+    if (csize > 1) cluster_sync();
     return;
   }
 
   // ---- consumers
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
   const int c = wg - 1;
   const int warp = tid >> 5, lane = tid & 31;
+  // hand ring slot `slot` back: to this CTA's producer, or to the producers of every CTA of the cluster (each may have
+  // multicast a slice into it), one lane per CTA
+  auto release = [&](int slot) {
+    __syncwarp();
+    if (csize == 1) {
+      if (lane == 0) mbar_arrive(&empty_bar[slot]);
+    } else if (lane < csize) {
+      mbar_arrive_cluster(&empty_bar[slot], (uint32_t)lane);
+    }
+  };
   int s = 0;
   uint32_t ph = 0;
-  for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
-    const int tile = unit / p.splits, split = unit % p.splits;
-    const int tm_idx = tile % tiles_m_total;
-    const int tn_idx = tile / tiles_m_total;
+  for (int unit = first_unit; unit < num_units; unit += unit_step) {
+    const int ctile = unit / p.splits, split = unit % p.splits;
+    const int tm_idx = (ctile % cluster_tiles_m) * p.cm + rm;
+    const int tn_idx = (ctile / cluster_tiles_m) * p.cn + rn;
     const int b = tm_idx / p.m_tiles;
     const int m0 = (tm_idx % p.m_tiles) * (MT * 128);
     const int n0 = tn_idx * BN;
@@ -203,16 +244,12 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       wgmma_commit();
       // one k-block of MMAs stays in flight; the slot read by the previous one is handed back to the producer
       wgmma_wait<1>();
-      if (prev >= 0) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[prev]);
-      }
+      if (prev >= 0) release(prev);
       prev = s;
       if (++s == stages) { s = 0; ph ^= 1u; }
     }
     wgmma_wait<0>();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+    release(prev);
 
     // ---- epilogue from registers: this thread holds rows r0 (+8) of each 64-row sub-tile, columns 8j + 2(lane % 4) (+1)
     const int rq = warp * 16 + (lane >> 2);
@@ -326,6 +363,7 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
     }
   }
+  if (csize > 1) cluster_sync();
 }
 
 // Split-K second pass: sums the fp32 partials in split order and applies the same epilogue as the direct path.
@@ -683,14 +721,25 @@ static int finish_gemm(const uvx_gemm_args* a, const GemmParams& p, cudaStream_t
   return uvx_rmsnorm(a->C, a->norm_w, a->norm_out, a->a_batch * a->a_rows, a->N, a->c_row_stride, 0, 0, 0, a->norm_eps, stream);
 }
 
+// cluster shape (cm, cn) actually run for an (MT, BN) tiling: an axis whose tile count it does not divide, or whose operand box
+// it cannot cut into whole 8-row swizzle atoms, falls back to 1; at most 8 CTAs (the portable cluster size)
+static void legal_cluster(int mt, int bn, int tiles_m_total, int n_tiles, int* cm, int* cn) {
+  if (*cm < 1 || *cm > 4 || tiles_m_total % *cm != 0 || bn % (8 * *cm) != 0) *cm = 1;
+  if (*cn < 1 || *cn > 4 || n_tiles % *cn != 0 || (mt * 128) % (8 * *cn) != 0) *cn = 1;
+  if (*cm * *cn > 8) *cm = *cn = 1;
+}
+
 template <int MT, int BN>
-static int launch_gemm(const uvx_gemm_args* a, int splits, cudaStream_t stream) {
+static int launch_gemm(const uvx_gemm_args* a, int splits, int cm, int cn, cudaStream_t stream) {
   using L = WgLayout<MT, BN>;
+  const int m_tiles = (int)((a->a_rows + MT * 128 - 1) / (MT * 128));
+  const int n_tiles = (int)((a->N + BN - 1) / BN);
+  legal_cluster(MT, BN, m_tiles * (int)a->a_batch, n_tiles, &cm, &cn);
   CUtensorMap tmA, tmW;
   {
     uint64_t dims[3] = {(uint64_t)a->K, (uint64_t)a->a_rows, (uint64_t)a->a_batch};
     uint64_t st[2] = {(uint64_t)a->a_row_stride * 2, (uint64_t)(a->a_batch > 1 ? a->a_batch_stride : a->a_row_stride) * 2};
-    uint32_t box[3] = {kBK, (uint32_t)(MT * 128), 1};
+    uint32_t box[3] = {kBK, (uint32_t)(MT * 128 / cn), 1};  // a CTA loads its 1/cn share of the A box
     int rc = encode_map(&tmA, a->A, 3, dims, st, box, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
     if (rc) return rc;
   }
@@ -702,13 +751,13 @@ static int launch_gemm(const uvx_gemm_args* a, int splits, cudaStream_t stream) 
     const uint64_t n_tiles_w = (uint64_t)((a->N + BN - 1) / BN);
     uint64_t dims[2] = {(uint64_t)kBK, n_tiles_w * (uint64_t)(a->K / kBK) * (uint64_t)BN};
     uint64_t st[1] = {(uint64_t)kBK * 2};
-    uint32_t box[2] = {kBK, (uint32_t)BN};
+    uint32_t box[2] = {kBK, (uint32_t)(BN / cm)};  // and its 1/cm share of the W box
     int rc = encode_map(&tmW, a->W, 2, dims, st, box, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
     if (rc) return rc;
   } else {
     uint64_t dims[2] = {(uint64_t)a->K, (uint64_t)a->N};
     uint64_t st[1] = {(uint64_t)a->w_row_stride * 2};
-    uint32_t box[2] = {kBK, (uint32_t)BN};
+    uint32_t box[2] = {kBK, (uint32_t)(BN / cm)};
     int rc = encode_map(&tmW, a->W, 2, dims, st, box, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
     if (rc) return rc;
   }
@@ -743,9 +792,11 @@ static int launch_gemm(const uvx_gemm_args* a, int splits, cudaStream_t stream) 
   p.norm_w = (const bf16*)a->norm_w;
   p.norm_out = (bf16*)a->norm_out;
   p.norm_eps = a->norm_eps;
-  p.m_tiles = (int)((a->a_rows + MT * 128 - 1) / (MT * 128));
-  p.n_tiles = (int)((a->N + BN - 1) / BN);
+  p.m_tiles = m_tiles;
+  p.n_tiles = n_tiles;
   p.num_tiles = p.m_tiles * (int)a->a_batch * p.n_tiles;
+  p.cm = cm;
+  p.cn = cn;
   const int num_kb = (int)((a->K + kBK - 1) / kBK);
   if (a->N % BN != 0) splits = 1;  // ragged column tiles exist only in the direct epilogue
   // split-K needs the caller's workspace: [splits][rows][N] fp32 partial sums
@@ -768,10 +819,42 @@ static int launch_gemm(const uvx_gemm_args* a, int splits, cudaStream_t stream) 
     }
     attr_set = true;
   }
-  const int units = p.num_tiles * p.splits;
-  int grid = units < num_sms() ? units : num_sms();
-  if (g_grid_cap > 0 && grid > g_grid_cap) grid = g_grid_cap;
-  launch_k(gemm_wg_kernel<MT, BN>, dim3((unsigned)grid), dim3(kGemmThreads), (size_t)smem, stream, tmA, tmW, p);
+  // persistent grid: a whole number of clusters, no more than fit on the GPU at once (clusters stay inside one GPC, so with
+  // 4-CTA clusters a few SMs stay idle)
+  const int csize = cm * cn;
+  const int units = p.num_tiles / csize * p.splits;
+  int max_units = num_sms();
+  if (csize > 1) {
+    static int max_clusters[9] = {0};
+    if (!max_clusters[csize]) {
+      cudaLaunchConfig_t cfg = {};
+      cfg.gridDim = dim3((unsigned)csize);
+      cfg.blockDim = dim3(kGemmThreads);
+      cfg.dynamicSmemBytes = (size_t)smem;
+      cudaLaunchAttribute attr;
+      attr.id = cudaLaunchAttributeClusterDimension;
+      attr.val.clusterDim.x = (unsigned)csize;
+      attr.val.clusterDim.y = 1;
+      attr.val.clusterDim.z = 1;
+      cfg.attrs = &attr;
+      cfg.numAttrs = 1;
+      cudaError_t e = cudaOccupancyMaxActiveClusters(&max_clusters[csize], gemm_wg_kernel<MT, BN>, &cfg);
+      if (e != cudaSuccess || max_clusters[csize] < 1) {
+        set_error("cudaOccupancyMaxActiveClusters(gemm_wg_kernel<%d,%d>, %d CTAs): %s", MT, BN, csize,
+                  e != cudaSuccess ? cudaGetErrorString(e) : "no cluster fits");
+        max_clusters[csize] = 0;
+        return UVX_ERR_CUDA;
+      }
+    }
+    max_units = max_clusters[csize];
+  }
+  int clusters = units < max_units ? units : max_units;
+  if (g_grid_cap > 0 && clusters * csize > g_grid_cap) clusters = g_grid_cap / csize > 1 ? g_grid_cap / csize : 1;
+  const dim3 grid((unsigned)(clusters * csize));
+  if (csize > 1)
+    launch_k_cluster(gemm_wg_kernel<MT, BN>, grid, dim3(kGemmThreads), (size_t)smem, stream, (unsigned)csize, tmA, tmW, p);
+  else
+    launch_k(gemm_wg_kernel<MT, BN>, grid, dim3(kGemmThreads), (size_t)smem, stream, tmA, tmW, p);
   int rc = check_launch("gemm_wg_kernel");
   if (rc) return rc;
   return finish_gemm(a, p, stream);
@@ -929,13 +1012,23 @@ extern "C" int uvx_debug_gemm_ws(int enable, int mode, int grid) {
   return UVX_OK;
 }
 
-// Hooks of tuning knobs this kernel does not have (TMA-store epilogue, L2 prefetch distance, phase timestamps, pipeline isolation,
-// thread-block cluster shape): accepted for ABI compatibility, no effect.
+static int forced_cm = 0, forced_cn = 0;
+static int g_cluster_enable = -1;  // -1: UVX_GEMM_CLUSTER env (0 = no clusters), default on
+
+// tuning hook: thread-block cluster shape of gemm_wg_kernel, cm tiles along M x cn along N ((0, 0) = heuristic, (1, 1) = none);
+// an axis that does not divide the tile grid falls back to 1
+extern "C" int uvx_debug_gemm_cluster(int cm, int cn) {
+  forced_cm = cm;
+  forced_cn = cn;
+  return UVX_OK;
+}
+
+// Hooks of tuning knobs this kernel does not have (TMA-store epilogue, L2 prefetch distance, phase timestamps, pipeline isolation):
+// accepted for ABI compatibility, no effect.
 extern "C" int uvx_debug_gemm_mode(int mode) { (void)mode; return UVX_OK; }
 extern "C" int uvx_debug_gemm_tma_store(int on) { (void)on; return UVX_OK; }
 extern "C" int uvx_debug_gemm_times(void* dev_buf) { (void)dev_buf; return UVX_OK; }
 extern "C" int uvx_debug_gemm_pf(int pf) { (void)pf; return UVX_OK; }
-extern "C" int uvx_debug_gemm_cluster(int cm, int cn) { (void)cm; (void)cn; return UVX_OK; }
 extern "C" int uvx_debug_gemm_ws_times(void* dev_buf) { (void)dev_buf; return UVX_OK; }
 
 static void read_forced() {
@@ -955,13 +1048,17 @@ static void pick_cfg(int64_t rows, int64_t batch, int64_t N, int64_t K, int sms,
   if (rows <= 256 && batch == 1) {
     mt = rows > 128 ? 2 : 1;
     bn = N % 128 == 0 ? 128 : 64;
-    // enough 128 x 128 tiles to fill most SMs without split-K: no reduce pass, and the same tiling as the fused-RoPE q|k|v GEMM
-    if (bn == 128 && 2 * (N / 128) >= (sms * 3) / 5 && num_kb <= 80) mt = 1;
+    // enough 128 x 128 tiles to fill most SMs without split-K: no reduce pass, and the same tiling as the fused-RoPE q|k|v GEMM;
+    // unless 256 x 128 tiles alone fill every SM (gate|up): then one W read per tile instead of two is faster (same bits)
+    if (bn == 128 && 2 * (N / 128) >= (sms * 3) / 5 && N / 128 < sms && num_kb <= 80) mt = 1;
   } else {
-    // tensor-bound regime (encoder, training): 128-row tiles; 256 wide when that still fills one wave of SMs
+    // tensor-bound regime (encoder, training): 128-row tiles; 256 wide when that still fills one wave of SMs and K is long (the
+    // Llama GEMMs of adapter training: the cfg3 step is ~3 % slower with them 128 wide).  With the 20 k-blocks of the Whisper
+    // encoder (K = 1280) 128-wide tiles win (H100 at 400 W, T = 1500: q|k|v 1500 x 3840 63.6 -> 47.6 us, fc1 1500 x 5120
+    // 80.5 -> 69.1 us)
     mt = 1;
     const int64_t m_tiles = (rows + 127) / 128 * batch;
-    if (N % 256 == 0 && m_tiles * (N / 256) >= sms) bn = 256;
+    if (N % 256 == 0 && m_tiles * (N / 256) >= sms && num_kb >= 32) bn = 256;
     else bn = (N % 128 == 0 && m_tiles * (N / 128) >= sms / 2) ? 128 : 64;
   }
   const int64_t tiles = ((rows + mt * 128 - 1) / (mt * 128)) * batch * ((N + bn - 1) / bn);
@@ -975,6 +1072,33 @@ static void pick_cfg(int64_t rows, int64_t batch, int64_t N, int64_t K, int sms,
   *mt_out = mt;
   *bn_out = bn;
   *splits = sp;
+}
+
+// Cluster shape for the final (MT, BN).  Prefill rows (<= 256, one batch) against a large weight: every CTA pulled its own copy of
+// the A box for each k-block (2-3 bytes of L2 -> SM traffic per weight byte); multicast along N cuts the A share to 1/cn and
+// along M lets 128-row tiles share one W read.  Chosen per tiling by scripts/gemm_cluster_sweep.py (DESIGN §3).  The
+// tensor-bound regime (encoder, training) runs without clusters.
+static void pick_cluster(int64_t rows, int64_t batch, int mt, int* cm, int* cn) {
+  *cm = *cn = 1;
+  if (g_cluster_enable < 0) {
+    const char* e = getenv("UVX_GEMM_CLUSTER");
+    g_cluster_enable = e ? atoi(e) : 1;
+  }
+  if (forced_cm > 0 || forced_cn > 0) {
+    *cm = forced_cm > 0 ? forced_cm : 1;
+    *cn = forced_cn > 0 ? forced_cn : 1;
+    return;
+  }
+  if (!g_cluster_enable || rows > 256 || batch != 1) return;
+  // H100 80GB HBM3 at 400 W, M = 201, us per call (scripts/gemm_cluster_sweep.py; (cm, cn) = (1, 1) first):
+  //   q|k|v  6144 x 4096  MT 1: 42.2 | (2,1) 36.5 | (2,2) 33.9 | (1,2) 41.5 | (1,4) 34.9
+  //   gate|up 28672 x 4096 MT 2: 135.9 | (1,2) 148.6 | (1,4) 137.4   (MT 1: 169.6 | (2,2) 141.9)
+  //   o 4096 x 4096 MT 2 split 4: 34.5 | (1,2) 35.2 | (1,4) 48.0;  down 4096 x 14336 MT 2 split 4: 81.1 | (1,2) 76.8 | (1,4) 126.8
+  // so two 128-row tiles share both boxes; 256-row tiles (W already read once per tile) run without a cluster
+  if (mt == 1 && rows > 128) {
+    *cm = 2;
+    *cn = 2;
+  }
 }
 
 extern "C" int uvx_gemm_bf16(const uvx_gemm_args* a, uvx_stream_t stream_) {
@@ -1034,13 +1158,15 @@ extern "C" int uvx_gemm_bf16(const uvx_gemm_args* a, uvx_stream_t stream_) {
     bn = 128;
   }
   if (bn > 128) mt = 1;                  // register budget of the consumers
+  int cm, cn;
+  pick_cluster(a->a_rows, a->a_batch, mt, &cm, &cn);
   switch (mt * 1000 + bn) {
-    case 1064: return launch_gemm<1, 64>(a, splits, stream);
-    case 1128: return launch_gemm<1, 128>(a, splits, stream);
-    case 1208: return launch_gemm<1, 208>(a, splits, stream);
-    case 1256: return launch_gemm<1, 256>(a, splits, stream);
-    case 2064: return launch_gemm<2, 64>(a, splits, stream);
-    case 2128: return launch_gemm<2, 128>(a, splits, stream);
-    default: return launch_gemm<1, 64>(a, splits, stream);
+    case 1064: return launch_gemm<1, 64>(a, splits, cm, cn, stream);
+    case 1128: return launch_gemm<1, 128>(a, splits, cm, cn, stream);
+    case 1208: return launch_gemm<1, 208>(a, splits, cm, cn, stream);
+    case 1256: return launch_gemm<1, 256>(a, splits, cm, cn, stream);
+    case 2064: return launch_gemm<2, 64>(a, splits, cm, cn, stream);
+    case 2128: return launch_gemm<2, 128>(a, splits, cm, cn, stream);
+    default: return launch_gemm<1, 64>(a, splits, cm, cn, stream);
   }
 }

@@ -1,5 +1,5 @@
-// PTX wrappers of the Hopper GEMM (gemm_tc.cu) and flash attention (attention_wg.cu): mbarrier, TMA tensor loads, warpgroup MMA (wgmma) and its shared-memory
-// operand descriptors.  sm_90a.
+// PTX wrappers of the Hopper GEMM (gemm_tc.cu) and flash attention (attention_wg.cu): mbarrier, TMA tensor loads (multicast to a
+// thread-block cluster too), warpgroup MMA (wgmma) and its shared-memory operand descriptors.  sm_90a.
 #pragma once
 #include "uvx_common.cuh"
 
@@ -43,6 +43,41 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* tm, in
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::
           "r"(smem_u32(dst)),
       "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
+
+// ---- thread-block clusters (gemm_tc.cu: TMA multicast of the shared operand boxes)
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster: prior writes (mbarrier init, remote arrivals) are visible to the cluster after it
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;" ::: "memory");
+  asm volatile("barrier.cluster.wait.acquire;" ::: "memory");
+}
+// arrive on the mbarrier at the same shared-memory offset as `bar` in CTA `cta` of the cluster (this CTA included).  Default
+// (CTA-scope) release: what it orders are this warp's wgmma reads of the slot, already complete at wgmma.wait_group
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  uint32_t remote;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+}
+// TMA loads whose box lands at the same shared-memory offset in every CTA of `mask` (bit = cluster rank), each of which
+// gets complete_tx on its own mbarrier at the offset of `bar`
+__device__ __forceinline__ void tma_load_2d_mc(void* dst, const CUtensorMap* tm, int c0, int c1, uint64_t* bar, uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;" ::
+          "r"(smem_u32(dst)),
+      "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
+      : "memory");
+}
+__device__ __forceinline__ void tma_load_3d_mc(void* dst, const CUtensorMap* tm, int c0, int c1, int c2, uint64_t* bar, uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5}], [%2], %6;" ::
+          "r"(smem_u32(dst)),
+      "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "h"(mask)
       : "memory");
 }
 
