@@ -265,6 +265,14 @@ int uvx_kv_write(const void* qkv, int64_t row_stride, int64_t k_col, int64_t v_c
  * uvx_sample              out[b] ~ softmax(logits[b] / temperature) restricted to the top_k largest logits (top_k <= 0: all),
  *                         by inverse CDF on the uniform u[step_idx[0] * u_stride + b] (step_idx NULL = 0): the do_sample branch of
  *                         ref:ultravox/inference/infer.py:319-328.  Deterministic given u.
+ * uvx_sample_top_p        uvx_sample with nucleus filtering after the top-k cut, in HF's order (hf:generation/logits_process.py
+ *                         TemperatureLogitsWarper -> TopKLogitsWarper -> TopPLogitsWarper): with P = softmax(logits[b] / temperature)
+ *                         over the top-k survivors, token i stays iff sum_{j: x_j <= x_i} P_j > 1 - top_p, and the largest logit
+ *                         always stays (min_tokens_to_keep = 1, so top_p = 0 is the argmax).  The draw is the inverse CDF of P
+ *                         renormalised over the kept tokens, on the same u as uvx_sample.  0 <= top_p <= 1 (else UVX_ERR_ARG);
+ *                         top_p = 1 is uvx_sample bit for bit.  V <= 2^24.  Ties: equal logits are kept or dropped as one group,
+ *                         whereas HF's unstable sort may split a tie group that straddles the cut - the one intended difference.
+ *                         The masses are summed in 64-bit fixed point (2^-40 resolution), so the result is deterministic given u.
  * uvx_token_finish        tok[b] = done[b] ? pad_id : tok[b]; seq[b, cur_len[0]] = tok[b]; done[b] |= tok[b] in eos_ids;
  *                         cur_len[0]++, step_idx[0]++ (if given), bump{0,1,2}[b]++ (if given: cache slot / visible keys / RoPE
  *                         position); all_done[0] = all(done).                                                                 */
@@ -272,6 +280,8 @@ int uvx_repetition_penalty(float* logits, int64_t B, int64_t V, const int64_t* s
                            float penalty, float* scratch, uvx_stream_t stream);
 int uvx_sample(const float* logits, int64_t B, int64_t V, float temperature, int32_t top_k, const float* u, const int32_t* step_idx,
                int64_t u_stride, int64_t* out_idx, uvx_stream_t stream);
+int uvx_sample_top_p(const float* logits, int64_t B, int64_t V, float temperature, int32_t top_k, float top_p, const float* u,
+                     const int32_t* step_idx, int64_t u_stride, int64_t* out_idx, uvx_stream_t stream);
 int uvx_token_finish(int64_t* tok, int32_t* done, const int64_t* eos_ids, int32_t n_eos, int64_t pad_id, int64_t* seq,
                      int64_t seq_stride, int32_t* cur_len, int32_t* step_idx, int32_t* bump0, int32_t* bump1, int32_t* bump2,
                      int32_t* all_done, int64_t B, uvx_stream_t stream);

@@ -74,6 +74,7 @@ SIGNATURES = {
     "uvx_kv_write": (C.c_int, [c_vp, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_vp]),
     "uvx_repetition_penalty": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_f32, c_vp, c_vp]),
     "uvx_sample": (C.c_int, [c_vp, c_i64, c_i64, c_f32, c_i32, c_vp, c_vp, c_i64, c_vp, c_vp]),
+    "uvx_sample_top_p": (C.c_int, [c_vp, c_i64, c_i64, c_f32, c_i32, c_f32, c_vp, c_vp, c_i64, c_vp, c_vp]),
     "uvx_token_finish": (C.c_int, [c_vp, c_vp, c_vp, c_i32, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
     "uvx_argmax": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_vp]),
     "uvx_rope_bwd": (C.c_int, [c_vp, c_i64, c_i64, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp]),

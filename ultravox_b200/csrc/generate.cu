@@ -4,6 +4,7 @@
 //   uvx_repetition_penalty  hf:generation/logits_process.py RepetitionPenaltyLogitsProcessor (ref ultravox_pipeline.py:95-113)
 //   uvx_sample              temperature / top-k multinomial sampling (ref:ultravox/inference/infer.py:319-328: do_sample when
 //                           temperature > 0; hf:generation/utils.py _sample: softmax(logits / T) -> multinomial)
+//   uvx_sample_top_p        the same with nucleus (top-p) filtering after top-k (hf:generation/logits_process.py TopPLogitsWarper)
 //   uvx_token_finish        EOS / pad bookkeeping of the finished rows, append to `sequences`, advance positions
 #include "uvx_common.cuh"
 
@@ -60,12 +61,17 @@ __device__ __forceinline__ uint32_t f2key(float f) {  // order-preserving float 
 }
 
 // One CTA (1024 threads) per row: max, optional exact k-th-largest threshold by 4-pass radix select on the float keys,
-// sum of exp((x - max) / T) over the kept entries, then the inverse-CDF pick for the uniform u: thread t owns the contiguous
-// chunk [t*c, (t+1)*c), a block scan of the chunk sums finds the chunk, a serial walk finds the index.  Deterministic for a
-// given u (the host draws u from a seeded torch generator).
-__global__ void __launch_bounds__(1024) sample_kernel(const float* __restrict__ logits, int64_t V, float inv_temp, int top_k,
-                                                     const float* __restrict__ u_all, const int32_t* __restrict__ step_idx,
-                                                     int64_t u_stride, int64_t* __restrict__ out) {
+// (TOP_P) optional nucleus threshold by a 4-pass radix select on probability mass, sum of exp((x - max) / T) over the kept
+// entries, then the inverse-CDF pick for the uniform u: thread t owns the contiguous chunk [t*c, (t+1)*c), a block scan of
+// the chunk sums finds the chunk, a serial walk finds the index.  Deterministic for a given u (the host draws u from a
+// seeded torch generator).  sample_kernel<false> is uvx_sample; top_p is read only by sample_kernel<true>.
+constexpr float kMassOne = 1099511627776.f;  // 2^40: fixed-point unit of the top-p mass (sum <= V * 2^40 < 2^64 for V <= 2^24)
+
+template <bool TOP_P>  // (1024, 1): lets ptxas use the 64 registers a lone 1024-thread CTA may have (the top-p form uses 56)
+__global__ void __launch_bounds__(1024, 1) sample_kernel(const float* __restrict__ logits, int64_t V, float inv_temp, int top_k,
+                                                     float top_p, const float* __restrict__ u_all,
+                                                     const int32_t* __restrict__ step_idx, int64_t u_stride,
+                                                     int64_t* __restrict__ out) {
   pdl_trigger();
   pdl_wait();
   __shared__ float red[32];
@@ -111,6 +117,91 @@ __global__ void __launch_bounds__(1024) sample_kernel(const float* __restrict__ 
       __syncthreads();
     }
     thr_key = sel_prefix;
+  }
+  if constexpr (TOP_P) {
+    // ---- top-p threshold over the top-k survivors (HF TopPLogitsWarper after TopKLogitsWarper): with m_i = exp((x_i - max) / T),
+    // the smallest key v such that the mass of the keys <= v exceeds (1 - top_p) * (total mass); keys >= v are kept.  Radix
+    // select from the top byte down: a 256-bin mass histogram of the keys that match the prefix, scanned upward from the mass
+    // carried below the prefix.  Masses are 64-bit fixed point (kMassOne = 1), so the atomics are order-free and the result
+    // deterministic; a tie group has one key and is kept or dropped whole.  Entries whose mass rounds to 0 never cross the
+    // threshold and are skipped.  target <= total - 1 makes the maximum (mass exactly kMassOne) always kept: top_p = 0 -> argmax.
+    __shared__ unsigned long long mhist[256];
+    __shared__ unsigned long long p_below, p_target;
+    __shared__ uint32_t p_prefix;
+    if (tid == 0) { p_prefix = 0u; p_below = 0ull; p_target = 0ull; }
+    for (int pass = 3; pass >= 0; --pass) {
+      if (tid < 256) mhist[tid] = 0ull;
+      __syncthreads();
+      const uint32_t prefix = p_prefix;
+      const uint32_t hi_mask = pass == 3 ? 0u : (0xFFFFFFFFu << ((pass + 1) * 8));
+      // a per-thread cache of 4 (bin, mass) slots in registers: without top-k most of the row carries mass, and the first pass
+      // puts it in the few top-byte bins its exponents span, where shared atomics would serialise on a handful of addresses
+      uint32_t cb[4] = {~0u, ~0u, ~0u, ~0u};
+      unsigned long long cs[4] = {0ull, 0ull, 0ull, 0ull};
+      constexpr int kLoads = 8;  // independent loads in flight per thread: one at a time, a pass is bound by L2 latency
+      for (int64_t base = tid; base < V; base += 1024 * kLoads) {
+        float xs[kLoads];
+#pragma unroll
+        for (int j = 0; j < kLoads; ++j) {
+          const int64_t i = base + (int64_t)j * 1024;
+          xs[j] = i < V ? row[i] : -INFINITY;
+        }
+#pragma unroll
+        for (int j = 0; j < kLoads; ++j) {
+          const float x = xs[j];
+          const uint32_t k = f2key(x);
+          if (base + (int64_t)j * 1024 >= V || k < thr_key || (k & hi_mask) != (prefix & hi_mask)) continue;
+          const unsigned long long m = __float2ull_rn(__expf((x - mx) * inv_temp) * kMassOne);
+          if (m == 0ull) continue;
+          const uint32_t bin = (k >> (pass * 8)) & 255u;
+          bool held = false;
+#pragma unroll
+          for (int s = 0; s < 4; ++s)
+            if (!held && cb[s] == bin) { cs[s] += m; held = true; }
+#pragma unroll
+          for (int s = 0; s < 4; ++s)
+            if (!held && cs[s] == 0ull) { cb[s] = bin; cs[s] = m; held = true; }
+          if (!held) atomicAdd(&mhist[bin], m);
+        }
+      }
+#pragma unroll
+      for (int s = 0; s < 4; ++s)
+        if (cs[s] != 0ull) atomicAdd(&mhist[cb[s]], cs[s]);
+      __syncthreads();
+      if (w == 0) {  // lane l scans bins [8l, 8l + 8)
+        unsigned long long s = 0ull;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) s += mhist[lane * 8 + j];
+        unsigned long long incl = s;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+          const unsigned long long t = __shfl_up_sync(0xffffffffu, incl, o);
+          if (lane >= o) incl += t;
+        }
+        if (pass == 3) {  // the first pass sees every survivor: its histogram total is the whole mass
+          const unsigned long long total = __shfl_sync(0xffffffffu, incl, 31);
+          if (lane == 0 && total > 0ull) {
+            const unsigned long long t = (unsigned long long)((1.0 - (double)top_p) * (double)total);
+            p_target = t < total - 1ull ? t : total - 1ull;
+          }
+          __syncwarp();
+        }
+        const unsigned long long below = p_below, target = p_target;
+        const unsigned hit = __ballot_sync(0xffffffffu, below + incl > target);
+        if (hit != 0u && lane == __ffs(hit) - 1) {  // no hit only for a row without mass (all -inf): no top-p cut
+          unsigned long long acc = below + incl - s;
+          int d = lane * 8;
+          for (; d < lane * 8 + 7; ++d) {
+            if (acc + mhist[d] > target) break;
+            acc += mhist[d];
+          }
+          p_prefix = prefix | ((uint32_t)d << (pass * 8));
+          p_below = acc;
+        }
+      }
+      __syncthreads();
+    }
+    thr_key = max(thr_key, p_prefix);
   }
   // ---- chunk sums
   const int64_t c = (V + 1023) / 1024;
@@ -232,9 +323,21 @@ extern "C" int uvx_sample(const float* logits, int64_t B, int64_t V, float tempe
                           const int32_t* step_idx, int64_t u_stride, int64_t* out_idx, uvx_stream_t stream) {
   using namespace uvx;
   UVX_REQUIRE(logits && u && out_idx && B >= 1 && V >= 1 && temperature > 0.f, "uvx_sample: bad arguments");
-  launch_k(sample_kernel, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, 1.0f / temperature, (int)top_k, u,
-           step_idx, u_stride, out_idx);
+  launch_k(sample_kernel<false>, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, 1.0f / temperature, (int)top_k,
+           1.0f, u, step_idx, u_stride, out_idx);
   return check_launch("sample_kernel");
+}
+
+extern "C" int uvx_sample_top_p(const float* logits, int64_t B, int64_t V, float temperature, int32_t top_k, float top_p,
+                                const float* u, const int32_t* step_idx, int64_t u_stride, int64_t* out_idx, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(logits && u && out_idx && B >= 1 && V >= 1 && V <= (int64_t)1 << 24 && temperature > 0.f && top_p >= 0.f &&
+                  top_p <= 1.f,
+              "uvx_sample_top_p: bad arguments");
+  if (top_p >= 1.f) return uvx_sample(logits, B, V, temperature, top_k, u, step_idx, u_stride, out_idx, stream);
+  launch_k(sample_kernel<true>, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, 1.0f / temperature, (int)top_k,
+           top_p, u, step_idx, u_stride, out_idx);
+  return check_launch("sample_kernel_top_p");
 }
 
 extern "C" int uvx_token_finish(int64_t* tok, int32_t* done, const int64_t* eos_ids, int32_t n_eos, int64_t pad_id, int64_t* seq,

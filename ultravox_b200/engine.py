@@ -114,12 +114,13 @@ class DecodeEngine:
     the graph changes between steps and the host never has to synchronise inside the loop.  Linear layers are weight-streaming
     matrix-vector kernels (uvx_gemv_bf16, slabs of 8 streams).  This is the serving loop of ``LocalInference._generate``
     (ref:ultravox/inference/infer.py:309-342 -> ``GenerationMixin.generate``): greedy when ``temperature in {None, 0}``,
-    multinomial sampling otherwise; repetition penalty as the reference pipeline sets it (ref ultravox_pipeline.py:95-113);
-    left-padded batches (``kv_start`` + mask-derived RoPE positions, hf:generation/utils.py:707-729)."""
+    multinomial sampling otherwise (top-k, then top-p when ``top_p < 1``); repetition penalty as the reference pipeline sets it
+    (ref ultravox_pipeline.py:95-113); left-padded batches (``kv_start`` + mask-derived RoPE positions,
+    hf:generation/utils.py:707-729)."""
 
     def __init__(self, model: UltravoxModel, batch: int, max_len: int, use_graph: bool = True, cache=None,
                  eos_token_ids=None, pad_token_id: int = 0, temperature: float = 0.0, top_k: int = 0,
-                 repetition_penalty: float = 1.0, generator: Optional[torch.Generator] = None):
+                 repetition_penalty: float = 1.0, generator: Optional[torch.Generator] = None, top_p: Optional[float] = None):
         self.model, self.B = model, batch
         dev = model.device
         self.cache = cache if cache is not None else model.new_cache(batch, max_len)
@@ -138,6 +139,9 @@ class DecodeEngine:
         self.eos = torch.tensor(eos, dtype=torch.int64, device=dev) if eos else None
         self.pad_id = int(pad_token_id)
         self.temperature, self.top_k = float(temperature or 0.0), int(top_k or 0)
+        self.top_p = 1.0 if top_p is None else float(top_p)         # a kernel argument of the captured step, like top_k
+        if not 0.0 <= self.top_p <= 1.0:
+            raise ValueError(f"top_p must be in [0, 1], got {top_p}")
         self.penalty = float(repetition_penalty or 1.0)
         self.u = None
         if self.temperature > 0:
@@ -189,7 +193,7 @@ class DecodeEngine:
             ops.repetition_penalty_(logits, self.seq, self.cur_len, self.penalty, self.scratch)
         tok = self.token.view(-1)
         if self.temperature > 0:
-            ops.sample(logits, self.temperature, self.top_k, self.u, self.step_idx, out=tok)
+            ops.sample(logits, self.temperature, self.top_k, self.u, self.step_idx, out=tok, top_p=self.top_p)
         else:
             ops.argmax(logits, out=tok)
         ops.token_finish(tok, self.done, self.eos, self.pad_id, self.seq, self.cur_len, self.step_idx,

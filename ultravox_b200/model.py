@@ -880,7 +880,11 @@ class UltravoxModel(nn.Module):
 
         Greedy when ``do_sample`` is false (the reference's default: temperature None / 0, ref infer.py:319-328); with
         ``do_sample=True`` tokens are drawn from softmax(logits / temperature) over the ``top_k`` largest logits (HF
-        ``GenerationConfig`` defaults: temperature 1.0, top_k 50), reproducibly for a seeded ``generator``.
+        ``GenerationConfig`` defaults: temperature 1.0, top_k 50), reproducibly for a seeded ``generator``.  ``top_p < 1``
+        then keeps the nucleus of that distribution, as HF's ``TopPLogitsWarper`` after ``TopKLogitsWarper``: the smallest
+        set of largest logits whose probability exceeds ``top_p`` (always the largest one, so ``top_p=0`` is greedy; a tie
+        group at the cut is kept whole).  ``top_p`` must lie in [0, 1] (``ValueError`` otherwise); it is ignored when not
+        sampling, and ``None`` or 1.0 means no nucleus filter.
         ``past_key_values``: conversation KV reuse (ref infer.py:126-148): the cache already holds the first
         ``past_key_values.length`` positions of ``input_ids`` (earlier turns incl. the reply), so only the new suffix is
         embedded, spliced and prefilled; ``return_dict_in_generate=True`` hands the cache back for the next turn.
@@ -894,11 +898,12 @@ class UltravoxModel(nn.Module):
         unknown = [k for k, v in kwargs.items() if isinstance(v, torch.Tensor)]
         if unknown:
             raise TypeError(f"generate() got unexpected tensor arguments {unknown}")
-        if top_p is not None and float(top_p) < 1.0:
-            raise NotImplementedError("top_p (nucleus) filtering is not built; use top_k")
+        if top_p is not None and not 0.0 <= float(top_p) <= 1.0:       # NaN fails too
+            raise ValueError(f"`top_p` has to be a float in [0, 1], but is {top_p}")
         sampling = bool(do_sample) and (temperature is None or float(temperature) > 0)
         temp = (1.0 if temperature is None else float(temperature)) if sampling else 0.0
         k_top = (50 if top_k is None else int(top_k)) if sampling else 0
+        p_top = float(top_p) if sampling and top_p is not None else 1.0
         dev = self.device
         input_ids = input_ids.to(dev)
         B, S = input_ids.shape
@@ -941,7 +946,8 @@ class UltravoxModel(nn.Module):
         eos = sorted(set([eos_token_id] if isinstance(eos_token_id, int) else (eos_token_id or [])))
         pad_id = pad_token_id if pad_token_id is not None else (min(eos) if eos else 0)
         eng = DecodeEngine(self, B, cache.capacity, use_graph=use_graph, cache=cache, eos_token_ids=eos, pad_token_id=pad_id,
-                           temperature=temp, top_k=k_top, repetition_penalty=repetition_penalty or 1.0, generator=generator)
+                           temperature=temp, top_k=k_top, top_p=p_top, repetition_penalty=repetition_penalty or 1.0,
+                           generator=generator)
         if streamer is not None:
             streamer.put(input_ids)
         tok = eng.begin(input_ids, out.logits.view(B, -1), kv_start)

@@ -608,14 +608,20 @@ def repetition_penalty_(logits: torch.Tensor, seq: torch.Tensor, cur_len: torch.
 
 
 def sample(logits: torch.Tensor, temperature: float, top_k: int, u: torch.Tensor, step_idx: Optional[torch.Tensor] = None,
-           out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """logits [B, V] fp32, u [steps, B] (or [B]) uniforms in [0, 1) -> sampled ids [B] int64."""
+           out: Optional[torch.Tensor] = None, top_p: float = 1.0) -> torch.Tensor:
+    """logits [B, V] fp32, u [steps, B] (or [B]) uniforms in [0, 1) -> sampled ids [B] int64.  ``top_p < 1`` adds nucleus
+    filtering after the top-k cut (``uvx_sample_top_p``); ``top_p >= 1`` is plain ``uvx_sample``."""
     _cuda(logits, torch.float32, "logits"), _cuda(u, torch.float32, "u")
     B, V = logits.shape
     if out is None:
         out = torch.empty(B, dtype=torch.int64, device=logits.device)
-    check(lib().uvx_sample(logits.data_ptr(), B, V, float(temperature), int(top_k or 0), u.data_ptr(), _p(step_idx),
-                           u.stride(0) if u.dim() == 2 else 0, out.data_ptr(), _stream()), "uvx_sample")
+    u_stride = u.stride(0) if u.dim() == 2 else 0
+    if top_p >= 1.0:
+        check(lib().uvx_sample(logits.data_ptr(), B, V, float(temperature), int(top_k or 0), u.data_ptr(), _p(step_idx), u_stride,
+                               out.data_ptr(), _stream()), "uvx_sample")
+    else:
+        check(lib().uvx_sample_top_p(logits.data_ptr(), B, V, float(temperature), int(top_k or 0), float(top_p), u.data_ptr(),
+                                     _p(step_idx), u_stride, out.data_ptr(), _stream()), "uvx_sample_top_p")
     return out
 
 
