@@ -319,7 +319,9 @@ int uvx_attention_bwd(const uvx_attn_args* a, const void* o, const void* dout, v
 int uvx_transpose_bf16(const void* in, int64_t rows, int64_t cols, int64_t in_row_stride, void* out,
                        int64_t out_row_stride, uvx_stream_t stream);
 /* dx = dres + d(rmsnorm)/dx . dy (dx may be NULL), dw[cols] += sum_rows dy * xhat (fp32, dw may be NULL);
- * group_* as in uvx_rmsnorm (stack mode: no dx).                                                              */
+ * dy / dres / dx are dense [rows, cols].  group_* as in uvx_rmsnorm; in stack mode dx is written in the stacked
+ * layout [rows, cols] (the frames of a group in order, the zero tail of the last row included), which the
+ * projector backward views as [N, group_rows * stack, C] to get d(encoder output).                          */
 int uvx_rmsnorm_bwd(const void* dy, const void* x, const void* w, const void* dres, void* dx, float* dw,
                     int64_t rows, int64_t cols, int64_t x_row_stride, int64_t group_rows, int64_t group_stride,
                     int64_t valid_elems, float eps, uvx_stream_t stream);

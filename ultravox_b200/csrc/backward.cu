@@ -31,7 +31,7 @@ __global__ void transpose_kernel(const bf16* __restrict__ in, int64_t rows, int6
 // ------------------------------------------------------------------------------------- RMSNorm backward
 // y = w * bf16(x * rstd); dx = rstd * (g - xhat * mean(g * xhat)) with g = dy * w, xhat = x * rstd.
 // Optional: dres is added to dx (residual-stream gradient), dw[cols] += sum_rows dy * xhat (fp32 atomics, one per
-// column per CTA of kRowsPerCta rows).  Stack mode as in rmsnorm_kernel (elements past `valid` are zero, no dx needed).
+// column per CTA of kRowsPerCta rows).  Stack mode as in rmsnorm_kernel (elements past `valid` are zero); dx is stacked.
 static constexpr int kNbThreads = 256;
 static constexpr int kNbMaxVec = 5;  // up to 256*5*8 = 10240 columns
 static constexpr int kRowsPerCta = 8;

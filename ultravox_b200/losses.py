@@ -16,7 +16,11 @@ def causal_lm_loss(logits: torch.Tensor, labels: torch.Tensor, ignore_index: int
         logits = logits[None]
         labels = labels.reshape(1, -1)
     B, S, V = logits.shape
+    if labels.shape != (B, S):
+        raise ValueError(f"labels {tuple(labels.shape)} do not match logits {tuple(logits.shape)}")
     lg = logits.reshape(B * S, V)
+    if lg.stride(-1) != 1 or lg.stride(0) % 4 != 0 or lg.data_ptr() % 16 != 0:
+        lg = lg.contiguous()                      # the kernels read unit-stride rows with 128-bit loads
     labels = labels.contiguous()
     row_loss = torch.empty(B * S, dtype=torch.float32, device=logits.device)
     row_lse = torch.empty_like(row_loss)
@@ -62,6 +66,10 @@ def kl_distill_loss(student: torch.Tensor, teacher: torch.Tensor, is_eot: torch.
     """KL(teacher || student) at temperature T, "batchmean" over the rows, + eot_loss_weight x the same over the EOT rows
     (ref ultravox_model.py:228-255).  student / teacher: [R, V] fp32 rows gathered at the prediction positions."""
     _cuda(student, torch.float32, "student"), _cuda(teacher, torch.float32, "teacher")
+    if student.dim() != 2 or teacher.shape != student.shape:
+        raise ValueError(f"student {tuple(student.shape)} and teacher {tuple(teacher.shape)} must be the same [R, V]")
+    # the kernels take ONE row stride for both: hand them contiguous rows (a no-op for the lm_head outputs of training)
+    student, teacher = student.contiguous(), teacher.contiguous()
     R, V = student.shape
     n_eot = int(is_eot.sum())
     w = torch.full((R,), 1.0 / R, dtype=torch.float32)

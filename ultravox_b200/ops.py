@@ -416,14 +416,28 @@ def transpose(x: torch.Tensor, out: Optional[torch.Tensor] = None, pad_cols_to: 
 def rmsnorm_bwd(dy: torch.Tensor, x: torch.Tensor, w: torch.Tensor, eps: float, dres: Optional[torch.Tensor] = None,
                 want_dx: bool = True, dw: Optional[torch.Tensor] = None, stack: Optional[tuple] = None,
                 out: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
-    """dx (bf16, + dres) and/or dw (fp32, accumulated) of uvx_rmsnorm.  ``stack=(group_rows, T*C)`` for ln_pre."""
-    _cuda(dy, BF16, "dy")
+    """dx (bf16, + dres) and/or dw (fp32, accumulated) of uvx_rmsnorm.  ``stack=(group_rows, T*C)`` for ln_pre: x is the
+    encoder output [N, T, C] and dx comes back in the stacked layout [N * group_rows, stack * C]."""
+    _cuda(dy, BF16, "dy"), _cuda(x, BF16, "x")
     cols = dy.shape[-1]
+    dy = dy.contiguous()                          # the kernel reads dy / dres / dx as dense [rows, cols]
     rows = dy.numel() // cols
+    if dres is not None:
+        assert dres.shape == dy.shape, "dres must have dy's shape"
+        dres = dres.contiguous()
     if want_dx and out is None:
         out = torch.empty(dy.shape, dtype=BF16, device=dy.device)
+    assert not want_dx or (out.is_contiguous() and out.numel() == dy.numel()), "out must be a dense [rows, cols] buffer"
+    assert dw is None or (dw.dtype == torch.float32 and dw.is_contiguous() and dw.numel() == cols)
     g_rows, g_stride, valid = (stack[0], stack[1], stack[1]) if stack else (0, 0, 0)
-    xs = cols if stack else x.reshape(-1, cols).stride(0)
+    if stack:
+        x = x.contiguous()
+        xs = cols
+    else:
+        x = x.reshape(-1, cols)
+        if x.stride(-1) != 1 or x.stride(0) % 8 != 0:
+            x = x.contiguous()
+        xs = x.stride(0)
     check(lib().uvx_rmsnorm_bwd(dy.data_ptr(), x.data_ptr(), w.data_ptr(), _p(dres), _p(out) if want_dx else None, _p(dw), rows,
                                 cols, xs, g_rows, g_stride, valid, eps, _stream()), "uvx_rmsnorm_bwd")
     return out if want_dx else None
@@ -463,10 +477,16 @@ def gelu_bwd(x: torch.Tensor, dy: torch.Tensor, out: Optional[torch.Tensor] = No
 
 
 def swiglu_bwd(x: torch.Tensor, dout: torch.Tensor, gate_first: bool, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    _cuda(x, BF16, "x"), _cuda(dout, BF16, "dout")
     H = x.shape[-1] // 2
     x2 = x.reshape(-1, 2 * H)
+    if x2.stride(-1) != 1 or x2.stride(0) % 8 != 0:
+        x2 = x2.contiguous()
+    assert dout.numel() == x2.shape[0] * H, "dout must be [rows, H]"
+    dout = dout.contiguous()                      # the kernel reads dout as dense [rows, H]
     if out is None:
         out = torch.empty(x2.shape, dtype=BF16, device=x.device)
+    assert out.is_contiguous() and out.numel() == x2.numel(), "out must be a dense [rows, 2H] buffer"
     check(lib().uvx_swiglu_bwd(x2.data_ptr(), dout.data_ptr(), out.data_ptr(), x2.shape[0], H, x2.stride(0), int(gate_first),
                                _stream()), "uvx_swiglu_bwd")
     return out
@@ -498,10 +518,15 @@ def attention_fused_qkv_bwd(qkv: torch.Tensor, o: torch.Tensor, dout: torch.Tens
                             Hkv: int, D: int, scale: float, causal: bool, dqkv: Optional[torch.Tensor] = None,
                             kv_len: Optional[torch.Tensor] = None) -> torch.Tensor:
     """dqkv [B*S, (Hq+2Hkv)*D] (same fused layout as qkv) from dout [B*S, Hq*D]."""
+    _cuda(qkv, BF16, "qkv"), _cuda(o, BF16, "o"), _cuda(dout, BF16, "dout"), _cuda(lse, torch.float32, "lse")
+    assert qkv.shape[-1] == (Hq + 2 * Hkv) * D and qkv.stride(-1) == 1
+    assert o.numel() == dout.numel() == B * S * Hq * D and lse.numel() == B * Hq * S and lse.is_contiguous()
+    o, dout = o.contiguous(), dout.contiguous()  # o and dout are read as dense [B*S, Hq*D]
     rs = qkv.stride(-2)
     base = qkv.data_ptr()
     if dqkv is None:
         dqkv = torch.empty_like(qkv)
+    assert dqkv.shape == qkv.shape and dqkv.stride(-1) == 1
     a = AttnArgs()
     a.q, a.k, a.v, a.o = base, base + 2 * Hq * D, base + 2 * (Hq + Hkv) * D, o.data_ptr()
     a.B, a.Hq, a.Hkv, a.Sq, a.Skv, a.D = B, Hq, Hkv, S, S, D
