@@ -286,6 +286,42 @@ int uvx_token_finish(int64_t* tok, int32_t* done, const int64_t* eos_ids, int32_
                      int64_t seq_stride, int32_t* cur_len, int32_t* step_idx, int32_t* bump0, int32_t* bump1, int32_t* bump2,
                      int32_t* all_done, int64_t B, uvx_stream_t stream);
 
+/* Beam search (hf:generation/utils.py _beam_search, transformers 5.5, and the helpers above it), one decode step as four
+ * launches that read every per-step scalar from device memory.  B prompts, nb <= 8 beams each: row r = b * nb + j.
+ * uvx_log_softmax   out[r] = log_softmax(in[r]) in fp32 (in == out allowed).  Beam search scores log-probs; the repetition
+ *                   penalty (uvx_repetition_penalty on the running sequences) then applies to these, not to the logits.
+ * uvx_beam_select   per prompt, the K (1 <= K <= 64, K <= V) largest a[b, j * V + v] = logprobs[r, v] + run_score[r] (one
+ *                   fp32 add), sorted descending: out_s[b, :K] the values, out_i[b, :K] the flat index j * V + v.
+ *                   row_s / row_i [B * nb * K] are scratch (the per-row top K, merged per prompt).
+ * uvx_beam_update   one CTA per prompt on the K candidates (K = max(2, 1 + n_eos) * nb): a candidate hits the stopping criteria
+ *                   if its token is in eos_ids or step_idx[0] + 1 >= max_new; the next running beams are the top nb of
+ *                   score + hit * -1e9 (run_score, tok, parent = the source row, run_seq rows gathered by parent and extended at
+ *                   cur_len[0]); the finished pool (pool_seq / pool_score / pool_len = generated length / pool_fin) keeps the top
+ *                   nb of itself merged with score / len_div[step_idx + 1] + the -1e9 masks (early_stopping 1 and a full pool,
+ *                   heur[b] cleared, not a top-nb finisher).  heur[b] &= the early-stop heuristic (early_stopping 0 = False,
+ *                   1 = True, 2 = "never"; lp_positive = length_penalty > 0), evaluated at the new length with the divisor
+ *                   len_div[len] = fp32(double(len) ** length_penalty).  The last prompt's CTA writes done[0] = !(loop
+ *                   condition over the batch), advances cur_len[0] and step_idx[0] and resets ticket[0] (0 before the first
+ *                   launch); bump{0,1,2}[r]++ (if given).  flags [B] is scratch.  While done[0] is set a launch changes nothing
+ *                   but parent, which becomes the identity.  All scores are fp32 in HF's operation order.
+ * uvx_kv_reorder    k / v caches [L, B * nb, S_max, row_elems] bf16 (contiguous): row r <- row parent[r] (parent in the same
+ *                   prompt) at positions [0, n_pos[0]), in place, for every layer in one launch.  A row whose parent is itself
+ *                   is not written, and is read only when another beam descends from it; positions >= n_pos[0] are untouched.
+ *                   With parent[b * nb + j] = b * nb it broadcasts each prompt's prefilled row to its beams.
+ * Ties: where two values are exactly equal (in both selections and in the pool merge) the lower flat / candidate / merged
+ * index ranks first.  torch.topk leaves that order unspecified; in a search it matters only at a top-k cut.               */
+int uvx_log_softmax(const float* in, float* out, int64_t rows, int64_t V, uvx_stream_t stream);
+int uvx_beam_select(const float* logprobs, int64_t B, int32_t nb, int64_t V, const float* run_score, int32_t K, float* row_s,
+                    int64_t* row_i, float* out_s, int64_t* out_i, uvx_stream_t stream);
+int uvx_beam_update(const float* cand_s, const int64_t* cand_i, int64_t B, int32_t nb, int32_t K, int64_t V, const int64_t* eos_ids,
+                    int32_t n_eos, int32_t max_new, const float* len_div, int32_t early_stopping, int32_t lp_positive,
+                    float* run_score, int64_t* run_seq, int64_t* pool_seq, int64_t seq_stride, float* pool_score, int32_t* pool_len,
+                    int32_t* pool_fin, int32_t* parent, int64_t* tok, int32_t* heur, int32_t* flags, uint32_t* ticket,
+                    int32_t* cur_len, int32_t* step_idx, int32_t* bump0, int32_t* bump1, int32_t* bump2, int32_t* done,
+                    uvx_stream_t stream);
+int uvx_kv_reorder(void* k_cache, void* v_cache, int64_t L, int64_t B, int32_t nb, int64_t S_max, int64_t row_elems,
+                   const int32_t* parent, const int32_t* n_pos, uvx_stream_t stream);
+
 /* Shifted causal-LM cross entropy (hf:loss/loss_utils.py:28-67; called through LlamaForCausalLM.forward(labels=)
  * from ref:ultravox/model/ultravox_model.py:328-334).  logits [B*S, V] fp32 (row_stride elements), labels [B, S]
  * un-shifted (the shift and the ignore_index padding happen inside).  row_loss/row_lse [B*S] are kept for the

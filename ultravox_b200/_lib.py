@@ -76,6 +76,12 @@ SIGNATURES = {
     "uvx_sample": (C.c_int, [c_vp, c_i64, c_i64, c_f32, c_i32, c_vp, c_vp, c_i64, c_vp, c_vp]),
     "uvx_sample_top_p": (C.c_int, [c_vp, c_i64, c_i64, c_f32, c_i32, c_f32, c_vp, c_vp, c_i64, c_vp, c_vp]),
     "uvx_token_finish": (C.c_int, [c_vp, c_vp, c_vp, c_i32, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
+    "uvx_log_softmax": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_vp]),
+    "uvx_beam_select": (C.c_int, [c_vp, c_i64, c_i32, c_i64, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "uvx_beam_update": (C.c_int, [c_vp, c_vp, c_i64, c_i32, c_i32, c_i64, c_vp, c_i32, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp,
+                                  c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                  c_vp]),
+    "uvx_kv_reorder": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_i32, c_i64, c_i64, c_vp, c_vp, c_vp]),
     "uvx_argmax": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_vp]),
     "uvx_rope_bwd": (C.c_int, [c_vp, c_i64, c_i64, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp]),
     "uvx_attention_bwd": (C.c_int, [C.POINTER(AttnArgs), c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64,

@@ -6,6 +6,10 @@
 //                           temperature > 0; hf:generation/utils.py _sample: softmax(logits / T) -> multinomial)
 //   uvx_sample_top_p        the same with nucleus (top-p) filtering after top-k (hf:generation/logits_process.py TopPLogitsWarper)
 //   uvx_token_finish        EOS / pad bookkeeping of the finished rows, append to `sequences`, advance positions
+//   uvx_log_softmax         beam search scores: log_softmax over each logits row (hf:generation/utils.py _beam_search)
+//   uvx_beam_select         the top K of (log-prob + running beam score) over each prompt's nb * V continuations
+//   uvx_beam_update         running beams, finished-hypothesis pool, early-stop heuristic and loop condition of one step
+//   uvx_kv_reorder          in-place gather of the KV cache rows by parent beam (and the prefill broadcast to the beams)
 #include "uvx_common.cuh"
 
 namespace uvx {
@@ -294,6 +298,362 @@ __global__ void token_finish_kernel(int64_t* __restrict__ tok, int32_t* __restri
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// Beam search (hf:generation/utils.py _beam_search and the helpers above it).  Row r = b * nb + j is beam j of prompt b.
+// Inputs written by the preceding kernel are plain (not const __restrict__) pointers: nvcc may hoist a read-only (.nc)
+// load above griddepcontrol.wait, and under PDL that reads the previous kernel's output before it is complete.
+constexpr int kBeamMax = 8;     // beams per prompt
+constexpr int kBeamMaxK = 64;   // candidates per prompt, K = max(2, 1 + n_eos) * nb
+constexpr int kSeqChunk = 128;  // token positions staged per round by beam_update_kernel
+
+// One CTA per row: y = (x - max) - log(sum exp(x - max)), in fp32 (in == out allowed).
+__global__ void __launch_bounds__(1024) log_softmax_kernel(const float* in, float* out, int64_t V) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ float red[32];
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  const float* x = in + (int64_t)blockIdx.x * V;
+  float* y = out + (int64_t)blockIdx.x * V;
+  float mx = -INFINITY;
+  for (int64_t i = tid; i < V; i += 1024) mx = fmaxf(mx, x[i]);
+  mx = warp_max(mx);
+  if (lane == 0) red[w] = mx;
+  __syncthreads();
+  mx = warp_max(red[lane]);
+  __syncthreads();
+  float s = 0.f;
+  for (int64_t i = tid; i < V; i += 1024) s += expf(x[i] - mx);
+  s = warp_sum(s);
+  if (lane == 0) red[w] = s;
+  __syncthreads();
+  const float lse = logf(warp_sum(red[lane]));
+  for (int64_t i = tid; i < V; i += 1024) y[i] = (x[i] - mx) - lse;
+}
+
+// One CTA (1024 threads) per row: the K largest of lp[r, v] + run_score[r] (one fp32 add, as HF adds the running score),
+// sorted by (value desc, v asc).  The K-th largest key comes from the 4-pass radix select of sample_kernel; the keys above it
+// (fewer than K) are appended in any order, the missing ones are taken from the keys equal to it in index order (thread t
+// owns the chunk [t*c, (t+1)*c), an exclusive scan of the per-chunk counts ranks them), and the K survivors are sorted by
+// rank.  out_i holds the prompt-flat index j * V + v.
+__global__ void __launch_bounds__(1024, 1) beam_row_topk_kernel(const float* lp, int64_t V, const float* run_score, int nb, int K,
+                                                                float* __restrict__ out_s, int64_t* __restrict__ out_i) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ uint32_t hist[256];
+  __shared__ uint32_t sel_prefix, sel_remaining;
+  __shared__ int n_gt;
+  __shared__ int scan[32];
+  __shared__ float s_val[kBeamMaxK];
+  __shared__ int64_t s_idx[kBeamMaxK];
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  const int64_t r = blockIdx.x;
+  const float* row = lp + r * V;
+  const float sc = run_score[r];
+  if (tid == 0) { sel_prefix = 0u; sel_remaining = (uint32_t)K; n_gt = 0; }
+  for (int pass = 3; pass >= 0; --pass) {
+    if (tid < 256) hist[tid] = 0u;
+    __syncthreads();
+    const uint32_t prefix = sel_prefix;
+    const uint32_t hi_mask = pass == 3 ? 0u : (0xFFFFFFFFu << ((pass + 1) * 8));
+    for (int64_t i = tid; i < V; i += 1024) {
+      const uint32_t k = f2key(row[i] + sc);
+      if ((k & hi_mask) == (prefix & hi_mask)) atomicAdd(&hist[(k >> (pass * 8)) & 255u], 1u);
+    }
+    __syncthreads();
+    if (tid == 0) {
+      uint32_t rem = sel_remaining;
+      int d = 255;
+      for (; d > 0; --d) {
+        if (hist[d] >= rem) break;
+        rem -= hist[d];
+      }
+      sel_prefix = prefix | ((uint32_t)d << (pass * 8));
+      sel_remaining = rem;
+    }
+    __syncthreads();
+  }
+  const uint32_t thr = sel_prefix;
+  const int need_eq = (int)sel_remaining;  // keys equal to thr to take; K - need_eq keys lie above it
+  for (int64_t i = tid; i < V; i += 1024) {
+    const float x = row[i] + sc;
+    if (f2key(x) > thr) {
+      const int s = atomicAdd(&n_gt, 1);
+      s_val[s] = x;
+      s_idx[s] = i;
+    }
+  }
+  const int64_t c = (V + 1023) / 1024;
+  const int64_t lo = (int64_t)tid * c, hi = lo + c < V ? lo + c : V;
+  int cnt = 0;
+  for (int64_t i = lo; i < hi; ++i) cnt += f2key(row[i] + sc) == thr;
+  int incl = cnt;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += t;
+  }
+  if (lane == 31) scan[w] = incl;
+  __syncthreads();
+  if (w == 0) {
+    const int v = scan[lane];
+    int s = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, s, o);
+      if (lane >= o) s += t;
+    }
+    scan[lane] = s - v;
+  }
+  __syncthreads();
+  int rank = scan[w] + incl - cnt;
+  const int base = K - need_eq;
+  for (int64_t i = lo; i < hi && rank < need_eq; ++i) {
+    const float x = row[i] + sc;
+    if (f2key(x) == thr) {
+      s_val[base + rank] = x;
+      s_idx[base + rank] = i;
+      ++rank;
+    }
+  }
+  __syncthreads();
+  if (tid < K) {
+    const float x = s_val[tid];
+    const int64_t ix = s_idx[tid];
+    int pos = 0;
+    for (int m = 0; m < K; ++m) pos += s_val[m] > x || (s_val[m] == x && s_idx[m] < ix);
+    out_s[r * K + pos] = x;
+    out_i[r * K + pos] = (r % nb) * V + ix;
+  }
+}
+
+// One CTA per prompt: the top K of its nb row lists (nb * K entries), by (value desc, flat index asc).
+__global__ void __launch_bounds__(kBeamMax * kBeamMaxK) beam_merge_kernel(const float* row_s, const int64_t* row_i, int nb, int K,
+                                                                          float* __restrict__ out_s, int64_t* __restrict__ out_i) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ float sv[kBeamMax * kBeamMaxK];
+  __shared__ int64_t si[kBeamMax * kBeamMaxK];
+  const int64_t b = blockIdx.x;
+  const int n = nb * K;
+  for (int t = threadIdx.x; t < n; t += blockDim.x) {
+    sv[t] = row_s[b * n + t];
+    si[t] = row_i[b * n + t];
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < n; t += blockDim.x) {
+    const float x = sv[t];
+    const int64_t ix = si[t];
+    int pos = 0;
+    for (int m = 0; m < n; ++m) pos += sv[m] > x || (sv[m] == x && si[m] < ix);
+    if (pos < K) {
+      out_s[b * K + pos] = x;
+      out_i[b * K + pos] = ix;
+    }
+  }
+}
+
+// One CTA per prompt: steps d-g of one _beam_search iteration on the K sorted candidates of uvx_beam_select.  Every fp32
+// operation is HF's, in HF's order; top-k ties are broken towards the lower index.  The last CTA to finish (ticket) folds the
+// per-prompt flags into the loop condition and advances the step counters.  With done[0] set nothing changes except parent,
+// which becomes the identity (so the uvx_kv_reorder that follows is a no-op).
+__global__ void __launch_bounds__(256) beam_update_kernel(
+    const float* cand_s, const int64_t* cand_i, int64_t V, int nb, int K, const int64_t* __restrict__ eos,
+    int n_eos, int max_new, const float* __restrict__ len_div, int early_stopping, int lp_positive, float* __restrict__ run_score,
+    int64_t* __restrict__ run_seq, int64_t* __restrict__ pool_seq, int64_t seq_stride, float* __restrict__ pool_score,
+    int32_t* __restrict__ pool_len, int32_t* __restrict__ pool_fin, int32_t* __restrict__ parent, int64_t* __restrict__ tok,
+    int32_t* __restrict__ heur, int32_t* __restrict__ flags, uint32_t* __restrict__ ticket, int32_t* __restrict__ cur_len,
+    int32_t* __restrict__ step_idx, int32_t* __restrict__ bump0, int32_t* __restrict__ bump1, int32_t* __restrict__ bump2,
+    int32_t* __restrict__ done, int64_t B) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ float rsc[kBeamMaxK], psc[kBeamMaxK];  // running-selection / pool-merge scores of the candidates
+  __shared__ int cj[kBeamMaxK], chit[kBeamMaxK];
+  __shared__ int64_t ct[kBeamMaxK];
+  __shared__ float old_ps[kBeamMax];
+  __shared__ int old_pl[kBeamMax], old_pf[kBeamMax];
+  __shared__ int run_src[kBeamMax], pool_src[kBeamMax];
+  __shared__ int64_t stage[2 * kBeamMax * kSeqChunk];
+  const int tid = threadIdx.x;
+  const int64_t b = blockIdx.x, r0 = b * nb;
+  if (*done) {
+    if (tid < nb) parent[r0 + tid] = (int32_t)(r0 + tid);
+    return;
+  }
+  const int n = *cur_len, gen = *step_idx + 1;  // HF: cur_len = n, the candidates' generated length cur_len + 1 - prompt = gen
+  const int heur_old = heur[b];
+  if (tid < nb) {
+    old_ps[tid] = pool_score[r0 + tid];
+    old_pl[tid] = pool_len[r0 + tid];
+    old_pf[tid] = pool_fin[r0 + tid];
+  }
+  __syncthreads();
+  int full = early_stopping == 1;  // beams_in_batch_are_full
+  for (int j = 0; j < nb; ++j) full &= old_pf[j] != 0;
+  if (tid < K) {
+    const float s = cand_s[b * K + tid];
+    const int64_t idx = cand_i[b * K + tid];
+    const int64_t t = idx % V;
+    int hit = gen >= max_new;  // MaxLengthCriteria: cur_len + 1 >= prompt + max_new_tokens
+    for (int e = 0; e < n_eos; ++e) hit |= t == eos[e];
+    cj[tid] = (int)(idx / V);
+    ct[tid] = t;
+    chit[tid] = hit;
+    rsc[tid] = s + (hit ? -1.0e9f : -0.0f);  // _get_running_beams_for_next_iteration
+    const int did = hit && tid < nb;         // _update_finished_beams: only the top nb may finish
+    float p = s / len_div[gen];
+    p = p + (full ? -1.0e9f : -0.0f);
+    p = p + (heur_old ? -0.0f : -1.0e9f);
+    p = p + (did ? -0.0f : -1.0e9f);
+    psc[tid] = p;
+  }
+  __syncthreads();
+  if (tid < K) {
+    const float x = rsc[tid];
+    int pos = 0;
+    for (int m = 0; m < K; ++m) pos += rsc[m] > x || (rsc[m] == x && m < tid);
+    if (pos < nb) run_src[pos] = tid;
+  }
+  if (tid < nb + K) {  // merged pool: old entries [0, nb), then the K candidates
+    const float x = tid < nb ? old_ps[tid] : psc[tid - nb];
+    int pos = 0;
+    for (int m = 0; m < nb + K; ++m) {
+      const float y = m < nb ? old_ps[m] : psc[m - nb];
+      pos += y > x || (y == x && m < tid);
+    }
+    if (pos < nb) pool_src[pos] = tid;
+  }
+  __syncthreads();
+  // sequences [0, n): every new row is a copy of an old running or pool row of this prompt, staged through shared memory
+  for (int c0 = 0; c0 < n; c0 += kSeqChunk) {
+    const int len = min(kSeqChunk, n - c0);
+    for (int e = tid; e < nb * len; e += blockDim.x) {
+      const int j = e / len, p = e % len;
+      stage[j * kSeqChunk + p] = run_seq[(r0 + j) * seq_stride + c0 + p];
+      stage[(nb + j) * kSeqChunk + p] = pool_seq[(r0 + j) * seq_stride + c0 + p];
+    }
+    __syncthreads();
+    for (int e = tid; e < nb * len; e += blockDim.x) {
+      const int i = e / len, p = e % len;
+      const int m = pool_src[i];
+      run_seq[(r0 + i) * seq_stride + c0 + p] = stage[cj[run_src[i]] * kSeqChunk + p];
+      pool_seq[(r0 + i) * seq_stride + c0 + p] = m < nb ? stage[(nb + m) * kSeqChunk + p] : stage[cj[m - nb] * kSeqChunk + p];
+    }
+    __syncthreads();
+  }
+  if (tid < nb) {
+    const int k = run_src[tid], m = pool_src[tid];
+    run_seq[(r0 + tid) * seq_stride + n] = ct[k];
+    run_score[r0 + tid] = rsc[k];
+    parent[r0 + tid] = (int32_t)(r0 + cj[k]);
+    tok[r0 + tid] = ct[k];
+    if (m < nb) {  // an older hypothesis ends before position n
+      pool_score[r0 + tid] = old_ps[m];
+      pool_len[r0 + tid] = old_pl[m];
+      pool_fin[r0 + tid] = old_pf[m];
+    } else {
+      pool_seq[(r0 + tid) * seq_stride + n] = ct[m - nb];
+      pool_score[r0 + tid] = psc[m - nb];
+      pool_len[r0 + tid] = gen;
+      pool_fin[r0 + tid] = chit[m - nb] && m - nb < nb;
+    }
+    if (bump0) bump0[r0 + tid] += 1;
+    if (bump1) bump1[r0 + tid] += 1;
+    if (bump2) bump2[r0 + tid] += 1;
+  }
+  if (tid == 0) {
+    // _check_early_stop_heuristic at cur_len + 1 on the new running scores and pool
+    float worst = INFINITY;
+    int all_fin = 1;
+    for (int i = 0; i < nb; ++i) {
+      const int m = pool_src[i];
+      worst = fminf(worst, m < nb ? old_ps[m] : psc[m - nb]);
+      all_fin &= m < nb ? old_pf[m] != 0 : (chit[m - nb] && m - nb < nb);
+    }
+    const int best_len = (early_stopping == 2 && lp_positive) ? max_new : gen;
+    const float best = rsc[run_src[0]] / len_div[best_len];
+    int improvable = 0;
+    for (int i = 0; i < nb; ++i) {
+      const int m = pool_src[i];
+      const int fin = m < nb ? old_pf[m] != 0 : (chit[m - nb] && m - nb < nb);
+      improvable |= best > (fin ? worst : -1.0e9f);
+    }
+    const int h = heur_old && improvable;
+    heur[b] = h;
+    int all_hit = 1;
+    for (int k = 0; k < K; ++k) all_hit &= chit[k];
+    flags[b] = h | (all_fin << 1) | (all_hit << 2);
+    __threadfence();
+    if (atomicAdd(ticket, 1u) == (uint32_t)(B - 1)) {  // last prompt: _beam_search_has_unfinished_sequences over the batch
+      __threadfence();
+      int any_h = 0, every_fin = 1, every_hit = 1;
+      for (int64_t q = 0; q < B; ++q) {
+        const int f = ((volatile int32_t*)flags)[q];
+        any_h |= f & 1;
+        every_fin &= (f >> 1) & 1;
+        every_hit &= (f >> 2) & 1;
+      }
+      const int open = any_h && !(every_fin && early_stopping == 1) && !every_hit;
+      *done = open ? 0 : 1;
+      *cur_len = n + 1;
+      *step_idx = gen;
+      *ticket = 0u;
+    }
+  }
+}
+
+// k / v [L, G * nb, S_max, row_elems] bf16.  Tiles (layer, prompt, P positions) are spread over the grid; each stages the
+// rows of its prompt that some other beam descends from, synchronises, then rewrites every beam whose parent is another row.
+// A tile owns its positions of its prompt's rows, so duplicates, swaps and cycles need no scratch copy of the cache.
+__global__ void __launch_bounds__(256) kv_reorder_kernel(bf16* k, bf16* v, int64_t L, int64_t G, int nb, int64_t S_max,
+                                                         int64_t row_elems, const int32_t* parent, const int32_t* n_pos, int P) {
+  pdl_trigger();
+  pdl_wait();
+  extern __shared__ uint4 kv_stage[];  // [nb][k, v][P * row_elems / 8]
+  __shared__ int par[kBeamMax], need[kBeamMax];
+  const int tid = threadIdx.x;
+  const int n = *n_pos;
+  const int64_t slices = (n + P - 1) / P;
+  const int64_t tiles = L * G * slices;
+  const int64_t vec = row_elems / 8;
+  const int64_t row_vec = S_max * vec;
+  const int64_t slot = (int64_t)P * vec;
+  uint4* K4 = reinterpret_cast<uint4*>(k);
+  uint4* V4 = reinterpret_cast<uint4*>(v);
+  for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int64_t s = tile % slices, g = (tile / slices) % G, l = tile / (slices * G);
+    const int64_t row0 = l * G * nb + g * nb;
+    if (tid < nb) par[tid] = parent[g * nb + tid] - (int32_t)(g * nb);
+    __syncthreads();
+    if (tid < nb) {
+      int nd = 0;
+      for (int c = 0; c < nb; ++c) nd |= c != tid && par[c] == tid;
+      need[tid] = nd;
+    }
+    __syncthreads();
+    const int64_t p0 = s * P;
+    const int64_t cnt = (p0 + P < n ? (int64_t)P : n - p0) * vec;
+    for (int j = 0; j < nb; ++j) {
+      if (!need[j]) continue;
+      const int64_t src = (row0 + j) * row_vec + p0 * vec;
+      for (int64_t e = tid; e < cnt; e += blockDim.x) {
+        kv_stage[(2 * j) * slot + e] = K4[src + e];
+        kv_stage[(2 * j + 1) * slot + e] = V4[src + e];
+      }
+    }
+    __syncthreads();
+    for (int c = 0; c < nb; ++c) {
+      const int p = par[c];
+      if (p == c) continue;
+      const int64_t dst = (row0 + c) * row_vec + p0 * vec;
+      for (int64_t e = tid; e < cnt; e += blockDim.x) {
+        K4[dst + e] = kv_stage[(2 * p) * slot + e];
+        V4[dst + e] = kv_stage[(2 * p + 1) * slot + e];
+      }
+    }
+    __syncthreads();
+  }
+}
+
 }  // namespace uvx
 
 extern "C" int uvx_kv_write(const void* qkv, int64_t row_stride, int64_t k_col, int64_t v_col, int64_t kv_width, void* k_cache,
@@ -348,4 +708,65 @@ extern "C" int uvx_token_finish(int64_t* tok, int32_t* done, const int64_t* eos_
   launch_k(token_finish_kernel, dim3(1), dim3(128), 0, (cudaStream_t)stream, tok, done, eos_ids, (int)n_eos, pad_id, seq, seq_stride,
            cur_len, step_idx, bump0, bump1, bump2, all_done, B);
   return check_launch("token_finish_kernel");
+}
+
+extern "C" int uvx_log_softmax(const float* in, float* out, int64_t rows, int64_t V, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(in && out && rows >= 1 && V >= 1, "uvx_log_softmax: bad arguments");
+  launch_k(log_softmax_kernel, dim3((unsigned)rows), dim3(1024), 0, (cudaStream_t)stream, in, out, V);
+  return check_launch("log_softmax_kernel");
+}
+
+extern "C" int uvx_beam_select(const float* logprobs, int64_t B, int32_t nb, int64_t V, const float* run_score, int32_t K,
+                               float* row_s, int64_t* row_i, float* out_s, int64_t* out_i, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(logprobs && run_score && row_s && row_i && out_s && out_i && B >= 1 && nb >= 1 && nb <= kBeamMax && K >= 1 &&
+                  K <= kBeamMaxK && V >= K && V <= ((int64_t)1 << 40),
+              "uvx_beam_select: bad arguments (1 <= nb <= %d, 1 <= K <= min(%d, V))", kBeamMax, kBeamMaxK);
+  launch_k(beam_row_topk_kernel, dim3((unsigned)(B * nb)), dim3(1024), 0, (cudaStream_t)stream, logprobs, V, run_score, (int)nb, (int)K,
+           row_s, row_i);
+  if (int rc = check_launch("beam_row_topk_kernel")) return rc;
+  launch_k(beam_merge_kernel, dim3((unsigned)B), dim3(kBeamMax * kBeamMaxK), 0, (cudaStream_t)stream, (const float*)row_s,
+           (const int64_t*)row_i, (int)nb, (int)K, out_s, out_i);
+  return check_launch("beam_merge_kernel");
+}
+
+extern "C" int uvx_beam_update(const float* cand_s, const int64_t* cand_i, int64_t B, int32_t nb, int32_t K, int64_t V,
+                               const int64_t* eos_ids, int32_t n_eos, int32_t max_new, const float* len_div, int32_t early_stopping,
+                               int32_t lp_positive, float* run_score, int64_t* run_seq, int64_t* pool_seq, int64_t seq_stride,
+                               float* pool_score, int32_t* pool_len, int32_t* pool_fin, int32_t* parent, int64_t* tok,
+                               int32_t* heur, int32_t* flags, uint32_t* ticket, int32_t* cur_len, int32_t* step_idx, int32_t* bump0,
+                               int32_t* bump1, int32_t* bump2, int32_t* done, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(cand_s && cand_i && len_div && run_score && run_seq && pool_seq && pool_score && pool_len && pool_fin && parent && tok &&
+                  heur && flags && ticket && cur_len && step_idx && done && B >= 1 && nb >= 1 && nb <= kBeamMax && K >= nb &&
+                  K <= kBeamMaxK && V >= 1 && (n_eos == 0 || eos_ids) && n_eos >= 0 && max_new >= 1 && early_stopping >= 0 &&
+                  early_stopping <= 2,
+              "uvx_beam_update: bad arguments");
+  launch_k(beam_update_kernel, dim3((unsigned)B), dim3(256), 0, (cudaStream_t)stream, cand_s, cand_i, V, (int)nb, (int)K, eos_ids,
+           (int)n_eos, (int)max_new, len_div, (int)early_stopping, (int)lp_positive, run_score, run_seq, pool_seq, seq_stride,
+           pool_score, pool_len, pool_fin, parent, tok, heur, flags, ticket, cur_len, step_idx, bump0, bump1, bump2, done, B);
+  return check_launch("beam_update_kernel");
+}
+
+extern "C" int uvx_kv_reorder(void* k_cache, void* v_cache, int64_t L, int64_t B, int32_t nb, int64_t S_max, int64_t row_elems,
+                              const int32_t* parent, const int32_t* n_pos, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(k_cache && v_cache && parent && n_pos && L >= 1 && B >= 1 && nb >= 1 && nb <= kBeamMax && S_max >= 1 && row_elems >= 8 &&
+                  row_elems % 8 == 0,
+              "uvx_kv_reorder: bad arguments");
+  const int64_t per_pos = (int64_t)nb * 2 * row_elems * 2;  // staged bytes per position: nb rows of k and v
+  int64_t P = 32768 / per_pos;  // (the static 64 bytes of the kernel count towards the 48 KB default as well)
+  P = P < 1 ? 1 : (P > 64 ? 64 : P);
+  const size_t smem = (size_t)(P * per_pos);
+  UVX_REQUIRE(smem <= 227 * 1024, "uvx_kv_reorder: %lld-element rows do not fit in shared memory", (long long)row_elems);
+  if (smem > 40 * 1024) {
+    const cudaError_t e = cudaFuncSetAttribute(kv_reorder_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    UVX_REQUIRE(e == cudaSuccess, "uvx_kv_reorder: %s", cudaGetErrorString(e));
+  }
+  const int64_t tiles = L * B * ((S_max + P - 1) / P);
+  const int64_t blocks = tiles < 132 * 6 ? tiles : 132 * 6;
+  launch_k(kv_reorder_kernel, dim3((unsigned)blocks), dim3(256), smem, (cudaStream_t)stream, (bf16*)k_cache, (bf16*)v_cache, L, B,
+           (int)nb, S_max, row_elems, parent, n_pos, (int)P);
+  return check_launch("kv_reorder_kernel");
 }

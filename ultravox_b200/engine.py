@@ -266,3 +266,123 @@ class DecodeEngine:
             t.copy_(s0)
         torch.cuda.synchronize()
         self.graph = g
+
+
+class BeamDecodeEngine(DecodeEngine):
+    """Beam search over ``batch`` prompts with ``num_beams`` beams each (row b * num_beams + j), as
+    hf:generation/utils.py ``_beam_search``: the forward of ``DecodeEngine._step`` runs unchanged over the batch * num_beams
+    rows, and the pick becomes log_softmax -> repetition penalty on the log-probs -> top-K continuations per prompt ->
+    running beams / finished pool / early-stop heuristic -> KV cache rows gathered by parent beam, all on the device, so a
+    step is still one CUDA graph replay.  ``all_done`` is HF's loop condition (negated); ``logprobs`` holds the last step's
+    processed log-probs [batch * num_beams, V] and ``logits`` the raw ones.  The cache must have batch * num_beams rows with
+    each prompt prefilled into row b * num_beams (``begin`` broadcasts it to the other beams)."""
+
+    def __init__(self, model: UltravoxModel, batch: int, num_beams: int, max_len: int, max_new_tokens: int, use_graph: bool = True,
+                 cache=None, eos_token_ids=None, length_penalty: float = 1.0, early_stopping=False, repetition_penalty: float = 1.0):
+        nb = int(num_beams)
+        if not 1 <= nb <= ops.BEAM_MAX:
+            raise ValueError(f"num_beams must be in [1, {ops.BEAM_MAX}], got {num_beams}")
+        if early_stopping not in (False, True, "never"):
+            raise ValueError(f"early_stopping must be True, False or 'never', got {early_stopping!r}")
+        eos_list = [eos_token_ids] if isinstance(eos_token_ids, int) else list(eos_token_ids or [])
+        super().__init__(model, batch * nb, max_len, use_graph=use_graph, cache=cache, eos_token_ids=eos_list,
+                         repetition_penalty=repetition_penalty)
+        dev = model.device
+        R = batch * nb
+        self.prompts, self.nb = batch, nb
+        self.K = max(2, 1 + len(eos_list)) * nb                 # HF's beams_to_keep
+        if self.K > ops.BEAM_MAX_K:
+            raise ValueError(f"max(2, 1 + {len(eos_list)} EOS ids) * {nb} beams = {self.K} candidates; at most {ops.BEAM_MAX_K}")
+        self.max_new = int(max_new_tokens)
+        if not 1 <= self.max_new <= self.max_len:
+            raise ValueError(f"max_new_tokens must be in [1, {self.max_len}], got {max_new_tokens}")
+        self.length_penalty = float(length_penalty)
+        self.es = 2 if early_stopping == "never" else int(early_stopping is True)
+        # divisor of a hypothesis of n generated tokens: HF divides by the Python float n ** length_penalty, which torch rounds
+        # once to fp32 (entry 0 is never read)
+        self.len_div = torch.tensor([1.0] + [float(n) ** self.length_penalty for n in range(1, self.max_len + 2)],
+                                    dtype=torch.float32, device=dev)
+        self.V = model.language_model.lm_head.weight.shape[0]
+        i32 = dict(dtype=torch.int32, device=dev)
+        self.run_score = torch.zeros(R, dtype=torch.float32, device=dev)
+        self.pool_seq = torch.zeros_like(self.seq)
+        self.pool_score = torch.full((R,), -1e9, dtype=torch.float32, device=dev)
+        self.pool_len = torch.zeros(R, **i32)
+        self.pool_fin = torch.zeros(R, **i32)
+        self.parent = torch.arange(R, **i32)
+        self.heur = torch.ones(batch, **i32)
+        self.flags = torch.zeros(batch, **i32)
+        self.ticket = torch.zeros(1, **i32)
+        self.n_pos = torch.zeros(1, **i32)
+        self.logprobs = torch.empty(R, self.V, dtype=torch.float32, device=dev)
+        self.row_buf = (torch.empty(R * self.K, dtype=torch.float32, device=dev), torch.empty(R * self.K, dtype=torch.int64, device=dev))
+        self.cand = (torch.empty(batch, self.K, dtype=torch.float32, device=dev), torch.empty(batch, self.K, dtype=torch.int64, device=dev))
+        self._beam = dict(run_score=self.run_score, run_seq=self.seq, pool_seq=self.pool_seq, pool_score=self.pool_score,
+                          pool_len=self.pool_len, pool_fin=self.pool_fin, parent=self.parent, tok=self.token.view(-1),
+                          heur=self.heur, flags=self.flags, ticket=self.ticket)
+        self._counters = dict(cur_len=self.cur_len, step_idx=self.step_idx, done=self.all_done)
+
+    def begin(self, input_ids: torch.Tensor, first_logits: torch.Tensor, kv_start: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``input_ids`` [batch, S] prompts prefilled into cache rows b * num_beams, ``first_logits`` [batch, V] their last
+        positions: broadcasts both to the beams and runs the first beam step (HF's running scores [0, -1e9, ...] and a pool of
+        -1e9 entries).  Returns the device token tensor [batch * num_beams]."""
+        B, S = input_ids.shape
+        nb = self.nb
+        rows = input_ids.repeat_interleave(nb, 0)
+        self.pool_seq[:, :S].copy_(rows)
+        self.run_score.view(B, nb).fill_(-1e9)
+        self.run_score.view(B, nb)[:, 0] = 0.0
+        self.pool_score.fill_(-1e9)
+        self.pool_len.zero_()
+        self.pool_fin.zero_()
+        self.heur.fill_(1)
+        self.flags.zero_()
+        self.ticket.zero_()
+        self.parent.copy_(torch.arange(B * nb, dtype=torch.int32, device=self.parent.device) // nb * nb)
+        self.n_pos.fill_(S)
+        ops.kv_reorder_(self.cache.k, self.cache.v, self.parent, self.n_pos, nb)
+        kv = kv_start.repeat_interleave(nb) if kv_start is not None else None
+        return super().begin(rows, first_logits.repeat_interleave(nb, 0), kv)
+
+    def prefill(self, inputs_embeds: torch.Tensor) -> torch.Tensor:
+        """Prefills the batch prompts [batch, S, D] once each into rows b * num_beams, then ``begin`` (prompt ids taken as 0)."""
+        m = self.model
+        B, S, _ = inputs_embeds.shape
+        L, _, smax, hkv, d = self.cache.k.shape
+        view = type(self.cache)(self.cache.k.view(L, B, self.nb * smax, hkv, d), self.cache.v.view(L, B, self.nb * smax, hkv, d))
+        hid = m.llama_hidden(inputs_embeds, view)
+        logits = ops.lm_head(hid[:, -1, :], m.language_model.lm_head.weight)
+        ids = torch.zeros(B, S, dtype=torch.int64, device=logits.device)
+        return self.begin(ids, logits).clone()
+
+    def _pick(self, logits: torch.Tensor):
+        """logits [batch * nb, V] fp32 -> the next running beams in ``token`` / ``seq``, the pool, the cache rows reordered."""
+        self.logits = logits
+        lp = ops.log_softmax(logits, out=self.logprobs)
+        if self.penalty != 1.0:
+            ops.repetition_penalty_(lp, self.seq, self.cur_len, self.penalty, self.scratch)
+        s, i = ops.beam_select(lp, self.run_score, self.nb, self.K, scratch=self.row_buf, out=self.cand)
+        ops.beam_update(s, i, self.V, self.nb, self.eos, self.max_new, self.len_div, self.es, self.length_penalty > 0.0, self._beam,
+                        self._counters, (self.pos, self.lens, self.rope_pos))
+        # the update advanced pos to the slot of the token fed next: the cache holds positions [0, pos)
+        ops.kv_reorder_(self.cache.k, self.cache.v, self.parent, self.pos, self.nb)
+
+    def _step_warm(self):
+        # the warm-up and capture steps run with the search marked done, so they leave the beams, the pool and the cache rows
+        # alone (the update then only sets the identity parent map)
+        prev = self.all_done.clone()
+        self.all_done.fill_(1)
+        super()._step_warm()
+        self.all_done.copy_(prev)
+
+    def result(self, prompt_len: int, num_return_sequences: int, fill_value: int):
+        """(sequences [batch * n, prompt_len + longest], scores [batch * n]) of the n best finished hypotheses per prompt, cropped
+        to the longest of them and filled with ``fill_value`` past each one's end (HF's output)."""
+        dev = self.pool_seq.device
+        idx = (torch.arange(self.prompts, device=dev)[:, None] * self.nb
+               + torch.arange(num_return_sequences, device=dev)[None, :]).reshape(-1)
+        lens = self.pool_len[idx].to(torch.int64)
+        width = prompt_len + int(lens.max())
+        seq = self.pool_seq[idx, :width]
+        keep = torch.arange(width, device=dev)[None, :] < (prompt_len + lens)[:, None]
+        return torch.where(keep, seq, torch.full_like(seq, fill_value)), self.pool_score[idx].clone()

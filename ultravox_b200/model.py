@@ -219,9 +219,11 @@ class KVCache:
 
 @dataclasses.dataclass
 class GenerateOutput:
-    """``return_dict_in_generate=True`` result: what the reference's conversation mode reads (ref infer.py:131-148)."""
+    """``return_dict_in_generate=True`` result: what the reference's conversation mode reads (ref infer.py:131-148), plus the
+    final beam scores of a beam search asked for with ``output_scores=True`` (HF's ``sequences_scores``)."""
     sequences: torch.Tensor
-    past_key_values: KVCache
+    past_key_values: Optional[KVCache]
+    sequences_scores: Optional[torch.Tensor] = None
 
 
 # ------------------------------------------------------------------------------------------------ the model
@@ -874,7 +876,9 @@ class UltravoxModel(nn.Module):
                  repetition_penalty: float = 1.0, temperature: Optional[float] = None, do_sample: bool = False,
                  top_k: Optional[int] = None, top_p: Optional[float] = None, generator: Optional[torch.Generator] = None,
                  audio_waveforms: Optional[torch.Tensor] = None, audio_num_frames: Optional[torch.Tensor] = None,
-                 audio_pad_frames: Optional[torch.Tensor] = None, use_graph: bool = True, **kwargs):
+                 audio_pad_frames: Optional[torch.Tensor] = None, use_graph: bool = True, num_beams: int = 1,
+                 length_penalty: float = 1.0, early_stopping=False, num_return_sequences: int = 1, output_scores: bool = False,
+                 **kwargs):
         """``GenerationMixin.generate`` for this model (ref :398-426; arguments as ``LocalInference._generate`` passes them, ref
         infer.py:309-342).  Returns prompt ids followed by the new tokens.
 
@@ -893,11 +897,35 @@ class UltravoxModel(nn.Module):
 
         The prompt is prefilled by the tensor-core path; every later token is one replay of a CUDA graph holding the whole
         decode step (``engine.DecodeEngine``: GEMV linears, device-side positions / EOS / sequence bookkeeping), so the loop
-        has no per-token host synchronisation unless a streamer asks for the token."""
+        has no per-token host synchronisation unless a streamer asks for the token.
+
+        ``num_beams > 1`` runs beam search as hf:generation/utils.py ``_beam_search`` does (the reference passes the argument
+        through to ``language_model.generate``, ref :398-426): log-probs, ``repetition_penalty`` applied to them, the top
+        ``max(2, 1 + #EOS) * num_beams`` continuations per prompt, hypotheses scored ``sum log-prob / generated_len **
+        length_penalty``, ``early_stopping`` in {False, True, "never"}.  Each prompt is prefilled once and its cache rows are
+        broadcast to its beams; every later step is one graph replay (``engine.BeamDecodeEngine``).  Returns the best
+        ``num_return_sequences`` hypotheses per prompt, [B * num_return_sequences, S + longest], filled past each one's end with
+        ``pad_token_id`` (or the first EOS id when that is unset or 0).  With ``return_dict_in_generate=True`` and
+        ``output_scores=True`` their scores are in ``sequences_scores``; ``past_key_values`` is None, because the cache rows
+        belong to the running beams, not to the returned hypotheses.  Not built: beam sampling (``do_sample=True``), a
+        streamer, conversation KV reuse and per-step ``scores`` / ``beam_indices``."""
         from .engine import DecodeEngine
         unknown = [k for k, v in kwargs.items() if isinstance(v, torch.Tensor)]
         if unknown:
             raise TypeError(f"generate() got unexpected tensor arguments {unknown}")
+        if not isinstance(num_beams, int) or not 1 <= num_beams <= ops.BEAM_MAX:
+            raise ValueError(f"num_beams must be an integer in [1, {ops.BEAM_MAX}], got {num_beams!r}")
+        if not isinstance(num_return_sequences, int) or not 1 <= num_return_sequences <= num_beams:
+            raise ValueError(f"num_return_sequences ({num_return_sequences!r}) must be in [1, num_beams = {num_beams}]")
+        if num_beams > 1:
+            if do_sample:
+                raise NotImplementedError("beam sampling (num_beams > 1 with do_sample=True) is not built")
+            if streamer is not None:
+                raise ValueError("`streamer` cannot be used with beam search (yet!). Make sure that `num_beams` is set to 1.")
+            if past_key_values is not None:
+                raise NotImplementedError("conversation KV reuse with beam search is not built")
+            if early_stopping not in (False, True, "never"):
+                raise ValueError(f"early_stopping must be True, False or 'never', got {early_stopping!r}")
         if top_p is not None and not 0.0 <= float(top_p) <= 1.0:       # NaN fails too
             raise ValueError(f"`top_p` has to be a float in [0, 1], but is {top_p}")
         sampling = bool(do_sample) and (temperature is None or float(temperature) > 0)
@@ -919,6 +947,17 @@ class UltravoxModel(nn.Module):
             if past_key_values is not None:
                 raise NotImplementedError("conversation KV reuse with padded batches (the reference has none either, infer.py:155)")
             position_ids = (am.to(torch.int64).cumsum(-1) - 1).clamp_min(0)
+        if num_beams > 1:
+            seqs, scores = self._beam_search(
+                input_ids, dict(audio_values=audio_values, inputs_embeds=inputs_embeds, attention_mask=attention_mask,
+                                audio_token_start_idx=audio_token_start_idx, audio_lens=audio_lens, audio_token_len=audio_token_len,
+                                audio_batch_size=audio_batch_size, position_ids=position_ids, audio_waveforms=audio_waveforms,
+                                audio_num_frames=audio_num_frames, audio_pad_frames=audio_pad_frames),
+                kv_start, max_new_tokens, eos_token_id, pad_token_id, num_beams, length_penalty, early_stopping,
+                num_return_sequences, repetition_penalty or 1.0, use_graph)
+            if return_dict_in_generate:
+                return GenerateOutput(seqs, None, scores if output_scores else None)
+            return seqs
         has_wave = audio_waveforms is not None and len(audio_waveforms) > 0
         has_mel = audio_values is not None and len(audio_values) > 0
         if past_key_values is None:
@@ -975,6 +1014,46 @@ class UltravoxModel(nn.Module):
         cache.length = S + n_new - 1                        # the last new token has not been fed yet
         sequences = torch.cat([input_ids, new], dim=1)
         return GenerateOutput(sequences, cache) if return_dict_in_generate else sequences
+
+    def _beam_search(self, input_ids: torch.Tensor, forward_kw: dict, kv_start: Optional[torch.Tensor], max_new_tokens: int,
+                     eos_token_id, pad_token_id: Optional[int], num_beams: int, length_penalty: float, early_stopping,
+                     num_return_sequences: int, repetition_penalty: float, use_graph: bool, step_hook=None):
+        """``generate``'s beam branch -> (sequences [B * num_return_sequences, S + longest], their scores).  The B prompts are
+        prefilled once into cache rows b * num_beams (a view of the [L, B * num_beams, S_max, ...] cache as B rows of
+        num_beams * S_max positions).  ``step_hook(engine)``, if given, runs after every beam step (the host then checks
+        the done flag every step)."""
+        from .engine import BeamDecodeEngine
+        B, S = input_ids.shape
+        if max_new_tokens < 1:
+            raise ValueError(f"max_new_tokens must be >= 1, got {max_new_tokens}")
+        eos_list = [eos_token_id] if isinstance(eos_token_id, int) else list(eos_token_id or [])
+        cache = self.new_cache(B * num_beams, S + max_new_tokens)
+        L, _, smax, hkv, hd = cache.k.shape
+        prompt_rows = KVCache(cache.k.view(L, B, num_beams * smax, hkv, hd), cache.v.view(L, B, num_beams * smax, hkv, hd))
+        fk = dict(forward_kw)
+        out = self.forward(input_ids, fk.pop("audio_values"), fk.pop("inputs_embeds"), None, fk.pop("attention_mask"),
+                           fk.pop("audio_token_start_idx"), fk.pop("audio_lens"), fk.pop("audio_token_len"),
+                           fk.pop("audio_batch_size"), prompt_rows, logits_to_keep=1, **fk)
+        eng = BeamDecodeEngine(self, B, num_beams, cache.capacity, max_new_tokens, use_graph=use_graph, cache=cache,
+                               eos_token_ids=eos_list, length_penalty=length_penalty, early_stopping=early_stopping,
+                               repetition_penalty=repetition_penalty)
+        eng.begin(input_ids, out.logits.view(B, -1), kv_start)
+        n_new = 1
+        sync_every = 8          # the host looks at the device's done flag every few steps only
+        while True:
+            if step_hook is not None:
+                step_hook(eng)
+            stop = n_new >= max_new_tokens
+            if not stop and (step_hook is not None or n_new % sync_every == 0):
+                stop = bool(int(eng.all_done))
+            if stop:
+                break
+            eng.step()
+            n_new += 1
+        # hf:generation/utils.py _beam_search: `pad_token_id or eos_token_id[0] if eos_token_id is not None else -1`, with the
+        # pad id defaulting to the first EOS id
+        fill = (pad_token_id if pad_token_id else eos_list[0]) if eos_list else -1
+        return eng.result(S, num_return_sequences, fill)
 
 
 class SwiGLU(nn.Module):

@@ -658,3 +658,62 @@ def token_finish(tok: torch.Tensor, done: torch.Tensor, eos_ids: Optional[torch.
     check(lib().uvx_token_finish(tok.data_ptr(), done.data_ptr(), _p(eos_ids), 0 if eos_ids is None else eos_ids.numel(), int(pad_id),
                                  _p(seq), seq.stride(0) if seq is not None else 0, cur_len.data_ptr(), _p(step_idx), _p(b[0]), _p(b[1]),
                                  _p(b[2]), _p(all_done), tok.numel(), _stream()), "uvx_token_finish")
+
+
+# ------------------------------------------------------------------------------------------ beam search
+BEAM_MAX = 8        # beams per prompt (kBeamMax in generate.cu)
+BEAM_MAX_K = 64     # candidates per prompt, max(2, 1 + n_eos) * num_beams
+
+
+def log_softmax(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """[R, V] fp32 -> log_softmax over each row, fp32 (``out`` may be ``x``)."""
+    _cuda(x, torch.float32, "x")
+    R, V = x.shape
+    if out is None:
+        out = torch.empty_like(x)
+    check(lib().uvx_log_softmax(x.data_ptr(), out.data_ptr(), R, V, _stream()), "uvx_log_softmax")
+    return out
+
+
+def beam_select(logprobs: torch.Tensor, run_score: torch.Tensor, num_beams: int, k: int, scratch=None, out=None):
+    """logprobs [B*nb, V] fp32, run_score [B*nb] fp32 -> (scores [B, k] fp32, flat ids [B, k] int64 = beam * V + token): the
+    k largest logprobs + run_score per prompt, descending, equal values in flat-index order."""
+    _cuda(logprobs, torch.float32, "logprobs"), _cuda(run_score, torch.float32, "run_score")
+    R, V = logprobs.shape
+    B = R // num_beams
+    dev = logprobs.device
+    if scratch is None:
+        scratch = (torch.empty(R * k, dtype=torch.float32, device=dev), torch.empty(R * k, dtype=torch.int64, device=dev))
+    if out is None:
+        out = (torch.empty(B, k, dtype=torch.float32, device=dev), torch.empty(B, k, dtype=torch.int64, device=dev))
+    check(lib().uvx_beam_select(logprobs.data_ptr(), B, num_beams, V, run_score.data_ptr(), k, scratch[0].data_ptr(),
+                                scratch[1].data_ptr(), out[0].data_ptr(), out[1].data_ptr(), _stream()), "uvx_beam_select")
+    return out
+
+
+def beam_update(cand_s: torch.Tensor, cand_i: torch.Tensor, V: int, num_beams: int, eos_ids: Optional[torch.Tensor], max_new: int,
+                len_div: torch.Tensor, early_stopping: int, lp_positive: bool, state: dict, counters: dict, bumps: tuple = ()) -> None:
+    """``uvx_beam_update`` on the candidates of ``beam_select``.  ``state`` holds the device tensors run_score, run_seq,
+    pool_seq, pool_score, pool_len, pool_fin, parent, tok, heur, flags, ticket; ``counters`` cur_len, step_idx, done."""
+    B, K = cand_s.shape
+    s, c = state, counters
+    b = list(bumps) + [None] * (3 - len(bumps))
+    check(lib().uvx_beam_update(cand_s.data_ptr(), cand_i.data_ptr(), B, num_beams, K, V, _p(eos_ids),
+                                0 if eos_ids is None else eos_ids.numel(), int(max_new), len_div.data_ptr(), int(early_stopping),
+                                int(bool(lp_positive)), s["run_score"].data_ptr(), s["run_seq"].data_ptr(), s["pool_seq"].data_ptr(),
+                                s["run_seq"].stride(0), s["pool_score"].data_ptr(), s["pool_len"].data_ptr(), s["pool_fin"].data_ptr(),
+                                s["parent"].data_ptr(), s["tok"].data_ptr(), s["heur"].data_ptr(), s["flags"].data_ptr(),
+                                s["ticket"].data_ptr(), c["cur_len"].data_ptr(), c["step_idx"].data_ptr(), _p(b[0]), _p(b[1]), _p(b[2]),
+                                c["done"].data_ptr(), _stream()), "uvx_beam_update")
+
+
+def kv_reorder_(k_cache: torch.Tensor, v_cache: torch.Tensor, parent: torch.Tensor, n_pos: torch.Tensor, num_beams: int) -> None:
+    """k / v caches [L, B*nb, S_max, Hkv, D] bf16: row r <- row parent[r] (int32, same prompt) at positions [0, n_pos[0]), in place."""
+    _cuda(k_cache, BF16, "k_cache"), _cuda(v_cache, BF16, "v_cache"), _cuda(parent, torch.int32, "parent")
+    _cuda(n_pos, torch.int32, "n_pos")
+    if not (k_cache.is_contiguous() and v_cache.is_contiguous() and k_cache.shape == v_cache.shape):
+        raise ValueError("kv_reorder_ needs two contiguous caches of one shape")
+    L, R, S_max = k_cache.shape[:3]
+    row_elems = k_cache[0, 0, 0].numel()
+    check(lib().uvx_kv_reorder(k_cache.data_ptr(), v_cache.data_ptr(), L, R // num_beams, num_beams, S_max, row_elems,
+                               parent.data_ptr(), n_pos.data_ptr(), _stream()), "uvx_kv_reorder")
