@@ -226,7 +226,8 @@ int uvx_embed_splice(const int64_t* input_ids, const void* embed_tokens, int64_t
 
 /* Last-position LM head: logits[b, v] = sum_k h[b, k] * W[v, k] (bf16 x bf16 -> f32), HBM-streaming GEMV
  * (hf:modeling_llama.py:485-491 with logits_to_keep = 1), and greedy argmax (first maximal index, like
- * torch.argmax; ref:ultravox/inference/infer.py:319-328 greedy path).                                  */
+ * torch.argmax; ref:ultravox/inference/infer.py:319-328 greedy path).  uvx_argmax takes finite or -inf logits
+ * (a row that is all -inf gives 0, as torch.argmax does); NaN is out of contract.                        */
 int uvx_lm_head(const void* h, int64_t B, int64_t h_row_stride, const void* W, int64_t V, int64_t d,
                 float* logits, uvx_stream_t stream);
 int uvx_argmax(const float* logits, int64_t B, int64_t V, int64_t* out_idx, uvx_stream_t stream);

@@ -65,7 +65,9 @@ __global__ void __launch_bounds__(1024) argmax_kernel(const float* __restrict__ 
     const float xs[4] = {t.x, t.y, t.z, t.w};
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
-      if (xs[e] > best) {  // within a thread indices grow monotonically: strict > keeps the first maximum
+      // within a thread indices grow monotonically: strict > keeps the first maximum.  A thread's first element is always taken,
+      // so a -inf element still carries its index and a row that is all -inf resolves to 0 below, as torch.argmax does.
+      if (xs[e] > best || bi == INT64_MAX) {
         best = xs[e];
         bi = i * 4 + e;
       }
@@ -78,7 +80,7 @@ __global__ void __launch_bounds__(1024) argmax_kernel(const float* __restrict__ 
       bi = i;
     }
   }
-  // NaN handling is out of contract (torch would return the NaN position); finite logits only.
+  // Finite or -inf logits only: NaN handling is out of contract (torch would return the NaN position).
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     const float ob = __shfl_xor_sync(0xffffffffu, best, o);
