@@ -384,6 +384,58 @@ int uvx_adamw(void* p, const float* g, float* m, float* v, int64_t n, float lr, 
               float weight_decay, int64_t step, float grad_scale, uvx_stream_t stream);
 int uvx_cast_f32_bf16(const float* in, void* out, int64_t n, uvx_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * a14: the optimizer step of the released recipes (HF Trainer, ref train.py:250-307): global-norm gradient clipping
+ * (torch.nn.utils.clip_grad_norm_, max_grad_norm), AdamW (adamw_torch) with a learning-rate schedule read from a device
+ * table, and gradient accumulation over micro-batches.  Every trained tensor of a step (the projector's flat buffer, the
+ * encoder-LoRA A / Bq / Bk) goes through one launch per entry, described by a tensor list passed by value at launch time.
+ * Entry i: numel[i] > 0 elements; the pointers an entry reads are named below, the others are ignored.  Tensors of one
+ * list must not overlap.  Vector accesses are used where a tensor's pointers are 16-byte (fp32) / 8-byte (bf16) aligned.  */
+#define UVX_TL_MAX 8
+typedef struct uvx_tensor_list {
+  int64_t count;                /* 1 .. UVX_TL_MAX                                                                 */
+  int64_t numel[UVX_TL_MAX];
+  const float* g[UVX_TL_MAX];   /* fp32 gradients                                                                  */
+  float* acc[UVX_TL_MAX];       /* fp32 gradient accumulators (uvx_grad_accumulate)                                */
+  void* p[UVX_TL_MAX];          /* bf16 parameters (uvx_adamw_multi)                                               */
+  float* m[UVX_TL_MAX];         /* fp32 first / second moments (uvx_adamw_multi)                                   */
+  float* v[UVX_TL_MAX];
+} uvx_tensor_list;
+
+/* Size of the workspace of uvx_grad_norm_clip: UVX_NORM_BLOCKS fp64 block partials + a 4-byte ticket.                  */
+#define UVX_NORM_BLOCKS 1024
+#define UVX_NORM_WS_BYTES (8 * UVX_NORM_BLOCKS + 8)
+
+/* uvx_grad_norm_clip   reads g[i].  norm = || scale[0] * g ||_2 over all tensors of the list, where each element is first
+ *                      rounded to fp32 as fl(g * scale[0]) (the gradient the reference would hold after the all-reduce mean
+ *                      and the 1 / accumulation-steps loss division), squared and summed in fp64.  Deterministic: a fixed
+ *                      grid of UVX_NORM_BLOCKS blocks, a fixed per-thread order, fp64 block partials, and the last block to
+ *                      finish (ticket in the workspace) sums the partials in index order; the result depends on the inputs
+ *                      only.  norm_coef[0] = fp32(sqrt(sum)); norm_coef[1] = coef = min(max_norm / (norm + 1e-6), 1) in
+ *                      fp32 as torch.nn.utils.clip_grad_norm_ computes it (error_if_nonfinite=False; the division is
+ *                      torch's reciprocal-then-multiply): a NaN norm gives a NaN
+ *                      coef, an Inf norm coef 0; max_norm <= 0 means no clipping, coef = 1 (the norm is still written).
+ *                      If step is not NULL the same final block does step[0] += 1 (int64, device) and writes
+ *                      lr[0] = lr_table[min(step[0], table_len) - 1] (the lr of the optimizer step about to run).
+ *                      workspace: UVX_NORM_WS_BYTES bytes, zero before the first call; the last block resets the ticket,
+ *                      so calls (and graph replays) may follow each other on one stream without re-initialisation.
+ *                      Nothing is read from the host but the list and max_norm: the call is graph-capturable.
+ * uvx_adamw_multi      reads g[i], p[i], m[i], v[i]; writes p, m, v.  torch.optim.AdamW (decoupled weight decay,
+ *                      adamw_torch) with lr = lr[0], step = step[0] (>= 1), coef = coef[0] (NULL = 1) and scale = scale[0]
+ *                      read from device memory: effective gradient fl(fl(g * scale) * coef); p *= 1 - lr * wd;
+ *                      m = lerp(m, g, 1 - beta1); v = beta2 v + (1 - beta2) g^2; p -= (lr / bc1) * m / (sqrt(v) / sqrt(bc2) + eps)
+ *                      with bc = 1 - beta ** step, the scalars formed in double from the device values and rounded to
+ *                      fp32 where torch's foreach implementation rounds them.  Moments fp32, parameters bf16
+ *                      (round-to-nearest once per step).  A NaN gradient makes its own elements NaN; a NaN coef makes every
+ *                      element NaN, as torch's clip + step does.  Elementwise: deterministic.
+ * uvx_grad_accumulate  reads g[i]; acc[i] = g[i] if assign else acc[i] + g[i] (fp32), the micro-batch accumulation of a
+ *                      gradient-accumulation step.  acc may not alias g.  Deterministic.                                */
+int uvx_grad_norm_clip(const uvx_tensor_list* tl, const float* scale, float max_norm, void* workspace, float* norm_coef,
+                       int64_t* step, const float* lr_table, int64_t table_len, float* lr, uvx_stream_t stream);
+int uvx_adamw_multi(const uvx_tensor_list* tl, const float* lr, const int64_t* step, const float* coef, const float* scale,
+                    double beta1, double beta2, double eps, double weight_decay, uvx_stream_t stream);
+int uvx_grad_accumulate(const uvx_tensor_list* tl, int32_t assign, uvx_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -35,6 +35,16 @@ class AttnArgs(C.Structure):
                 ("causal", c_i32), ("block", c_i32), ("scale", c_f32), ("lse", c_vp), ("kv_start", c_vp)]
 
 
+TL_MAX = 8                 # UVX_TL_MAX
+NORM_WS_BYTES = 8 * 1024 + 8   # UVX_NORM_WS_BYTES
+
+
+class TensorList(C.Structure):
+    """``struct uvx_tensor_list`` (include/uvx.h)."""
+    _fields_ = [("count", c_i64), ("numel", c_i64 * TL_MAX), ("g", c_vp * TL_MAX), ("acc", c_vp * TL_MAX), ("p", c_vp * TL_MAX),
+                ("m", c_vp * TL_MAX), ("v", c_vp * TL_MAX)]
+
+
 # name -> (restype, argtypes); must list every symbol include/uvx.h declares (tests check this)
 SIGNATURES = {
     "uvx_abi_version": (C.c_int, []),
@@ -97,6 +107,10 @@ SIGNATURES = {
     "uvx_splice_inverse": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp]),
     "uvx_adamw": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_f32, c_f32, c_f32, c_i64, c_f32, c_vp]),
     "uvx_cast_f32_bf16": (C.c_int, [c_vp, c_vp, c_i64, c_vp]),
+    "uvx_grad_norm_clip": (C.c_int, [C.POINTER(TensorList), c_vp, c_f32, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp]),
+    "uvx_adamw_multi": (C.c_int, [C.POINTER(TensorList), c_vp, c_vp, c_vp, c_vp, C.c_double, C.c_double, C.c_double, C.c_double,
+                                  c_vp]),
+    "uvx_grad_accumulate": (C.c_int, [C.POINTER(TensorList), c_i32, c_vp]),
     "uvx_kl_loss": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_i64, c_f32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "uvx_kl_bwd": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_i64, c_f32, c_vp, c_vp, c_vp, c_f32, c_vp, c_vp]),
     "uvx_ce_loss": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_i64, c_i64, c_i64, C.c_int, c_vp, c_vp, c_vp, c_vp]),

@@ -27,6 +27,13 @@ def shard_indices(n_items: int, shard: int, n_shards: int) -> list[int]:
     return [i for i in range(n_items) if i % n_shards == shard]
 
 
+def group_world_size(group=None) -> int:
+    """Ranks in the data-parallel group (1 without an initialised process group)."""
+    if dist.is_available() and dist.is_initialized():
+        return dist.get_world_size(group)
+    return 1
+
+
 def allreduce_sum_(flat: torch.Tensor, group=None) -> float:
     """In-place SUM over the data-parallel group; returns 1 / world for the caller to fold into its next kernel (the optimizer
     step reads the gradient anyway: a separate x 1/world pass over the flat buffer is a wasted HBM round trip)."""

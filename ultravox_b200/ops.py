@@ -561,6 +561,70 @@ def adamw_(p: torch.Tensor, g: torch.Tensor, m: torch.Tensor, v: torch.Tensor, s
                           weight_decay, step, grad_scale, _stream()), "uvx_adamw")
 
 
+def _tensor_list(g, acc=None, p=None, m=None, v=None) -> _lib.TensorList:
+    """``uvx_tensor_list`` over parallel lists of contiguous CUDA tensors (g / acc / m / v fp32, p bf16)."""
+    if not 1 <= len(g) <= _lib.TL_MAX:
+        raise ValueError(f"1 .. {_lib.TL_MAX} tensors per launch, got {len(g)}")
+    tl = _lib.TensorList()
+    tl.count = len(g)
+    for field, ts, dtype in (("g", g, torch.float32), ("acc", acc, torch.float32), ("p", p, BF16), ("m", m, torch.float32),
+                             ("v", v, torch.float32)):
+        if ts is None:
+            continue
+        if len(ts) != len(g):
+            raise ValueError(f"{field}: {len(ts)} tensors for {len(g)} gradients")
+        for i, t in enumerate(ts):
+            _cuda(t, dtype, f"{field}[{i}]")
+            if not t.is_contiguous() or t.numel() != g[i].numel():
+                raise ValueError(f"{field}[{i}] must be contiguous with {g[i].numel()} elements")
+            getattr(tl, field)[i] = t.data_ptr()
+            tl.numel[i] = t.numel()
+    return tl
+
+
+def norm_workspace(device) -> torch.Tensor:
+    """Zeroed workspace of ``grad_norm_clip`` (block partials + the self-resetting ticket); one per stream of calls."""
+    return torch.zeros(_lib.NORM_WS_BYTES, dtype=torch.uint8, device=device)
+
+
+def grad_norm_clip(grads, scale: torch.Tensor, max_norm: Optional[float], workspace: torch.Tensor,
+                   out: Optional[torch.Tensor] = None, step: Optional[torch.Tensor] = None, lr_table: Optional[torch.Tensor] = None,
+                   lr: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out = [norm, coef] (fp32 device): norm = ||scale[0] * g||_2 over all ``grads`` (deterministic fp64 sum) and
+    coef = min(max_norm / (norm + 1e-6), 1) as ``torch.nn.utils.clip_grad_norm_`` forms it; ``max_norm`` None / <= 0 gives
+    coef = 1.  With ``step`` (int64 [1]) the same launch does step += 1 and lr[0] = lr_table[min(step, len) - 1]."""
+    _cuda(scale, torch.float32, "scale"), _cuda(workspace, torch.uint8, "workspace")
+    if workspace.numel() < _lib.NORM_WS_BYTES:
+        raise ValueError(f"workspace needs {_lib.NORM_WS_BYTES} bytes")
+    if out is None:
+        out = torch.empty(2, dtype=torch.float32, device=scale.device)
+    if step is not None:
+        _cuda(step, torch.int64, "step"), _cuda(lr_table, torch.float32, "lr_table"), _cuda(lr, torch.float32, "lr")
+    tl = _tensor_list(list(grads))
+    check(lib().uvx_grad_norm_clip(C.byref(tl), scale.data_ptr(), float(max_norm or 0.0), workspace.data_ptr(), out.data_ptr(),
+                                   _p(step), _p(lr_table), 0 if lr_table is None else lr_table.numel(), _p(lr), _stream()),
+          "uvx_grad_norm_clip")
+    return out
+
+
+def adamw_multi_(params, grads, ms, vs, lr: torch.Tensor, step: torch.Tensor, scale: torch.Tensor,
+                 coef: Optional[torch.Tensor] = None, betas=(0.9, 0.999), eps: float = 1e-8, weight_decay: float = 0.0) -> None:
+    """torch.optim.AdamW over every tensor of the lists in one launch; lr / step / coef / scale are device scalars (``coef`` may be
+    a view of ``grad_norm_clip``'s output)."""
+    _cuda(lr, torch.float32, "lr"), _cuda(step, torch.int64, "step"), _cuda(scale, torch.float32, "scale")
+    if coef is not None:
+        _cuda(coef, torch.float32, "coef")
+    tl = _tensor_list(list(grads), p=list(params), m=list(ms), v=list(vs))
+    check(lib().uvx_adamw_multi(C.byref(tl), lr.data_ptr(), step.data_ptr(), _p(coef), scale.data_ptr(), betas[0], betas[1], eps,
+                                weight_decay, _stream()), "uvx_adamw_multi")
+
+
+def grad_accumulate_(accs, grads, assign: bool = False) -> None:
+    """acc[i] (+)= g[i] in fp32 for every pair, one launch; ``assign`` starts a new accumulation (acc = g)."""
+    tl = _tensor_list(list(grads), acc=list(accs))
+    check(lib().uvx_grad_accumulate(C.byref(tl), int(bool(assign)), _stream()), "uvx_grad_accumulate")
+
+
 # ------------------------------------------------------------------------------------------ decode step (a13)
 def gemv(x: torch.Tensor, w: torch.Tensor, residual: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
          out_dtype=BF16, norm: Optional[tuple] = None, swiglu: bool = False) -> torch.Tensor:
