@@ -287,6 +287,27 @@ int uvx_token_finish(int64_t* tok, int32_t* done, const int64_t* eos_ids, int32_
                      int64_t seq_stride, int32_t* cur_len, int32_t* step_idx, int32_t* bump0, int32_t* bump1, int32_t* bump2,
                      int32_t* all_done, int64_t B, uvx_stream_t stream);
 
+/* Continuous batching (ultravox_b200/engine.py SlotDecodeEngine): B decode rows ("slots") that each carry their own request, so
+ * every per-request scalar is a device array [B] and rows with active[b] == 0 are idle.
+ * uvx_sample_slots              active rows only: temperature[b] <= 0 -> out[b] = uvx_argmax of the row (first maximal index, an
+ *                               all -inf row gives 0); otherwise out[b] = uvx_sample (top_p[b] >= 1) or uvx_sample_top_p
+ *                               (top_p[b] < 1) of the row with temperature[b], top_k[b], top_p[b] and the uniform
+ *                               u[b * u_stride + n_new[b]] - bit for bit the pick those entries make.  Inactive rows are not written.
+ * uvx_repetition_penalty_slots  uvx_repetition_penalty on active rows with penalty[b] != 1, over seq[b, 0:cur_len[b]], scratch
+ *                               [B, seq_stride] fp32.
+ * uvx_slot_finish               for each active row that is not done: seq[b, cur_len[b]] = tok[b]; cur_len[b]++, n_new[b]++;
+ *                               done[b] = tok[b] in eos_ids or n_new[b] >= max_new[b]; pos / lens / rope_pos [b]++ only if the
+ *                               row is still open.  Done and inactive rows are frozen (their decode KV writes stay at one
+ *                               position).  n_open[0] = number of active rows still open.                                         */
+int uvx_sample_slots(const float* logits, int64_t B, int64_t V, const float* temperature, const int32_t* top_k, const float* top_p,
+                     const float* u, int64_t u_stride, const int32_t* n_new, const int32_t* active, int64_t* out_idx,
+                     uvx_stream_t stream);
+int uvx_repetition_penalty_slots(float* logits, int64_t B, int64_t V, const int64_t* seq, int64_t seq_stride, const int32_t* cur_len,
+                                 const float* penalty, const int32_t* active, float* scratch, uvx_stream_t stream);
+int uvx_slot_finish(const int64_t* tok, int32_t* done, const int64_t* eos_ids, int32_t n_eos, int64_t* seq, int64_t seq_stride,
+                    int32_t* cur_len, int32_t* n_new, const int32_t* max_new, const int32_t* active, int32_t* pos, int32_t* lens,
+                    int32_t* rope_pos, int32_t* n_open, int64_t B, uvx_stream_t stream);
+
 /* Beam search (hf:generation/utils.py _beam_search, transformers 5.5, and the helpers above it), one decode step as four
  * launches that read every per-step scalar from device memory.  B prompts, nb <= 8 beams each: row r = b * nb + j.
  * uvx_log_softmax   out[r] = log_softmax(in[r]) in fp32 (in == out allowed).  Beam search scores log-probs; the repetition

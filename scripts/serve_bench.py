@@ -1,0 +1,180 @@
+"""Continuous batching against static batches on a serving workload.
+
+64 independent requests to the 8B backbone with the large-v3 encoder (`preset("v0_5_8b")`, random weights), all submitted at
+t = 0.  Each is one clip of 5, 10, 20 or 30 s between 8 and 5 text tokens, with a budget of 16-256 new tokens drawn uniformly
+(fixed seed).  There are no EOS ids (random weights almost never emit one), so each budget sets its reply length.  Greedy.
+
+Arms, alternated over `--rounds` rounds in one process after a warm-up of each:
+- static: batches of 8 in submission order, left-padded as `LocalInference.infer_batch` collates them, one `generate()` per
+  batch with `max_new_tokens` = the batch's largest budget (every row decodes until the longest reply ends);
+- slots: `serving.SlotScheduler` with 8 slots (one engine, captured once before the rounds).
+
+Per arm: wall time (host clock, synchronised), useful tokens per second (the sum of the budgets over the wall time), decode
+milliseconds per step (CUDA events around every decode step), time to first token p50 / p90 over the 64 requests (CUDA events
+from t = 0 to the request's first picked token) and the share of decode row-steps (rows x steps) that decode padding or idle slots.
+
+Prints the device name and power limit first, then one JSON line per arm."""
+import argparse, json, os, statistics, sys, time
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import numpy as np
+import torch
+from sample_bench import device_info
+from ultravox_b200 import ops
+
+SR, PRE, POST = 16000, 8, 5
+
+
+def make_requests(cfg, n, seed):
+    rng = np.random.default_rng(seed)
+    secs = rng.choice([5, 10, 20, 30], size=n)
+    budgets = rng.integers(16, 257, size=n)
+    g = torch.Generator().manual_seed(seed)
+    reqs = []
+    for i in range(n):
+        wave = torch.from_numpy(rng.standard_normal(int(secs[i]) * SR).astype(np.float32)).cuda()
+        mel = ops.logmel(wave[None], cfg.audio_config.num_mel_bins)
+        frames = mel.shape[-1]
+        tok = -(-frames // 16)
+        ids = torch.randint(0, 128000, (1, PRE + tok + POST), generator=g)
+        reqs.append(dict(feats=dict(input_ids=ids.cuda(), audio_values=mel, audio_token_start_idx=torch.tensor([PRE]).cuda(),
+                                    audio_lens=torch.tensor([frames]).cuda(), audio_token_len=torch.tensor([tok], dtype=torch.int32).cuda(),
+                                    audio_batch_size=torch.ones(1, dtype=torch.int64).cuda()),
+                         budget=int(budgets[i])))
+    return reqs
+
+
+def collate(batch):
+    """Left padding, as the inference collator does: ids padded with 0 on the left, the audio start shifted, mel padded."""
+    S = max(r["feats"]["input_ids"].shape[1] for r in batch)
+    T = max(r["feats"]["audio_values"].shape[-1] for r in batch)
+    ids, am, start, mels = [], [], [], []
+    for r in batch:
+        f = r["feats"]
+        p = S - f["input_ids"].shape[1]
+        ids.append(torch.nn.functional.pad(f["input_ids"], (p, 0)))
+        am.append(torch.nn.functional.pad(torch.ones_like(f["input_ids"]), (p, 0)))
+        start.append(f["audio_token_start_idx"] + p)
+        mels.append(torch.nn.functional.pad(f["audio_values"], (0, T - f["audio_values"].shape[-1])))
+    cat = lambda k: torch.cat([r["feats"][k] for r in batch])
+    return dict(input_ids=torch.cat(ids), attention_mask=torch.cat(am), audio_token_start_idx=torch.cat(start),
+                audio_values=torch.cat(mels), audio_lens=cat("audio_lens"), audio_token_len=cat("audio_token_len"),
+                audio_batch_size=cat("audio_batch_size"))
+
+
+class _Events:
+    """A streamer that records a CUDA event per new token and never synchronises."""
+
+    def __init__(self):
+        self.events, self.seen_prompt = [], False
+
+    def put(self, _):
+        if not self.seen_prompt:
+            self.seen_prompt = True
+            return
+        e = torch.cuda.Event(enable_timing=True)
+        e.record()
+        self.events.append(e)
+
+    def end(self):
+        pass
+
+
+def run_static(model, reqs, batch=8):
+    t0 = torch.cuda.Event(enable_timing=True)
+    torch.cuda.synchronize()
+    w0 = time.perf_counter()
+    t0.record()
+    ttft, steps_ms, row_steps = [], [], 0
+    for i in range(0, len(reqs), batch):
+        chunk = reqs[i:i + batch]
+        n = max(r["budget"] for r in chunk)
+        st = _Events()
+        model.generate(**collate(chunk), max_new_tokens=n, streamer=st)
+        ttft.append((st.events[0], len(chunk)))
+        steps_ms.append(st.events)
+        row_steps += (n - 1) * len(chunk)                   # the first token comes from the prefill
+    torch.cuda.synchronize()
+    wall = time.perf_counter() - w0
+    first = [t0.elapsed_time(e) for e, k in ttft for _ in range(k)]
+    step = [a.elapsed_time(b) for evs in steps_ms for a, b in zip(evs, evs[1:])]
+    return wall, first, step, row_steps
+
+
+def run_slots(sched, reqs):
+    eng = sched.engine
+    marks = []
+    plain = eng.step
+
+    def timed():
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        plain()
+        b.record()
+        marks.append((a, b))
+
+    eng.step = timed
+    t0 = torch.cuda.Event(enable_timing=True)
+    torch.cuda.synchronize()
+    w0 = time.perf_counter()
+    t0.record()
+    steps0 = sched.steps
+    ids = [sched.submit(r["feats"], max_new_tokens=r["budget"]) for r in reqs]
+    sched.run()
+    torch.cuda.synchronize()
+    wall = time.perf_counter() - w0
+    eng.step = plain
+    first = [t0.elapsed_time(sched.first_token[i]) for i in ids]
+    step = [a.elapsed_time(b) for a, b in marks]
+    return wall, first, step, (sched.steps - steps0) * eng.slots
+
+
+def pct(xs, q):
+    return float(np.percentile(np.asarray(xs), q))
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
+    ap.add_argument("--requests", type=int, default=64)
+    ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--seed", type=int, default=0)
+    args = ap.parse_args()
+    print(json.dumps({"device": device_info()}), flush=True)
+    from ultravox_b200.config import preset
+    from ultravox_b200.model import UltravoxModel
+    from ultravox_b200.serving import SlotScheduler
+    torch.set_grad_enabled(False)
+    cfg = preset("v0_5_8b")
+    model = UltravoxModel(cfg, device="cuda").init_random_(seed=42)
+    reqs = make_requests(cfg, args.requests, args.seed)
+    useful = sum(r["budget"] for r in reqs)
+    useful_steps = useful - len(reqs)                         # tokens picked by decode steps (the first comes from the prefill)
+    max_len = max(r["feats"]["input_ids"].shape[1] for r in reqs) + 256
+    c0 = time.perf_counter()
+    sched = SlotScheduler(model, slots=8, max_len=max_len)
+    torch.cuda.synchronize()
+    build_s = time.perf_counter() - c0
+    warm = [dict(r, budget=16) for r in reqs[:8]]
+    run_static(model, warm)
+    run_slots(sched, warm)
+    out = {"static": [], "slots": []}
+    for _ in range(args.rounds):
+        out["static"].append(run_static(model, reqs))
+        out["slots"].append(run_slots(sched, reqs))
+    for arm, runs in out.items():
+        walls = [r[0] for r in runs]
+        k = walls.index(sorted(walls)[len(walls) // 2])
+        wall, first, step, row_steps = runs[k]
+        line = {"bench": "serve 64 requests, 8B + large-v3, clips 5-30 s, budgets 16-256, greedy", "arm": arm,
+                "wall_s_median": wall, "wall_s_all": [round(w, 3) for w in walls], "useful_tokens": useful,
+                "tokens_per_s": useful / wall, "decode_ms_per_step_mean": statistics.fmean(step), "decode_steps": len(step),
+                "ttft_ms_p50": pct(first, 50), "ttft_ms_p90": pct(first, 90), "row_steps": row_steps,
+                "wasted_row_step_share": 1.0 - useful_steps / row_steps}
+        if arm == "slots":
+            line["engine_build_s"] = build_s
+            line["launches_per_step"] = sched.engine.launches_per_step
+        print(json.dumps(line), flush=True)
+
+
+if __name__ == "__main__":
+    main()

@@ -86,6 +86,9 @@ SIGNATURES = {
     "uvx_sample": (C.c_int, [c_vp, c_i64, c_i64, c_f32, c_i32, c_vp, c_vp, c_i64, c_vp, c_vp]),
     "uvx_sample_top_p": (C.c_int, [c_vp, c_i64, c_i64, c_f32, c_i32, c_f32, c_vp, c_vp, c_i64, c_vp, c_vp]),
     "uvx_token_finish": (C.c_int, [c_vp, c_vp, c_vp, c_i32, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
+    "uvx_sample_slots": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp]),
+    "uvx_repetition_penalty_slots": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "uvx_slot_finish": (C.c_int, [c_vp, c_vp, c_vp, c_i32, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
     "uvx_log_softmax": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_vp]),
     "uvx_beam_select": (C.c_int, [c_vp, c_i64, c_i32, c_i64, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "uvx_beam_update": (C.c_int, [c_vp, c_vp, c_i64, c_i32, c_i32, c_i64, c_vp, c_i32, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp,

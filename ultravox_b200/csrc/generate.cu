@@ -6,6 +6,9 @@
 //                           temperature > 0; hf:generation/utils.py _sample: softmax(logits / T) -> multinomial)
 //   uvx_sample_top_p        the same with nucleus (top-p) filtering after top-k (hf:generation/logits_process.py TopPLogitsWarper)
 //   uvx_token_finish        EOS / pad bookkeeping of the finished rows, append to `sequences`, advance positions
+//   uvx_sample_slots        continuous batching: per-row greedy / sampled pick with each row's own settings and uniform
+//   uvx_repetition_penalty_slots   the repetition penalty with each row's own penalty and length
+//   uvx_slot_finish         per-row append / budget / EOS bookkeeping; finished and idle rows stay frozen
 //   uvx_log_softmax         beam search scores: log_softmax over each logits row (hf:generation/utils.py _beam_search)
 //   uvx_beam_select         the top K of (log-prob + running beam score) over each prompt's nb * V continuations
 //   uvx_beam_update         running beams, finished-hypothesis pool, early-stop heuristic and loop condition of one step
@@ -71,21 +74,18 @@ __device__ __forceinline__ uint32_t f2key(float f) {  // order-preserving float 
 // seeded torch generator).  sample_kernel<false> is uvx_sample; top_p is read only by sample_kernel<true>.
 constexpr float kMassOne = 1099511627776.f;  // 2^40: fixed-point unit of the top-p mass (sum <= V * 2^40 < 2^64 for V <= 2^24)
 
-template <bool TOP_P>  // (1024, 1): lets ptxas use the 64 registers a lone 1024-thread CTA may have (the top-p form uses 56)
-__global__ void __launch_bounds__(1024, 1) sample_kernel(const float* __restrict__ logits, int64_t V, float inv_temp, int top_k,
-                                                     float top_p, const float* __restrict__ u_all,
-                                                     const int32_t* __restrict__ step_idx, int64_t u_stride,
-                                                     int64_t* __restrict__ out) {
-  pdl_trigger();
-  pdl_wait();
+// The body is sample_row, shared with uvx_sample_slots: TOP_P = 0 never runs the nucleus pass, 1 always does, 2 does when the
+// row's top_p < 1 (the per-row form of uvx_sample_top_p routing top_p >= 1 to uvx_sample).  The caller's CTA handles one row.
+template <int TOP_P>
+__device__ __forceinline__ void sample_row(const float* __restrict__ row, int64_t V, float inv_temp, int top_k, float top_p,
+                                           const float* __restrict__ u_all, const int32_t* __restrict__ step_idx, int64_t u_stride,
+                                           int64_t col, int64_t* __restrict__ out_ptr) {
   __shared__ float red[32];
   __shared__ uint32_t hist[256];
   __shared__ uint32_t sel_prefix, sel_remaining;
   __shared__ float chunk_base[32];
   __shared__ int win_thread;
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  const int64_t b = blockIdx.x;
-  const float* row = logits + b * V;
   // ---- max
   float mx = -INFINITY;
   for (int64_t i = tid; i < V; i += 1024) mx = fmaxf(mx, row[i]);
@@ -122,7 +122,7 @@ __global__ void __launch_bounds__(1024, 1) sample_kernel(const float* __restrict
     }
     thr_key = sel_prefix;
   }
-  if constexpr (TOP_P) {
+  if (TOP_P == 1 || (TOP_P == 2 && top_p < 1.f)) {
     // ---- top-p threshold over the top-k survivors (HF TopPLogitsWarper after TopKLogitsWarper): with m_i = exp((x_i - max) / T),
     // the smallest key v such that the mass of the keys <= v exceeds (1 - top_p) * (total mass); keys >= v are kept.  Radix
     // select from the top byte down: a 256-bin mass histogram of the keys that match the prefix, scanned upward from the mass
@@ -238,7 +238,7 @@ __global__ void __launch_bounds__(1024, 1) sample_kernel(const float* __restrict
   __syncthreads();
   const float total = red[0];
   const float excl = chunk_base[w] + incl - local;
-  const float u = u_all[(int64_t)(step_idx ? *step_idx : 0) * u_stride + b];
+  const float u = u_all[(int64_t)(step_idx ? *step_idx : 0) * u_stride + col];
   const float target = fminf(u, 0.99999994f) * total;
   if (local > 0.f && target >= excl && target < excl + local) atomicMax(&win_thread, tid);
   __syncthreads();
@@ -260,8 +260,135 @@ __global__ void __launch_bounds__(1024, 1) sample_kernel(const float* __restrict
       if (acc > target) { pick = i; break; }
     }
     if (pick < 0) pick = last >= 0 ? last : 0;
-    out[b] = pick;
+    *out_ptr = pick;
   }
+}
+
+template <bool TOP_P>  // (1024, 1): lets ptxas use the 64 registers a lone 1024-thread CTA may have (the top-p form uses 56)
+__global__ void __launch_bounds__(1024, 1) sample_kernel(const float* __restrict__ logits, int64_t V, float inv_temp, int top_k,
+                                                     float top_p, const float* __restrict__ u_all,
+                                                     const int32_t* __restrict__ step_idx, int64_t u_stride,
+                                                     int64_t* __restrict__ out) {
+  pdl_trigger();
+  pdl_wait();
+  const int64_t b = blockIdx.x;
+  sample_row<TOP_P ? 1 : 0>(logits + b * V, V, inv_temp, top_k, top_p, u_all, step_idx, u_stride, b, out + b);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// Continuous batching: a fixed set of decode rows ("slots"), each with its own request state.  The state written by the
+// preceding kernel (or by the host between graph replays) is read through plain pointers, as in the beam kernels below.
+
+// One CTA per row: first index of the row maximum (uvx_argmax's rule: an all -inf row gives 0).
+__device__ __forceinline__ void argmax_row(const float* row, int64_t V, int64_t* out_ptr) {
+  __shared__ float red[32];
+  __shared__ unsigned long long ired[32];
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  float mx = -INFINITY;
+  for (int64_t i = tid; i < V; i += 1024) mx = fmaxf(mx, row[i]);
+  mx = warp_max(mx);
+  if (lane == 0) red[w] = mx;
+  __syncthreads();
+  mx = warp_max(red[lane]);
+  unsigned long long first = ~0ull;
+  for (int64_t i = tid; i < V; i += 1024)
+    if (row[i] == mx) { first = (unsigned long long)i; break; }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const unsigned long long t = __shfl_xor_sync(0xffffffffu, first, o);
+    first = t < first ? t : first;
+  }
+  if (lane == 0) ired[w] = first;
+  __syncthreads();
+  if (w == 0) {
+    first = ired[lane];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const unsigned long long t = __shfl_xor_sync(0xffffffffu, first, o);
+      first = t < first ? t : first;
+    }
+    if (lane == 0) *out_ptr = (int64_t)first;
+  }
+}
+
+// One CTA per row: inactive rows are left alone; temperature <= 0 takes the argmax, otherwise sample_row with the row's own
+// settings and the uniform u[row * u_stride + n_new[row]].
+__global__ void __launch_bounds__(1024, 1) sample_slots_kernel(const float* logits, int64_t V, const float* temperature,
+                                                               const int32_t* top_k, const float* top_p, const float* u,
+                                                               int64_t u_stride, const int32_t* n_new, const int32_t* active,
+                                                               int64_t* out) {
+  pdl_trigger();
+  pdl_wait();
+  const int64_t b = blockIdx.x;
+  if (!active[b]) return;
+  const float t = temperature[b];
+  const float* row = logits + b * V;
+  if (!(t > 0.f)) {
+    argmax_row(row, V, out + b);
+    return;
+  }
+  sample_row<2>(row, V, __frcp_rn(t), top_k[b], top_p[b], u + b * u_stride, n_new + b, 1, 0, out + b);
+}
+
+// One CTA per row: uvx_repetition_penalty's rule with the row's own penalty over seq[b, 0:cur_len[b]]; inactive rows and
+// penalty 1 are skipped.
+__global__ void __launch_bounds__(1024) rep_penalty_slots_kernel(float* logits, int64_t V, const int64_t* seq, int64_t seq_stride,
+                                                                 const int32_t* cur_len, const float* penalty, const int32_t* active,
+                                                                 float* __restrict__ scratch) {
+  pdl_trigger();
+  pdl_wait();
+  const int64_t b = blockIdx.x;
+  if (!active[b]) return;
+  const float pen = penalty[b];
+  if (pen == 1.f) return;
+  const int n = cur_len[b];
+  float* row = logits + b * V;
+  const int64_t* sq = seq + b * seq_stride;
+  float* sc = scratch + b * seq_stride;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const int64_t t = sq[i];
+    sc[i] = (t >= 0 && t < V) ? row[t] : 0.f;
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const int64_t t = sq[i];
+    if (t >= 0 && t < V) {
+      const float x = sc[i];
+      row[t] = x < 0.f ? x * pen : x / pen;
+    }
+  }
+}
+
+// One CTA: for each active, unfinished row append tok at seq[b, cur_len[b]], advance cur_len / n_new, finish on an EOS id or
+// at the budget, and advance pos / lens / rope_pos only while the row stays open.  n_open[0] = active rows still open.
+__global__ void slot_finish_kernel(const int64_t* tok, int32_t* done, const int64_t* __restrict__ eos, int n_eos, int64_t* seq,
+                                   int64_t seq_stride, int32_t* cur_len, int32_t* n_new, const int32_t* max_new, const int32_t* active,
+                                   int32_t* pos, int32_t* lens, int32_t* rope_pos, int32_t* n_open, int64_t B) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ int open;
+  if (threadIdx.x == 0) open = 0;
+  __syncthreads();
+  for (int64_t b = threadIdx.x; b < B; b += blockDim.x) {
+    if (!active[b] || done[b]) continue;
+    const int64_t t = tok[b];
+    const int n = cur_len[b];
+    seq[b * seq_stride + n] = t;
+    cur_len[b] = n + 1;
+    const int k = n_new[b] + 1;
+    n_new[b] = k;
+    int d = k >= max_new[b];
+    for (int e = 0; e < n_eos; ++e) d |= (t == eos[e]);
+    done[b] = d;
+    if (!d) {
+      pos[b] += 1;
+      lens[b] += 1;
+      rope_pos[b] += 1;
+      atomicAdd(&open, 1);
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) *n_open = open;
 }
 
 // One CTA: rows that already produced an EOS emit pad_id (HF semantics), the token is appended to `sequences`, rows whose token
@@ -698,6 +825,41 @@ extern "C" int uvx_sample_top_p(const float* logits, int64_t B, int64_t V, float
   launch_k(sample_kernel<true>, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, 1.0f / temperature, (int)top_k,
            top_p, u, step_idx, u_stride, out_idx);
   return check_launch("sample_kernel_top_p");
+}
+
+extern "C" int uvx_sample_slots(const float* logits, int64_t B, int64_t V, const float* temperature, const int32_t* top_k,
+                                const float* top_p, const float* u, int64_t u_stride, const int32_t* n_new, const int32_t* active,
+                                int64_t* out_idx, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(logits && temperature && top_k && top_p && u && n_new && active && out_idx && B >= 1 && V >= 1 &&
+                  V <= (int64_t)1 << 24 && u_stride >= 0,
+              "uvx_sample_slots: bad arguments");
+  launch_k(sample_slots_kernel, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, temperature, top_k, top_p, u,
+           u_stride, n_new, active, out_idx);
+  return check_launch("sample_slots_kernel");
+}
+
+extern "C" int uvx_repetition_penalty_slots(float* logits, int64_t B, int64_t V, const int64_t* seq, int64_t seq_stride,
+                                            const int32_t* cur_len, const float* penalty, const int32_t* active, float* scratch,
+                                            uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(logits && seq && cur_len && penalty && active && scratch && B >= 1 && V >= 1,
+              "uvx_repetition_penalty_slots: bad arguments");
+  launch_k(rep_penalty_slots_kernel, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, seq, seq_stride, cur_len,
+           penalty, active, scratch);
+  return check_launch("rep_penalty_slots_kernel");
+}
+
+extern "C" int uvx_slot_finish(const int64_t* tok, int32_t* done, const int64_t* eos_ids, int32_t n_eos, int64_t* seq,
+                               int64_t seq_stride, int32_t* cur_len, int32_t* n_new, const int32_t* max_new, const int32_t* active,
+                               int32_t* pos, int32_t* lens, int32_t* rope_pos, int32_t* n_open, int64_t B, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(tok && done && seq && cur_len && n_new && max_new && active && pos && lens && rope_pos && n_open && B >= 1 &&
+                  n_eos >= 0 && (n_eos == 0 || eos_ids),
+              "uvx_slot_finish: bad arguments");
+  launch_k(slot_finish_kernel, dim3(1), dim3(128), 0, (cudaStream_t)stream, tok, done, eos_ids, (int)n_eos, seq, seq_stride, cur_len,
+           n_new, max_new, active, pos, lens, rope_pos, n_open, B);
+  return check_launch("slot_finish_kernel");
 }
 
 extern "C" int uvx_token_finish(int64_t* tok, int32_t* done, const int64_t* eos_ids, int32_t n_eos, int64_t pad_id, int64_t* seq,

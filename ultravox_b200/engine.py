@@ -386,3 +386,128 @@ class BeamDecodeEngine(DecodeEngine):
         seq = self.pool_seq[idx, :width]
         keep = torch.arange(width, device=dev)[None, :] < (prompt_len + lens)[:, None]
         return torch.where(keep, seq, torch.full_like(seq, fill_value)), self.pool_score[idx].clone()
+
+
+class SlotDecodeEngine(DecodeEngine):
+    """Continuous batching: ``slots`` decode rows that each carry their own request.  The step is the forward of
+    ``DecodeEngine._step`` over all rows followed by three per-row kernels (``uvx_repetition_penalty_slots``,
+    ``uvx_sample_slots``, ``uvx_slot_finish``); every per-request value - positions, lengths, budget, active / done flags,
+    sampling settings, the uniforms - lives in a device array [slots], so the step is captured once per engine and admission
+    and retirement only write into those arrays between replays.
+
+    An idle slot holds ``pos = 0``, ``lens = 1`` and the pad token: it writes its own K / V at position 0 and attends to that
+    alone, so it stays finite whatever its cache row held.  A finished slot is frozen (no sequence writes, no position bumps)
+    until ``retire``.  ``n_open[0]`` counts the active slots still decoding after each step."""
+
+    def __init__(self, model: UltravoxModel, slots: int, max_len: int, eos_token_ids=None, pad_token_id: int = 0,
+                 use_graph: bool = True):
+        super().__init__(model, slots, max_len, use_graph=use_graph, eos_token_ids=eos_token_ids, pad_token_id=pad_token_id)
+        dev = model.device
+        i32, f32 = dict(dtype=torch.int32, device=dev), dict(dtype=torch.float32, device=dev)
+        self.slots = int(slots)
+        self.cur_len = torch.zeros(slots, **i32)
+        self.n_new = torch.zeros(slots, **i32)
+        self.max_new = torch.ones(slots, **i32)
+        self.active = torch.zeros(slots, **i32)
+        self.temps = torch.zeros(slots, **f32)
+        self.top_ks = torch.zeros(slots, **i32)
+        self.top_ps = torch.ones(slots, **f32)
+        self.penalties = torch.ones(slots, **f32)
+        self.u = torch.zeros(slots, self.max_len + 1, **f32)
+        self.scratch = torch.empty(slots, self.max_len + 1, **f32)
+        self.n_open = torch.zeros(1, **i32)
+        self._admit_open = torch.zeros(1, **i32)     # the count an admission's one-row pick writes (not the step's)
+        self.captures = 0
+        self.busy = [False] * self.slots
+        for j in range(self.slots):
+            self._idle(j)
+        if use_graph:
+            self._step_warm()
+
+    def _idle(self, j: int) -> None:
+        self.active[j] = 0
+        self.done[j] = 0
+        self.cur_len[j] = 0
+        self.n_new[j] = 0
+        self.pos[j] = 0
+        self.lens[j] = 1
+        self.rope_pos[j] = 0
+        self.token[j] = self.pad_id
+        self.busy[j] = False
+
+    def _state(self):
+        return [self.pos, self.lens, self.rope_pos, self.token, self.cur_len, self.n_new, self.done, self.n_open]
+
+    def _step_warm(self):
+        self.captures += 1
+        super()._step_warm()
+
+    def _pick_rows(self, logits: torch.Tensor, r: slice, n_open: torch.Tensor) -> None:
+        tok = self.token.view(-1)[r]
+        ops.repetition_penalty_slots_(logits, self.seq[r], self.cur_len[r], self.penalties[r], self.active[r], self.scratch[r])
+        ops.sample_slots(logits, self.temps[r], self.top_ks[r], self.top_ps[r], self.u[r], self.n_new[r], self.active[r], tok)
+        ops.slot_finish(tok, self.done[r], self.eos, self.seq[r], self.cur_len[r], self.n_new[r], self.max_new[r], self.active[r],
+                        self.pos[r], self.lens[r], self.rope_pos[r], n_open)
+
+    def _pick(self, logits: torch.Tensor):
+        self.logits = logits
+        self._pick_rows(logits, slice(None), self.n_open)
+
+    def begin(self, *args, **kwargs):
+        raise NotImplementedError("SlotDecodeEngine takes requests through admit()")
+
+    def prefill(self, *args, **kwargs):
+        raise NotImplementedError("SlotDecodeEngine takes requests through admit()")
+
+    def admit(self, slot: int, input_ids: torch.Tensor, max_new_tokens: int, temperature: float = 0.0, top_k: int = 0,
+              top_p: float = 1.0, repetition_penalty: float = 1.0, u: Optional[torch.Tensor] = None, **features) -> torch.Tensor:
+        """Prefills one request (``input_ids`` [1, S] plus the processor's audio features, passed to ``model.forward``) at B = 1
+        into cache row ``slot``, sets the slot's state and picks its first token from the prefill logits with the slot kernels.
+        ``temperature <= 0`` is greedy; a sampled request reads ``u`` (its uniforms, one per step, as ``generate()`` draws them
+        for a batch of one).  Returns the device token tensor [slots] (no sync)."""
+        from .model import KVCache
+        j = int(slot)
+        if not 0 <= j < self.slots:
+            raise ValueError(f"slot {slot} out of range [0, {self.slots})")
+        if self.busy[j]:
+            raise ValueError(f"slot {j} is busy; retire it first")
+        if input_ids.dim() != 2 or input_ids.shape[0] != 1:
+            raise ValueError(f"admit() takes one request: input_ids [1, S], got {tuple(input_ids.shape)}")
+        S, n = int(input_ids.shape[1]), int(max_new_tokens)
+        if n < 1 or S < 1 or S + n > self.max_len:
+            raise ValueError(f"a prompt of {S} tokens plus max_new_tokens={n} does not fit a slot of {self.max_len} positions")
+        if temperature > 0 and (u is None or u.numel() < S + n):
+            raise ValueError(f"a sampled request needs at least {S + n} uniforms")
+        dev = self.pos.device
+        input_ids = input_ids.to(dev)
+        row = KVCache(self.cache.k[:, j:j + 1], self.cache.v[:, j:j + 1])
+        logits = self.model.forward(input_ids, past_key_values=row, logits_to_keep=1, **features).logits.view(1, -1)
+        self.seq[j, :S].copy_(input_ids[0])
+        self.cur_len[j] = S
+        self.n_new[j] = 0
+        self.max_new[j] = n
+        self.done[j] = 0
+        self.active[j] = 1
+        # the pick's slot_finish bumps all three: the first new token sits at slot S, sees S + 1 keys, RoPE position S
+        self.pos[j] = S - 1
+        self.lens[j] = S
+        self.rope_pos[j] = S - 1
+        self.temps[j] = float(temperature) if temperature > 0 else 0.0
+        self.top_ks[j] = int(top_k or 0)
+        self.top_ps[j] = float(top_p)
+        self.penalties[j] = float(repetition_penalty or 1.0)
+        if u is not None:
+            w = min(u.numel(), self.max_len + 1)
+            self.u[j, :w].copy_(u.reshape(-1)[:w])
+        self.busy[j] = True
+        self._pick_rows(logits, slice(j, j + 1), self._admit_open)
+        return self.token.view(-1)
+
+    def retire(self, slot: int, length: Optional[int] = None) -> torch.Tensor:
+        """The slot's sequence [1, prompt + new tokens] (a copy; ``length`` = its ``cur_len`` if the caller already read it, else
+        one sync), then the slot goes back to idle."""
+        j = int(slot)
+        n = int(self.cur_len[j]) if length is None else int(length)
+        out = self.seq[j:j + 1, :n].clone()
+        self._idle(j)
+        return out

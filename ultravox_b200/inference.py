@@ -184,16 +184,20 @@ class LocalInference(VoiceInference):
         dev = self.model.device
         return {k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in inputs.items()}
 
+    def _terminators(self) -> List[int]:
+        terminators = [self.tokenizer.eos_token_id]
+        extra = getattr(self.tokenizer, "added_tokens_encoder", {})
+        if "<|eot_id|>" in extra:
+            terminators.append(self.tokenizer.convert_tokens_to_ids("<|eot_id|>"))
+        return terminators
+
     @torch.inference_mode()
     def _generate(self, inputs: Dict[str, torch.Tensor], max_new_tokens: Optional[int] = None,
                   temperature: Optional[float] = None, streamer=None, past_key_values=None,
                   return_dict_in_generate: bool = True):
         # ref infer.py:319-328: temperature None -> model default (greedy here), 0 -> greedy, > 0 -> sample
         do_sample = temperature is not None and temperature > 0
-        terminators = [self.tokenizer.eos_token_id]
-        extra = getattr(self.tokenizer, "added_tokens_encoder", {})
-        if "<|eot_id|>" in extra:
-            terminators.append(self.tokenizer.convert_tokens_to_ids("<|eot_id|>"))
+        terminators = self._terminators()
         return self.model.generate(**inputs, max_new_tokens=max_new_tokens or MAX_NEW_TOKENS, eos_token_id=terminators,
                                    streamer=streamer, past_key_values=past_key_values, do_sample=do_sample,
                                    temperature=temperature if do_sample else None,
@@ -234,6 +238,36 @@ class LocalInference(VoiceInference):
         outs = []
         for row in seqs:
             new_tokens = row[input_len:]
+            text, thinking = self._postprocess_response(self.tokenizer.decode(new_tokens, skip_special_tokens=True))
+            outs.append(VoiceOutput(text, input_len, len(new_tokens), thinking_content=thinking))
+        return outs
+
+    @torch.inference_mode()
+    def infer_many(self, samples: List[VoiceSample], max_tokens: Optional[int] = None, temperature: Optional[float] = None,
+                   slots: int = 8, max_len: Optional[int] = None) -> List[VoiceOutput]:
+        """Serves independent samples through ``slots`` continuous-batching slots (``serving.SlotScheduler``): a finished reply
+        frees its slot for the next sample at once, instead of a static batch decoding until its longest reply ends.  Same
+        data processing, terminators and sampling rule as ``infer``; each result is what ``infer`` gives for that sample alone
+        (no conversation mode, like ``infer_batch``).  Results come back in input order.  ``max_len`` is the slot capacity in
+        positions (default: the longest prompt plus ``max_tokens``); a sample that does not fit raises ``ValueError``."""
+        assert not self.conversation_mode
+        from .serving import SlotScheduler
+        feats = [self._dataproc(s) for s in samples]
+        if not feats:
+            return []
+        max_new = max_tokens or MAX_NEW_TOKENS
+        need = max(int(f["input_ids"].shape[1]) for f in feats) + max_new
+        if max_len is not None and need > max_len:
+            raise ValueError(f"a sample needs {need} positions (prompt + max_tokens); the slots hold {max_len}")
+        sched = SlotScheduler(self.model, slots=slots, max_len=max_len or need, eos_token_ids=self._terminators())
+        do_sample = temperature is not None and temperature > 0
+        ids = [sched.submit(f, max_new_tokens=max_new, do_sample=do_sample, temperature=temperature if do_sample else None)
+               for f in feats]
+        res = sched.run()
+        outs = []
+        for f, rid in zip(feats, ids):
+            input_len = int(f["input_ids"].shape[1])
+            new_tokens = res[rid][0, input_len:]
             text, thinking = self._postprocess_response(self.tokenizer.decode(new_tokens, skip_special_tokens=True))
             outs.append(VoiceOutput(text, input_len, len(new_tokens), thinking_content=thinking))
         return outs

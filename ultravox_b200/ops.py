@@ -724,6 +724,77 @@ def token_finish(tok: torch.Tensor, done: torch.Tensor, eos_ids: Optional[torch.
                                  _p(b[2]), _p(all_done), tok.numel(), _stream()), "uvx_token_finish")
 
 
+# ------------------------------------------------------------------------------------------ continuous batching (slots)
+def _rows(t: torch.Tensor, dtype, B: int, name: str) -> torch.Tensor:
+    """A contiguous per-row device array [B] of ``dtype``."""
+    _cuda(t, dtype, name)
+    if t.shape != (B,) or not t.is_contiguous():
+        raise ValueError(f"{name} must be a contiguous [{B}] tensor, got {tuple(t.shape)}")
+    return t
+
+
+def _seq_rows(t: torch.Tensor, dtype, B: int, name: str) -> torch.Tensor:
+    """A [B, W] device tensor with unit column stride (its row stride is passed to the kernel)."""
+    _cuda(t, dtype, name)
+    if t.dim() != 2 or t.shape[0] != B or t.stride(1) != 1:
+        raise ValueError(f"{name} must be [{B}, W] with unit column stride, got {tuple(t.shape)} strides {t.stride()}")
+    return t
+
+
+def sample_slots(logits: torch.Tensor, temperature: torch.Tensor, top_k: torch.Tensor, top_p: torch.Tensor, u: torch.Tensor,
+                 n_new: torch.Tensor, active: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """Per-row pick of ``uvx_sample_slots``: logits [B, V] fp32, temperature / top_p [B] fp32, top_k [B] int32, u [B, W] fp32
+    (row b reads u[b, n_new[b]]), n_new / active [B] int32 -> out [B] int64 (inactive rows untouched)."""
+    _cuda(logits, torch.float32, "logits")
+    if logits.dim() != 2 or not logits.is_contiguous():
+        raise ValueError("logits must be a contiguous [B, V] tensor")
+    B, V = logits.shape
+    _rows(temperature, torch.float32, B, "temperature"), _rows(top_k, torch.int32, B, "top_k"), _rows(top_p, torch.float32, B, "top_p")
+    _rows(n_new, torch.int32, B, "n_new"), _rows(active, torch.int32, B, "active"), _rows(out, torch.int64, B, "out")
+    _seq_rows(u, torch.float32, B, "u")
+    check(lib().uvx_sample_slots(logits.data_ptr(), B, V, temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), u.data_ptr(),
+                                 u.stride(0), n_new.data_ptr(), active.data_ptr(), out.data_ptr(), _stream()), "uvx_sample_slots")
+    return out
+
+
+def repetition_penalty_slots_(logits: torch.Tensor, seq: torch.Tensor, cur_len: torch.Tensor, penalty: torch.Tensor,
+                              active: torch.Tensor, scratch: torch.Tensor) -> torch.Tensor:
+    """HF's repetition penalty on each active row b with penalty[b] over seq[b, :cur_len[b]], in place on logits [B, V] fp32;
+    scratch is fp32 [B, >= seq.stride(0)]."""
+    _cuda(logits, torch.float32, "logits")
+    if logits.dim() != 2 or not logits.is_contiguous():
+        raise ValueError("logits must be a contiguous [B, V] tensor")
+    B, V = logits.shape
+    _seq_rows(seq, torch.int64, B, "seq")
+    _rows(cur_len, torch.int32, B, "cur_len"), _rows(penalty, torch.float32, B, "penalty"), _rows(active, torch.int32, B, "active")
+    _seq_rows(scratch, torch.float32, B, "scratch")
+    if scratch.stride(0) < seq.stride(0) or scratch.shape[1] < seq.shape[1]:
+        raise ValueError("scratch rows must be at least as long as the seq rows")
+    if scratch.stride(0) != seq.stride(0):
+        raise ValueError("scratch and seq must share a row stride")
+    check(lib().uvx_repetition_penalty_slots(logits.data_ptr(), B, V, seq.data_ptr(), seq.stride(0), cur_len.data_ptr(), penalty.data_ptr(),
+                                             active.data_ptr(), scratch.data_ptr(), _stream()), "uvx_repetition_penalty_slots")
+    return logits
+
+
+def slot_finish(tok: torch.Tensor, done: torch.Tensor, eos_ids: Optional[torch.Tensor], seq: torch.Tensor, cur_len: torch.Tensor,
+                n_new: torch.Tensor, max_new: torch.Tensor, active: torch.Tensor, pos: torch.Tensor, lens: torch.Tensor,
+                rope_pos: torch.Tensor, n_open: torch.Tensor) -> None:
+    """``uvx_slot_finish``: tok [B] int64, seq [B, W] int64, every other per-row array [B] int32, eos_ids int64 or None,
+    n_open [1] int32 (the count of active rows still open)."""
+    B = tok.numel()
+    _rows(tok, torch.int64, B, "tok"), _seq_rows(seq, torch.int64, B, "seq")
+    for t, name in ((done, "done"), (cur_len, "cur_len"), (n_new, "n_new"), (max_new, "max_new"), (active, "active"), (pos, "pos"),
+                    (lens, "lens"), (rope_pos, "rope_pos")):
+        _rows(t, torch.int32, B, name)
+    _rows(n_open, torch.int32, 1, "n_open")
+    if eos_ids is not None:
+        _cuda(eos_ids, torch.int64, "eos_ids")
+    check(lib().uvx_slot_finish(tok.data_ptr(), done.data_ptr(), _p(eos_ids), 0 if eos_ids is None else eos_ids.numel(), seq.data_ptr(),
+                                seq.stride(0), cur_len.data_ptr(), n_new.data_ptr(), max_new.data_ptr(), active.data_ptr(), pos.data_ptr(),
+                                lens.data_ptr(), rope_pos.data_ptr(), n_open.data_ptr(), B, _stream()), "uvx_slot_finish")
+
+
 # ------------------------------------------------------------------------------------------ beam search
 BEAM_MAX = 8        # beams per prompt (kBeamMax in generate.cu)
 BEAM_MAX_K = 64     # candidates per prompt, max(2, 1 + n_eos) * num_beams

@@ -1,0 +1,150 @@
+"""Request-level continuous batching over ``engine.SlotDecodeEngine``.
+
+Requests queue FIFO.  Between decode steps the host admits one waiting request into each free slot (a B = 1 prefill into that
+slot's cache row, which pauses the other slots for its duration) and every ``sync_every`` steps it reads the device count of
+open slots to retire the finished ones and deliver their tokens.  A slot is also retired as soon as the host knows that its
+budget is spent.  Each request gets exactly what ``model.generate()`` returns for that request alone: its prompt ids, then the
+new tokens up to and including its first EOS, or ``max_new_tokens`` of them.
+"""
+from __future__ import annotations
+
+import collections
+import dataclasses
+from typing import Callable, Deque, Dict, List, Optional
+
+import torch
+
+from .engine import SlotDecodeEngine
+
+
+@dataclasses.dataclass
+class _Request:
+    rid: int
+    input_ids: torch.Tensor
+    features: dict
+    max_new: int
+    temperature: float
+    top_k: int
+    top_p: float
+    penalty: float
+    u: Optional[torch.Tensor]
+    admitted_at: int = -1
+    first_token: Optional[torch.cuda.Event] = None
+
+
+class SlotScheduler:
+    """``SlotDecodeEngine(model, slots, max_len, ...)`` plus a FIFO queue.  ``submit`` validates and queues a request and
+    returns its id; ``run`` serves until the queue is empty and returns {id: sequence [1, S + n] on the device}.
+    ``first_token[id]`` is a CUDA event recorded when the request's first token has been picked (time-to-first-token)."""
+
+    def __init__(self, model, slots: int = 8, max_len: int = 2048, eos_token_ids=None, pad_token_id: Optional[int] = None,
+                 sync_every: int = 8, use_graph: bool = True):
+        eos = sorted(set([eos_token_ids] if isinstance(eos_token_ids, int) else (eos_token_ids or [])))
+        pad = pad_token_id if pad_token_id is not None else (min(eos) if eos else 0)     # generate()'s default
+        if int(sync_every) < 1:
+            raise ValueError(f"sync_every must be >= 1, got {sync_every}")
+        self.model = model
+        self.engine = SlotDecodeEngine(model, slots, max_len, eos_token_ids=eos, pad_token_id=pad, use_graph=use_graph)
+        self.sync_every = int(sync_every)
+        self.steps = 0
+        self.first_token: Dict[int, torch.cuda.Event] = {}
+        self._queue: Deque[_Request] = collections.deque()
+        self._running: Dict[int, _Request] = {}        # slot -> request
+        self._next_id = 0
+        self._last_poll = 0
+
+    @property
+    def capacity(self) -> int:
+        return self.engine.max_len
+
+    def submit(self, features: dict, max_new_tokens: int = 20, do_sample: bool = False, temperature: Optional[float] = None,
+               top_k: Optional[int] = None, top_p: Optional[float] = None, repetition_penalty: float = 1.0,
+               generator: Optional[torch.Generator] = None, num_beams: int = 1) -> int:
+        """Queues one request: ``features`` is the processor's output for it (``input_ids`` [1, S] and, for audio, its mel or
+        waveform fields).  Arguments and defaults are ``generate()``'s: greedy unless ``do_sample``; sampling defaults to
+        temperature 1 and top_k 50; ``top_p`` must lie in [0, 1].  A sampled request draws its uniforms here, as ``generate()``
+        does for a batch of one, so a seeded generator gives the same tokens in both."""
+        if num_beams != 1:
+            raise NotImplementedError("beam search is not built into the slot engine; use generate(num_beams=...)")
+        if top_p is not None and not 0.0 <= float(top_p) <= 1.0:       # NaN fails too
+            raise ValueError(f"`top_p` has to be a float in [0, 1], but is {top_p}")
+        ids = features.get("input_ids")
+        if ids is None or ids.dim() != 2 or ids.shape[0] != 1:
+            raise ValueError("submit() takes one request: features['input_ids'] must be [1, S]")
+        am = features.get("attention_mask")
+        if am is not None and not bool(am.to(torch.bool).all()):
+            raise NotImplementedError("a single request has no padding; its attention_mask must be all ones")
+        S, n = int(ids.shape[1]), int(max_new_tokens)
+        if n < 1:
+            raise ValueError(f"max_new_tokens must be >= 1, got {max_new_tokens}")
+        if S + n > self.capacity:
+            raise ValueError(f"a prompt of {S} tokens plus max_new_tokens={n} exceeds the slot capacity of {self.capacity} positions")
+        sampling = bool(do_sample) and (temperature is None or float(temperature) > 0)
+        temp = (1.0 if temperature is None else float(temperature)) if sampling else 0.0
+        k_top = (50 if top_k is None else int(top_k)) if sampling else 0
+        p_top = float(top_p) if sampling and top_p is not None else 1.0
+        u = None
+        if sampling:
+            u = torch.rand(S + n + 1, 1, device=self.engine.pos.device, dtype=torch.float32, generator=generator)
+        feats = {k: v for k, v in features.items() if k not in ("input_ids", "attention_mask", "labels")}
+        rid = self._next_id
+        self._next_id += 1
+        self._queue.append(_Request(rid, ids, feats, n, temp, k_top, p_top, float(repetition_penalty or 1.0), u))
+        return rid
+
+    def _admit(self) -> None:
+        eng = self.engine
+        dev = eng.pos.device
+        for j in range(eng.slots):
+            if not self._queue:
+                return
+            if eng.busy[j]:
+                continue
+            r = self._queue.popleft()
+            feats = {k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in r.features.items()}
+            eng.admit(j, r.input_ids, r.max_new, r.temperature, r.top_k, r.top_p, r.penalty, r.u, **feats)
+            ev = torch.cuda.Event(enable_timing=True)
+            ev.record()
+            self.first_token[r.rid] = ev
+            r.admitted_at = self.steps
+            r.features, r.u = {}, None
+            self._running[j] = r
+
+    def _retire(self, results: Dict[int, torch.Tensor], on_tokens: Optional[Callable]) -> int:
+        eng = self.engine
+        if int(eng.n_open) >= len(self._running) and not any(self._budget_spent(r) for r in self._running.values()):
+            return 0                    # n_open counts the slots still open after the last step: nothing finished
+        state = torch.stack([eng.done, eng.cur_len]).cpu()
+        freed = 0
+        for j in sorted(self._running):
+            if not int(state[0, j]):
+                continue
+            r = self._running.pop(j)
+            seq = eng.retire(j, int(state[1, j]))
+            results[r.rid] = seq
+            freed += 1
+            if on_tokens is not None:
+                on_tokens(r.rid, seq)
+        return freed
+
+    def _budget_spent(self, r: _Request) -> bool:
+        return 1 + self.steps - r.admitted_at >= r.max_new
+
+    def run(self, on_tokens: Optional[Callable[[int, torch.Tensor], None]] = None) -> Dict[int, torch.Tensor]:
+        """Serves every queued request; ``on_tokens(id, sequence)`` is called as each one finishes."""
+        results: Dict[int, torch.Tensor] = {}
+        while self._queue or self._running:
+            self._admit()
+            due = any(self._budget_spent(r) for r in self._running.values())
+            if due or self.steps - self._last_poll >= self.sync_every:
+                self._last_poll = self.steps
+                if self._retire(results, on_tokens):
+                    continue
+                if due:
+                    raise RuntimeError("a slot reached its budget on the host but not on the device")
+            self.engine.step()
+            self.steps += 1
+        return results
+
+    def pending(self) -> List[int]:
+        return [r.rid for r in self._queue] + [r.rid for r in self._running.values()]
