@@ -326,7 +326,20 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         continue;
       }
     }
-    // plain epilogue: alpha, bias, GELU, residual, row remap; bf16 or fp32 out
+    // plain epilogue: alpha, bias, GELU, residual, row remap; bf16 or fp32 out.  The operands are loaded before the first store
+    // that could depend on them: the bias columns once per tile, a row's residual before that row's stores.  The compiler cannot
+    // move a load above a store to C (C may alias R: the in-place residual stream), so loads interleaved with the stores each
+    // waited out a full memory latency.  Hoisting is safe: a thread reads residual elements only at the positions it writes.  Only
+    // tiles with MT * BN <= 128 have the registers for it (wider ones spill, and keep the loads next to their use).
+    constexpr bool kHoist = MT * BN <= 128;
+    __nv_bfloat162 bias_v[BN / 8];
+    if constexpr (kHoist) {
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int64_t n = n0 + tile_col(8 * j + cq, p.w_perm);
+        if (p.bias && n < p.N) bias_v[j] = *reinterpret_cast<const __nv_bfloat162*>(p.bias + n);
+      }
+    }
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt) {
 #pragma unroll
@@ -336,13 +349,21 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int64_t orow = out_row(p, b, m);
         if (orow < 0) continue;
         const bf16* rrow = p.R ? p.R + (int64_t)b * p.r_batch_stride + m * p.r_row_stride : nullptr;
+        __nv_bfloat162 res_v[BN / 8];
+        if (kHoist && rrow) {
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int64_t n = n0 + tile_col(8 * j + cq, p.w_perm);
+            if (n < p.N) res_v[j] = *reinterpret_cast<const __nv_bfloat162*>(rrow + n);
+          }
+        }
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
           const int64_t n = n0 + tile_col(8 * j + cq, p.w_perm);
           if (n >= p.N) continue;  // ragged last column tile (N % BN != 0); N % 64 == 0 keeps both columns in range
           float v0 = acc[mt][4 * j + 2 * h] * p.alpha, v1 = acc[mt][4 * j + 2 * h + 1] * p.alpha;
           if (p.bias) {
-            const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.bias + n));
+            const float2 t = __bfloat1622float2(kHoist ? bias_v[j] : *reinterpret_cast<const __nv_bfloat162*>(p.bias + n));
             v0 += t.x;
             v1 += t.y;
           }
@@ -351,7 +372,7 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             v1 = gelu_fast(v1);
           }
           if (rrow) {
-            const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(rrow + n));
+            const float2 t = __bfloat1622float2(kHoist ? res_v[j] : *reinterpret_cast<const __nv_bfloat162*>(rrow + n));
             v0 += t.x;
             v1 += t.y;
           }
