@@ -133,9 +133,13 @@ int uvx_debug_gemm_stages(int n);
 /* tuning hook of the weight-streaming forms: enable (0 = never, 1 = decode form + single-pass form, 2 = decode form only; -1 =
  * UVX_GEMM_WS env, default 2), `mode` (ignored), upper bound on the persistent grid of every uvx_gemm_bf16 launch (0 = one CTA per SM) */
 int uvx_debug_gemm_ws(int enable, int mode, int grid);
-/* hooks of tuning knobs the Hopper kernel does not have (TMA-store epilogue, phase timestamps, L2 prefetch distance, pipeline
- * isolation): accepted for ABI compatibility, no effect */
+/* tuning hook: the staged epilogue of the tensor-bound calls (more than 256 rows or a batch; plain bias / GELU / residual epilogue,
+ * no row map, one split, 128 x 64 or 128 x 128 tiles): the output tile goes through shared memory and leaves by TMA store, the
+ * residual is loaded by TMA ahead of the epilogue.  -1 (default) or > 0 = staged wherever it applies, 0 = register epilogue
+ * everywhere.  Never changes the result bits. */
 int uvx_debug_gemm_tma_store(int on);
+/* hooks of tuning knobs the Hopper kernel does not have (phase timestamps, L2 prefetch distance, pipeline isolation): accepted
+ * for ABI compatibility, no effect */
 int uvx_debug_gemm_times(void* dev_buf);
 int uvx_debug_gemm_pf(int pf);
 int uvx_debug_gemm_ws_times(void* dev_buf);

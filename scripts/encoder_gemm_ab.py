@@ -1,6 +1,8 @@
 """Times the Whisper-large-v3 encoder GEMMs (T = 1500 rows; q|k|v, out, fc1, fc2) at K in {320, 640, 1280, 2560, 5120} with each
 epilogue (plain, +bias, +bias+GELU, +bias+residual) at 128 x 128 and 128 x 64 tiles (forced with uvx_debug_gemm_override) and on
-the default path.  Run it from two trees (this library and another one) to compare them call by call.
+the default path, each with the staged (shared memory + TMA store) epilogue and, in the `_reg` arms, with the register epilogue
+(uvx_debug_gemm_tma_store(0)); the arms alternate call shape by call shape.  Run it from two trees (this library and another one)
+to compare them call by call.
 
 Each (shape, K, epilogue, arm) is captured in a CUDA graph of `--calls` back-to-back calls (two weight copies alternating) and
 timed with CUDA events over `--reps` replays.  Per (shape, epilogue, arm) the time per call is fitted as t = waves * (F + c * kb)
@@ -20,19 +22,21 @@ SHAPES = {"qkv": (3 * E, E), "out": (E, E), "fc1": (4 * E, E), "fc2": (E, 4 * E)
 MODEL_EPI = {"qkv": "bias", "out": "bias_res", "fc1": "bias_gelu", "fc2": "bias_res"}
 EPILOGUES = ("plain", "bias", "bias_gelu", "bias_res")
 KS = (320, 640, 1280, 2560, 5120)
-ARMS = {"wg128": 1128, "wg64": 1064, "default": 0}   # arm -> forced MT*1000 + BN (0: heuristic)
+# arm -> (forced MT*1000 + BN (0: heuristic), uvx_debug_gemm_tma_store value (-1: default, staged where it applies; 0: registers))
+ARMS = {"wg128": (1128, -1), "wg64": (1064, -1), "default": (0, -1), "wg128_reg": (1128, 0), "wg64_reg": (1064, 0), "default_reg": (0, 0)}
 
 
 def waves(N, arm, sms):
-    bn = 64 if arm == "wg64" else 128
+    bn = 64 if arm.startswith("wg64") else 128
     tiles = -(-T // 128) * (N // bn)
     return -(-tiles // min(tiles, sms))
 
 
 def time_call(call, arm, calls, reps):
     lib = _lib.lib()
-    cfg = ARMS[arm]
+    cfg, tma = ARMS[arm]
     lib.uvx_debug_gemm_override(cfg, 1 if cfg else 0)
+    lib.uvx_debug_gemm_tma_store(tma)
     try:
         call(0), call(1)
         torch.cuda.synchronize()
@@ -51,13 +55,14 @@ def time_call(call, arm, calls, reps):
         torch.cuda.synchronize()
     finally:
         lib.uvx_debug_gemm_override(0, 0)
+        lib.uvx_debug_gemm_tma_store(-1)
     return e0.elapsed_time(e1) * 1e3 / (reps * calls)
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--shapes", default="qkv,out,fc1,fc2")
-    ap.add_argument("--arms", default="wg128,wg64,default")
+    ap.add_argument("--arms", default="wg128,wg128_reg,wg64,wg64_reg,default,default_reg")
     ap.add_argument("--calls", type=int, default=20)
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--out", default=None, help="also write every row to this JSON file")
@@ -91,7 +96,7 @@ def main():
                 pts = [(r["K"] // 64, r["us"]) for r in rows if r["shape"] == name and r["epilogue"] == epi and r["arm"] == arm]
                 kb, us = np.array(pts, dtype=np.float64).T
                 slope, icpt = np.polyfit(kb, us, 1)
-                w = waves(N, arm, sms) if arm != "default" else None
+                w = waves(N, arm, sms) if not arm.startswith("default") else None
                 fit = {"fit": name, "epilogue": epi, "arm": arm, "intercept_us": round(icpt, 2), "slope_us_per_kb": round(slope, 4)}
                 if w:
                     F, c = icpt / w, slope / w

@@ -12,7 +12,8 @@
 //   warpgroups 1-2 consumers: warpgroup c owns rows [64c, 64c+64) of each 128-row sub-tile and issues wgmma m64 x BN x 16
 //                  from shared memory with fp32 accumulators in registers, keeping one k-block of MMAs in flight while it
 //                  releases the previous ring slot; then the fused epilogue (bias / GELU / residual / row remap, fused SwiGLU or
-//                  RoPE) straight from the accumulator registers.
+//                  RoPE) straight from the accumulator registers, or - tensor-bound calls with the plain epilogue - staged
+//                  through a shared-memory tile and written by TMA store, the residual loaded into that tile by the producer.
 // A is described by a 3-D tensor map (k, row, batch) with caller-chosen strides, so overlapping rows (implicit-GEMM conv over
 // a time-major activation) and batch-strided inputs need no im2col copy; rows or k beyond the tensor bounds are zero-filled
 // by TMA, which is how M / K tails are handled.  K is always summed in k-block order, so a result depends only on the split
@@ -52,11 +53,15 @@ struct GemmParams {
   int rope_cols;
   int stages;              // ring depth
   int cm, cn;              // thread-block cluster of cm x cn tiles (1 x 1: no cluster); cm divides m_tiles * a_batch, cn n_tiles
+  int staged_bytes;        // staged epilogue (gemm_wg_kernel<., ., true>): its output tile in shared memory, between the ring and
+                           // the barriers (0: register epilogue)
+  int r_bcast;             // the residual has batch stride 0: its map (tmR) has no batch dimension
 };
 
 static constexpr int kSmemTotal = 227 * 1024;
 static constexpr int kMaxStages = 8;
 static constexpr int kGemmThreads = 384;  // producer warpgroup + two consumer warpgroups
+static constexpr int kPanelBytes = 128 * 128;  // staged output: 128 rows x 128 bytes (64 bf16 / 32 fp32 columns), 128B swizzle
 
 template <int MT, int BN>
 struct WgLayout {
@@ -114,15 +119,23 @@ __device__ __forceinline__ void rope_store(const GemmParams& p, float x1a, float
   *reinterpret_cast<__nv_bfloat162*>(crow + d + 64) = __floats2bfloat162_rn(o2a, o2b);
 }
 
-template <int MT, int BN>
+// STAGED: the staged epilogue (the output tile goes through shared memory and leaves by TMA store, the residual is loaded by TMA
+// ahead of the epilogue) and no other; its own instantiation, so the register-epilogue kernels keep their register budget.
+// tmC / tmR: its output and residual maps, 3-D (n, row, batch) with 128-row x 128-byte boxes.
+template <int MT, int BN, bool STAGED>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const GemmParams p) {
+gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmC,
+               const __grid_constant__ CUtensorMap tmR, const GemmParams p) {
   using L = WgLayout<MT, BN>;
+  static_assert(!STAGED || (MT == 1 && BN <= 128), "the staged epilogue is built for 128 x 64 and 128 x 128 tiles");
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);  // 128B-swizzle atoms need 1 KB alignment
-  uint64_t* full_bar = (uint64_t*)(smem + p.stages * L::kStageBytes);
+  uint8_t* stage_c = smem + p.stages * L::kStageBytes;                             // staged output tile (1 KB aligned)
+  uint64_t* full_bar = (uint64_t*)(stage_c + p.staged_bytes);
   uint64_t* empty_bar = full_bar + kMaxStages;
+  uint64_t* res_full = empty_bar + kMaxStages;  // staged: the tile's residual box has landed in stage_c
+  uint64_t* stage_free = res_full + 1;          // staged: the previous tile's TMA store has finished reading stage_c
 
   const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   const int tiles_m_total = p.m_tiles * (int)p.a_batch;
@@ -133,10 +146,12 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   // split's k range, so every member runs the same k-blocks in the same ring order.  It loads its 1/cn share of the A box and
   // multicasts it along its row (same m-tile), and its 1/cm share of the W box to its column (same n-tile).  1 x 1 is the plain
   // persistent walk: unit u = blockIdx.x + i * gridDim.x, tiles consecutive along M.
-  const int csize = p.cm * p.cn;
+  // the staged kernel runs without clusters (tensor-bound calls): a compile-time 1 x 1 keeps its producer within 40 registers
+  const int cm = STAGED ? 1 : p.cm, cn = STAGED ? 1 : p.cn;
+  const int csize = cm * cn;
   const int rank = csize > 1 ? (int)cluster_ctarank() : 0;
-  const int rm = rank / p.cn, rn = rank % p.cn;
-  const int cluster_tiles_m = tiles_m_total / p.cm;
+  const int rm = rank / cn, rn = rank % cn;
+  const int cluster_tiles_m = tiles_m_total / cm;
   const int num_units = p.num_tiles / csize * p.splits;
   const int first_unit = blockIdx.x / csize, unit_step = gridDim.x / csize;
 
@@ -144,6 +159,10 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     for (int s = 0; s < stages; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 8 * csize);  // one arrival per consumer warp of every CTA of the cluster
+    }
+    if (STAGED) {
+      mbar_init(res_full, 1);
+      mbar_init(stage_free, 1);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -162,16 +181,16 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"(&tmW) : "memory");
       // slices are whole 8-row (1 KB) swizzle atoms; each lands at its own offset of the box in every CTA of the mask
-      const int a_slice = MT * 128 / p.cn, w_slice = BN / p.cm;
-      const uint16_t row_mask = (uint16_t)(((1u << p.cn) - 1u) << (rm * p.cn));
+      const int a_slice = MT * 128 / cn, w_slice = BN / cm;
+      const uint16_t row_mask = (uint16_t)(((1u << cn) - 1u) << (rm * cn));
       uint16_t col_mask = 0;
-      for (int j = 0; j < p.cm; ++j) col_mask |= (uint16_t)(1u << (j * p.cn + rn));
+      for (int j = 0; j < cm; ++j) col_mask |= (uint16_t)(1u << (j * cn + rn));
       int s = 0;
       uint32_t ph = 0;
-      for (int unit = first_unit; unit < num_units; unit += unit_step) {
+      for (int unit = first_unit, tile_i = 0; unit < num_units; unit += unit_step, ++tile_i) {
         const int ctile = unit / p.splits, split = unit % p.splits;
-        const int tm_idx = (ctile % cluster_tiles_m) * p.cm + rm;  // consecutive tiles share the W tile
-        const int tn_idx = (ctile / cluster_tiles_m) * p.cn + rn;
+        const int tm_idx = (ctile % cluster_tiles_m) * cm + rm;  // consecutive tiles share the W tile
+        const int tn_idx = (ctile / cluster_tiles_m) * cn + rn;
         const int b = tm_idx / p.m_tiles;
         const int m0 = (tm_idx % p.m_tiles) * (MT * 128);
         const int kb_begin = split * p.kb_per_split;
@@ -179,20 +198,31 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         // W box of k-block kb: canonical [N, K] weights -> (kb * 64, n0); pre-tiled image [tile][kb][BN][64] viewed as
         // [rows, 64] -> (0, (tn_idx * num_kb + kb) * BN): one contiguous BN * 128-byte run of DRAM
         const int wt_base = tn_idx * num_kb * BN;
+        // staged epilogue with a residual: the tile's residual box is loaded into the staging tile ahead of the epilogue, after
+        // the k-block `stages` before the last one.  Not earlier, since waiting for the previous tile's store to leave the staging
+        // tile (the consumers signal it once this tile's first MMAs are issued) must not hold up the ring; and never before the
+        // tile's first k-block is loaded, which those MMAs need.
+        const int r_kb = max(kb_begin, kb_end - stages);
         for (int kb = kb_begin; kb < kb_end; ++kb) {
           mbar_wait(&empty_bar[s], ph ^ 1u);
           uint8_t* sa = smem + s * L::kStageBytes;
           // the whole stage lands in every CTA (own slices and the peers'); TMA zero fill counts toward the bytes
           mbar_expect_tx(&full_bar[s], (uint32_t)L::kStageBytes);
           uint8_t* da = sa + rn * a_slice * (kBK * 2);
-          if (p.cn > 1) tma_load_3d_mc(da, &tmA, kb * kBK, m0 + rn * a_slice, b, &full_bar[s], row_mask);
+          if (cn > 1) tma_load_3d_mc(da, &tmA, kb * kBK, m0 + rn * a_slice, b, &full_bar[s], row_mask);
           else tma_load_3d(da, &tmA, kb * kBK, m0, b, &full_bar[s]);
           uint8_t* dw = sa + L::kABytes + rm * w_slice * (kBK * 2);
           const int w0 = p.w_tiled ? 0 : kb * kBK;
           const int w1 = (p.w_tiled ? wt_base + kb * BN : tn_idx * BN) + rm * w_slice;
-          if (p.cm > 1) tma_load_2d_mc(dw, &tmW, w0, w1, &full_bar[s], col_mask);
+          if (cm > 1) tma_load_2d_mc(dw, &tmW, w0, w1, &full_bar[s], col_mask);
           else tma_load_2d(dw, &tmW, w0, w1, &full_bar[s]);
           if (++s == stages) { s = 0; ph ^= 1u; }
+          if (STAGED && p.R && kb == r_kb) {
+            mbar_wait(stage_free, (uint32_t)(tile_i & 1) ^ 1u);
+            const int n0 = tn_idx * BN, panels = (int)min((int64_t)BN, p.N - n0) / 64;
+            mbar_expect_tx(res_full, (uint32_t)(panels * kPanelBytes));
+            for (int q = 0; q < panels; ++q) tma_load_3d(stage_c + q * kPanelBytes, &tmR, n0 + 64 * q, m0, p.r_bcast ? 0 : b, res_full);
+          }
         }
       }
     }
@@ -215,12 +245,14 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       mbar_arrive_cluster(&empty_bar[slot], (uint32_t)lane);
     }
   };
+  // staged epilogue: consumer thread 0 issues the tile's TMA stores and tracks their completion
+  auto store_thread = [&]() { return STAGED && threadIdx.x == 128; };
   int s = 0;
   uint32_t ph = 0;
   for (int unit = first_unit; unit < num_units; unit += unit_step) {
     const int ctile = unit / p.splits, split = unit % p.splits;
-    const int tm_idx = (ctile % cluster_tiles_m) * p.cm + rm;
-    const int tn_idx = (ctile / cluster_tiles_m) * p.cn + rn;
+    const int tm_idx = (ctile % cluster_tiles_m) * cm + rm;
+    const int tn_idx = (ctile / cluster_tiles_m) * cn + rn;
     const int b = tm_idx / p.m_tiles;
     const int m0 = (tm_idx % p.m_tiles) * (MT * 128);
     const int n0 = tn_idx * BN;
@@ -242,6 +274,12 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           Wgmma<BN>::mma(acc[mt], da + (uint64_t)(2 * k), dw + (uint64_t)(2 * k), (kb > kb_begin || k > 0) ? 1u : 0u);
       }
       wgmma_commit();
+      // staged epilogue: with this tile's first MMAs in flight, wait for the previous tile's store to finish reading the staging
+      // tile and hand it on (to the producer's residual load, or to this tile's epilogue)
+      if (store_thread() && kb == kb_begin && unit != first_unit) {
+        bulk_wait_read0();
+        mbar_arrive(stage_free);
+      }
       // one k-block of MMAs stays in flight; the slot read by the previous one is handed back to the producer
       wgmma_wait<1>();
       if (prev >= 0) release(prev);
@@ -254,6 +292,71 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     // ---- epilogue from registers: this thread holds rows r0 (+8) of each 64-row sub-tile, columns 8j + 2(lane % 4) (+1)
     const int rq = warp * 16 + (lane >> 2);
     const int cq = 2 * (lane & 3);
+    if constexpr (STAGED) {
+      {
+        // ---- staged epilogue (plain epilogue, one split, no row map): the same arithmetic in the same order as below, written
+        // into the staging tile and stored by TMA, so the consumers go straight on to the next tile's MMAs.  The tile is
+        // 128-byte panels (64 bf16 / 32 fp32 columns x 128 rows, 128B swizzle: 16-byte chunk q of row r sits at chunk q ^ (r % 8)).
+        // A warp's bf16 write of one (h, j) covers 8 rows r (r % 8 = lane / 4) x 16 bytes of chunk j % 8: the swizzle puts
+        // the 8 rows in 8 different chunks, so the 32 lanes hit 32 different banks.  An fp32 write (8 bytes per lane) covers
+        // chunks 2(j % 4) and 2(j % 4) + 1, which rows r and r ^ 1 share: a 2-way conflict, accepted for the rare fp32 output.
+        // The residual (bf16 output only) was loaded into the tile by the producer, in the output's layout: each element is
+        // read at the position its result is written to.
+        const uint32_t tile_par = (uint32_t)((unit - first_unit) / unit_step) & 1u;  // parity of the tile's ordinal in this CTA
+        if (p.R) mbar_wait(res_full, tile_par);
+        else mbar_wait(stage_free, tile_par ^ 1u);
+        __nv_bfloat162 bias_v[BN / 8];
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int64_t n = n0 + 8 * j + cq;
+          if (p.bias && n < p.N) bias_v[j] = *reinterpret_cast<const __nv_bfloat162*>(p.bias + n);
+        }
+        const uint32_t st0 = smem_u32(stage_c);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = c * 64 + rq + 8 * h;  // tile row; rows past a_rows are clipped by the TMA store
+          const uint32_t row = st0 + (uint32_t)r * 128u, sw = (uint32_t)(r & 7);
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            float v0 = acc[0][4 * j + 2 * h] * p.alpha, v1 = acc[0][4 * j + 2 * h + 1] * p.alpha;
+            if (p.bias) {
+              const float2 t = __bfloat1622float2(bias_v[j]);
+              v0 += t.x;
+              v1 += t.y;
+            }
+            if (p.act == UVX_ACT_GELU) {
+              v0 = gelu_fast(v0);
+              v1 = gelu_fast(v1);
+            }
+            if (p.out_f32) {
+              const uint32_t chunk = (uint32_t)(2 * (j % 4) + (lane & 3) / 2);
+              st_shared_f32x2(row + (j / 4) * kPanelBytes + ((chunk ^ sw) << 4) + (lane & 1) * 8, v0, v1);
+            } else {
+              const uint32_t addr = row + (j / 8) * kPanelBytes + (((uint32_t)(j % 8) ^ sw) << 4) + (lane & 3) * 4;
+              if (p.R) {
+                const uint32_t rv = ld_shared_u32(addr);
+                const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&rv));
+                v0 += t.x;
+                v1 += t.y;
+              }
+              const __nv_bfloat162 o = __floats2bfloat162_rn(v0, v1);
+              st_shared_u32(addr, *reinterpret_cast<const uint32_t*>(&o));
+            }
+          }
+        }
+        // every writer makes its shared-memory writes visible to the async proxy; then one thread stores the panels that lie
+        // inside N (TMA clips the M tail and the last panel's columns past N)
+        fence_proxy_async();
+        named_bar_sync<1, 256>();
+        if (store_thread()) {
+          const int cols = p.out_f32 ? 32 : 64;
+          const int panels = (int)min((int64_t)BN, p.N - n0) / cols;
+          for (int q = 0; q < panels; ++q) tma_store_3d(&tmC, stage_c + q * kPanelBytes, n0 + cols * q, m0, b);
+          bulk_commit();
+        }
+        continue;
+      }
+    }
     if (p.splits > 1) {
       // split-K: park the raw fp32 partial tile in the workspace; splitk_reduce_kernel sums the splits in a fixed order and
       // applies the epilogue (deterministic, and the reduction is spread over every SM)
@@ -384,6 +487,8 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
     }
   }
+  // the stores are complete in global memory before the CTA exits (the next kernel's griddepcontrol.wait must see them)
+  if (store_thread()) bulk_wait0();
   if (csize > 1) cluster_sync();
 }
 
@@ -682,7 +787,8 @@ static EncodeTiledFn get_encode() {
 }
 
 static int encode_map(CUtensorMap* tm, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                      const uint32_t* box, CUtensorMapL2promotion promo) {
+                      const uint32_t* box, CUtensorMapL2promotion promo,
+                      CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16) {
   EncodeTiledFn enc = get_encode();
   if (!enc) {
     set_error("cuTensorMapEncodeTiled entry point not available");
@@ -697,7 +803,7 @@ static int encode_map(CUtensorMap* tm, const void* base, int rank, const uint64_
     es[i] = 1;
   }
   for (int i = 0; i < rank - 1; ++i) gs[i] = strides_bytes[i];
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gd, gs, bx, es,
+  CUresult r = enc(tm, dtype, (cuuint32_t)rank, const_cast<void*>(base), gd, gs, bx, es,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled failed with CUresult %d (rank %d dims %llu %llu stride %llu)", (int)r, rank,
@@ -720,6 +826,7 @@ static int num_sms() {
 
 static int g_gemm_stage_cap = 0;  // tuning only (uvx_debug_gemm_stages): upper bound on the ring depth
 static int g_grid_cap = 0;        // tuning only (uvx_debug_gemm_ws grid): upper bound on the persistent grid
+static int g_tma_store = -1;      // uvx_debug_gemm_tma_store: 0 = register epilogue everywhere, otherwise staged where it applies
 
 // after the main kernel: split-K reduce (fused RMSNorm where it applies) or the row norm of a direct epilogue
 static int finish_gemm(const uvx_gemm_args* a, const GemmParams& p, cudaStream_t stream) {
@@ -748,6 +855,12 @@ static void legal_cluster(int mt, int bn, int tiles_m_total, int n_tiles, int* c
   if (*cm < 1 || *cm > 4 || tiles_m_total % *cm != 0 || bn % (8 * *cm) != 0) *cm = 1;
   if (*cn < 1 || *cn > 4 || n_tiles % *cn != 0 || (mt * 128) % (8 * *cn) != 0) *cn = 1;
   if (*cm * *cn > 8) *cm = *cn = 1;
+}
+
+template <int MT, int BN, bool STAGED>
+static cudaError_t set_smem_attr() {
+  if constexpr (STAGED && !(MT == 1 && BN <= 128)) return cudaErrorInvalidValue;
+  else return cudaFuncSetAttribute(gemm_wg_kernel<MT, BN, STAGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal);
 }
 
 template <int MT, int BN>
@@ -828,17 +941,47 @@ static int launch_gemm(const uvx_gemm_args* a, int splits, int cm, int cn, cudaS
   p.kb_per_split = (num_kb + splits - 1) / splits;
   p.splits = (num_kb + p.kb_per_split - 1) / p.kb_per_split;  // no empty split
   p.ws_partial = (float*)a->workspace;
-  p.stages = L::kStages;
+  // Staged epilogue (output tile through shared memory, TMA store; the residual loaded by TMA ahead of the epilogue): the
+  // tensor-bound calls (more than 256 rows, or a batch) with the plain epilogue on 128 x 64 / 128 x 128 tiles.  Same bits as
+  // the register epilogue.  The tile's shared memory comes out of the ring (128 x 128 bf16: 7 -> 6 stages, fp32: 5).
+  CUtensorMap tmC, tmR;
+  memset(&tmC, 0, sizeof(tmC));
+  memset(&tmR, 0, sizeof(tmR));
+  const bool staged = MT == 1 && BN <= 128 && g_tma_store != 0 && (a->a_rows > 256 || a->a_batch > 1) && p.splits == 1 &&
+                      cm * cn == 1 && !a->c_row_map && !p.swiglu && !p.rope_cos && !p.w_perm && !(a->norm_w && a->norm_out) &&
+                      (!a->R || (!p.out_f32 && a->r_row_stride > 0 && (uintptr_t)a->R % 16 == 0));
+  if (staged) {
+    const uint64_t es = p.out_f32 ? 4 : 2;
+    const uint64_t row_bytes = (uint64_t)a->c_row_stride * es;
+    uint64_t dims[3] = {(uint64_t)a->N, (uint64_t)a->a_rows, (uint64_t)a->a_batch};
+    uint64_t st[2] = {row_bytes, a->a_batch > 1 ? (uint64_t)a->c_batch_rows * row_bytes : row_bytes};
+    uint32_t box[3] = {(uint32_t)(128 / es), 128, 1};
+    int rc = encode_map(&tmC, (const char*)a->C + a->c_row_offset * (int64_t)row_bytes, 3, dims, st, box,
+                        CU_TENSOR_MAP_L2_PROMOTION_NONE, p.out_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
+    if (rc) return rc;
+    if (a->R) {
+      // a residual shared by every batch (the conv stem's positional embedding) gets a map without the batch dimension
+      p.r_bcast = a->a_batch == 1 || a->r_batch_stride == 0;
+      uint64_t rdims[3] = {(uint64_t)a->N, (uint64_t)a->a_rows, p.r_bcast ? 1 : (uint64_t)a->a_batch};
+      uint64_t rst[2] = {(uint64_t)a->r_row_stride * 2, (uint64_t)(p.r_bcast ? a->r_row_stride : a->r_batch_stride) * 2};
+      uint32_t rbox[3] = {64, 128, 1};
+      rc = encode_map(&tmR, a->R, 3, rdims, rst, rbox, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+      if (rc) return rc;
+    }
+    p.staged_bytes = BN / 64 * (p.out_f32 ? 2 : 1) * kPanelBytes;
+  }
+  p.stages = (L::kRingMax - p.staged_bytes) / L::kStageBytes;
+  if (p.stages > L::kStages) p.stages = L::kStages;
   if (g_gemm_stage_cap >= 2 && p.stages > g_gemm_stage_cap) p.stages = g_gemm_stage_cap;
-  const int smem = p.stages * L::kStageBytes + 1024 + 2 * kMaxStages * 8;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_wg_kernel<MT, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal);
+  const int smem = p.stages * L::kStageBytes + p.staged_bytes + 1024 + 2 * kMaxStages * 8 + 16;
+  static bool attr_set[2] = {false, false};
+  if (!attr_set[staged]) {
+    cudaError_t e = staged ? set_smem_attr<MT, BN, true>() : set_smem_attr<MT, BN, false>();
     if (e != cudaSuccess) {
-      set_error("cudaFuncSetAttribute(gemm_wg_kernel<%d,%d>, smem %d): %s", MT, BN, kSmemTotal, cudaGetErrorString(e));
+      set_error("cudaFuncSetAttribute(gemm_wg_kernel<%d,%d,%d>, smem %d): %s", MT, BN, (int)staged, kSmemTotal, cudaGetErrorString(e));
       return UVX_ERR_CUDA;
     }
-    attr_set = true;
+    attr_set[staged] = true;
   }
   // persistent grid: a whole number of clusters, no more than fit on the GPU at once (clusters stay inside one GPC, so with
   // 4-CTA clusters a few SMs stay idle)
@@ -859,7 +1002,7 @@ static int launch_gemm(const uvx_gemm_args* a, int splits, int cm, int cn, cudaS
       attr.val.clusterDim.z = 1;
       cfg.attrs = &attr;
       cfg.numAttrs = 1;
-      cudaError_t e = cudaOccupancyMaxActiveClusters(&max_clusters[csize], gemm_wg_kernel<MT, BN>, &cfg);
+      cudaError_t e = cudaOccupancyMaxActiveClusters(&max_clusters[csize], gemm_wg_kernel<MT, BN, false>, &cfg);
       if (e != cudaSuccess || max_clusters[csize] < 1) {
         set_error("cudaOccupancyMaxActiveClusters(gemm_wg_kernel<%d,%d>, %d CTAs): %s", MT, BN, csize,
                   e != cudaSuccess ? cudaGetErrorString(e) : "no cluster fits");
@@ -873,9 +1016,11 @@ static int launch_gemm(const uvx_gemm_args* a, int splits, int cm, int cn, cudaS
   if (g_grid_cap > 0 && clusters * csize > g_grid_cap) clusters = g_grid_cap / csize > 1 ? g_grid_cap / csize : 1;
   const dim3 grid((unsigned)(clusters * csize));
   if (csize > 1)
-    launch_k_cluster(gemm_wg_kernel<MT, BN>, grid, dim3(kGemmThreads), (size_t)smem, stream, (unsigned)csize, tmA, tmW, p);
+    launch_k_cluster(gemm_wg_kernel<MT, BN, false>, grid, dim3(kGemmThreads), (size_t)smem, stream, (unsigned)csize, tmA, tmW, tmC, tmR, p);
+  else if (staged)
+    launch_k(gemm_wg_kernel<MT, BN, (MT == 1 && BN <= 128)>, grid, dim3(kGemmThreads), (size_t)smem, stream, tmA, tmW, tmC, tmR, p);
   else
-    launch_k(gemm_wg_kernel<MT, BN>, grid, dim3(kGemmThreads), (size_t)smem, stream, tmA, tmW, p);
+    launch_k(gemm_wg_kernel<MT, BN, false>, grid, dim3(kGemmThreads), (size_t)smem, stream, tmA, tmW, tmC, tmR, p);
   int rc = check_launch("gemm_wg_kernel");
   if (rc) return rc;
   return finish_gemm(a, p, stream);
@@ -1044,10 +1189,16 @@ extern "C" int uvx_debug_gemm_cluster(int cm, int cn) {
   return UVX_OK;
 }
 
-// Hooks of tuning knobs this kernel does not have (TMA-store epilogue, L2 prefetch distance, phase timestamps, pipeline isolation):
-// accepted for ABI compatibility, no effect.
+// tuning hook: the staged (shared memory + TMA store) epilogue of the tensor-bound calls: 0 = register epilogue everywhere,
+// -1 (default) or > 0 = staged wherever it applies.  Never changes the result bits.
+extern "C" int uvx_debug_gemm_tma_store(int on) {
+  uvx::g_tma_store = on;
+  return UVX_OK;
+}
+
+// Hooks of tuning knobs this kernel does not have (L2 prefetch distance, phase timestamps, pipeline isolation): accepted for ABI
+// compatibility, no effect.
 extern "C" int uvx_debug_gemm_mode(int mode) { (void)mode; return UVX_OK; }
-extern "C" int uvx_debug_gemm_tma_store(int on) { (void)on; return UVX_OK; }
 extern "C" int uvx_debug_gemm_times(void* dev_buf) { (void)dev_buf; return UVX_OK; }
 extern "C" int uvx_debug_gemm_pf(int pf) { (void)pf; return UVX_OK; }
 extern "C" int uvx_debug_gemm_ws_times(void* dev_buf) { (void)dev_buf; return UVX_OK; }

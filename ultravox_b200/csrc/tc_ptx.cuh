@@ -46,6 +46,36 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* tm, in
       : "memory");
 }
 
+// ---- TMA stores (gemm_tc.cu: the staged epilogue).  The box at `src` is read by the async proxy: a thread's generic-proxy writes
+// to it need fence_proxy_async() before the store is issued.  Completion is tracked per issuing thread in bulk async-groups.
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* tm, const void* src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(tm), "r"(smem_u32(src)),
+               "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// this thread's committed stores have finished reading shared memory (the box may be overwritten)
+__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// ... and their writes to global memory are complete
+__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// named barrier `id` over `n` threads (a multiple of 32); id 0 is __syncthreads
+template <int ID, int N>
+__device__ __forceinline__ void named_bar_sync() {
+  asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(N) : "memory");
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void st_shared_f32x2(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
+
 // ---- thread-block clusters (gemm_tc.cu: TMA multicast of the shared operand boxes)
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
