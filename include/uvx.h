@@ -178,7 +178,11 @@ int uvx_rmsnorm(const void* x, const void* w, void* y, int64_t rows, int64_t col
  *   Whisper encoder self-attention (hf:modeling_whisper.py:215-238,305-349): non-causal, keys >= kv_len[b]
  *   masked (ref:ultravox_model.py:915-926), optional block-causal streaming mask (ref :834-863,928-936);
  *   Llama attention (hf:modeling_llama.py:199-289): causal, grouped-query.
- * q[b, i, h, :] = q + b*q_bs + i*q_rs + h*D  (same for k, v with h / (Hq/Hkv), and o).                  */
+ * q[b, i, h, :] = q + b*q_bs + i*q_rs + h*D  (same for k, v with h / (Hq/Hkv), and o).
+ * Visible keys of sequence b: [clamp(kv_start[b], 0, end), end) with end = clamp(kv_len[b], 0, Skv), further cut by the causal
+ * and block rules.  Key / value rows outside that range (left padding, rows from kv_len on, a cache's rows from Skv on) may
+ * hold anything, NaN and Inf included: they change no output bit.  A query that sees no key (inside the left padding of a
+ * causal call, or kv_len[b] <= kv_start[b]) writes an output row of exactly 0 and lse = -inf (the log of an empty sum).   */
 typedef struct uvx_attn_args {
   const void *q, *k, *v;
   void* o;
@@ -205,7 +209,9 @@ int uvx_attention_enc_tc(const void* qkv, int64_t row_stride, int64_t B, int64_t
 /* RoPE on the q and k sections of a fused [rows, (Hq + 2*Hkv) * D] projection, in place
  * (hf:modeling_llama.py:124-168; cos/sin tables [max_pos, D/2] fp32 built by the host exactly like
  * LlamaRotaryEmbedding incl. llama3 scaling, hf:modeling_rope_utils.py:550-626).
- * position of row r = positions ? positions[r] : pos_offset + (r % rows_per_seq).                      */
+ * position of row r = positions ? positions[r] : pos_offset + (r % rows_per_seq); with positions, rows_per_seq and
+ * pos_offset are not read.  Every row is rotated, pad rows too: the caller gives them a position inside the tables
+ * (generate() gives position 0, where cos = 1 and sin = 0, so a pad row keeps its bits).  The v section is not touched. */
 int uvx_rope(void* qkv, int64_t rows, int64_t row_stride, int Hq, int Hkv, int D, const float* cos_tab,
              const float* sin_tab, const int32_t* positions, int64_t rows_per_seq, int64_t pos_offset,
              uvx_stream_t stream);

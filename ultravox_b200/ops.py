@@ -300,7 +300,8 @@ def attention_fused_qkv(qkv: torch.Tensor, B: int, S: int, Hq: int, Hkv: int, D:
 
 def attention_encoder_tc(qkv: torch.Tensor, B: int, S: int, H: int, scale: float, kv_len: Optional[torch.Tensor] = None,
                          block: int = 0, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """Encoder attention (mma.sync flash kernel) over a fused [B*S, 3*H*64] q|k|v projection (head_dim 64), no q / k / v copies."""
+    """Encoder attention over a fused [B*S, 3*H*64] q|k|v projection (head_dim 64), no q / k / v copies: the TMA + wgmma flash
+    kernel from 16 queries on, the mma.sync kernel below that (``uvx_attention``'s dispatch)."""
     _cuda(qkv, BF16, "qkv")
     d = H * 64
     assert qkv.shape[-1] == 3 * d and qkv.stride(-1) == 1
