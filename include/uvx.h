@@ -205,6 +205,16 @@ int uvx_debug_attn_tc(int on);
 int uvx_attention_enc_tc(const void* qkv, int64_t row_stride, int64_t B, int64_t S, int64_t H, int64_t q_col, int64_t k_col,
                          int64_t v_col, void* o, int64_t o_rs, const int32_t* kv_len, int32_t block, float scale,
                          uvx_stream_t stream);
+/* Device-indexed causal attention of a prompt chunk against a slot KV cache (chunked prefill inside the captured decode step of
+ * continuous batching, ultravox_b200/engine.py).  The q side is a->B sequences of a->Sq queries as in uvx_attention; k / v
+ * cover the whole cache [kv_batch, Skv = S_max, Hkv, D] (batch strides k_bs / v_bs), so the tensor maps never change between
+ * graph replays.  Query batch b reads cache row kv_row[b] and has past[b] keys before its first query: query i sees keys
+ * j <= i + past[b], j < kv_len[b] (a->kv_len required, normally past + valid queries).  Same kernel, tile schedule, masks
+ * and arithmetic as the wgmma path of uvx_attention (bit-identical to it on a cache row with Skv = past + Sq, Sq >= 16);
+ * cache rows other than kv_row[b] and keys from kv_len[b] on may hold anything, NaN included.  Requires causal = 1,
+ * block = 0, kv_start = NULL, lse = NULL; kv_row / past / kv_len are read on the device, so they may change between replays. */
+int uvx_attention_indexed(const uvx_attn_args* a, int64_t kv_batch, const int32_t* kv_row, const int32_t* past,
+                          uvx_stream_t stream);
 
 /* RoPE on the q and k sections of a fused [rows, (Hq + 2*Hkv) * D] projection, in place
  * (hf:modeling_llama.py:124-168; cos/sin tables [max_pos, D/2] fp32 built by the host exactly like
@@ -260,6 +270,12 @@ int uvx_gemv_fused_bf16(const void* x, int64_t B, int64_t x_row_stride, const vo
 int uvx_rope_kv_append(void* qkv, int64_t B, int64_t row_stride, int Hq, int Hkv, int D, const float* cos_tab, const float* sin_tab,
                        const int32_t* rope_positions, void* k_cache, void* v_cache, int64_t cache_batch_stride,
                        const int32_t* positions, uvx_stream_t stream);
+/* uvx_rope_kv_append with a per-row map (the mixed decode + prompt-chunk step): row r is rotated at rope_positions[r] and,
+ * when cache_row[r] >= 0, its k / v go to cache row cache_row[r] at positions[r]; cache_row[r] < 0 writes nothing (q and k are
+ * still rotated in qkv).  Same bits as uvx_rope_kv_append for the rows it writes; shares its kernel body.                    */
+int uvx_rope_kv_append_map(void* qkv, int64_t rows, int64_t row_stride, int Hq, int Hkv, int D, const float* cos_tab,
+                           const float* sin_tab, const int32_t* rope_positions, void* k_cache, void* v_cache,
+                           int64_t cache_batch_stride, const int32_t* cache_row, const int32_t* positions, uvx_stream_t stream);
 /* a[i] += delta (and b[i] += delta when b != NULL): advances the device-side positions / lengths after each step     */
 int uvx_add_i32(int32_t* a, int32_t* b, int64_t n, int32_t delta, uvx_stream_t stream);
 /* prefill counterpart of uvx_kv_append: rows b*S + s of the fused projection -> cache[b, past + s] (k and v sections),

@@ -12,6 +12,14 @@ Arms, alternated over `--rounds` rounds in one process after a warm-up of each:
 Per arm: wall time (host clock, synchronised), useful tokens per second (the sum of the budgets over the wall time), decode
 milliseconds per step (CUDA events around every decode step), time to first token p50 / p90 over the 64 requests (CUDA events
 from t = 0 to the request's first picked token) and the share of decode row-steps (rows x steps) that decode padding or idle slots.
+The slots arm also reports the inter-token gaps of every request (p50 / p99 over all gaps, the largest gap of each request at
+p50 and its maximum; from the same per-step events) and, apart, the mean time of plain steps and of mixed steps (steps that
+carry a chunk of a long prompt, see below).
+
+`--workload long`: the same 64 budgets, but each clip lasts 40-90 s, cut into 30 s encoder chunks as the processor does
+(`processing.frame_chunks`), so prompts hold 264-577 rows.  Every such prompt is over the 256 rows up to which a prompt is
+prefilled whole at admission, so the slot engine prefills it in chunks inside its decode steps; the default workload (at most
+201 rows) never does.  `--arms slots` skips the static arm.
 
 Prints the device name and power limit first, then one JSON line per arm."""
 import argparse, json, os, statistics, sys, time
@@ -25,21 +33,26 @@ from ultravox_b200 import ops
 SR, PRE, POST = 16000, 8, 5
 
 
-def make_requests(cfg, n, seed):
+def make_requests(cfg, n, seed, workload="default"):
+    from ultravox_b200.processing import frame_chunks
     rng = np.random.default_rng(seed)
-    secs = rng.choice([5, 10, 20, 30], size=n)
+    secs = rng.choice([5, 10, 20, 30] if workload == "default" else [40, 50, 60, 70, 80, 90], size=n)
     budgets = rng.integers(16, 257, size=n)
     g = torch.Generator().manual_seed(seed)
     reqs = []
     for i in range(n):
         wave = torch.from_numpy(rng.standard_normal(int(secs[i]) * SR).astype(np.float32)).cuda()
         mel = ops.logmel(wave[None], cfg.audio_config.num_mel_bins)
-        frames = mel.shape[-1]
-        tok = -(-frames // 16)
-        ids = torch.randint(0, 128000, (1, PRE + tok + POST), generator=g)
-        reqs.append(dict(feats=dict(input_ids=ids.cuda(), audio_values=mel, audio_token_start_idx=torch.tensor([PRE]).cuda(),
-                                    audio_lens=torch.tensor([frames]).cuda(), audio_token_len=torch.tensor([tok], dtype=torch.int32).cuda(),
-                                    audio_batch_size=torch.ones(1, dtype=torch.int64).cuda()),
+        plan, _ = frame_chunks([mel.shape[-1]], 3000)          # one chunk per 30 s, continuations zero-padded to 3000 frames
+        pieces = [torch.nn.functional.pad(mel[0, :, off:off + 3000], (0, 3000 - min(3000, mel.shape[-1] - off)) if cont else (0, 0))
+                  for _, off, _, cont in plan]
+        frames = [p[2] for p in plan]
+        tok = [-(-f // 16) for f in frames]
+        starts = [PRE + sum(tok[:k]) for k in range(len(tok))]
+        ids = torch.randint(0, 128000, (1, PRE + sum(tok) + POST), generator=g)
+        reqs.append(dict(feats=dict(input_ids=ids.cuda(), audio_values=torch.stack(pieces), audio_token_start_idx=torch.tensor(starts).cuda(),
+                                    audio_lens=torch.tensor(frames).cuda(), audio_token_len=torch.tensor(tok, dtype=torch.int32).cuda(),
+                                    audio_batch_size=torch.tensor([len(plan)]).cuda()),
                          budget=int(budgets[i])))
     return reqs
 
@@ -101,17 +114,31 @@ def run_static(model, reqs, batch=8):
     return wall, first, step, row_steps
 
 
+class _FirstTokens(dict):
+    """``SlotScheduler.first_token`` that also notes the scheduler's step count when each request's first token is picked."""
+
+    def __init__(self, sched):
+        super().__init__()
+        self.sched, self.at = sched, {}
+
+    def __setitem__(self, rid, ev):
+        self.at[rid] = self.sched.steps
+        super().__setitem__(rid, ev)
+
+
 def run_slots(sched, reqs):
     eng = sched.engine
     marks = []
     plain = eng.step
+    sched.first_token = _FirstTokens(sched)
 
     def timed():
+        mixed = getattr(eng, "prefilling", None) is not None
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
         plain()
         b.record()
-        marks.append((a, b))
+        marks.append((a, b, mixed))
 
     eng.step = timed
     t0 = torch.cuda.Event(enable_timing=True)
@@ -125,8 +152,16 @@ def run_slots(sched, reqs):
     wall = time.perf_counter() - w0
     eng.step = plain
     first = [t0.elapsed_time(sched.first_token[i]) for i in ids]
-    step = [a.elapsed_time(b) for a, b in marks]
-    return wall, first, step, (sched.steps - steps0) * eng.slots
+    step = [a.elapsed_time(b) for a, b, _ in marks]
+    ends = [t0.elapsed_time(b) for _, b, _ in marks]
+    # a request whose first token came at step count k gets its next tokens from steps k + 1, k + 2, ... (no EOS ids)
+    gaps = []
+    for i, r, f in zip(ids, reqs, first):
+        k = sched.first_token.at[i] - steps0
+        times = [f] + ends[k:k + r["budget"] - 1]
+        gaps.append([b - a for a, b in zip(times, times[1:])])
+    split = {m: [t for t, (_, _, x) in zip(step, marks) if x == m] for m in (False, True)}
+    return wall, first, step, (sched.steps - steps0) * eng.slots, gaps, split
 
 
 def pct(xs, q):
@@ -138,7 +173,10 @@ def main():
     ap.add_argument("--requests", type=int, default=64)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--workload", choices=["default", "long"], default="default")
+    ap.add_argument("--arms", default="static,slots")
     args = ap.parse_args()
+    arms = args.arms.split(",")
     print(json.dumps({"device": device_info()}), flush=True)
     from ultravox_b200.config import preset
     from ultravox_b200.model import UltravoxModel
@@ -146,7 +184,7 @@ def main():
     torch.set_grad_enabled(False)
     cfg = preset("v0_5_8b")
     model = UltravoxModel(cfg, device="cuda").init_random_(seed=42)
-    reqs = make_requests(cfg, args.requests, args.seed)
+    reqs = make_requests(cfg, args.requests, args.seed, args.workload)
     useful = sum(r["budget"] for r in reqs)
     useful_steps = useful - len(reqs)                         # tokens picked by decode steps (the first comes from the prefill)
     max_len = max(r["feats"]["input_ids"].shape[1] for r in reqs) + 256
@@ -155,22 +193,30 @@ def main():
     torch.cuda.synchronize()
     build_s = time.perf_counter() - c0
     warm = [dict(r, budget=16) for r in reqs[:8]]
-    run_static(model, warm)
+    if "static" in arms:
+        run_static(model, warm)
     run_slots(sched, warm)
-    out = {"static": [], "slots": []}
+    out = {a: [] for a in ("static", "slots") if a in arms}
     for _ in range(args.rounds):
-        out["static"].append(run_static(model, reqs))
+        if "static" in arms:
+            out["static"].append(run_static(model, reqs))
         out["slots"].append(run_slots(sched, reqs))
+    clips = "5-30 s" if args.workload == "default" else "40-90 s"
     for arm, runs in out.items():
         walls = [r[0] for r in runs]
         k = walls.index(sorted(walls)[len(walls) // 2])
-        wall, first, step, row_steps = runs[k]
-        line = {"bench": "serve 64 requests, 8B + large-v3, clips 5-30 s, budgets 16-256, greedy", "arm": arm,
+        wall, first, step, row_steps = runs[k][:4]
+        line = {"bench": f"serve {len(reqs)} requests, 8B + large-v3, clips {clips}, budgets 16-256, greedy", "arm": arm,
                 "wall_s_median": wall, "wall_s_all": [round(w, 3) for w in walls], "useful_tokens": useful,
                 "tokens_per_s": useful / wall, "decode_ms_per_step_mean": statistics.fmean(step), "decode_steps": len(step),
                 "ttft_ms_p50": pct(first, 50), "ttft_ms_p90": pct(first, 90), "row_steps": row_steps,
                 "wasted_row_step_share": 1.0 - useful_steps / row_steps}
         if arm == "slots":
+            gaps, split = runs[k][4:]
+            flat, worst = [g for gs in gaps for g in gs], [max(gs) for gs in gaps if gs]
+            line.update(gap_ms_p50=pct(flat, 50), gap_ms_p99=pct(flat, 99), max_gap_ms_p50=pct(worst, 50), max_gap_ms_max=max(worst),
+                        plain_step_ms_mean=statistics.fmean(split[False]) if split[False] else None, plain_steps=len(split[False]),
+                        mixed_step_ms_mean=statistics.fmean(split[True]) if split[True] else None, mixed_steps=len(split[True]))
             line["engine_build_s"] = build_s
             line["launches_per_step"] = sched.engine.launches_per_step
         print(json.dumps(line), flush=True)

@@ -70,6 +70,7 @@ SIGNATURES = {
     "uvx_attention": (C.c_int, [C.POINTER(AttnArgs), c_vp]),
     "uvx_debug_attn_tc": (C.c_int, [C.c_int]),
     "uvx_attention_enc_tc": (C.c_int, [c_vp, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_vp, c_i64, c_vp, c_i32, c_f32, c_vp]),
+    "uvx_attention_indexed": (C.c_int, [C.POINTER(AttnArgs), c_i64, c_vp, c_vp, c_vp]),
     "uvx_rope": (C.c_int, [c_vp, c_i64, c_i64, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp]),
     "uvx_swiglu": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_i64, C.c_int, c_vp]),
     "uvx_splice_plan": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp]),
@@ -80,6 +81,8 @@ SIGNATURES = {
     "uvx_gemv_fused_bf16": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_i64, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, C.c_int, c_vp, C.c_float,
                                       C.c_int, c_vp]),
     "uvx_rope_kv_append": (C.c_int, [c_vp, c_i64, c_i64, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp]),
+    "uvx_rope_kv_append_map": (C.c_int, [c_vp, c_i64, c_i64, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp,
+                                         c_vp]),
     "uvx_add_i32": (C.c_int, [c_vp, c_vp, c_i64, c_i32, c_vp]),
     "uvx_kv_write": (C.c_int, [c_vp, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_vp]),
     "uvx_repetition_penalty": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_f32, c_vp, c_vp]),

@@ -22,6 +22,8 @@ struct AttnWgParams {
   int Sq, Skv, group, Hq;
   int causal, block;
   float scale_log2;
+  const int32_t* kv_row;  // device-indexed form: K / V batch coordinate of query batch b
+  const int32_t* past;    // device-indexed form: causal shift (keys already in the cache) of query batch b
 };
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
@@ -43,7 +45,9 @@ struct AttnWgSmem {
   static constexpr int kBytes = kBar + 64 + 1024;     // + barriers + alignment slack
 };
 
-template <int D>
+// kIndexed: the K / V batch coordinate and the causal shift come from device memory (p.kv_row[b], p.past[b]) instead of b and
+// Skv - Sq, so one captured launch serves whichever cache row and prompt offset the host writes between replays.
+template <int D, bool kIndexed = false>
 __global__ void __launch_bounds__(128, 1)
 attn_wg_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                const AttnWgParams p) {
@@ -57,10 +61,11 @@ attn_wg_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
   const int m0 = blockIdx.x * kWQ;
   const int h = blockIdx.y, b = blockIdx.z;
   const int hk = h / p.group;
+  const int kb = kIndexed ? p.kv_row[b] : b;
 
   int kv_end = p.Skv;
   if (p.kv_len) kv_end = min(kv_end, max(p.kv_len[b], 0));
-  const int shift = p.Skv - p.Sq;
+  const int shift = kIndexed ? p.past[b] : p.Skv - p.Sq;
   const int last_q = min(m0 + kWQ, p.Sq) - 1;
   if (p.causal) kv_end = min(kv_end, last_q + shift + 1);
   if (p.block > 0) kv_end = min(kv_end, (last_q / p.block + 1) * p.block);
@@ -81,8 +86,8 @@ attn_wg_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
     mbar_expect_tx(&full[stage], (uint32_t)(2 * P * kPanel));
 #pragma unroll
     for (int pn = 0; pn < P; ++pn) {
-      tma_load_4d(smem + L::kK + (stage * P + pn) * kPanel, &tmK, pn * 64, hk, tile * kWK, b, &full[stage]);
-      tma_load_4d(smem + L::kV + (stage * P + pn) * kPanel, &tmV, pn * 64, hk, tile * kWK, b, &full[stage]);
+      tma_load_4d(smem + L::kK + (stage * P + pn) * kPanel, &tmK, pn * 64, hk, tile * kWK, kb, &full[stage]);
+      tma_load_4d(smem + L::kV + (stage * P + pn) * kPanel, &tmV, pn * 64, hk, tile * kWK, kb, &full[stage]);
     }
   };
   if (tid == 0 && n_tiles > tile0) {
@@ -249,17 +254,17 @@ bool attn_wg_eligible(const uvx_attn_args* a) {
   return true;
 }
 
-template <int D>
-static int launch_wg(const uvx_attn_args* a, cudaStream_t st) {
+template <int D, bool kIndexed>
+static int launch_wg(const uvx_attn_args* a, int64_t kv_batch, const int32_t* kv_row, const int32_t* past, cudaStream_t st) {
   using L = AttnWgSmem<D>;
   CUtensorMap tq, tk, tv;
   int rc = aw_encode(&tq, a->q, D, a->Hq, a->Sq, a->B, a->q_rs, a->q_bs);
-  if (!rc) rc = aw_encode(&tk, a->k, D, a->Hkv, a->Skv, a->B, a->k_rs, a->k_bs);
-  if (!rc) rc = aw_encode(&tv, a->v, D, a->Hkv, a->Skv, a->B, a->v_rs, a->v_bs);
+  if (!rc) rc = aw_encode(&tk, a->k, D, a->Hkv, a->Skv, kv_batch, a->k_rs, a->k_bs);
+  if (!rc) rc = aw_encode(&tv, a->v, D, a->Hkv, a->Skv, kv_batch, a->v_rs, a->v_bs);
   if (rc) return rc;
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(attn_wg_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kBytes);
+    cudaError_t e = cudaFuncSetAttribute(attn_wg_kernel<D, kIndexed>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kBytes);
     if (e != cudaSuccess) {
       set_error("cudaFuncSetAttribute(attn_wg_kernel<%d>): %s", D, cudaGetErrorString(e));
       return UVX_ERR_CUDA;
@@ -280,13 +285,34 @@ static int launch_wg(const uvx_attn_args* a, cudaStream_t st) {
   p.causal = a->causal;
   p.block = a->block;
   p.scale_log2 = a->scale * 1.4426950408889634f;
+  p.kv_row = kv_row;
+  p.past = past;
   dim3 grid((unsigned)((a->Sq + kWQ - 1) / kWQ), (unsigned)a->Hq, (unsigned)a->B);
-  launch_k(attn_wg_kernel<D>, grid, dim3(128), (size_t)L::kBytes, st, tq, tk, tv, p);
+  launch_k(attn_wg_kernel<D, kIndexed>, grid, dim3(128), (size_t)L::kBytes, st, tq, tk, tv, p);
   return check_launch("attn_wg_kernel");
 }
 
 int launch_attn_wg(const uvx_attn_args* a, cudaStream_t st) {
-  return a->D == 64 ? launch_wg<64>(a, st) : launch_wg<128>(a, st);
+  return a->D == 64 ? launch_wg<64, false>(a, a->B, nullptr, nullptr, st) : launch_wg<128, false>(a, a->B, nullptr, nullptr, st);
 }
 
 }  // namespace uvx
+
+extern "C" int uvx_attention_indexed(const uvx_attn_args* a, int64_t kv_batch, const int32_t* kv_row, const int32_t* past,
+                                     uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(a && a->q && a->k && a->v && a->o && kv_row && past && a->kv_len, "uvx_attention_indexed: null pointer");
+  UVX_REQUIRE(a->D == 64 || a->D == 128, "uvx_attention_indexed: head_dim must be 64 or 128 (got %lld)", (long long)a->D);
+  UVX_REQUIRE(a->B >= 1 && a->B < 65536 && a->Hq >= 1 && a->Hq < 65536 && a->Hkv >= 1 && a->Hq % a->Hkv == 0 && a->Sq >= 1 &&
+                  a->Skv >= 1 && kv_batch >= 1,
+              "uvx_attention_indexed: bad shape");
+  UVX_REQUIRE(a->causal == 1 && a->block == 0 && !a->kv_start && !a->lse,
+              "uvx_attention_indexed: causal, no block mask, no kv_start, no lse");
+  UVX_REQUIRE(a->q_rs % 8 == 0 && a->k_rs % 8 == 0 && a->v_rs % 8 == 0 && a->q_bs % 8 == 0 && a->k_bs % 8 == 0 &&
+                  a->v_bs % 8 == 0 && a->o_rs % 2 == 0,
+              "uvx_attention_indexed: strides must keep 16-byte alignment");
+  UVX_REQUIRE(((uintptr_t)a->q | (uintptr_t)a->k | (uintptr_t)a->v) % 16 == 0 && (uintptr_t)a->o % 4 == 0,
+              "uvx_attention_indexed: base pointers must be 16-byte aligned");
+  return a->D == 64 ? launch_wg<64, true>(a, kv_batch, kv_row, past, (cudaStream_t)stream)
+                    : launch_wg<128, true>(a, kv_batch, kv_row, past, (cudaStream_t)stream);
+}

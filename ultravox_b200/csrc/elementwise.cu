@@ -162,14 +162,17 @@ __global__ void kv_append_kernel(const bf16* __restrict__ qkv, int64_t row_strid
 }
 
 
-// One launch for the two row-local steps between the q|k|v projection and the attention of a decode step: RoPE on the q and k heads
-// (in place, same arithmetic as rope_kernel) and the append of the rotated k and of v to the static KV cache at positions[b].
-__global__ void rope_kv_append_kernel(bf16* __restrict__ qkv, int64_t row_stride, int Hq, int Hkv, int D,
-                                      const float* __restrict__ cos_tab, const float* __restrict__ sin_tab,
-                                      const int32_t* __restrict__ rope_pos, bf16* __restrict__ k_cache, bf16* __restrict__ v_cache,
-                                      int64_t cache_batch_stride, const int32_t* __restrict__ positions, int64_t B) {
-  pdl_trigger();
-  pdl_wait();
+// The two row-local steps between the q|k|v projection and the attention: RoPE on the q and k heads (in place, same arithmetic
+// as rope_kernel) and the append of the rotated k and of v to the static KV cache.  Row b goes to cache row b at positions[b]
+// (kMap = false: the decode step), or to cache row cache_row[b] at positions[b], nowhere when cache_row[b] < 0 (kMap = true:
+// the mixed decode + prompt-chunk step of continuous batching).  q and k are rotated either way.
+template <bool kMap>
+__device__ __forceinline__ void rope_kv_append_body(bf16* __restrict__ qkv, int64_t row_stride, int Hq, int Hkv, int D,
+                                                    const float* __restrict__ cos_tab, const float* __restrict__ sin_tab,
+                                                    const int32_t* __restrict__ rope_pos, bf16* __restrict__ k_cache,
+                                                    bf16* __restrict__ v_cache, int64_t cache_batch_stride,
+                                                    const int32_t* __restrict__ positions, const int32_t* __restrict__ cache_row,
+                                                    int64_t B) {
   const int half = D / 2;
   const int vec_per_head = half / 8;
   const int heads = Hq + 2 * Hkv;
@@ -180,9 +183,11 @@ __global__ void rope_kv_append_kernel(bf16* __restrict__ qkv, int64_t row_stride
     const int h = (int)((idx / vec_per_head) % heads);
     const int64_t b = idx / ((int64_t)vec_per_head * heads);
     bf16* base = qkv + b * row_stride + (int64_t)h * D + jv * 8;
+    const int64_t crow = kMap ? (int64_t)cache_row[b] : b;
     const int64_t slot = (int64_t)positions[b];
     if (h >= Hq + Hkv) {   // v head: copy both halves
-      bf16* dst = v_cache + b * cache_batch_stride + slot * kv_width + (int64_t)(h - Hq - Hkv) * D + jv * 8;
+      if (kMap && crow < 0) continue;
+      bf16* dst = v_cache + crow * cache_batch_stride + slot * kv_width + (int64_t)(h - Hq - Hkv) * D + jv * 8;
       *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(base);
       *reinterpret_cast<uint4*>(dst + half) = *reinterpret_cast<const uint4*>(base + half);
       continue;
@@ -202,12 +207,33 @@ __global__ void rope_kv_append_kernel(bf16* __restrict__ qkv, int64_t row_stride
     const bf16x8 p1 = pack8(o1), p2 = pack8(o2);
     *reinterpret_cast<bf16x8*>(base) = p1;
     *reinterpret_cast<bf16x8*>(base + half) = p2;
-    if (h >= Hq) {         // k head: the rotated row also goes to the cache
-      bf16* dst = k_cache + b * cache_batch_stride + slot * kv_width + (int64_t)(h - Hq) * D + jv * 8;
+    if (h >= Hq && (!kMap || crow >= 0)) {         // k head: the rotated row also goes to the cache
+      bf16* dst = k_cache + crow * cache_batch_stride + slot * kv_width + (int64_t)(h - Hq) * D + jv * 8;
       *reinterpret_cast<bf16x8*>(dst) = p1;
       *reinterpret_cast<bf16x8*>(dst + half) = p2;
     }
   }
+}
+
+__global__ void rope_kv_append_kernel(bf16* __restrict__ qkv, int64_t row_stride, int Hq, int Hkv, int D,
+                                      const float* __restrict__ cos_tab, const float* __restrict__ sin_tab,
+                                      const int32_t* __restrict__ rope_pos, bf16* __restrict__ k_cache, bf16* __restrict__ v_cache,
+                                      int64_t cache_batch_stride, const int32_t* __restrict__ positions, int64_t B) {
+  pdl_trigger();
+  pdl_wait();
+  rope_kv_append_body<false>(qkv, row_stride, Hq, Hkv, D, cos_tab, sin_tab, rope_pos, k_cache, v_cache, cache_batch_stride, positions,
+                             nullptr, B);
+}
+
+__global__ void rope_kv_append_map_kernel(bf16* __restrict__ qkv, int64_t row_stride, int Hq, int Hkv, int D,
+                                          const float* __restrict__ cos_tab, const float* __restrict__ sin_tab,
+                                          const int32_t* __restrict__ rope_pos, bf16* __restrict__ k_cache, bf16* __restrict__ v_cache,
+                                          int64_t cache_batch_stride, const int32_t* __restrict__ cache_row,
+                                          const int32_t* __restrict__ positions, int64_t B) {
+  pdl_trigger();
+  pdl_wait();
+  rope_kv_append_body<true>(qkv, row_stride, Hq, Hkv, D, cos_tab, sin_tab, rope_pos, k_cache, v_cache, cache_batch_stride, positions,
+                            cache_row, B);
 }
 
 __global__ void add_i32_kernel(int32_t* __restrict__ a, int32_t* __restrict__ b2, int64_t n, int32_t delta) {
@@ -370,6 +396,20 @@ extern "C" int uvx_rope_kv_append(void* qkv, int64_t B, int64_t row_stride, int 
   launch_k(rope_kv_append_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, (cudaStream_t)stream, (bf16*)qkv, row_stride, Hq,
            Hkv, D, cos_tab, sin_tab, rope_positions, (bf16*)k_cache, (bf16*)v_cache, cache_batch_stride, positions, B);
   return check_launch("rope_kv_append_kernel");
+}
+
+extern "C" int uvx_rope_kv_append_map(void* qkv, int64_t rows, int64_t row_stride, int Hq, int Hkv, int D, const float* cos_tab,
+                                      const float* sin_tab, const int32_t* rope_positions, void* k_cache, void* v_cache,
+                                      int64_t cache_batch_stride, const int32_t* cache_row, const int32_t* positions,
+                                      uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(qkv && cos_tab && sin_tab && rope_positions && k_cache && v_cache && cache_row && positions,
+              "uvx_rope_kv_append_map: null pointer");
+  UVX_REQUIRE(D % 16 == 0 && row_stride % 8 == 0 && cache_batch_stride % 8 == 0 && rows >= 1, "uvx_rope_kv_append_map: alignment");
+  const int64_t total = rows * (Hq + 2 * Hkv) * (D / 16);
+  launch_k(rope_kv_append_map_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, (cudaStream_t)stream, (bf16*)qkv, row_stride,
+           Hq, Hkv, D, cos_tab, sin_tab, rope_positions, (bf16*)k_cache, (bf16*)v_cache, cache_batch_stride, cache_row, positions, rows);
+  return check_launch("rope_kv_append_map_kernel");
 }
 
 extern "C" int uvx_add_i32(int32_t* a, int32_t* b, int64_t n, int32_t delta, uvx_stream_t stream) {

@@ -18,6 +18,9 @@ from . import _lib, ops
 from .model import UltravoxModel
 
 GEMV_MAX_B = int(os.environ.get("UVX_GEMV_MAX_B", "1"))     # decode streams up to which the linears run as matrix-vector kernels
+# Rows up to which the LLM GEMMs stay on the weight-bound tiling (gemm_tc.cu pick_cfg: more rows take the tensor-bound tiles).
+# SlotDecodeEngine prefills a prompt of more rows in chunks of PREFILL_ROWS - slots rows inside a mixed decode step.
+PREFILL_ROWS = 256
 
 
 class PrefillEngine:
@@ -250,22 +253,25 @@ class DecodeEngine:
         return [self.pos, self.lens, self.rope_pos, self.token, self.cur_len, self.step_idx, self.done, self.all_done]
 
     def _step_warm(self):
+        self.graph, self.launches_per_step = self._capture(self._step)
+
+    def _capture(self, step):
         # warm-up on a scratch copy of the state, then capture; the state is restored so no token is lost (the cache row and the
         # sequence column the two trial steps write are rewritten with the same values by the first real step)
         saved = [t.clone() for t in self._state()]
-        self._step()
+        step()
         torch.cuda.synchronize()
         for t, s0 in zip(self._state(), saved):
             t.copy_(s0)
         before = _lib.launch_count()
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g, capture_error_mode="thread_local"):
-            self._step()
-        self.launches_per_step = _lib.launch_count() - before
+            step()
+        launches = _lib.launch_count() - before
         for t, s0 in zip(self._state(), saved):
             t.copy_(s0)
         torch.cuda.synchronize()
-        self.graph = g
+        return g, launches
 
 
 class BeamDecodeEngine(DecodeEngine):
@@ -397,7 +403,18 @@ class SlotDecodeEngine(DecodeEngine):
 
     An idle slot holds ``pos = 0``, ``lens = 1`` and the pad token: it writes its own K / V at position 0 and attends to that
     alone, so it stays finite whatever its cache row held.  A finished slot is frozen (no sequence writes, no position bumps)
-    until ``retire``.  ``n_open[0]`` counts the active slots still decoding after each step."""
+    until ``retire``.  ``n_open[0]`` counts the active slots still decoding after each step.
+
+    A prompt of more than ``PREFILL_ROWS`` rows is prefilled in chunks instead of one B = 1 prefill that would stall every
+    other slot: ``admit`` runs the audio side and the splice and parks the slot as prefilling, and each following ``step``
+    is a mixed step - a second graph, captured on the first such admission - whose GEMMs carry the ``slots`` decode rows
+    followed by ``chunk = PREFILL_ROWS - slots`` prompt rows (so they stay on the weight-bound tiling).  The chunk rows take
+    RoPE + the KV append through a per-row map and attend to the prefilling slot's cache row through the device-indexed
+    attention; the LM head runs over the decode rows plus the chunk's last valid row.  While it prefills, the slot's own
+    decode row writes nothing to the cache and picks nothing; after the last chunk its first token is picked from that row's
+    logits and the slot becomes active.  One slot prefills at a time.  A chunk's rows are independent of the decode rows
+    (every kernel is row-independent at the fixed row count), so a chunked request gets the same bits whatever else is
+    decoding; the decode rows of a mixed step run at 256 rows instead of ``slots`` and are not bit-identical to a plain step."""
 
     def __init__(self, model: UltravoxModel, slots: int, max_len: int, eos_token_ids=None, pad_token_id: int = 0,
                  use_graph: bool = True):
@@ -417,6 +434,21 @@ class SlotDecodeEngine(DecodeEngine):
         self.scratch = torch.empty(slots, self.max_len + 1, **f32)
         self.n_open = torch.zeros(1, **i32)
         self._admit_open = torch.zeros(1, **i32)     # the count an admission's one-row pick writes (not the step's)
+        # mixed-step rows: [0, slots) decode rows, [slots, slots + chunk) prompt-chunk rows.  pos / rope_pos are the decode part
+        # of the per-row position arrays the mixed step's RoPE + KV append reads; the host writes the chunk part, the cache-row
+        # map, the attention scalars (cache row, past, past + valid) and the LM-head row list between replays.
+        self.chunk = PREFILL_ROWS - self.slots
+        R = self.slots + max(self.chunk, 0)
+        self._mpos, self._mrope = torch.zeros(R, **i32), torch.zeros(R, **i32)
+        self.pos, self.rope_pos = self._mpos[:self.slots], self._mrope[:self.slots]
+        self._mrow = torch.arange(R, **i32)
+        self._mscal = torch.zeros(3, **i32)
+        self._head_rows = torch.arange(self.slots + 1, **i32)
+        self._mixed_in = None
+        self._mixed_graph = None
+        self._chunk_logits = None
+        self._prefill: Optional[dict] = None
+        self.launches_per_mixed_step = 0
         self.captures = 0
         self.busy = [False] * self.slots
         for j in range(self.slots):
@@ -453,6 +485,78 @@ class SlotDecodeEngine(DecodeEngine):
         self.logits = logits
         self._pick_rows(logits, slice(None), self.n_open)
 
+    def _mixed_step(self):
+        """The forward of ``DecodeEngine._step`` (multi-stream form) over the decode rows and the prompt-chunk rows."""
+        m = self.model
+        lm, tc = m.language_model, m.config.text_config
+        nq, nkv, hd, Dm = tc.num_attention_heads, tc.num_key_value_heads, lm.head_dim, tc.hidden_size
+        B, R = self.slots, self.slots + self.chunk
+        eps = tc.rms_norm_eps
+        h = self._mixed_in
+        ops.embed_splice(self.token, lm.model.embed_tokens.weight, None, None, out=h[:B])
+        smax = self.cache.k.shape[2]
+        kv_row, past, kv_len = self._mscal[0:1], self._mscal[1:2], self._mscal[2:3]
+        for li, layer in enumerate(lm.model.layers):
+            sa, mlp = layer.self_attn, layer.mlp
+            kc, vc = self.cache.k[li], self.cache.v[li]
+            qkv = ops.linear(ops.rmsnorm(h, layer.input_layernorm.weight, eps), sa.qkv_w)
+            ops.rope_kv_append_map_(qkv, nq, nkv, hd, self.cos, self.sin, self._mrope, kc, vc, self._mrow, self._mpos)
+            att = torch.empty(R, nq * hd, dtype=torch.bfloat16, device=h.device)
+            rs = qkv.stride(0)
+            ops.attention(qkv.data_ptr(), kc.data_ptr(), vc.data_ptr(), att, B, nq, nkv, 1, smax, hd,
+                          (rs, rs, nkv * hd, smax * nkv * hd, nkv * hd, smax * nkv * hd, nq * hd, nq * hd), hd ** -0.5, False,
+                          self.lens, 0, self.kv_start)
+            ops.attention_indexed(qkv[B:, :nq * hd].unsqueeze(0), kc, vc, att[B:].unsqueeze(0), nq, hd ** -0.5, kv_row, past, kv_len)
+            h = ops.linear(att, sa.o_proj.weight, residual=h)
+            x = ops.rmsnorm(h, layer.post_attention_layernorm.weight, eps)
+            act = ops.swiglu(ops.linear(x, mlp.gate_up_w), gate_first=True)
+            h = ops.linear(act, mlp.down_proj.weight, residual=h)
+        hn = ops.rmsnorm(ops.gather_rows(h, self._head_rows), lm.model.norm.weight, eps)
+        logits = ops.lm_head(hn, lm.lm_head.weight)
+        self._chunk_logits = logits[B:]
+        self._pick(logits[:B])
+
+    @property
+    def prefilling(self) -> Optional[int]:
+        """The slot whose prompt is being prefilled in chunks, or None."""
+        return None if self._prefill is None else self._prefill["slot"]
+
+    def step(self) -> torch.Tensor:
+        """A plain decode step, or a mixed step while a chunked prompt is pending (whose last chunk activates its slot)."""
+        pf = self._prefill
+        if pf is None:
+            return super().step()
+        j, S, a, C, B = pf["slot"], pf["S"], pf["done"], self.chunk, self.slots
+        n = min(C, S - a)
+        self._mixed_in[B:B + n].copy_(pf["embeds"][a:a + n])
+        # cache row per chunk row (-1: padding, no write) | its position (padding: 0, inside the RoPE tables) | attention scalars
+        # | the LM head's chunk row; one pinned buffer per step (the host allocator keeps it until its copies have run)
+        hv = torch.tensor([j] * n + [-1] * (C - n) + list(range(a, a + n)) + [0] * (C - n) + [j, a, a + n, B + n - 1],
+                          dtype=torch.int32).pin_memory()
+        self._mrow[B:].copy_(hv[:C], non_blocking=True)
+        self._mpos[B:].copy_(hv[C:2 * C], non_blocking=True)
+        self._mrope[B:].copy_(hv[C:2 * C], non_blocking=True)
+        self._mscal.copy_(hv[2 * C:2 * C + 3], non_blocking=True)
+        self._head_rows[B:].copy_(hv[2 * C + 3:], non_blocking=True)
+        if self.use_graph:
+            if self._mixed_graph is None:
+                self.captures += 1
+                self._mixed_graph, self.launches_per_mixed_step = self._capture(self._mixed_step)
+            self._mixed_graph.replay()
+        else:
+            self._mixed_step()
+        pf["done"] = a + n
+        if a + n == S:
+            self._prefill = None
+            self.active[j] = 1
+            # the pick's slot_finish bumps all three: the first new token sits at slot S, sees S + 1 keys, RoPE position S
+            self.pos[j] = S - 1
+            self.lens[j] = S
+            self.rope_pos[j] = S - 1
+            self._mrow[j] = j
+            self._pick_rows(self._chunk_logits, slice(j, j + 1), self._admit_open)
+        return self.token
+
     def begin(self, *args, **kwargs):
         raise NotImplementedError("SlotDecodeEngine takes requests through admit()")
 
@@ -464,7 +568,11 @@ class SlotDecodeEngine(DecodeEngine):
         """Prefills one request (``input_ids`` [1, S] plus the processor's audio features, passed to ``model.forward``) at B = 1
         into cache row ``slot``, sets the slot's state and picks its first token from the prefill logits with the slot kernels.
         ``temperature <= 0`` is greedy; a sampled request reads ``u`` (its uniforms, one per step, as ``generate()`` draws them
-        for a batch of one).  Returns the device token tensor [slots] (no sync)."""
+        for a batch of one).  Returns the device token tensor [slots] (no sync).
+
+        A prompt of more than ``PREFILL_ROWS`` rows is only embedded here (audio encoder, projector, splice); its LLM prefill
+        runs in chunks inside the following steps, and its first token is picked after the last one (``prefilling`` is the
+        slot until then).  Only one slot prefills at a time."""
         from .model import KVCache
         j = int(slot)
         if not 0 <= j < self.slots:
@@ -478,20 +586,34 @@ class SlotDecodeEngine(DecodeEngine):
             raise ValueError(f"a prompt of {S} tokens plus max_new_tokens={n} does not fit a slot of {self.max_len} positions")
         if temperature > 0 and (u is None or u.numel() < S + n):
             raise ValueError(f"a sampled request needs at least {S + n} uniforms")
+        chunked = S > PREFILL_ROWS
+        if chunked and self.chunk < 1:
+            raise ValueError(f"a prompt of {S} > {PREFILL_ROWS} rows is prefilled in chunks of {PREFILL_ROWS} - slots rows; "
+                             f"{self.slots} slots leave none")
+        if chunked and self._prefill is not None:
+            raise ValueError(f"slot {self._prefill['slot']} is still prefilling; one long prompt at a time")
         dev = self.pos.device
         input_ids = input_ids.to(dev)
-        row = KVCache(self.cache.k[:, j:j + 1], self.cache.v[:, j:j + 1])
-        logits = self.model.forward(input_ids, past_key_values=row, logits_to_keep=1, **features).logits.view(1, -1)
+        if chunked:
+            embeds = self.model.prompt_embeds(input_ids, **features).view(S, -1)
+            if self._mixed_in is None:
+                self._mixed_in = torch.zeros(self.slots + self.chunk, embeds.shape[1], dtype=embeds.dtype, device=dev)
+            self._prefill = dict(slot=j, S=S, done=0, embeds=embeds)
+            self._mrow[j] = -1          # the slot's idle decode row must not overwrite position 0 of the prompt
+        else:
+            row = KVCache(self.cache.k[:, j:j + 1], self.cache.v[:, j:j + 1])
+            logits = self.model.forward(input_ids, past_key_values=row, logits_to_keep=1, **features).logits.view(1, -1)
         self.seq[j, :S].copy_(input_ids[0])
         self.cur_len[j] = S
         self.n_new[j] = 0
         self.max_new[j] = n
         self.done[j] = 0
-        self.active[j] = 1
-        # the pick's slot_finish bumps all three: the first new token sits at slot S, sees S + 1 keys, RoPE position S
-        self.pos[j] = S - 1
-        self.lens[j] = S
-        self.rope_pos[j] = S - 1
+        if not chunked:
+            self.active[j] = 1
+            # the pick's slot_finish bumps all three: the first new token sits at slot S, sees S + 1 keys, RoPE position S
+            self.pos[j] = S - 1
+            self.lens[j] = S
+            self.rope_pos[j] = S - 1
         self.temps[j] = float(temperature) if temperature > 0 else 0.0
         self.top_ks[j] = int(top_k or 0)
         self.top_ps[j] = float(top_p)
@@ -500,13 +622,16 @@ class SlotDecodeEngine(DecodeEngine):
             w = min(u.numel(), self.max_len + 1)
             self.u[j, :w].copy_(u.reshape(-1)[:w])
         self.busy[j] = True
-        self._pick_rows(logits, slice(j, j + 1), self._admit_open)
+        if not chunked:
+            self._pick_rows(logits, slice(j, j + 1), self._admit_open)
         return self.token.view(-1)
 
     def retire(self, slot: int, length: Optional[int] = None) -> torch.Tensor:
         """The slot's sequence [1, prompt + new tokens] (a copy; ``length`` = its ``cur_len`` if the caller already read it, else
         one sync), then the slot goes back to idle."""
         j = int(slot)
+        if j == self.prefilling:
+            raise ValueError(f"slot {j} is still prefilling")
         n = int(self.cur_len[j]) if length is None else int(length)
         out = self.seq[j:j + 1, :n].clone()
         self._idle(j)

@@ -783,15 +783,8 @@ class UltravoxModel(nn.Module):
                 from .autograd import EncoderLoraFn
                 inputs_embeds = EncoderLoraFn.apply(self, tm, audio_lens, lora.A, lora.Bq, lora.Bk)
         elif inputs_embeds is None:
-            if audio_waveforms is not None and len(audio_waveforms) > 0:
-                tm = self.mel_chunks_from_waveforms(audio_waveforms, audio_num_frames, audio_pad_frames=audio_pad_frames)
-                inputs_embeds = self._prepare_audio_embeds(input_ids, None, audio_token_start_idx, audio_lens,
-                                                           audio_token_len, audio_batch_size, audio_tm=tm)
-            elif audio_values is not None and len(audio_values) > 0:
-                inputs_embeds = self._prepare_audio_embeds(input_ids, audio_values, audio_token_start_idx, audio_lens,
-                                                           audio_token_len, audio_batch_size)
-            else:
-                inputs_embeds = ops.embed_splice(input_ids, self.language_model.model.embed_tokens.weight, None, None)
+            inputs_embeds = self.prompt_embeds(input_ids, audio_values, audio_token_start_idx, audio_lens, audio_token_len,
+                                               audio_batch_size, audio_waveforms, audio_num_frames, audio_pad_frames)
         else:
             inputs_embeds = inputs_embeds.clone()
         if self.training and self.loss_config.loss_function not in (LossFunction.CrossEntropy, LossFunction.KL_Divergence):
@@ -816,6 +809,23 @@ class UltravoxModel(nn.Module):
         if self.training and self.loss_config.loss_function == LossFunction.KL_Divergence:
             loss = self._compute_kl_loss(logits, labels, alt_input_ids, alt_labels)
         return CausalLMOutputWithPast(loss=loss, logits=logits, past_key_values=past_key_values)
+
+    def prompt_embeds(self, input_ids: torch.Tensor, audio_values: Optional[torch.Tensor] = None,
+                      audio_token_start_idx: Optional[torch.Tensor] = None, audio_lens: Optional[torch.Tensor] = None,
+                      audio_token_len: Optional[torch.Tensor] = None, audio_batch_size: Optional[torch.Tensor] = None,
+                      audio_waveforms: Optional[torch.Tensor] = None, audio_num_frames: Optional[torch.Tensor] = None,
+                      audio_pad_frames: Optional[torch.Tensor] = None, **kwargs) -> torch.Tensor:
+        """The spliced ``inputs_embeds`` [B, S, D] that ``forward`` feeds the LLM: log-mel (for waveforms), encoder, projector,
+        token embeddings and the audio splice; token embeddings alone without audio."""
+        input_ids = input_ids.to(self.device)
+        if audio_waveforms is not None and len(audio_waveforms) > 0:
+            tm = self.mel_chunks_from_waveforms(audio_waveforms, audio_num_frames, audio_pad_frames=audio_pad_frames)
+            return self._prepare_audio_embeds(input_ids, None, audio_token_start_idx, audio_lens, audio_token_len, audio_batch_size,
+                                              audio_tm=tm)
+        if audio_values is not None and len(audio_values) > 0:
+            return self._prepare_audio_embeds(input_ids, audio_values, audio_token_start_idx, audio_lens, audio_token_len,
+                                              audio_batch_size)
+        return ops.embed_splice(input_ids, self.language_model.model.embed_tokens.weight, None, None)
 
     def _forward_with_grad(self, input_ids, enc, labels, attention_mask, audio_token_start_idx, audio_token_len,
                            audio_batch_size, alt_input_ids, alt_labels, logits_to_keep) -> CausalLMOutputWithPast:

@@ -284,6 +284,33 @@ def attention(q_ptr: int, k_ptr: int, v_ptr: int, out: torch.Tensor, B: int, Hq:
     return out
 
 
+def attention_indexed(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, out: torch.Tensor, Hq: int, scale: float,
+                      kv_row: torch.Tensor, past: torch.Tensor, kv_len: torch.Tensor) -> torch.Tensor:
+    """Causal attention of one prompt chunk per query batch against a slot cache, with the cache row and the offset read on
+    the device (``uvx_attention_indexed``): q [B, Sq, Hq * D] (rows of any stride), k_cache / v_cache one layer [slots, S_max,
+    Hkv, D], kv_row / past / kv_len [B] int32 -> out [B, Sq, Hq * D].  Query i of batch b sees keys j <= i + past[b] and
+    j < kv_len[b] of cache row kv_row[b]."""
+    _cuda(q, BF16, "q"), _cuda(k_cache, BF16, "k_cache"), _cuda(v_cache, BF16, "v_cache"), _cuda(out, BF16, "out")
+    B, Sq = q.shape[0], q.shape[1]
+    slots, smax, Hkv, D = k_cache.shape
+    if q.shape[2] != Hq * D or q.stride(2) != 1 or out.shape != (B, Sq, Hq * D) or out.stride(2) != 1:
+        raise ValueError(f"q / out must be [B, Sq, {Hq * D}] with unit column stride")
+    if v_cache.shape != k_cache.shape or v_cache.stride() != k_cache.stride() or not k_cache.is_contiguous():
+        raise ValueError("k_cache / v_cache must be contiguous [slots, S_max, Hkv, D] of the same shape")
+    for t, name in ((kv_row, "kv_row"), (past, "past"), (kv_len, "kv_len")):
+        _rows(t, torch.int32, B, name)
+    a = AttnArgs()
+    a.q, a.k, a.v, a.o = q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), out.data_ptr()
+    a.B, a.Hq, a.Hkv, a.Sq, a.Skv, a.D = B, Hq, Hkv, Sq, smax, D
+    (a.q_rs, a.q_bs, a.k_rs, a.k_bs, a.v_rs, a.v_bs, a.o_rs, a.o_bs) = (q.stride(1), q.stride(0), Hkv * D, smax * Hkv * D, Hkv * D,
+                                                                        smax * Hkv * D, out.stride(1), out.stride(0))
+    a.kv_len = kv_len.data_ptr()
+    a.kv_start = None
+    a.causal, a.block, a.scale = 1, 0, float(scale)
+    check(lib().uvx_attention_indexed(C.byref(a), slots, kv_row.data_ptr(), past.data_ptr(), _stream()), "uvx_attention_indexed")
+    return out
+
+
 def attention_fused_qkv(qkv: torch.Tensor, B: int, S: int, Hq: int, Hkv: int, D: int, scale: float, causal: bool,
                         kv_len: Optional[torch.Tensor] = None, block: int = 0,
                         out: Optional[torch.Tensor] = None, kv_start: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -675,6 +702,20 @@ def rope_kv_append_(qkv: torch.Tensor, Hq: int, Hkv: int, D: int, cos: torch.Ten
     check(lib().uvx_rope_kv_append(qkv.data_ptr(), B, qkv.stride(0), Hq, Hkv, D, cos.data_ptr(), sin.data_ptr(), rope_positions.data_ptr(),
                                    k_cache.data_ptr(), v_cache.data_ptr(), k_cache.stride(0), positions.data_ptr(), _stream()),
           "uvx_rope_kv_append")
+
+
+def rope_kv_append_map_(qkv: torch.Tensor, Hq: int, Hkv: int, D: int, cos: torch.Tensor, sin: torch.Tensor,
+                        rope_positions: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, cache_row: torch.Tensor,
+                        positions: torch.Tensor) -> None:
+    """``rope_kv_append_`` with a per-row map: row r is rotated at rope_positions[r] and appended to cache row cache_row[r] at
+    positions[r], or not appended when cache_row[r] < 0 (all three [rows] int32 on the device)."""
+    _cuda(qkv, BF16, "qkv")
+    R = qkv.shape[0]
+    for t, name in ((rope_positions, "rope_positions"), (cache_row, "cache_row"), (positions, "positions")):
+        _rows(t, torch.int32, R, name)
+    check(lib().uvx_rope_kv_append_map(qkv.data_ptr(), R, qkv.stride(0), Hq, Hkv, D, cos.data_ptr(), sin.data_ptr(),
+                                       rope_positions.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), k_cache.stride(0),
+                                       cache_row.data_ptr(), positions.data_ptr(), _stream()), "uvx_rope_kv_append_map")
 
 
 def add_i32_(a: torch.Tensor, b: Optional[torch.Tensor], delta: int) -> None:

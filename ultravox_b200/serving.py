@@ -1,7 +1,9 @@
 """Request-level continuous batching over ``engine.SlotDecodeEngine``.
 
 Requests queue FIFO.  Between decode steps the host admits one waiting request into each free slot (a B = 1 prefill into that
-slot's cache row, which pauses the other slots for its duration) and every ``sync_every`` steps it reads the device count of
+slot's cache row, which pauses the other slots for its duration; a prompt of more than ``engine.PREFILL_ROWS`` rows is
+prefilled in chunks inside the following decode steps instead, one such prompt at a time, and a long prompt at the head of the
+queue waits for the previous one to finish) and every ``sync_every`` steps it reads the device count of
 open slots to retire the finished ones and deliver their tokens.  A slot is also retired as soon as the host knows that its
 budget is spent.  Each request gets exactly what ``model.generate()`` returns for that request alone: its prompt ids, then the
 new tokens up to and including its first EOS, or ``max_new_tokens`` of them.
@@ -14,7 +16,7 @@ from typing import Callable, Deque, Dict, List, Optional
 
 import torch
 
-from .engine import SlotDecodeEngine
+from .engine import PREFILL_ROWS, SlotDecodeEngine
 
 
 @dataclasses.dataclass
@@ -50,6 +52,7 @@ class SlotScheduler:
         self.first_token: Dict[int, torch.cuda.Event] = {}
         self._queue: Deque[_Request] = collections.deque()
         self._running: Dict[int, _Request] = {}        # slot -> request
+        self._prefilling: Optional[tuple] = None        # (slot, request) of the prompt being prefilled in chunks
         self._next_id = 0
         self._last_poll = 0
 
@@ -100,15 +103,25 @@ class SlotScheduler:
                 return
             if eng.busy[j]:
                 continue
+            long = int(self._queue[0].input_ids.shape[1]) > PREFILL_ROWS
+            if long and self._prefilling is not None:
+                return                  # FIFO: it waits until the prompt in flight has been prefilled
             r = self._queue.popleft()
             feats = {k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in r.features.items()}
             eng.admit(j, r.input_ids, r.max_new, r.temperature, r.top_k, r.top_p, r.penalty, r.u, **feats)
-            ev = torch.cuda.Event(enable_timing=True)
-            ev.record()
-            self.first_token[r.rid] = ev
-            r.admitted_at = self.steps
             r.features, r.u = {}, None
-            self._running[j] = r
+            if long:
+                self._prefilling = (j, r)
+            else:
+                self._started(j, r)
+
+    def _started(self, j: int, r: _Request) -> None:
+        """The request's first token has been picked: its budget counts from here."""
+        ev = torch.cuda.Event(enable_timing=True)
+        ev.record()
+        self.first_token[r.rid] = ev
+        r.admitted_at = self.steps
+        self._running[j] = r
 
     def _retire(self, results: Dict[int, torch.Tensor], on_tokens: Optional[Callable]) -> int:
         eng = self.engine
@@ -133,7 +146,7 @@ class SlotScheduler:
     def run(self, on_tokens: Optional[Callable[[int, torch.Tensor], None]] = None) -> Dict[int, torch.Tensor]:
         """Serves every queued request; ``on_tokens(id, sequence)`` is called as each one finishes."""
         results: Dict[int, torch.Tensor] = {}
-        while self._queue or self._running:
+        while self._queue or self._running or self._prefilling is not None:
             self._admit()
             due = any(self._budget_spent(r) for r in self._running.values())
             if due or self.steps - self._last_poll >= self.sync_every:
@@ -144,7 +157,12 @@ class SlotScheduler:
                     raise RuntimeError("a slot reached its budget on the host but not on the device")
             self.engine.step()
             self.steps += 1
+            if self._prefilling is not None and self.engine.prefilling is None:
+                j, r = self._prefilling
+                self._prefilling = None
+                self._started(j, r)
         return results
 
     def pending(self) -> List[int]:
-        return [r.rid for r in self._queue] + [r.rid for r in self._running.values()]
+        pf = [] if self._prefilling is None else [self._prefilling[1].rid]
+        return [r.rid for r in self._queue] + pf + [r.rid for r in self._running.values()]
