@@ -215,6 +215,23 @@ int uvx_attention_enc_tc(const void* qkv, int64_t row_stride, int64_t B, int64_t
  * block = 0, kv_start = NULL, lse = NULL; kv_row / past / kv_len are read on the device, so they may change between replays. */
 int uvx_attention_indexed(const uvx_attn_args* a, int64_t kv_batch, const int32_t* kv_row, const int32_t* past,
                           uvx_stream_t stream);
+/* Paged KV cache (continuous batching with conversation sessions, ultravox_b200/engine.py PagedSlotDecodeEngine): one layer of the
+ * K / V pool is [n_pages, 64, Hkv, D]; a page holds 64 positions, exactly one key tile of both attention kernels, so the same
+ * keys meet in the same order and the results are bit-identical to the contiguous forms.  table [rows, table_stride] int32:
+ * key tile t of table row b is page table[b * table_stride + t].  Only entries of tiles below the key bound are read (entries past a
+ * sequence's pages may hold -1).
+ * uvx_attention_paged          uvx_attention on the mma.sync kernel with K / V read through the table: a->k / a->v point at the
+ *                              pool layer, k_rs / v_rs are the row strides inside a page and k_bs / v_bs = 64 rows (the page
+ *                              stride); batch row b uses table row b; a->kv_len required; Skv bounds the keys (<= 64 *
+ *                              table_stride).  Bit-identical to uvx_attention on a contiguous cache holding the same rows, for
+ *                              calls that take its mma.sync kernel.  Requires kv_start = NULL, lse = NULL, block = 0, causal only
+ *                              with Sq = 1.
+ * uvx_attention_indexed_paged  uvx_attention_indexed with kv_row[b] a table row: the K / V tensor maps cover the pool layer
+ *                              (n_pages pages) as {D, Hkv, 64, n_pages}, key tile t is loaded from page table[kv_row[b] *
+ *                              table_stride + t].  Same restrictions; bit-identical to uvx_attention_indexed.                 */
+int uvx_attention_paged(const uvx_attn_args* a, const int32_t* table, int64_t table_stride, uvx_stream_t stream);
+int uvx_attention_indexed_paged(const uvx_attn_args* a, int64_t n_pages, const int32_t* table, int64_t table_stride,
+                                const int32_t* kv_row, const int32_t* past, uvx_stream_t stream);
 
 /* RoPE on the q and k sections of a fused [rows, (Hq + 2*Hkv) * D] projection, in place
  * (hf:modeling_llama.py:124-168; cos/sin tables [max_pos, D/2] fp32 built by the host exactly like
@@ -369,6 +386,23 @@ int uvx_beam_update(const float* cand_s, const int64_t* cand_i, int64_t B, int32
                     uvx_stream_t stream);
 int uvx_kv_reorder(void* k_cache, void* v_cache, int64_t L, int64_t B, int32_t nb, int64_t S_max, int64_t row_elems,
                    const int32_t* parent, const int32_t* n_pos, uvx_stream_t stream);
+
+/* Paged KV cache bookkeeping (pages of 64 positions, see uvx_attention_paged).
+ * uvx_kv_page_map    for each of `rows` step rows: cache_row[r] < 0, or r < n_frozen and frozen[r] != 0 (optional, e.g. the
+ *                    slots' done flags: a finished row that is still fed must not overwrite the last position its conversation
+ *                    keeps) -> page_out[r] = -1, off_out[r] = 0 (no table read); otherwise page_out[r] = table[cache_row[r] * table_stride + pos[r] / 64], off_out[r] = pos[r] % 64.
+ *                    uvx_rope_kv_append_map then appends into a pool layer viewed as [n_pages, 64, Hkv, D] with
+ *                    cache_row = page_out and positions = off_out.  Everything is read on the device (graph-capturable).
+ * uvx_kv_pages_copy  bit-exact copy of positions [p0, p1) of every layer, K and V, between a contiguous one-row cache (layer
+ *                    l, position p at l * row_layer_stride + p * row_elems) and the pool (page pages[p / 64], row p % 64, at
+ *                    l * pool_layer_stride + (page * 64 + p % 64) * row_elems), 16-byte accesses, one launch.  to_pages = 1:
+ *                    row -> pages (scatter); 0: pages -> row (gather).  `pages` (device) lists the pages of positions 0, 64,
+ *                    128, ...; nothing outside [p0, p1) is written.                                                       */
+int uvx_kv_page_map(const int32_t* table, int64_t table_stride, const int32_t* cache_row, const int32_t* pos, const int32_t* frozen,
+                    int64_t n_frozen, int64_t rows, int32_t* page_out, int32_t* off_out, uvx_stream_t stream);
+int uvx_kv_pages_copy(void* k_row, void* v_row, int64_t row_layer_stride, void* k_pool, void* v_pool, int64_t pool_layer_stride,
+                      int64_t L, int64_t row_elems, const int32_t* pages, int64_t p0, int64_t p1, int32_t to_pages,
+                      uvx_stream_t stream);
 
 /* Shifted causal-LM cross entropy (hf:loss/loss_utils.py:28-67; called through LlamaForCausalLM.forward(labels=)
  * from ref:ultravox/model/ultravox_model.py:328-334).  logits [B*S, V] fp32 (row_stride elements), labels [B, S]

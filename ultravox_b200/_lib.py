@@ -71,6 +71,10 @@ SIGNATURES = {
     "uvx_debug_attn_tc": (C.c_int, [C.c_int]),
     "uvx_attention_enc_tc": (C.c_int, [c_vp, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_vp, c_i64, c_vp, c_i32, c_f32, c_vp]),
     "uvx_attention_indexed": (C.c_int, [C.POINTER(AttnArgs), c_i64, c_vp, c_vp, c_vp]),
+    "uvx_attention_paged": (C.c_int, [C.POINTER(AttnArgs), c_vp, c_i64, c_vp]),
+    "uvx_attention_indexed_paged": (C.c_int, [C.POINTER(AttnArgs), c_i64, c_vp, c_i64, c_vp, c_vp, c_vp]),
+    "uvx_kv_page_map": (C.c_int, [c_vp, c_i64, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp]),
+    "uvx_kv_pages_copy": (C.c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp]),
     "uvx_rope": (C.c_int, [c_vp, c_i64, c_i64, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp]),
     "uvx_swiglu": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_i64, C.c_int, c_vp]),
     "uvx_splice_plan": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp]),

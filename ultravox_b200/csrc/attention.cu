@@ -7,6 +7,8 @@
 // the Llama prefill / training attention (head_dim 128) and the single-token decode steps.
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "uvx_common.cuh"
 
 namespace uvx {
@@ -25,6 +27,13 @@ struct AttnParams {
   int Sq, Skv, group, Hq;  // group = Hq / Hkv
   int causal, block;
   float scale_log2;  // scale * log2(e)
+};
+
+// Paged form: k / v address a pool layer [n_pages, 64, Hkv, D]; key tile t of batch row b is page table[b * table_stride + t]
+// (k_bs / v_bs are the page strides, k_rs / v_rs the row strides inside a page).
+struct PagedAttnParams : AttnParams {
+  const int32_t* table;
+  int64_t table_stride;
 };
 
 __device__ __forceinline__ void cp_async16(void* dst, const void* src, bool valid) {
@@ -58,8 +67,8 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&t);
 }
 
-template <int D>
-__global__ void __launch_bounds__(kAThreads) attn_fwd_kernel(const AttnParams p) {
+template <int D, bool kPaged = false>
+__global__ void __launch_bounds__(kAThreads) attn_fwd_kernel(const std::conditional_t<kPaged, PagedAttnParams, AttnParams> p) {
   pdl_trigger();
   pdl_wait();
   constexpr int LD = D + 8;  // padded row (bf16 elements): 16-byte aligned, conflict-free ldmatrix
@@ -74,8 +83,8 @@ __global__ void __launch_bounds__(kAThreads) attn_fwd_kernel(const AttnParams p)
   const int h = blockIdx.y, b = blockIdx.z;
   const int hk = h / p.group;
   const bf16* qb = p.q + (int64_t)b * p.q_bs + (int64_t)h * D;
-  const bf16* kb = p.k + (int64_t)b * p.k_bs + (int64_t)hk * D;
-  const bf16* vb = p.v + (int64_t)b * p.v_bs + (int64_t)hk * D;
+  const bf16* kb = p.k + (kPaged ? 0 : (int64_t)b * p.k_bs) + (int64_t)hk * D;
+  const bf16* vb = p.v + (kPaged ? 0 : (int64_t)b * p.v_bs) + (int64_t)hk * D;
 
   int kv_end = p.Skv;
   if (p.kv_len) kv_end = min(kv_end, max(p.kv_len[b], 0));
@@ -99,14 +108,28 @@ __global__ void __launch_bounds__(kAThreads) attn_fwd_kernel(const AttnParams p)
     const int n0 = tile * kAN;
     bf16* dk = sK + stage * kAN * LD;
     bf16* dv = sV + stage * kAN * LD;
-    for (int i = tid; i < kAN * CH; i += kAThreads) {
-      const int r = i / CH, c = i % CH;
-      // rows outside [kv_begin, kv_end) are zero-filled, never read: the cache tail past a sequence's length may hold
-      // anything (torch.empty), and a masked probability of 0 times a NaN/Inf V row would still poison P.V
-      const bool ok = (n0 + r) < kv_end && (n0 + r) >= kv_begin;
-      const int64_t row = ok ? n0 + r : 0;
-      cp_async16(dk + r * LD + c * 8, kb + row * p.k_rs + c * 8, ok);
-      cp_async16(dv + r * LD + c * 8, vb + row * p.v_rs + c * 8, ok);
+    if constexpr (kPaged) {
+      // the tile is one page: row r of the tile is row r of the page (only tiles below kv_end are ever looked up)
+      const int64_t pg = p.table[(int64_t)b * p.table_stride + tile];
+      const bf16* kp = kb + pg * p.k_bs;
+      const bf16* vp = vb + pg * p.v_bs;
+      for (int i = tid; i < kAN * CH; i += kAThreads) {
+        const int r = i / CH, c = i % CH;
+        const bool ok = (n0 + r) < kv_end;
+        const int64_t row = ok ? r : 0;
+        cp_async16(dk + r * LD + c * 8, kp + row * p.k_rs + c * 8, ok);
+        cp_async16(dv + r * LD + c * 8, vp + row * p.v_rs + c * 8, ok);
+      }
+    } else {
+      for (int i = tid; i < kAN * CH; i += kAThreads) {
+        const int r = i / CH, c = i % CH;
+        // rows outside [kv_begin, kv_end) are zero-filled, never read: the cache tail past a sequence's length may hold
+        // anything (torch.empty), and a masked probability of 0 times a NaN/Inf V row would still poison P.V
+        const bool ok = (n0 + r) < kv_end && (n0 + r) >= kv_begin;
+        const int64_t row = ok ? n0 + r : 0;
+        cp_async16(dk + r * LD + c * 8, kb + row * p.k_rs + c * 8, ok);
+        cp_async16(dv + r * LD + c * 8, vb + row * p.v_rs + c * 8, ok);
+      }
     }
   };
 
@@ -241,20 +264,24 @@ __global__ void __launch_bounds__(kAThreads) attn_fwd_kernel(const AttnParams p)
   }
 }
 
-template <int D>
-static int launch_attn(const uvx_attn_args* a, cudaStream_t st) {
+template <int D, bool kPaged = false>
+static int launch_attn(const uvx_attn_args* a, cudaStream_t st, const int32_t* table = nullptr, int64_t table_stride = 0) {
   constexpr int LD = D + 8;
   const size_t smem = (size_t)(kAM + 4 * kAN) * LD * 2;
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<D, kPaged>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) {
       set_error("cudaFuncSetAttribute(attn_fwd_kernel<%d>): %s", D, cudaGetErrorString(e));
       return UVX_ERR_CUDA;
     }
     attr = true;
   }
-  AttnParams p;
+  std::conditional_t<kPaged, PagedAttnParams, AttnParams> p;
+  if constexpr (kPaged) {
+    p.table = table;
+    p.table_stride = table_stride;
+  }
   p.q = (const bf16*)a->q;
   p.k = (const bf16*)a->k;
   p.v = (const bf16*)a->v;
@@ -272,7 +299,7 @@ static int launch_attn(const uvx_attn_args* a, cudaStream_t st) {
   p.block = a->block;
   p.scale_log2 = a->scale * 1.4426950408889634f;
   dim3 grid((unsigned)((a->Sq + kAM - 1) / kAM), (unsigned)a->Hq, (unsigned)a->B);
-  launch_k(attn_fwd_kernel<D>, dim3(grid), dim3(kAThreads), smem, st, p);
+  launch_k(attn_fwd_kernel<D, kPaged>, dim3(grid), dim3(kAThreads), smem, st, p);
   return check_launch("attn_fwd_kernel");
 }
 
@@ -309,6 +336,27 @@ extern "C" int uvx_attention(const uvx_attn_args* a, uvx_stream_t stream) {
   // mma.sync kernel below
   if (g_attn_wg && attn_wg_eligible(a)) return launch_attn_wg(a, (cudaStream_t)stream);
   return a->D == 64 ? launch_attn<64>(a, (cudaStream_t)stream) : launch_attn<128>(a, (cudaStream_t)stream);
+}
+
+extern "C" int uvx_attention_paged(const uvx_attn_args* a, const int32_t* table, int64_t table_stride, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(a && a->q && a->k && a->v && a->o && a->kv_len && table, "uvx_attention_paged: null pointer");
+  UVX_REQUIRE(a->D == 64 || a->D == 128, "uvx_attention_paged: head_dim must be 64 or 128 (got %lld)", (long long)a->D);
+  UVX_REQUIRE(a->B >= 1 && a->B < 65536 && a->Hq >= 1 && a->Hq < 65536 && a->Hkv >= 1 && a->Hq % a->Hkv == 0 && a->Sq >= 1 &&
+                  a->Skv >= 1,
+              "uvx_attention_paged: bad shape");
+  UVX_REQUIRE(table_stride >= (a->Skv + kAN - 1) / kAN, "uvx_attention_paged: a table row of %lld pages cannot cover Skv = %lld",
+              (long long)table_stride, (long long)a->Skv);
+  UVX_REQUIRE(!a->kv_start && !a->lse && a->block == 0 && (!a->causal || a->Sq == 1),
+              "uvx_attention_paged: no kv_start, no lse, no block mask, causal only with Sq == 1");
+  UVX_REQUIRE(a->k_bs == (int64_t)kAN * a->k_rs && a->v_bs == (int64_t)kAN * a->v_rs,
+              "uvx_attention_paged: k_bs / v_bs must be one page of 64 rows");
+  UVX_REQUIRE(a->q_rs % 8 == 0 && a->k_rs % 8 == 0 && a->v_rs % 8 == 0 && a->o_rs % 2 == 0 && a->q_bs % 8 == 0,
+              "uvx_attention_paged: strides must keep 16-byte alignment");
+  UVX_REQUIRE(((uintptr_t)a->q | (uintptr_t)a->k | (uintptr_t)a->v) % 16 == 0 && (uintptr_t)a->o % 4 == 0,
+              "uvx_attention_paged: base pointers must be 16-byte aligned");
+  return a->D == 64 ? launch_attn<64, true>(a, (cudaStream_t)stream, table, table_stride)
+                    : launch_attn<128, true>(a, (cudaStream_t)stream, table, table_stride);
 }
 
 // Whisper-encoder entry over the fused projection: qkv [B*S, row_stride] with head h's q / k / v at columns q_col + 64h,

@@ -8,6 +8,8 @@
 // fragment re-packed to bf16 is the A fragment) and V read MN-major from the same TMA layout.  Masks come from indices; key tiles
 // outside [kv_start, kv_len) / above the causal diagonal are never loaded, and V rows of a partly valid tile that lie outside
 // that range are zeroed in shared memory (a cache tail may hold anything, and 0 * NaN would still poison P V).
+#include <type_traits>
+
 #include "uvx_common.cuh"
 #include "tc_ptx.cuh"
 
@@ -24,6 +26,13 @@ struct AttnWgParams {
   float scale_log2;
   const int32_t* kv_row;  // device-indexed form: K / V batch coordinate of query batch b
   const int32_t* past;    // device-indexed form: causal shift (keys already in the cache) of query batch b
+};
+
+// Paged device-indexed form: kv_row[b] is a row of the page table, and key tile t lives in page table[kv_row[b] * table_stride + t]
+// of the pool layer the K / V tensor maps cover as {D, Hkv, 64, n_pages}.
+struct AttnWgPagedParams : AttnWgParams {
+  const int32_t* table;
+  int64_t table_stride;
 };
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
@@ -47,10 +56,11 @@ struct AttnWgSmem {
 
 // kIndexed: the K / V batch coordinate and the causal shift come from device memory (p.kv_row[b], p.past[b]) instead of b and
 // Skv - Sq, so one captured launch serves whichever cache row and prompt offset the host writes between replays.
-template <int D, bool kIndexed = false>
+template <int D, bool kIndexed = false, bool kPaged = false>
 __global__ void __launch_bounds__(128, 1)
 attn_wg_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-               const AttnWgParams p) {
+               const std::conditional_t<kPaged, AttnWgPagedParams, AttnWgParams> p) {
+  static_assert(!kPaged || kIndexed, "the paged form is device-indexed");
   using L = AttnWgSmem<D>;
   constexpr int P = L::kP;
   pdl_trigger();
@@ -84,10 +94,20 @@ attn_wg_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
   pdl_wait();
   auto load_kv = [&](int tile, int stage) {
     mbar_expect_tx(&full[stage], (uint32_t)(2 * P * kPanel));
+    if constexpr (kPaged) {
+      // the tile is one whole page (only tiles below kv_end are ever looked up)
+      const int pg = p.table[(int64_t)kb * p.table_stride + tile];
 #pragma unroll
-    for (int pn = 0; pn < P; ++pn) {
-      tma_load_4d(smem + L::kK + (stage * P + pn) * kPanel, &tmK, pn * 64, hk, tile * kWK, kb, &full[stage]);
-      tma_load_4d(smem + L::kV + (stage * P + pn) * kPanel, &tmV, pn * 64, hk, tile * kWK, kb, &full[stage]);
+      for (int pn = 0; pn < P; ++pn) {
+        tma_load_4d(smem + L::kK + (stage * P + pn) * kPanel, &tmK, pn * 64, hk, 0, pg, &full[stage]);
+        tma_load_4d(smem + L::kV + (stage * P + pn) * kPanel, &tmV, pn * 64, hk, 0, pg, &full[stage]);
+      }
+    } else {
+#pragma unroll
+      for (int pn = 0; pn < P; ++pn) {
+        tma_load_4d(smem + L::kK + (stage * P + pn) * kPanel, &tmK, pn * 64, hk, tile * kWK, kb, &full[stage]);
+        tma_load_4d(smem + L::kV + (stage * P + pn) * kPanel, &tmV, pn * 64, hk, tile * kWK, kb, &full[stage]);
+      }
     }
   };
   if (tid == 0 && n_tiles > tile0) {
@@ -254,24 +274,31 @@ bool attn_wg_eligible(const uvx_attn_args* a) {
   return true;
 }
 
-template <int D, bool kIndexed>
-static int launch_wg(const uvx_attn_args* a, int64_t kv_batch, const int32_t* kv_row, const int32_t* past, cudaStream_t st) {
+// kPaged: kv_batch is the pool's page count and the K / V maps cover it as {D, Hkv, 64, n_pages}
+template <int D, bool kIndexed, bool kPaged = false>
+static int launch_wg(const uvx_attn_args* a, int64_t kv_batch, const int32_t* kv_row, const int32_t* past, cudaStream_t st,
+                     const int32_t* table = nullptr, int64_t table_stride = 0) {
   using L = AttnWgSmem<D>;
   CUtensorMap tq, tk, tv;
+  const int64_t kv_rows = kPaged ? kWK : a->Skv;
   int rc = aw_encode(&tq, a->q, D, a->Hq, a->Sq, a->B, a->q_rs, a->q_bs);
-  if (!rc) rc = aw_encode(&tk, a->k, D, a->Hkv, a->Skv, kv_batch, a->k_rs, a->k_bs);
-  if (!rc) rc = aw_encode(&tv, a->v, D, a->Hkv, a->Skv, kv_batch, a->v_rs, a->v_bs);
+  if (!rc) rc = aw_encode(&tk, a->k, D, a->Hkv, kv_rows, kv_batch, a->k_rs, a->k_bs);
+  if (!rc) rc = aw_encode(&tv, a->v, D, a->Hkv, kv_rows, kv_batch, a->v_rs, a->v_bs);
   if (rc) return rc;
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(attn_wg_kernel<D, kIndexed>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kBytes);
+    cudaError_t e = cudaFuncSetAttribute(attn_wg_kernel<D, kIndexed, kPaged>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kBytes);
     if (e != cudaSuccess) {
       set_error("cudaFuncSetAttribute(attn_wg_kernel<%d>): %s", D, cudaGetErrorString(e));
       return UVX_ERR_CUDA;
     }
     attr = true;
   }
-  AttnWgParams p;
+  std::conditional_t<kPaged, AttnWgPagedParams, AttnWgParams> p;
+  if constexpr (kPaged) {
+    p.table = table;
+    p.table_stride = table_stride;
+  }
   p.o = (bf16*)a->o;
   p.o_rs = a->o_rs;
   p.o_bs = a->o_bs;
@@ -288,7 +315,7 @@ static int launch_wg(const uvx_attn_args* a, int64_t kv_batch, const int32_t* kv
   p.kv_row = kv_row;
   p.past = past;
   dim3 grid((unsigned)((a->Sq + kWQ - 1) / kWQ), (unsigned)a->Hq, (unsigned)a->B);
-  launch_k(attn_wg_kernel<D, kIndexed>, grid, dim3(128), (size_t)L::kBytes, st, tq, tk, tv, p);
+  launch_k(attn_wg_kernel<D, kIndexed, kPaged>, grid, dim3(128), (size_t)L::kBytes, st, tq, tk, tv, p);
   return check_launch("attn_wg_kernel");
 }
 
@@ -315,4 +342,26 @@ extern "C" int uvx_attention_indexed(const uvx_attn_args* a, int64_t kv_batch, c
               "uvx_attention_indexed: base pointers must be 16-byte aligned");
   return a->D == 64 ? launch_wg<64, true>(a, kv_batch, kv_row, past, (cudaStream_t)stream)
                     : launch_wg<128, true>(a, kv_batch, kv_row, past, (cudaStream_t)stream);
+}
+
+extern "C" int uvx_attention_indexed_paged(const uvx_attn_args* a, int64_t n_pages, const int32_t* table, int64_t table_stride,
+                                           const int32_t* kv_row, const int32_t* past, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(a && a->q && a->k && a->v && a->o && kv_row && past && a->kv_len && table, "uvx_attention_indexed_paged: null pointer");
+  UVX_REQUIRE(a->D == 64 || a->D == 128, "uvx_attention_indexed_paged: head_dim must be 64 or 128 (got %lld)", (long long)a->D);
+  UVX_REQUIRE(a->B >= 1 && a->B < 65536 && a->Hq >= 1 && a->Hq < 65536 && a->Hkv >= 1 && a->Hq % a->Hkv == 0 && a->Sq >= 1 &&
+                  a->Skv >= 1 && n_pages >= 1,
+              "uvx_attention_indexed_paged: bad shape");
+  UVX_REQUIRE(table_stride >= (a->Skv + kWK - 1) / kWK, "uvx_attention_indexed_paged: a table row of %lld pages cannot cover Skv = %lld",
+              (long long)table_stride, (long long)a->Skv);
+  UVX_REQUIRE(a->causal == 1 && a->block == 0 && !a->kv_start && !a->lse,
+              "uvx_attention_indexed_paged: causal, no block mask, no kv_start, no lse");
+  UVX_REQUIRE(a->k_bs == (int64_t)kWK * a->k_rs && a->v_bs == (int64_t)kWK * a->v_rs,
+              "uvx_attention_indexed_paged: k_bs / v_bs must be one page of 64 rows");
+  UVX_REQUIRE(a->q_rs % 8 == 0 && a->k_rs % 8 == 0 && a->v_rs % 8 == 0 && a->q_bs % 8 == 0 && a->o_rs % 2 == 0,
+              "uvx_attention_indexed_paged: strides must keep 16-byte alignment");
+  UVX_REQUIRE(((uintptr_t)a->q | (uintptr_t)a->k | (uintptr_t)a->v) % 16 == 0 && (uintptr_t)a->o % 4 == 0,
+              "uvx_attention_indexed_paged: base pointers must be 16-byte aligned");
+  return a->D == 64 ? launch_wg<64, true, true>(a, n_pages, kv_row, past, (cudaStream_t)stream, table, table_stride)
+                    : launch_wg<128, true, true>(a, n_pages, kv_row, past, (cudaStream_t)stream, table, table_stride);
 }

@@ -13,6 +13,8 @@
 //   uvx_beam_select         the top K of (log-prob + running beam score) over each prompt's nb * V continuations
 //   uvx_beam_update         running beams, finished-hypothesis pool, early-stop heuristic and loop condition of one step
 //   uvx_kv_reorder          in-place gather of the KV cache rows by parent beam (and the prefill broadcast to the beams)
+//   uvx_kv_page_map         paged KV cache: (table row, position) of each step row -> (page, offset) for the mapped RoPE + append
+//   uvx_kv_pages_copy       paged KV cache: positions of a contiguous one-row cache <-> their pages, all layers, K and V
 #include "uvx_common.cuh"
 
 namespace uvx {
@@ -781,6 +783,54 @@ __global__ void __launch_bounds__(256) kv_reorder_kernel(bf16* k, bf16* v, int64
   }
 }
 
+static constexpr int kPageRows = 64;  // positions per KV page = keys per attention tile
+
+// (cache_row[r], pos[r]) -> (page_out[r], off_out[r]) through the page table; cache_row < 0 or a frozen row -> (-1, 0), nothing
+// is looked up
+__global__ void kv_page_map_kernel(const int32_t* __restrict__ table, int64_t table_stride, const int32_t* __restrict__ cache_row,
+                                   const int32_t* __restrict__ pos, const int32_t* __restrict__ frozen, int64_t n_frozen,
+                                   int32_t* __restrict__ page_out, int32_t* __restrict__ off_out, int64_t rows) {
+  pdl_trigger();
+  pdl_wait();
+  const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= rows) return;
+  const int cr = cache_row[r];
+  if (cr < 0 || (r < n_frozen && frozen[r])) {
+    page_out[r] = -1;
+    off_out[r] = 0;
+    return;
+  }
+  const int p = pos[r];
+  page_out[r] = table[(int64_t)cr * table_stride + p / kPageRows];
+  off_out[r] = p % kPageRows;
+}
+
+// 16-byte vectors of positions [p0, p1) of every layer, K and V: row cache [L][S_max][row_elems] <-> pool [L][n_pages][64][row_elems]
+__global__ void __launch_bounds__(256) kv_pages_copy_kernel(uint4* __restrict__ k_row, uint4* __restrict__ v_row, int64_t row_layer_vec,
+                                                            uint4* __restrict__ k_pool, uint4* __restrict__ v_pool,
+                                                            int64_t pool_layer_vec, int64_t L, int64_t vec,
+                                                            const int32_t* __restrict__ pages, int64_t p0, int64_t n, int to_pages) {
+  pdl_trigger();
+  pdl_wait();
+  const int64_t per_layer = n * vec;
+  const int64_t total = 2 * L * per_layer;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int which = (int)(i / (L * per_layer));
+    const int64_t rem = i % (L * per_layer);
+    const int64_t l = rem / per_layer, e = rem % per_layer;
+    const int64_t p = p0 + e / vec, c = e % vec;
+    const int64_t pg = pages[p / kPageRows];
+    const int64_t ri = l * row_layer_vec + p * vec + c;
+    const int64_t pi = l * pool_layer_vec + (pg * kPageRows + p % kPageRows) * vec + c;
+    uint4* row = which ? v_row : k_row;
+    uint4* pool = which ? v_pool : k_pool;
+    if (to_pages)
+      pool[pi] = row[ri];
+    else
+      row[ri] = pool[pi];
+  }
+}
+
 }  // namespace uvx
 
 extern "C" int uvx_kv_write(const void* qkv, int64_t row_stride, int64_t k_col, int64_t v_col, int64_t kv_width, void* k_cache,
@@ -931,4 +981,36 @@ extern "C" int uvx_kv_reorder(void* k_cache, void* v_cache, int64_t L, int64_t B
   launch_k(kv_reorder_kernel, dim3((unsigned)blocks), dim3(256), smem, (cudaStream_t)stream, (bf16*)k_cache, (bf16*)v_cache, L, B,
            (int)nb, S_max, row_elems, parent, n_pos, (int)P);
   return check_launch("kv_reorder_kernel");
+}
+
+extern "C" int uvx_kv_page_map(const int32_t* table, int64_t table_stride, const int32_t* cache_row, const int32_t* pos,
+                               const int32_t* frozen, int64_t n_frozen, int64_t rows, int32_t* page_out, int32_t* off_out,
+                               uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(table && cache_row && pos && page_out && off_out && rows >= 1 && table_stride >= 1 && n_frozen >= 0 &&
+                  n_frozen <= rows && (frozen || n_frozen == 0),
+              "uvx_kv_page_map: bad arguments");
+  launch_k(kv_page_map_kernel, dim3((unsigned)((rows + 255) / 256)), dim3(256), 0, (cudaStream_t)stream, table, table_stride, cache_row,
+           pos, frozen, n_frozen, page_out, off_out, rows);
+  return check_launch("kv_page_map_kernel");
+}
+
+extern "C" int uvx_kv_pages_copy(void* k_row, void* v_row, int64_t row_layer_stride, void* k_pool, void* v_pool, int64_t pool_layer_stride,
+                                 int64_t L, int64_t row_elems, const int32_t* pages, int64_t p0, int64_t p1, int32_t to_pages,
+                                 uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(k_row && v_row && k_pool && v_pool && pages && L >= 1, "uvx_kv_pages_copy: null pointer");
+  UVX_REQUIRE(row_elems >= 8 && row_elems % 8 == 0 && row_layer_stride % 8 == 0 && pool_layer_stride % 8 == 0 && p0 >= 0 && p1 >= p0 &&
+                  p1 * row_elems <= row_layer_stride,
+              "uvx_kv_pages_copy: bad shape");
+  UVX_REQUIRE(((uintptr_t)k_row | (uintptr_t)v_row | (uintptr_t)k_pool | (uintptr_t)v_pool) % 16 == 0,
+              "uvx_kv_pages_copy: base pointers must be 16-byte aligned");
+  if (p1 == p0) return UVX_OK;
+  const int64_t total = 2 * L * (p1 - p0) * (row_elems / 8);
+  int64_t blocks = (total + 255) / 256;
+  if (blocks > 132 * 16) blocks = 132 * 16;
+  launch_k(kv_pages_copy_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, (uint4*)k_row, (uint4*)v_row,
+           row_layer_stride / 8, (uint4*)k_pool, (uint4*)v_pool, pool_layer_stride / 8, L, row_elems / 8, pages, p0, p1 - p0,
+           (int)to_pages);
+  return check_launch("kv_pages_copy_kernel");
 }

@@ -205,7 +205,7 @@ class DecodeEngine:
     def _step(self):
         m = self.model
         lm, tc = m.language_model, m.config.text_config
-        nq, nkv, hd, Dm = tc.num_attention_heads, tc.num_key_value_heads, lm.head_dim, tc.hidden_size
+        Dm = tc.hidden_size
         B = self.B
         # one stream: matrix-vector kernels (fp32 FMAs on the CUDA cores keep up with the weight stream) with RMSNorm / SwiGLU fused
         # into their prologues; more streams: the tensor-core GEMM (at B = 8 the FMA work per weight byte is 8x and the GEMV is
@@ -213,20 +213,13 @@ class DecodeEngine:
         one = B <= GEMV_MAX_B
         eps = tc.rms_norm_eps
         h = ops.embed_splice(self.token, lm.model.embed_tokens.weight, None, None).view(B, Dm)
-        smax = self.cache.k.shape[2]
         for li, layer in enumerate(lm.model.layers):
             sa, mlp = layer.self_attn, layer.mlp
-            kc, vc = self.cache.k[li], self.cache.v[li]
             if one:     # RMSNorm rides in the matrix-vector kernel's prologue
                 qkv = ops.gemv(h, sa.qkv_w, norm=(layer.input_layernorm.weight, eps))
             else:
                 qkv = ops.linear(ops.rmsnorm(h, layer.input_layernorm.weight, eps), sa.qkv_w)
-            ops.rope_kv_append_(qkv, nq, nkv, hd, self.cos, self.sin, self.rope_pos, kc, vc, self.pos)
-            att = torch.empty(B, nq * hd, dtype=torch.bfloat16, device=h.device)
-            rs = qkv.stride(0)
-            ops.attention(qkv.data_ptr(), kc.data_ptr(), vc.data_ptr(), att, B, nq, nkv, 1, smax, hd,
-                          (rs, rs, nkv * hd, smax * nkv * hd, nkv * hd, smax * nkv * hd, nq * hd, nq * hd), hd ** -0.5, False,
-                          self.lens, 0, self.kv_start)
+            att = self._attend(li, qkv)
             if one:
                 h = ops.gemv(att, sa.o_proj.weight, residual=h)
                 gu = ops.gemv(h, mlp.gate_up_w, norm=(layer.post_attention_layernorm.weight, eps))
@@ -238,6 +231,21 @@ class DecodeEngine:
                 h = ops.linear(act, mlp.down_proj.weight, residual=h)
         hn = ops.rmsnorm(h, lm.model.norm.weight, eps)
         self._pick(ops.lm_head(hn, lm.lm_head.weight))
+
+    def _attend(self, li: int, qkv: torch.Tensor) -> torch.Tensor:
+        """The two cache-touching calls of layer ``li`` of a step: RoPE on q / k + the KV append at ``pos``, then attention of the
+        B single-token queries over their cache rows -> [B, Hq * D]."""
+        lm, tc = self.model.language_model, self.model.config.text_config
+        nq, nkv, hd = tc.num_attention_heads, tc.num_key_value_heads, lm.head_dim
+        B, smax = self.B, self.cache.k.shape[2]
+        kc, vc = self.cache.k[li], self.cache.v[li]
+        ops.rope_kv_append_(qkv, nq, nkv, hd, self.cos, self.sin, self.rope_pos, kc, vc, self.pos)
+        att = torch.empty(B, nq * hd, dtype=torch.bfloat16, device=qkv.device)
+        rs = qkv.stride(0)
+        ops.attention(qkv.data_ptr(), kc.data_ptr(), vc.data_ptr(), att, B, nq, nkv, 1, smax, hd,
+                      (rs, rs, nkv * hd, smax * nkv * hd, nkv * hd, smax * nkv * hd, nq * hd, nq * hd), hd ** -0.5, False,
+                      self.lens, 0, self.kv_start)
+        return att
 
     def step(self) -> torch.Tensor:
         """Feeds ``self.token`` (the previous output), writes the next token into it; returns the device tensor."""
@@ -417,8 +425,9 @@ class SlotDecodeEngine(DecodeEngine):
     decoding; the decode rows of a mixed step run at 256 rows instead of ``slots`` and are not bit-identical to a plain step."""
 
     def __init__(self, model: UltravoxModel, slots: int, max_len: int, eos_token_ids=None, pad_token_id: int = 0,
-                 use_graph: bool = True):
-        super().__init__(model, slots, max_len, use_graph=use_graph, eos_token_ids=eos_token_ids, pad_token_id=pad_token_id)
+                 use_graph: bool = True, cache=None):
+        super().__init__(model, slots, max_len, use_graph=use_graph, cache=cache, eos_token_ids=eos_token_ids,
+                         pad_token_id=pad_token_id)
         dev = model.device
         i32, f32 = dict(dtype=torch.int32, device=dev), dict(dtype=torch.float32, device=dev)
         self.slots = int(slots)
@@ -489,24 +498,14 @@ class SlotDecodeEngine(DecodeEngine):
         """The forward of ``DecodeEngine._step`` (multi-stream form) over the decode rows and the prompt-chunk rows."""
         m = self.model
         lm, tc = m.language_model, m.config.text_config
-        nq, nkv, hd, Dm = tc.num_attention_heads, tc.num_key_value_heads, lm.head_dim, tc.hidden_size
-        B, R = self.slots, self.slots + self.chunk
+        B = self.slots
         eps = tc.rms_norm_eps
         h = self._mixed_in
         ops.embed_splice(self.token, lm.model.embed_tokens.weight, None, None, out=h[:B])
-        smax = self.cache.k.shape[2]
-        kv_row, past, kv_len = self._mscal[0:1], self._mscal[1:2], self._mscal[2:3]
         for li, layer in enumerate(lm.model.layers):
             sa, mlp = layer.self_attn, layer.mlp
-            kc, vc = self.cache.k[li], self.cache.v[li]
             qkv = ops.linear(ops.rmsnorm(h, layer.input_layernorm.weight, eps), sa.qkv_w)
-            ops.rope_kv_append_map_(qkv, nq, nkv, hd, self.cos, self.sin, self._mrope, kc, vc, self._mrow, self._mpos)
-            att = torch.empty(R, nq * hd, dtype=torch.bfloat16, device=h.device)
-            rs = qkv.stride(0)
-            ops.attention(qkv.data_ptr(), kc.data_ptr(), vc.data_ptr(), att, B, nq, nkv, 1, smax, hd,
-                          (rs, rs, nkv * hd, smax * nkv * hd, nkv * hd, smax * nkv * hd, nq * hd, nq * hd), hd ** -0.5, False,
-                          self.lens, 0, self.kv_start)
-            ops.attention_indexed(qkv[B:, :nq * hd].unsqueeze(0), kc, vc, att[B:].unsqueeze(0), nq, hd ** -0.5, kv_row, past, kv_len)
+            att = self._attend_mixed(li, qkv)
             h = ops.linear(att, sa.o_proj.weight, residual=h)
             x = ops.rmsnorm(h, layer.post_attention_layernorm.weight, eps)
             act = ops.swiglu(ops.linear(x, mlp.gate_up_w), gate_first=True)
@@ -515,6 +514,23 @@ class SlotDecodeEngine(DecodeEngine):
         logits = ops.lm_head(hn, lm.lm_head.weight)
         self._chunk_logits = logits[B:]
         self._pick(logits[:B])
+
+    def _attend_mixed(self, li: int, qkv: torch.Tensor) -> torch.Tensor:
+        """The cache-touching calls of layer ``li`` of a mixed step: mapped RoPE + KV append of every row, attention of the decode
+        rows over their cache rows and of the chunk rows over the prefilling slot's row -> [slots + chunk, Hq * D]."""
+        lm, tc = self.model.language_model, self.model.config.text_config
+        nq, nkv, hd = tc.num_attention_heads, tc.num_key_value_heads, lm.head_dim
+        B, R, smax = self.slots, self.slots + self.chunk, self.cache.k.shape[2]
+        kv_row, past, kv_len = self._mscal[0:1], self._mscal[1:2], self._mscal[2:3]
+        kc, vc = self.cache.k[li], self.cache.v[li]
+        ops.rope_kv_append_map_(qkv, nq, nkv, hd, self.cos, self.sin, self._mrope, kc, vc, self._mrow, self._mpos)
+        att = torch.empty(R, nq * hd, dtype=torch.bfloat16, device=qkv.device)
+        rs = qkv.stride(0)
+        ops.attention(qkv.data_ptr(), kc.data_ptr(), vc.data_ptr(), att, B, nq, nkv, 1, smax, hd,
+                      (rs, rs, nkv * hd, smax * nkv * hd, nkv * hd, smax * nkv * hd, nq * hd, nq * hd), hd ** -0.5, False,
+                      self.lens, 0, self.kv_start)
+        ops.attention_indexed(qkv[B:, :nq * hd].unsqueeze(0), kc, vc, att[B:].unsqueeze(0), nq, hd ** -0.5, kv_row, past, kv_len)
+        return att
 
     @property
     def prefilling(self) -> Optional[int]:
@@ -564,7 +580,8 @@ class SlotDecodeEngine(DecodeEngine):
         raise NotImplementedError("SlotDecodeEngine takes requests through admit()")
 
     def admit(self, slot: int, input_ids: torch.Tensor, max_new_tokens: int, temperature: float = 0.0, top_k: int = 0,
-              top_p: float = 1.0, repetition_penalty: float = 1.0, u: Optional[torch.Tensor] = None, **features) -> torch.Tensor:
+              top_p: float = 1.0, repetition_penalty: float = 1.0, u: Optional[torch.Tensor] = None, past: int = 0,
+              **features) -> torch.Tensor:
         """Prefills one request (``input_ids`` [1, S] plus the processor's audio features, passed to ``model.forward``) at B = 1
         into cache row ``slot``, sets the slot's state and picks its first token from the prefill logits with the slot kernels.
         ``temperature <= 0`` is greedy; a sampled request reads ``u`` (its uniforms, one per step, as ``generate()`` draws them
@@ -572,8 +589,11 @@ class SlotDecodeEngine(DecodeEngine):
 
         A prompt of more than ``PREFILL_ROWS`` rows is only embedded here (audio encoder, projector, splice); its LLM prefill
         runs in chunks inside the following steps, and its first token is picked after the last one (``prefilling`` is the
-        slot until then).  Only one slot prefills at a time."""
-        from .model import KVCache
+        slot until then).  Only one slot prefills at a time.
+
+        ``past`` > 0 (engines that keep a conversation's KV cache, ``PagedSlotDecodeEngine``): the slot's cache already holds the
+        first ``past`` positions of ``input_ids``, so only the suffix is prefilled, as ``generate(past_key_values=...)`` does; the
+        chunked form then starts at ``past`` and is taken when the suffix has more than ``PREFILL_ROWS`` rows."""
         j = int(slot)
         if not 0 <= j < self.slots:
             raise ValueError(f"slot {slot} out of range [0, {self.slots})")
@@ -581,12 +601,16 @@ class SlotDecodeEngine(DecodeEngine):
             raise ValueError(f"slot {j} is busy; retire it first")
         if input_ids.dim() != 2 or input_ids.shape[0] != 1:
             raise ValueError(f"admit() takes one request: input_ids [1, S], got {tuple(input_ids.shape)}")
-        S, n = int(input_ids.shape[1]), int(max_new_tokens)
+        S, n, P = int(input_ids.shape[1]), int(max_new_tokens), int(past)
         if n < 1 or S < 1 or S + n > self.max_len:
             raise ValueError(f"a prompt of {S} tokens plus max_new_tokens={n} does not fit a slot of {self.max_len} positions")
+        if not 0 <= P < S:
+            raise ValueError(f"past = {P}: the prompt of {S} tokens must extend the cached prefix")
+        if P and not self.keeps_kv:
+            raise ValueError("this engine keeps no KV cache between requests (past must be 0)")
         if temperature > 0 and (u is None or u.numel() < S + n):
             raise ValueError(f"a sampled request needs at least {S + n} uniforms")
-        chunked = S > PREFILL_ROWS
+        chunked = S - P > PREFILL_ROWS
         if chunked and self.chunk < 1:
             raise ValueError(f"a prompt of {S} > {PREFILL_ROWS} rows is prefilled in chunks of {PREFILL_ROWS} - slots rows; "
                              f"{self.slots} slots leave none")
@@ -598,11 +622,10 @@ class SlotDecodeEngine(DecodeEngine):
             embeds = self.model.prompt_embeds(input_ids, **features).view(S, -1)
             if self._mixed_in is None:
                 self._mixed_in = torch.zeros(self.slots + self.chunk, embeds.shape[1], dtype=embeds.dtype, device=dev)
-            self._prefill = dict(slot=j, S=S, done=0, embeds=embeds)
+            self._prefill = dict(slot=j, S=S, done=P, embeds=embeds)
             self._mrow[j] = -1          # the slot's idle decode row must not overwrite position 0 of the prompt
         else:
-            row = KVCache(self.cache.k[:, j:j + 1], self.cache.v[:, j:j + 1])
-            logits = self.model.forward(input_ids, past_key_values=row, logits_to_keep=1, **features).logits.view(1, -1)
+            logits = self._prefill_one(j, input_ids, P, features)
         self.seq[j, :S].copy_(input_ids[0])
         self.cur_len[j] = S
         self.n_new[j] = 0
@@ -626,6 +649,14 @@ class SlotDecodeEngine(DecodeEngine):
             self._pick_rows(logits, slice(j, j + 1), self._admit_open)
         return self.token.view(-1)
 
+    keeps_kv = False        # whether a request's KV cache can outlive its slot (conversation sessions)
+
+    def _prefill_one(self, j: int, input_ids: torch.Tensor, past: int, features: dict) -> torch.Tensor:
+        """B = 1 prefill of a whole prompt into cache row ``j`` -> its last position's logits [1, V]."""
+        from .model import KVCache
+        row = KVCache(self.cache.k[:, j:j + 1], self.cache.v[:, j:j + 1])
+        return self.model.forward(input_ids, past_key_values=row, logits_to_keep=1, **features).logits.view(1, -1)
+
     def retire(self, slot: int, length: Optional[int] = None) -> torch.Tensor:
         """The slot's sequence [1, prompt + new tokens] (a copy; ``length`` = its ``cur_len`` if the caller already read it, else
         one sync), then the slot goes back to idle."""
@@ -636,3 +667,119 @@ class SlotDecodeEngine(DecodeEngine):
         out = self.seq[j:j + 1, :n].clone()
         self._idle(j)
         return out
+
+
+class PagedSlotDecodeEngine(SlotDecodeEngine):
+    """``SlotDecodeEngine`` whose KV cache is a shared pool of 64-position pages instead of one ``[max_len]`` row per slot, so a
+    request's K / V can outlive its slot: a conversation keeps its pages between turns and each turn prefills only its new suffix.
+
+    The pool holds ``kv_pages`` shareable pages plus one private idle page per slot (an idle row writes its pad token at position
+    0 there, as the contiguous engine's idle row does in its own row): K and V are ``[L, kv_pages + slots, 64, Hkv, D]``.  The
+    page table ``[slots, ceil(max_len / 64)]`` int32 lives on the device; the host writes a slot's row between replays (its
+    pages at admission, its idle page at retirement).  A page is exactly one key tile of both attention kernels, so every step
+    computes the same bits as the contiguous engine: one ``uvx_kv_page_map`` launch per step turns each row's (slot, position)
+    into (page, offset) for the unchanged mapped RoPE + append, and the attention kernels read their key tiles through the table.
+    Rows that are done (finished, not yet retired) write nothing, so the last position a conversation keeps stays intact.
+
+    ``cache`` is the one-row admission scratch ``[L, 1, max_len, Hkv, D]``: a prompt of at most ``PREFILL_ROWS`` new rows
+    gathers its conversation's first ``past`` positions there, is prefilled at B = 1 like ``generate(past_key_values=...)``,
+    and its new positions are scattered into its pages.  Longer suffixes go through the mixed step from ``past`` on.  Page
+    ownership (which pages a request or a conversation holds) is the caller's bookkeeping (``serving.PagePool``)."""
+
+    keeps_kv = True
+
+    def __init__(self, model: UltravoxModel, slots: int, max_len: int, kv_pages: int, eos_token_ids=None, pad_token_id: int = 0,
+                 use_graph: bool = True):
+        lm, tc = model.language_model, model.config.text_config
+        dev = model.device
+        if int(kv_pages) < 1:
+            raise ValueError(f"kv_pages must be >= 1, got {kv_pages}")
+        self.kv_pages = int(kv_pages)
+        self.table_width = -(-int(max_len) // ops.PAGE)
+        L, nkv, hd = tc.num_hidden_layers, tc.num_key_value_heads, lm.head_dim
+        n = self.kv_pages + int(slots)
+        self.pool_k = torch.empty(L, n, ops.PAGE, nkv, hd, dtype=torch.bfloat16, device=dev)
+        self.pool_v = torch.empty_like(self.pool_k)
+        self.table = torch.full((int(slots), self.table_width), -1, dtype=torch.int32, device=dev)
+        R = int(slots) + max(PREFILL_ROWS - int(slots), 0)
+        self._pg_page = torch.zeros(R, dtype=torch.int32, device=dev)      # the page map's output: page / offset of every row
+        self._pg_off = torch.zeros(R, dtype=torch.int32, device=dev)
+        super().__init__(model, slots, max_len, eos_token_ids=eos_token_ids, pad_token_id=pad_token_id, use_graph=use_graph,
+                         cache=model.new_cache(1, max_len))
+
+    def idle_page(self, j: int) -> int:
+        return self.kv_pages + j
+
+    def _set_table_row(self, j: int, pages) -> None:
+        row = torch.full((self.table_width,), -1, dtype=torch.int32)
+        row[:len(pages)] = torch.tensor(list(pages), dtype=torch.int32)
+        self.table[j].copy_(row.pin_memory(), non_blocking=True)
+
+    def _idle(self, j: int) -> None:
+        super()._idle(j)
+        self._set_table_row(j, [self.idle_page(j)])
+
+    # -- the step: one page-map launch before the layers, then the forward with the paged cache calls ----------------------
+    def _step(self):
+        B = self.slots
+        ops.kv_page_map(self.table, self._mrow[:B], self.pos, self._pg_page[:B], self._pg_off[:B], frozen=self.done)
+        super()._step()
+
+    def _mixed_step(self):
+        ops.kv_page_map(self.table, self._mrow, self._mpos, self._pg_page, self._pg_off, frozen=self.done)
+        super()._mixed_step()
+
+    def _attend(self, li: int, qkv: torch.Tensor) -> torch.Tensor:
+        B = self.slots
+        return self._attend_rows(li, qkv, self._mrope[:B], self._pg_page[:B], self._pg_off[:B])
+
+    def _attend_mixed(self, li: int, qkv: torch.Tensor) -> torch.Tensor:
+        att = self._attend_rows(li, qkv, self._mrope, self._pg_page, self._pg_off)
+        B, nq, hd = self.slots, self.model.config.text_config.num_attention_heads, self.model.language_model.head_dim
+        ops.attention_indexed_paged(qkv[B:, :nq * hd].unsqueeze(0), self.pool_k[li], self.pool_v[li], att[B:].unsqueeze(0), nq,
+                                    hd ** -0.5, self.table, self._mscal[0:1], self._mscal[1:2], self._mscal[2:3])
+        return att
+
+    def _attend_rows(self, li, qkv, rope_pos, page, off) -> torch.Tensor:
+        """RoPE + append of every row of ``qkv`` into its (page, offset), then decode attention of the first ``slots`` rows."""
+        lm, tc = self.model.language_model, self.model.config.text_config
+        nq, nkv, hd = tc.num_attention_heads, tc.num_key_value_heads, lm.head_dim
+        B = self.slots
+        kp, vp = self.pool_k[li], self.pool_v[li]
+        ops.rope_kv_append_map_(qkv, nq, nkv, hd, self.cos, self.sin, rope_pos, kp, vp, page, off)
+        att = torch.empty(qkv.shape[0], nq * hd, dtype=torch.bfloat16, device=qkv.device)
+        ops.attention_paged(qkv[:B, :nq * hd], kp, vp, att[:B], nq, hd ** -0.5, self.table, self.lens)
+        return att
+
+    # -- admission ------------------------------------------------------------------------------------------------------------
+    def admit(self, slot: int, input_ids: torch.Tensor, max_new_tokens: int, temperature: float = 0.0, top_k: int = 0,
+              top_p: float = 1.0, repetition_penalty: float = 1.0, u: Optional[torch.Tensor] = None, past: int = 0,
+              pages=None, **features) -> torch.Tensor:
+        """``SlotDecodeEngine.admit`` into the pages ``pages`` (a list of page ids for positions 0, 64, 128, ...; it must cover
+        S + max_new_tokens positions, and its first ceil(past / 64) pages hold the conversation's first ``past`` positions)."""
+        j = int(slot)
+        S, n = int(input_ids.shape[1]), int(max_new_tokens)
+        pages = list(pages or [])
+        if len(pages) * ops.PAGE < S + n or len(pages) > self.table_width:
+            raise ValueError(f"{len(pages)} pages for a prompt of {S} tokens plus max_new_tokens={n}")
+        if not 0 <= j < self.slots or self.busy[j]:
+            raise ValueError(f"slot {slot} is out of range or busy")
+        self._set_table_row(j, pages)
+        self._pages_dev = torch.tensor(pages, dtype=torch.int32).to(self.pos.device, non_blocking=True)
+        return super().admit(j, input_ids, n, temperature, top_k, top_p, repetition_penalty, u, past=past, **features)
+
+    def _prefill_one(self, j: int, input_ids: torch.Tensor, past: int, features: dict) -> torch.Tensor:
+        """Gather [0, past) into the scratch row, prefill [past, S) there exactly as ``generate(past_key_values=...)`` does, scatter
+        [past, S) into the slot's pages."""
+        from .model import KVCache
+        m, S = self.model, int(input_ids.shape[1])
+        row = self.cache
+        if past:
+            ops.kv_pages_copy(row.k, row.v, self.pool_k, self.pool_v, self._pages_dev, 0, past, to_pages=False)
+            emb = m.prompt_embeds(input_ids, **features)       # embed + splice the whole prompt, prefill only the new suffix
+            out = m.forward(input_ids[:, past:], None, emb[:, past:].contiguous(), past_key_values=KVCache(row.k, row.v, past),
+                            logits_to_keep=1)
+        else:
+            out = m.forward(input_ids, past_key_values=KVCache(row.k, row.v), logits_to_keep=1, **features)
+        ops.kv_pages_copy(row.k, row.v, self.pool_k, self.pool_v, self._pages_dev, past, S, to_pages=True)
+        return out.logits.view(1, -1)

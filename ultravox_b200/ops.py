@@ -311,6 +311,114 @@ def attention_indexed(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Ten
     return out
 
 
+PAGE = 64      # positions per KV page: one key tile of both attention kernels
+
+
+def _pool(k_pool: torch.Tensor, v_pool: torch.Tensor, table: torch.Tensor):
+    """Checks of a paged pool layer [n_pages, 64, Hkv, D] pair and its table [rows, W] int32; returns (n_pages, Hkv, D, W)."""
+    _cuda(k_pool, BF16, "k_pool"), _cuda(v_pool, BF16, "v_pool"), _cuda(table, torch.int32, "table")
+    if k_pool.dim() != 4 or k_pool.shape[1] != PAGE or not k_pool.is_contiguous():
+        raise ValueError(f"k_pool must be a contiguous pool layer [n_pages, {PAGE}, Hkv, D], got {tuple(k_pool.shape)}")
+    if v_pool.shape != k_pool.shape or not v_pool.is_contiguous():
+        raise ValueError("k_pool / v_pool must be contiguous pool layers of the same shape")
+    if table.dim() != 2 or table.stride(1) != 1:
+        raise ValueError(f"table must be [rows, W] int32 with unit column stride, got {tuple(table.shape)}")
+    n_pages, _, Hkv, D = k_pool.shape
+    return n_pages, Hkv, D, table.shape[1]
+
+
+def attention_paged(q: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor, out: torch.Tensor, Hq: int, scale: float,
+                    table: torch.Tensor, kv_len: torch.Tensor) -> torch.Tensor:
+    """Decode attention through a page table (``uvx_attention_paged``): q [B, Hq * D] (rows of any stride), one pool layer
+    k_pool / v_pool [n_pages, 64, Hkv, D], table [>= B, W] int32 (row b: the pages of batch row b's key tiles), kv_len [B] int32
+    -> out [B, Hq * D].  Row b sees keys [0, kv_len[b]); bit-identical to ``attention`` on a contiguous cache holding them."""
+    _cuda(q, BF16, "q"), _cuda(out, BF16, "out")
+    n_pages, Hkv, D, W = _pool(k_pool, v_pool, table)
+    B = q.shape[0]
+    if q.dim() != 2 or q.shape[1] != Hq * D or q.stride(1) != 1 or out.shape != (B, Hq * D) or out.stride(1) != 1:
+        raise ValueError(f"q / out must be [B, {Hq * D}] with unit column stride")
+    if table.shape[0] < B:
+        raise ValueError(f"table has {table.shape[0]} rows for {B} batch rows")
+    _rows(kv_len, torch.int32, B, "kv_len")
+    a = AttnArgs()
+    a.q, a.k, a.v, a.o = q.data_ptr(), k_pool.data_ptr(), v_pool.data_ptr(), out.data_ptr()
+    a.B, a.Hq, a.Hkv, a.Sq, a.Skv, a.D = B, Hq, Hkv, 1, W * PAGE, D
+    (a.q_rs, a.q_bs, a.k_rs, a.k_bs, a.v_rs, a.v_bs, a.o_rs, a.o_bs) = (q.stride(0), q.stride(0), Hkv * D, PAGE * Hkv * D, Hkv * D,
+                                                                        PAGE * Hkv * D, out.stride(0), out.stride(0))
+    a.kv_len = kv_len.data_ptr()
+    a.kv_start = None
+    a.causal, a.block, a.scale = 0, 0, float(scale)
+    check(lib().uvx_attention_paged(C.byref(a), table.data_ptr(), table.stride(0), _stream()), "uvx_attention_paged")
+    return out
+
+
+def attention_indexed_paged(q: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor, out: torch.Tensor, Hq: int, scale: float,
+                            table: torch.Tensor, kv_row: torch.Tensor, past: torch.Tensor, kv_len: torch.Tensor) -> torch.Tensor:
+    """``attention_indexed`` through a page table (``uvx_attention_indexed_paged``): q [B, Sq, Hq * D], one pool layer
+    k_pool / v_pool [n_pages, 64, Hkv, D], table [rows, W] int32; kv_row [B] (a table row) / past / kv_len [B] int32 on the
+    device -> out [B, Sq, Hq * D].  Bit-identical to ``attention_indexed`` on a contiguous cache holding the same keys."""
+    _cuda(q, BF16, "q"), _cuda(out, BF16, "out")
+    n_pages, Hkv, D, W = _pool(k_pool, v_pool, table)
+    B, Sq = q.shape[0], q.shape[1]
+    if q.shape[2] != Hq * D or q.stride(2) != 1 or out.shape != (B, Sq, Hq * D) or out.stride(2) != 1:
+        raise ValueError(f"q / out must be [B, Sq, {Hq * D}] with unit column stride")
+    for t, name in ((kv_row, "kv_row"), (past, "past"), (kv_len, "kv_len")):
+        _rows(t, torch.int32, B, name)
+    a = AttnArgs()
+    a.q, a.k, a.v, a.o = q.data_ptr(), k_pool.data_ptr(), v_pool.data_ptr(), out.data_ptr()
+    a.B, a.Hq, a.Hkv, a.Sq, a.Skv, a.D = B, Hq, Hkv, Sq, W * PAGE, D
+    (a.q_rs, a.q_bs, a.k_rs, a.k_bs, a.v_rs, a.v_bs, a.o_rs, a.o_bs) = (q.stride(1), q.stride(0), Hkv * D, PAGE * Hkv * D, Hkv * D,
+                                                                        PAGE * Hkv * D, out.stride(1), out.stride(0))
+    a.kv_len = kv_len.data_ptr()
+    a.kv_start = None
+    a.causal, a.block, a.scale = 1, 0, float(scale)
+    check(lib().uvx_attention_indexed_paged(C.byref(a), n_pages, table.data_ptr(), table.stride(0), kv_row.data_ptr(), past.data_ptr(),
+                                            _stream()), "uvx_attention_indexed_paged")
+    return out
+
+
+def kv_page_map(table: torch.Tensor, cache_row: torch.Tensor, pos: torch.Tensor, page_out: torch.Tensor, off_out: torch.Tensor,
+                frozen: Optional[torch.Tensor] = None) -> None:
+    """(table row cache_row[r], position pos[r]) -> (page_out[r], off_out[r]) through ``table`` [rows, W] int32; cache_row < 0,
+    or frozen[r] != 0 for the first frozen.numel() rows, gives (-1, 0).  All int32 on the device (``uvx_kv_page_map``)."""
+    _cuda(table, torch.int32, "table")
+    if table.dim() != 2 or table.stride(1) != 1:
+        raise ValueError("table must be [rows, W] int32 with unit column stride")
+    R = cache_row.shape[0]
+    for t, name in ((cache_row, "cache_row"), (pos, "pos"), (page_out, "page_out"), (off_out, "off_out")):
+        _rows(t, torch.int32, R, name)
+    nf = 0
+    if frozen is not None:
+        nf = frozen.numel()
+        _rows(frozen, torch.int32, nf, "frozen")
+        if nf > R:
+            raise ValueError(f"{nf} frozen flags for {R} rows")
+    check(lib().uvx_kv_page_map(table.data_ptr(), table.stride(0), cache_row.data_ptr(), pos.data_ptr(), _p(frozen), nf, R,
+                                page_out.data_ptr(), off_out.data_ptr(), _stream()), "uvx_kv_page_map")
+
+
+def kv_pages_copy(k_row: torch.Tensor, v_row: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor, pages: torch.Tensor,
+                  p0: int, p1: int, to_pages: bool) -> None:
+    """Positions [p0, p1) of every layer, K and V, between a contiguous one-row cache [L, 1, S_max, Hkv, D] and the pool
+    [L, n_pages, 64, Hkv, D] (``uvx_kv_pages_copy``): position p lives in page pages[p // 64] (int32 on the device), row p % 64.
+    ``to_pages``: row -> pages (scatter), else pages -> row (gather).  Bit-exact."""
+    for t, name in ((k_row, "k_row"), (v_row, "v_row"), (k_pool, "k_pool"), (v_pool, "v_pool")):
+        _cuda(t, BF16, name)
+        if not t.is_contiguous() or t.dim() != 5:
+            raise ValueError(f"{name} must be a contiguous 5-D cache")
+    _cuda(pages, torch.int32, "pages")
+    L, one, smax, Hkv, D = k_row.shape
+    if one != 1 or v_row.shape != k_row.shape:
+        raise ValueError(f"k_row / v_row must be one-row caches [L, 1, S_max, Hkv, D], got {tuple(k_row.shape)}")
+    if k_pool.shape[0] != L or k_pool.shape[2:] != (PAGE, Hkv, D) or v_pool.shape != k_pool.shape:
+        raise ValueError(f"k_pool / v_pool must be [{L}, n_pages, {PAGE}, {Hkv}, {D}], got {tuple(k_pool.shape)}")
+    if not 0 <= p0 <= p1 <= smax or pages.numel() * PAGE < p1:
+        raise ValueError(f"positions [{p0}, {p1}) outside the row ({smax}) or the page list ({pages.numel()} pages)")
+    check(lib().uvx_kv_pages_copy(k_row.data_ptr(), v_row.data_ptr(), smax * Hkv * D, k_pool.data_ptr(), v_pool.data_ptr(),
+                                  k_pool.shape[1] * PAGE * Hkv * D, L, Hkv * D, pages.data_ptr(), int(p0), int(p1), int(bool(to_pages)),
+                                  _stream()), "uvx_kv_pages_copy")
+
+
 def attention_fused_qkv(qkv: torch.Tensor, B: int, S: int, Hq: int, Hkv: int, D: int, scale: float, causal: bool,
                         kv_len: Optional[torch.Tensor] = None, block: int = 0,
                         out: Optional[torch.Tensor] = None, kv_start: Optional[torch.Tensor] = None) -> torch.Tensor:
