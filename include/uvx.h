@@ -125,6 +125,19 @@ typedef struct uvx_gemm_args {
   int32_t w_perm;           /* row order inside the tiles of a w_tiled = 128 image: 0 = plain, 1 = UVX_TILE_ROPE_PAIRS          */
 } uvx_gemm_args;
 
+/* Contracts of uvx_gemm_bf16 (pinned per element by tests/test_gemm_gpu.py):
+ *  - workspace: its contents on entry do not matter.  Every partial sum the reduce reads was written by the same call, so a
+ *    workspace full of NaN gives the same bits as a zeroed one.
+ *  - accumulation: fp32, K summed in k-block order within a split and the splits summed in split order; the tile width, the
+ *    cluster shape, the grid and the epilogue form (registers or the staged shared-memory tile) never change a bit.
+ *  - epilogue rounding order (plain): v = acc * alpha, v += bias, v = GELU(v), v += R, all in fp32, then ONE round-to-nearest-even
+ *    to bf16 at the store (fp32 output: no rounding).  The fused SwiGLU rounds gate * alpha and up * alpha to bf16, silu(gate)
+ *    to bf16, and the product once more; the fused RoPE rounds the projection to bf16 and rotates it in fp32 with every
+ *    product and sum rounded (o1 = x1 cos - x2 sin, o2 = x2 cos + x1 sin, no FMA), then rounds once; the fused RMSNorm writes
+ *    norm_out = norm_w * bf16(bf16(C) * rsqrt(mean(bf16(C)^2) + eps)), the bits uvx_rmsnorm gives on the finished rows.
+ *  - GELU: the split-K reduce evaluates it with erff (gelu_erf); the direct, staged and decode-form epilogues use the
+ *    Abramowitz-Stegun 7.1.26 form with ex2 / rcp approximations (|error| <= 7.5e-8 |x| plus fp32 roundings).  The same call can
+ *    therefore differ in its low bits between split counts, and so between configurations that pick different split counts. */
 int uvx_gemm_bf16(const uvx_gemm_args* args, uvx_stream_t stream);
 /* tuning hook: force tile config MT*1000+BN (MT in {1,2}, BN in {64,128,208,256}; 0 = heuristic) and split-K count (0 = heuristic) */
 int uvx_debug_gemm_override(int cfg, int splits);
