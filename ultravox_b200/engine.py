@@ -15,7 +15,7 @@ import torch
 import os
 
 from . import _lib, ops
-from .model import UltravoxModel
+from .model import KVCache, UltravoxModel
 
 GEMV_MAX_B = int(os.environ.get("UVX_GEMV_MAX_B", "1"))     # decode streams up to which the linears run as matrix-vector kernels
 # Rows up to which the LLM GEMMs stay on the weight-bound tiling (gemm_tc.cu pick_cfg: more rows take the tensor-bound tiles).
@@ -110,116 +110,198 @@ class PrefillEngine:
         return self._host_token
 
 
-class DecodeEngine:
-    """Token-by-token decoding after a prefill, the whole step (embedding -> 32/80 layers -> lm head -> logits processing ->
-    greedy / sampled pick -> EOS + sequence bookkeeping -> position bump) captured ONCE in a CUDA graph and replayed per token:
-    positions, KV lengths, the current token, the output sequence and the step counter all live on the device, so nothing in
-    the graph changes between steps and the host never has to synchronise inside the loop.  Linear layers are weight-streaming
-    matrix-vector kernels (uvx_gemv_bf16, slabs of 8 streams).  This is the serving loop of ``LocalInference._generate``
-    (ref:ultravox/inference/infer.py:309-342 -> ``GenerationMixin.generate``): greedy when ``temperature in {None, 0}``,
-    multinomial sampling otherwise (top-k, then top-p when ``top_p < 1``); repetition penalty as the reference pipeline sets it
-    (ref ultravox_pipeline.py:95-113); left-padded batches (``kv_start`` + mask-derived RoPE positions,
-    hf:generation/utils.py:707-729)."""
+class _RowKV:
+    """The KV cache as one ``[S_max]`` row per decode row (stream, beam or slot): ``cache`` [L, rows, S_max, Hkv, D]."""
 
-    def __init__(self, model: UltravoxModel, batch: int, max_len: int, use_graph: bool = True, cache=None,
-                 eos_token_ids=None, pad_token_id: int = 0, temperature: float = 0.0, top_k: int = 0,
-                 repetition_penalty: float = 1.0, generator: Optional[torch.Generator] = None, top_p: Optional[float] = None):
-        self.model, self.B = model, batch
+    keeps_kv = False        # whether a request's KV cache can outlive its slot (conversation sessions)
+
+    def __init__(self, cache: KVCache):
+        self.cache = cache
+
+    def map_rows(self, e: "_Decoder", R: int) -> None:
+        """Before the embedding of a step over R rows: a row's cache row is its own (or ``_mrow``'s), nothing to map."""
+
+    def attend(self, e: "_Decoder", li: int, qkv: torch.Tensor) -> torch.Tensor:
+        """The cache-touching calls of layer ``li`` of a step over the R rows of ``qkv``: RoPE on q / k + the KV append, then
+        attention of the B decode rows over their cache rows and, in a mixed step (R > B), of the chunk rows over the prefilling
+        slot's row -> [R, Hq * D].  A plain step appends row b at ``pos[b]`` of cache row b, a mixed step through ``_mrow``."""
+        nq, nkv, hd = e.heads
+        B, R = e.B, qkv.shape[0]
+        kc, vc = self.cache.k[li], self.cache.v[li]
+        smax = kc.shape[1]
+        if R == B:
+            ops.rope_kv_append_(qkv, nq, nkv, hd, e.cos, e.sin, e.rope_pos, kc, vc, e.pos)
+        else:
+            ops.rope_kv_append_map_(qkv, nq, nkv, hd, e.cos, e.sin, e._mrope, kc, vc, e._mrow, e._mpos)
+        att = torch.empty(R, nq * hd, dtype=torch.bfloat16, device=qkv.device)
+        rs = qkv.stride(0)
+        ops.attention(qkv.data_ptr(), kc.data_ptr(), vc.data_ptr(), att, B, nq, nkv, 1, smax, hd,
+                      (rs, rs, nkv * hd, smax * nkv * hd, nkv * hd, smax * nkv * hd, nq * hd, nq * hd), hd ** -0.5, False,
+                      e.lens, 0, e.kv_start)
+        if R > B:
+            ops.attention_indexed(qkv[B:, :nq * hd].unsqueeze(0), kc, vc, att[B:].unsqueeze(0), nq, hd ** -0.5, *e._mscal.split(1))
+        return att
+
+    def prefill(self, model: UltravoxModel, j: int, input_ids: torch.Tensor, past: int, features: dict) -> torch.Tensor:
+        """B = 1 prefill of a whole prompt into cache row ``j`` -> its last position's logits [1, V]."""
+        row = KVCache(self.cache.k[:, j:j + 1], self.cache.v[:, j:j + 1])
+        return model.forward(input_ids, past_key_values=row, logits_to_keep=1, **features).logits.view(1, -1)
+
+    def install(self, j: int, S: int, n: int, pages) -> None:
+        if pages is not None:
+            raise ValueError("this engine keeps its KV cache in slot rows, not pages (pages must be None)")
+
+    def release(self, j: int) -> None:
+        pass
+
+
+class _PagedKV:
+    """The KV cache as a shared pool of 64-position pages, so a request's K / V can outlive its slot.  K and V are
+    ``[L, kv_pages + slots, 64, Hkv, D]``: the ``kv_pages`` shareable pages, then one private idle page per slot (an idle row
+    writes its pad token at position 0 there, as a contiguous idle row does in its own row).  The page table
+    ``[slots, ceil(max_len / 64)]`` int32 lives on the device; the host writes a slot's row between replays (its pages at
+    ``install``, its idle page at ``release``).  A page is exactly one key tile of both attention kernels, so every step computes
+    the same bits as with ``_RowKV``: one ``uvx_kv_page_map`` launch per step turns each row's (slot, position) into
+    (page, offset) for the unchanged mapped RoPE + append, and the attention kernels read their key tiles through the table.
+    Rows that are done (finished, not yet retired) write nothing, so the last position a conversation keeps stays intact.
+
+    ``cache`` is the one-row admission scratch ``[L, 1, max_len, Hkv, D]``: a prompt prefilled at B = 1 gathers its
+    conversation's first ``past`` positions there, is prefilled like ``generate(past_key_values=...)``, and its new positions
+    are scattered into its pages."""
+
+    keeps_kv = True
+
+    def __init__(self, model: UltravoxModel, slots: int, max_len: int, kv_pages: int):
+        lm, tc = model.language_model, model.config.text_config
         dev = model.device
-        self.cache = cache if cache is not None else model.new_cache(batch, max_len)
+        if int(kv_pages) < 1:
+            raise ValueError(f"kv_pages must be >= 1, got {kv_pages}")
+        self.kv_pages = int(kv_pages)
+        self.table_width = -(-int(max_len) // ops.PAGE)
+        L, nkv, hd = tc.num_hidden_layers, tc.num_key_value_heads, lm.head_dim
+        self.pool_k = torch.empty(L, self.kv_pages + slots, ops.PAGE, nkv, hd, dtype=torch.bfloat16, device=dev)
+        self.pool_v = torch.empty_like(self.pool_k)
+        self.table = torch.full((slots, self.table_width), -1, dtype=torch.int32, device=dev)
+        R = max(slots, PREFILL_ROWS)        # the rows of a mixed step (slots decode rows + PREFILL_ROWS - slots chunk rows)
+        self.page = torch.zeros(R, dtype=torch.int32, device=dev)      # the page map's output: page / offset of every row
+        self.off = torch.zeros(R, dtype=torch.int32, device=dev)
+        self.cache = model.new_cache(1, max_len)
+        self.pages = None                   # the admitted request's pages on the device
+
+    def map_rows(self, e: "_Decoder", R: int) -> None:
+        ops.kv_page_map(self.table, e._mrow[:R], e._mpos[:R], self.page[:R], self.off[:R], frozen=e.done)
+
+    def attend(self, e: "_Decoder", li: int, qkv: torch.Tensor) -> torch.Tensor:
+        """``_RowKV.attend`` through the page map and the table: every row appends at its (page, offset)."""
+        nq, nkv, hd = e.heads
+        B, R = e.B, qkv.shape[0]
+        kp, vp = self.pool_k[li], self.pool_v[li]
+        ops.rope_kv_append_map_(qkv, nq, nkv, hd, e.cos, e.sin, e._mrope[:R], kp, vp, self.page[:R], self.off[:R])
+        att = torch.empty(R, nq * hd, dtype=torch.bfloat16, device=qkv.device)
+        ops.attention_paged(qkv[:B, :nq * hd], kp, vp, att[:B], nq, hd ** -0.5, self.table, e.lens)
+        if R > B:
+            ops.attention_indexed_paged(qkv[B:, :nq * hd].unsqueeze(0), kp, vp, att[B:].unsqueeze(0), nq, hd ** -0.5, self.table,
+                                        *e._mscal.split(1))
+        return att
+
+    def prefill(self, model: UltravoxModel, j: int, input_ids: torch.Tensor, past: int, features: dict) -> torch.Tensor:
+        """Gather [0, past) into the scratch row, prefill [past, S) there exactly as ``generate(past_key_values=...)`` does, scatter
+        [past, S) into the pages ``install`` gave slot ``j``."""
+        S = int(input_ids.shape[1])
+        row = self.cache
+        if past:
+            ops.kv_pages_copy(row.k, row.v, self.pool_k, self.pool_v, self.pages, 0, past, to_pages=False)
+            emb = model.prompt_embeds(input_ids, **features)       # embed + splice the whole prompt, prefill only the new suffix
+            out = model.forward(input_ids[:, past:], None, emb[:, past:].contiguous(), past_key_values=KVCache(row.k, row.v, past),
+                                logits_to_keep=1)
+        else:
+            out = model.forward(input_ids, past_key_values=KVCache(row.k, row.v), logits_to_keep=1, **features)
+        ops.kv_pages_copy(row.k, row.v, self.pool_k, self.pool_v, self.pages, past, S, to_pages=True)
+        return out.logits.view(1, -1)
+
+    def install(self, j: int, S: int, n: int, pages) -> None:
+        """Slot ``j``'s table row <- ``pages`` (page ids for positions 0, 64, 128, ...), which must cover its S + n positions."""
+        pages = list(pages or [])
+        if len(pages) * ops.PAGE < S + n or len(pages) > self.table_width:
+            raise ValueError(f"{len(pages)} pages for a prompt of {S} tokens plus max_new_tokens={n}")
+        self._set_table_row(j, pages)
+        self.pages = torch.tensor(pages, dtype=torch.int32).to(self.table.device, non_blocking=True)
+
+    def release(self, j: int) -> None:
+        self._set_table_row(j, [self.kv_pages + j])
+
+    def _set_table_row(self, j: int, pages) -> None:
+        row = torch.full((self.table_width,), -1, dtype=torch.int32)
+        row[:len(pages)] = torch.tensor(list(pages), dtype=torch.int32)
+        self.table[j].copy_(row.pin_memory(), non_blocking=True)
+
+
+class _Decoder:
+    """What every decode engine shares: the KV cache ``kv`` (``_RowKV`` or ``_PagedKV``; ``cache`` is its contiguous part), the
+    B decode rows' fed token, sequence, done flag and positions, the EOS ids, the RoPE tables, the step loop and its CUDA-graph
+    capture.  ``extra`` rows after the decode rows carry a prompt chunk in a mixed step: ``_mpos`` / ``_mrope`` hold the cache
+    position and the RoPE position of every row, ``pos`` / ``rope_pos`` are their decode part."""
+
+    def __init__(self, model: UltravoxModel, rows: int, kv, eos_token_ids, pad_token_id: int, use_graph: bool, extra: int = 0):
+        lm, tc = model.language_model, model.config.text_config
+        dev = model.device
+        i32 = dict(dtype=torch.int32, device=dev)
+        self.model, self.B, self.kv = model, rows, kv
+        self.cache = kv.cache
         self.max_len = self.cache.capacity
-        self.pos = torch.zeros(batch, dtype=torch.int32, device=dev)        # cache slot of the token being fed
-        self.lens = torch.zeros(batch, dtype=torch.int32, device=dev)       # keys visible to it (= pos + 1)
-        self.rope_pos = torch.zeros(batch, dtype=torch.int32, device=dev)   # its RoPE position (= pos - left padding)
+        self.heads = (tc.num_attention_heads, tc.num_key_value_heads, lm.head_dim)
+        self._mpos = torch.zeros(rows + extra, **i32)
+        self.pos = self._mpos[:rows]            # cache slot of the token being fed
+        self.lens = torch.zeros(rows, **i32)    # keys visible to it (= pos + 1)
+        self._mrope = torch.zeros(rows + extra, **i32)
+        self.rope_pos = self._mrope[:rows]      # its RoPE position (= pos - left padding)
         self.kv_start: Optional[torch.Tensor] = None
-        self.token = torch.zeros(batch, 1, dtype=torch.int64, device=dev)
-        self.seq = torch.zeros(batch, self.max_len + 1, dtype=torch.int64, device=dev)
-        self.cur_len = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.step_idx = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.done = torch.zeros(batch, dtype=torch.int32, device=dev)
-        self.all_done = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.token = torch.zeros(rows, 1, dtype=torch.int64, device=dev)
+        self.seq = torch.zeros(rows, self.max_len + 1, dtype=torch.int64, device=dev)
+        self.done = torch.zeros(rows, **i32)
         eos = sorted(set([eos_token_ids] if isinstance(eos_token_ids, int) else (eos_token_ids or [])))
         self.eos = torch.tensor(eos, dtype=torch.int64, device=dev) if eos else None
         self.pad_id = int(pad_token_id)
-        self.temperature, self.top_k = float(temperature or 0.0), int(top_k or 0)
-        self.top_p = 1.0 if top_p is None else float(top_p)         # a kernel argument of the captured step, like top_k
-        if not 0.0 <= self.top_p <= 1.0:
-            raise ValueError(f"top_p must be in [0, 1], got {top_p}")
-        self.penalty = float(repetition_penalty or 1.0)
-        self.u = None
-        if self.temperature > 0:
-            # one uniform per (step, stream), drawn up front from the caller's (seedable) generator: the graph reads row step_idx
-            self.u = torch.rand(self.max_len + 1, batch, device=dev, dtype=torch.float32, generator=generator)
-        self.scratch = torch.empty(batch, self.max_len + 1, dtype=torch.float32, device=dev) if self.penalty != 1.0 else None
         self.cos, self.sin = model._rope_tables(self.max_len + 1)
         self.graph = None
         self.use_graph = use_graph
         self.launches_per_step = 0
+        self.captures = 0
         self.logits = None
 
-    # -- state ---------------------------------------------------------------------------------------------
-    def begin(self, input_ids: torch.Tensor, first_logits: torch.Tensor, kv_start: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """After the prompt has been prefilled into ``self.cache`` (S = input_ids.shape[1] positions): seeds the sequence buffer
-        and the counters, picks the first new token from ``first_logits`` [B, V] fp32.  Returns the device token tensor [B]."""
-        B, S = input_ids.shape
-        if S + 1 > self.max_len + 1:
-            raise ValueError("prompt longer than the KV cache")
-        self.seq[:, :S].copy_(input_ids)
-        self.cur_len.fill_(S)
-        self.step_idx.zero_()
-        self.done.zero_()
-        self.all_done.zero_()
-        self.kv_start = kv_start
-        pad = kv_start if kv_start is not None else torch.zeros(B, dtype=torch.int32, device=self.pos.device)
-        # the pick's token_finish bumps all three by one: the first new token sits at slot S, sees S + 1 keys, RoPE S - pad
-        self.pos.fill_(S - 1)
-        self.lens.fill_(S)
-        self.rope_pos.copy_((S - 1) - pad.to(torch.int32))
-        self._pick(first_logits.contiguous())
-        return self.token.view(-1)
-
-    def prefill(self, inputs_embeds: torch.Tensor) -> torch.Tensor:
-        """Runs the prompt through the LLM, fills the cache, returns the first generated token [B] (greedy or sampled)."""
-        m = self.model
-        B, S, _ = inputs_embeds.shape
-        self.cache.length = 0
-        hid = m.llama_hidden(inputs_embeds, self.cache)
-        logits = ops.lm_head(hid[:, -1, :], m.language_model.lm_head.weight)
-        self.seq[:, :S].zero_()
-        return self.begin(self.seq[:, :S], logits).clone()
+    def _seed(self, rows, S: int, pad=0) -> None:
+        """Positions of ``rows`` whose first new token is picked next from a prompt of S positions: the pick's finish kernel
+        bumps pos, lens and rope_pos by one, so the token sits at slot S, sees S + 1 keys and has RoPE position S - pad."""
+        self.pos[rows] = S - 1
+        self.lens[rows] = S
+        self.rope_pos[rows] = (S - 1) - pad
 
     # -- one step ------------------------------------------------------------------------------------------
-    def _pick(self, logits: torch.Tensor):
-        """logits [B, V] fp32 -> self.token (+ sequence / EOS / counter bookkeeping), all on the device."""
-        self.logits = logits
-        if self.penalty != 1.0:
-            ops.repetition_penalty_(logits, self.seq, self.cur_len, self.penalty, self.scratch)
-        tok = self.token.view(-1)
-        if self.temperature > 0:
-            ops.sample(logits, self.temperature, self.top_k, self.u, self.step_idx, out=tok, top_p=self.top_p)
-        else:
-            ops.argmax(logits, out=tok)
-        ops.token_finish(tok, self.done, self.eos, self.pad_id, self.seq, self.cur_len, self.step_idx,
-                         (self.pos, self.lens, self.rope_pos), self.all_done)
-
-    def _step(self):
+    def _forward(self, mixed_in: Optional[torch.Tensor] = None, head_rows: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Embedding -> layers -> final norm -> LM head of a step -> fp32 logits.  A plain step (``mixed_in`` None) feeds the B
+        rows of ``token``.  A mixed step feeds ``mixed_in`` [R, D]: the token embedding is written into its first B rows, the
+        prompt-chunk rows follow, and the LM head runs over rows ``head_rows`` only."""
         m = self.model
         lm, tc = m.language_model, m.config.text_config
-        Dm = tc.hidden_size
         B = self.B
         # one stream: matrix-vector kernels (fp32 FMAs on the CUDA cores keep up with the weight stream) with RMSNorm / SwiGLU fused
         # into their prologues; more streams: the tensor-core GEMM (at B = 8 the FMA work per weight byte is 8x and the GEMV is
         # instruction-bound)
-        one = B <= GEMV_MAX_B
+        one = mixed_in is None and B <= GEMV_MAX_B
         eps = tc.rms_norm_eps
-        h = ops.embed_splice(self.token, lm.model.embed_tokens.weight, None, None).view(B, Dm)
+        self.kv.map_rows(self, B if mixed_in is None else mixed_in.shape[0])
+        if mixed_in is None:
+            h = ops.embed_splice(self.token, lm.model.embed_tokens.weight, None, None).view(B, tc.hidden_size)
+        else:
+            h = mixed_in
+            ops.embed_splice(self.token, lm.model.embed_tokens.weight, None, None, out=h[:B])
         for li, layer in enumerate(lm.model.layers):
             sa, mlp = layer.self_attn, layer.mlp
             if one:     # RMSNorm rides in the matrix-vector kernel's prologue
                 qkv = ops.gemv(h, sa.qkv_w, norm=(layer.input_layernorm.weight, eps))
             else:
                 qkv = ops.linear(ops.rmsnorm(h, layer.input_layernorm.weight, eps), sa.qkv_w)
-            att = self._attend(li, qkv)
+            att = self.kv.attend(self, li, qkv)
             if one:
                 h = ops.gemv(att, sa.o_proj.weight, residual=h)
                 gu = ops.gemv(h, mlp.gate_up_w, norm=(layer.post_attention_layernorm.weight, eps))
@@ -229,23 +311,13 @@ class DecodeEngine:
                 x = ops.rmsnorm(h, layer.post_attention_layernorm.weight, eps)
                 act = ops.swiglu(ops.linear(x, mlp.gate_up_w), gate_first=True)
                 h = ops.linear(act, mlp.down_proj.weight, residual=h)
+        if head_rows is not None:
+            h = ops.gather_rows(h, head_rows)
         hn = ops.rmsnorm(h, lm.model.norm.weight, eps)
-        self._pick(ops.lm_head(hn, lm.lm_head.weight))
+        return ops.lm_head(hn, lm.lm_head.weight)
 
-    def _attend(self, li: int, qkv: torch.Tensor) -> torch.Tensor:
-        """The two cache-touching calls of layer ``li`` of a step: RoPE on q / k + the KV append at ``pos``, then attention of the
-        B single-token queries over their cache rows -> [B, Hq * D]."""
-        lm, tc = self.model.language_model, self.model.config.text_config
-        nq, nkv, hd = tc.num_attention_heads, tc.num_key_value_heads, lm.head_dim
-        B, smax = self.B, self.cache.k.shape[2]
-        kc, vc = self.cache.k[li], self.cache.v[li]
-        ops.rope_kv_append_(qkv, nq, nkv, hd, self.cos, self.sin, self.rope_pos, kc, vc, self.pos)
-        att = torch.empty(B, nq * hd, dtype=torch.bfloat16, device=qkv.device)
-        rs = qkv.stride(0)
-        ops.attention(qkv.data_ptr(), kc.data_ptr(), vc.data_ptr(), att, B, nq, nkv, 1, smax, hd,
-                      (rs, rs, nkv * hd, smax * nkv * hd, nkv * hd, smax * nkv * hd, nq * hd, nq * hd), hd ** -0.5, False,
-                      self.lens, 0, self.kv_start)
-        return att
+    def _step(self):
+        self._pick(self._forward())
 
     def step(self) -> torch.Tensor:
         """Feeds ``self.token`` (the previous output), writes the next token into it; returns the device tensor."""
@@ -257,15 +329,13 @@ class DecodeEngine:
             self._step()
         return self.token
 
-    def _state(self):
-        return [self.pos, self.lens, self.rope_pos, self.token, self.cur_len, self.step_idx, self.done, self.all_done]
-
     def _step_warm(self):
         self.graph, self.launches_per_step = self._capture(self._step)
 
     def _capture(self, step):
         # warm-up on a scratch copy of the state, then capture; the state is restored so no token is lost (the cache row and the
         # sequence column the two trial steps write are rewritten with the same values by the first real step)
+        self.captures += 1
         saved = [t.clone() for t in self._state()]
         step()
         torch.cuda.synchronize()
@@ -280,6 +350,81 @@ class DecodeEngine:
             t.copy_(s0)
         torch.cuda.synchronize()
         return g, launches
+
+
+class DecodeEngine(_Decoder):
+    """Token-by-token decoding after a prefill, the whole step (embedding -> 32/80 layers -> lm head -> logits processing ->
+    greedy / sampled pick -> EOS + sequence bookkeeping -> position bump) captured ONCE in a CUDA graph and replayed per token:
+    positions, KV lengths, the current token, the output sequence and the step counter all live on the device, so nothing in
+    the graph changes between steps and the host never has to synchronise inside the loop.  Linear layers are weight-streaming
+    matrix-vector kernels (uvx_gemv_bf16, slabs of 8 streams).  This is the serving loop of ``LocalInference._generate``
+    (ref:ultravox/inference/infer.py:309-342 -> ``GenerationMixin.generate``): greedy when ``temperature in {None, 0}``,
+    multinomial sampling otherwise (top-k, then top-p when ``top_p < 1``); repetition penalty as the reference pipeline sets it
+    (ref ultravox_pipeline.py:95-113); left-padded batches (``kv_start`` + mask-derived RoPE positions,
+    hf:generation/utils.py:707-729)."""
+
+    def __init__(self, model: UltravoxModel, batch: int, max_len: int, use_graph: bool = True, cache=None,
+                 eos_token_ids=None, pad_token_id: int = 0, temperature: float = 0.0, top_k: int = 0,
+                 repetition_penalty: float = 1.0, generator: Optional[torch.Generator] = None, top_p: Optional[float] = None):
+        super().__init__(model, batch, _RowKV(cache if cache is not None else model.new_cache(batch, max_len)), eos_token_ids,
+                         pad_token_id, use_graph)
+        dev = model.device
+        self.cur_len = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.step_idx = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.all_done = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.temperature, self.top_k = float(temperature or 0.0), int(top_k or 0)
+        self.top_p = 1.0 if top_p is None else float(top_p)         # a kernel argument of the captured step, like top_k
+        if not 0.0 <= self.top_p <= 1.0:
+            raise ValueError(f"top_p must be in [0, 1], got {top_p}")
+        self.penalty = float(repetition_penalty or 1.0)
+        self.u = None
+        if self.temperature > 0:
+            # one uniform per (step, stream), drawn up front from the caller's (seedable) generator: the graph reads row step_idx
+            self.u = torch.rand(self.max_len + 1, batch, device=dev, dtype=torch.float32, generator=generator)
+        self.scratch = torch.empty(batch, self.max_len + 1, dtype=torch.float32, device=dev) if self.penalty != 1.0 else None
+
+    # -- state ---------------------------------------------------------------------------------------------
+    def begin(self, input_ids: torch.Tensor, first_logits: torch.Tensor, kv_start: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """After the prompt has been prefilled into ``self.cache`` (S = input_ids.shape[1] positions): seeds the sequence buffer
+        and the counters, picks the first new token from ``first_logits`` [B, V] fp32.  Returns the device token tensor [B]."""
+        B, S = input_ids.shape
+        if S + 1 > self.max_len + 1:
+            raise ValueError("prompt longer than the KV cache")
+        self.seq[:, :S].copy_(input_ids)
+        self.cur_len.fill_(S)
+        self.step_idx.zero_()
+        self.done.zero_()
+        self.all_done.zero_()
+        self.kv_start = kv_start
+        self._seed(slice(None), S, 0 if kv_start is None else kv_start.to(torch.int32))
+        self._pick(first_logits.contiguous())
+        return self.token.view(-1)
+
+    def prefill(self, inputs_embeds: torch.Tensor) -> torch.Tensor:
+        """Runs the prompt through the LLM, fills the cache, returns the first generated token [B] (greedy or sampled)."""
+        m = self.model
+        B, S, _ = inputs_embeds.shape
+        self.cache.length = 0
+        hid = m.llama_hidden(inputs_embeds, self.cache)
+        logits = ops.lm_head(hid[:, -1, :], m.language_model.lm_head.weight)
+        self.seq[:, :S].zero_()
+        return self.begin(self.seq[:, :S], logits).clone()
+
+    def _pick(self, logits: torch.Tensor):
+        """logits [B, V] fp32 -> self.token (+ sequence / EOS / counter bookkeeping), all on the device."""
+        self.logits = logits
+        if self.penalty != 1.0:
+            ops.repetition_penalty_(logits, self.seq, self.cur_len, self.penalty, self.scratch)
+        tok = self.token.view(-1)
+        if self.temperature > 0:
+            ops.sample(logits, self.temperature, self.top_k, self.u, self.step_idx, out=tok, top_p=self.top_p)
+        else:
+            ops.argmax(logits, out=tok)
+        ops.token_finish(tok, self.done, self.eos, self.pad_id, self.seq, self.cur_len, self.step_idx,
+                         (self.pos, self.lens, self.rope_pos), self.all_done)
+
+    def _state(self):
+        return [self.pos, self.lens, self.rope_pos, self.token, self.cur_len, self.step_idx, self.done, self.all_done]
 
 
 class BeamDecodeEngine(DecodeEngine):
@@ -402,12 +547,12 @@ class BeamDecodeEngine(DecodeEngine):
         return torch.where(keep, seq, torch.full_like(seq, fill_value)), self.pool_score[idx].clone()
 
 
-class SlotDecodeEngine(DecodeEngine):
-    """Continuous batching: ``slots`` decode rows that each carry their own request.  The step is the forward of
-    ``DecodeEngine._step`` over all rows followed by three per-row kernels (``uvx_repetition_penalty_slots``,
-    ``uvx_sample_slots``, ``uvx_slot_finish``); every per-request value - positions, lengths, budget, active / done flags,
-    sampling settings, the uniforms - lives in a device array [slots], so the step is captured once per engine and admission
-    and retirement only write into those arrays between replays.
+class SlotDecodeEngine(_Decoder):
+    """Continuous batching: ``slots`` decode rows that each carry their own request.  The step is the shared step loop over
+    all rows followed by three per-row kernels (``uvx_repetition_penalty_slots``, ``uvx_sample_slots``, ``uvx_slot_finish``);
+    every per-request value - positions, lengths, budget, active / done flags, sampling settings, the uniforms - lives in a
+    device array [slots], so the step is captured once per engine and admission and retirement only write into those arrays
+    between replays.
 
     An idle slot holds ``pos = 0``, ``lens = 1`` and the pad token: it writes its own K / V at position 0 and attends to that
     alone, so it stays finite whatever its cache row held.  A finished slot is frozen (no sequence writes, no position bumps)
@@ -426,11 +571,18 @@ class SlotDecodeEngine(DecodeEngine):
 
     def __init__(self, model: UltravoxModel, slots: int, max_len: int, eos_token_ids=None, pad_token_id: int = 0,
                  use_graph: bool = True, cache=None):
-        super().__init__(model, slots, max_len, use_graph=use_graph, cache=cache, eos_token_ids=eos_token_ids,
-                         pad_token_id=pad_token_id)
+        kv = _RowKV(cache if cache is not None else model.new_cache(slots, max_len))
+        self._setup(model, int(slots), kv, eos_token_ids, pad_token_id, use_graph)
+
+    def _setup(self, model: UltravoxModel, slots: int, kv, eos_token_ids, pad_token_id: int, use_graph: bool):
+        self.slots = slots
+        self.chunk = PREFILL_ROWS - slots
+        # mixed-step rows: [0, slots) decode rows, [slots, slots + chunk) prompt-chunk rows.  The host writes the chunk part of
+        # the per-row position arrays (_mpos, _mrope), the cache-row map, the attention scalars (cache row, past, past + valid)
+        # and the LM-head row list between replays.
+        super().__init__(model, slots, kv, eos_token_ids, pad_token_id, use_graph, extra=max(self.chunk, 0))
         dev = model.device
         i32, f32 = dict(dtype=torch.int32, device=dev), dict(dtype=torch.float32, device=dev)
-        self.slots = int(slots)
         self.cur_len = torch.zeros(slots, **i32)
         self.n_new = torch.zeros(slots, **i32)
         self.max_new = torch.ones(slots, **i32)
@@ -443,24 +595,16 @@ class SlotDecodeEngine(DecodeEngine):
         self.scratch = torch.empty(slots, self.max_len + 1, **f32)
         self.n_open = torch.zeros(1, **i32)
         self._admit_open = torch.zeros(1, **i32)     # the count an admission's one-row pick writes (not the step's)
-        # mixed-step rows: [0, slots) decode rows, [slots, slots + chunk) prompt-chunk rows.  pos / rope_pos are the decode part
-        # of the per-row position arrays the mixed step's RoPE + KV append reads; the host writes the chunk part, the cache-row
-        # map, the attention scalars (cache row, past, past + valid) and the LM-head row list between replays.
-        self.chunk = PREFILL_ROWS - self.slots
-        R = self.slots + max(self.chunk, 0)
-        self._mpos, self._mrope = torch.zeros(R, **i32), torch.zeros(R, **i32)
-        self.pos, self.rope_pos = self._mpos[:self.slots], self._mrope[:self.slots]
-        self._mrow = torch.arange(R, **i32)
+        self._mrow = torch.arange(self._mpos.shape[0], **i32)
         self._mscal = torch.zeros(3, **i32)
-        self._head_rows = torch.arange(self.slots + 1, **i32)
+        self._head_rows = torch.arange(slots + 1, **i32)
         self._mixed_in = None
         self._mixed_graph = None
         self._chunk_logits = None
         self._prefill: Optional[dict] = None
         self.launches_per_mixed_step = 0
-        self.captures = 0
-        self.busy = [False] * self.slots
-        for j in range(self.slots):
+        self.busy = [False] * slots
+        for j in range(slots):
             self._idle(j)
         if use_graph:
             self._step_warm()
@@ -475,13 +619,10 @@ class SlotDecodeEngine(DecodeEngine):
         self.rope_pos[j] = 0
         self.token[j] = self.pad_id
         self.busy[j] = False
+        self.kv.release(j)
 
     def _state(self):
         return [self.pos, self.lens, self.rope_pos, self.token, self.cur_len, self.n_new, self.done, self.n_open]
-
-    def _step_warm(self):
-        self.captures += 1
-        super()._step_warm()
 
     def _pick_rows(self, logits: torch.Tensor, r: slice, n_open: torch.Tensor) -> None:
         tok = self.token.view(-1)[r]
@@ -495,42 +636,9 @@ class SlotDecodeEngine(DecodeEngine):
         self._pick_rows(logits, slice(None), self.n_open)
 
     def _mixed_step(self):
-        """The forward of ``DecodeEngine._step`` (multi-stream form) over the decode rows and the prompt-chunk rows."""
-        m = self.model
-        lm, tc = m.language_model, m.config.text_config
-        B = self.slots
-        eps = tc.rms_norm_eps
-        h = self._mixed_in
-        ops.embed_splice(self.token, lm.model.embed_tokens.weight, None, None, out=h[:B])
-        for li, layer in enumerate(lm.model.layers):
-            sa, mlp = layer.self_attn, layer.mlp
-            qkv = ops.linear(ops.rmsnorm(h, layer.input_layernorm.weight, eps), sa.qkv_w)
-            att = self._attend_mixed(li, qkv)
-            h = ops.linear(att, sa.o_proj.weight, residual=h)
-            x = ops.rmsnorm(h, layer.post_attention_layernorm.weight, eps)
-            act = ops.swiglu(ops.linear(x, mlp.gate_up_w), gate_first=True)
-            h = ops.linear(act, mlp.down_proj.weight, residual=h)
-        hn = ops.rmsnorm(ops.gather_rows(h, self._head_rows), lm.model.norm.weight, eps)
-        logits = ops.lm_head(hn, lm.lm_head.weight)
-        self._chunk_logits = logits[B:]
-        self._pick(logits[:B])
-
-    def _attend_mixed(self, li: int, qkv: torch.Tensor) -> torch.Tensor:
-        """The cache-touching calls of layer ``li`` of a mixed step: mapped RoPE + KV append of every row, attention of the decode
-        rows over their cache rows and of the chunk rows over the prefilling slot's row -> [slots + chunk, Hq * D]."""
-        lm, tc = self.model.language_model, self.model.config.text_config
-        nq, nkv, hd = tc.num_attention_heads, tc.num_key_value_heads, lm.head_dim
-        B, R, smax = self.slots, self.slots + self.chunk, self.cache.k.shape[2]
-        kv_row, past, kv_len = self._mscal[0:1], self._mscal[1:2], self._mscal[2:3]
-        kc, vc = self.cache.k[li], self.cache.v[li]
-        ops.rope_kv_append_map_(qkv, nq, nkv, hd, self.cos, self.sin, self._mrope, kc, vc, self._mrow, self._mpos)
-        att = torch.empty(R, nq * hd, dtype=torch.bfloat16, device=qkv.device)
-        rs = qkv.stride(0)
-        ops.attention(qkv.data_ptr(), kc.data_ptr(), vc.data_ptr(), att, B, nq, nkv, 1, smax, hd,
-                      (rs, rs, nkv * hd, smax * nkv * hd, nkv * hd, smax * nkv * hd, nq * hd, nq * hd), hd ** -0.5, False,
-                      self.lens, 0, self.kv_start)
-        ops.attention_indexed(qkv[B:, :nq * hd].unsqueeze(0), kc, vc, att[B:].unsqueeze(0), nq, hd ** -0.5, kv_row, past, kv_len)
-        return att
+        logits = self._forward(self._mixed_in, self._head_rows)
+        self._chunk_logits = logits[self.B:]
+        self._pick(logits[:self.B])
 
     @property
     def prefilling(self) -> Optional[int]:
@@ -556,7 +664,6 @@ class SlotDecodeEngine(DecodeEngine):
         self._head_rows[B:].copy_(hv[2 * C + 3:], non_blocking=True)
         if self.use_graph:
             if self._mixed_graph is None:
-                self.captures += 1
                 self._mixed_graph, self.launches_per_mixed_step = self._capture(self._mixed_step)
             self._mixed_graph.replay()
         else:
@@ -565,23 +672,14 @@ class SlotDecodeEngine(DecodeEngine):
         if a + n == S:
             self._prefill = None
             self.active[j] = 1
-            # the pick's slot_finish bumps all three: the first new token sits at slot S, sees S + 1 keys, RoPE position S
-            self.pos[j] = S - 1
-            self.lens[j] = S
-            self.rope_pos[j] = S - 1
+            self._seed(j, S)
             self._mrow[j] = j
             self._pick_rows(self._chunk_logits, slice(j, j + 1), self._admit_open)
         return self.token
 
-    def begin(self, *args, **kwargs):
-        raise NotImplementedError("SlotDecodeEngine takes requests through admit()")
-
-    def prefill(self, *args, **kwargs):
-        raise NotImplementedError("SlotDecodeEngine takes requests through admit()")
-
     def admit(self, slot: int, input_ids: torch.Tensor, max_new_tokens: int, temperature: float = 0.0, top_k: int = 0,
               top_p: float = 1.0, repetition_penalty: float = 1.0, u: Optional[torch.Tensor] = None, past: int = 0,
-              **features) -> torch.Tensor:
+              pages=None, **features) -> torch.Tensor:
         """Prefills one request (``input_ids`` [1, S] plus the processor's audio features, passed to ``model.forward``) at B = 1
         into cache row ``slot``, sets the slot's state and picks its first token from the prefill logits with the slot kernels.
         ``temperature <= 0`` is greedy; a sampled request reads ``u`` (its uniforms, one per step, as ``generate()`` draws them
@@ -593,7 +691,9 @@ class SlotDecodeEngine(DecodeEngine):
 
         ``past`` > 0 (engines that keep a conversation's KV cache, ``PagedSlotDecodeEngine``): the slot's cache already holds the
         first ``past`` positions of ``input_ids``, so only the suffix is prefilled, as ``generate(past_key_values=...)`` does; the
-        chunked form then starts at ``past`` and is taken when the suffix has more than ``PREFILL_ROWS`` rows."""
+        chunked form then starts at ``past`` and is taken when the suffix has more than ``PREFILL_ROWS`` rows.  ``pages``
+        (``PagedSlotDecodeEngine`` only): the request's page ids for positions 0, 64, 128, ...; they must cover
+        S + max_new_tokens positions, and the first ceil(past / 64) of them hold the conversation's first ``past`` positions."""
         j = int(slot)
         if not 0 <= j < self.slots:
             raise ValueError(f"slot {slot} out of range [0, {self.slots})")
@@ -606,7 +706,7 @@ class SlotDecodeEngine(DecodeEngine):
             raise ValueError(f"a prompt of {S} tokens plus max_new_tokens={n} does not fit a slot of {self.max_len} positions")
         if not 0 <= P < S:
             raise ValueError(f"past = {P}: the prompt of {S} tokens must extend the cached prefix")
-        if P and not self.keeps_kv:
+        if P and not self.kv.keeps_kv:
             raise ValueError("this engine keeps no KV cache between requests (past must be 0)")
         if temperature > 0 and (u is None or u.numel() < S + n):
             raise ValueError(f"a sampled request needs at least {S + n} uniforms")
@@ -616,6 +716,7 @@ class SlotDecodeEngine(DecodeEngine):
                              f"{self.slots} slots leave none")
         if chunked and self._prefill is not None:
             raise ValueError(f"slot {self._prefill['slot']} is still prefilling; one long prompt at a time")
+        self.kv.install(j, S, n, pages)
         dev = self.pos.device
         input_ids = input_ids.to(dev)
         if chunked:
@@ -625,7 +726,7 @@ class SlotDecodeEngine(DecodeEngine):
             self._prefill = dict(slot=j, S=S, done=P, embeds=embeds)
             self._mrow[j] = -1          # the slot's idle decode row must not overwrite position 0 of the prompt
         else:
-            logits = self._prefill_one(j, input_ids, P, features)
+            logits = self.kv.prefill(self.model, j, input_ids, P, features)
         self.seq[j, :S].copy_(input_ids[0])
         self.cur_len[j] = S
         self.n_new[j] = 0
@@ -633,10 +734,7 @@ class SlotDecodeEngine(DecodeEngine):
         self.done[j] = 0
         if not chunked:
             self.active[j] = 1
-            # the pick's slot_finish bumps all three: the first new token sits at slot S, sees S + 1 keys, RoPE position S
-            self.pos[j] = S - 1
-            self.lens[j] = S
-            self.rope_pos[j] = S - 1
+            self._seed(j, S)
         self.temps[j] = float(temperature) if temperature > 0 else 0.0
         self.top_ks[j] = int(top_k or 0)
         self.top_ps[j] = float(top_p)
@@ -648,14 +746,6 @@ class SlotDecodeEngine(DecodeEngine):
         if not chunked:
             self._pick_rows(logits, slice(j, j + 1), self._admit_open)
         return self.token.view(-1)
-
-    keeps_kv = False        # whether a request's KV cache can outlive its slot (conversation sessions)
-
-    def _prefill_one(self, j: int, input_ids: torch.Tensor, past: int, features: dict) -> torch.Tensor:
-        """B = 1 prefill of a whole prompt into cache row ``j`` -> its last position's logits [1, V]."""
-        from .model import KVCache
-        row = KVCache(self.cache.k[:, j:j + 1], self.cache.v[:, j:j + 1])
-        return self.model.forward(input_ids, past_key_values=row, logits_to_keep=1, **features).logits.view(1, -1)
 
     def retire(self, slot: int, length: Optional[int] = None) -> torch.Tensor:
         """The slot's sequence [1, prompt + new tokens] (a copy; ``length`` = its ``cur_len`` if the caller already read it, else
@@ -670,116 +760,17 @@ class SlotDecodeEngine(DecodeEngine):
 
 
 class PagedSlotDecodeEngine(SlotDecodeEngine):
-    """``SlotDecodeEngine`` whose KV cache is a shared pool of 64-position pages instead of one ``[max_len]`` row per slot, so a
-    request's K / V can outlive its slot: a conversation keeps its pages between turns and each turn prefills only its new suffix.
+    """``SlotDecodeEngine`` whose KV cache is a shared pool of ``kv_pages`` 64-position pages (``_PagedKV``) instead of one
+    ``[max_len]`` row per slot, so a request's K / V can outlive its slot: a conversation keeps its pages between turns and
+    each turn prefills only its new suffix.  Every step computes the same bits as the contiguous engine's.
 
-    The pool holds ``kv_pages`` shareable pages plus one private idle page per slot (an idle row writes its pad token at position
-    0 there, as the contiguous engine's idle row does in its own row): K and V are ``[L, kv_pages + slots, 64, Hkv, D]``.  The
-    page table ``[slots, ceil(max_len / 64)]`` int32 lives on the device; the host writes a slot's row between replays (its
-    pages at admission, its idle page at retirement).  A page is exactly one key tile of both attention kernels, so every step
-    computes the same bits as the contiguous engine: one ``uvx_kv_page_map`` launch per step turns each row's (slot, position)
-    into (page, offset) for the unchanged mapped RoPE + append, and the attention kernels read their key tiles through the table.
-    Rows that are done (finished, not yet retired) write nothing, so the last position a conversation keeps stays intact.
-
-    ``cache`` is the one-row admission scratch ``[L, 1, max_len, Hkv, D]``: a prompt of at most ``PREFILL_ROWS`` new rows
-    gathers its conversation's first ``past`` positions there, is prefilled at B = 1 like ``generate(past_key_values=...)``,
-    and its new positions are scattered into its pages.  Longer suffixes go through the mixed step from ``past`` on.  Page
-    ownership (which pages a request or a conversation holds) is the caller's bookkeeping (``serving.PagePool``)."""
-
-    keeps_kv = True
+    ``admit`` takes the request's ``pages``.  A prompt of at most ``PREFILL_ROWS`` new rows is prefilled at B = 1 in the
+    one-row scratch ``cache`` ``[L, 1, max_len, Hkv, D]`` and scattered into its pages; longer suffixes go through the mixed
+    step from ``past`` on.  Page ownership (which pages a request or a conversation holds) is the caller's bookkeeping
+    (``serving.PagePool``)."""
 
     def __init__(self, model: UltravoxModel, slots: int, max_len: int, kv_pages: int, eos_token_ids=None, pad_token_id: int = 0,
                  use_graph: bool = True):
-        lm, tc = model.language_model, model.config.text_config
-        dev = model.device
-        if int(kv_pages) < 1:
-            raise ValueError(f"kv_pages must be >= 1, got {kv_pages}")
-        self.kv_pages = int(kv_pages)
-        self.table_width = -(-int(max_len) // ops.PAGE)
-        L, nkv, hd = tc.num_hidden_layers, tc.num_key_value_heads, lm.head_dim
-        n = self.kv_pages + int(slots)
-        self.pool_k = torch.empty(L, n, ops.PAGE, nkv, hd, dtype=torch.bfloat16, device=dev)
-        self.pool_v = torch.empty_like(self.pool_k)
-        self.table = torch.full((int(slots), self.table_width), -1, dtype=torch.int32, device=dev)
-        R = int(slots) + max(PREFILL_ROWS - int(slots), 0)
-        self._pg_page = torch.zeros(R, dtype=torch.int32, device=dev)      # the page map's output: page / offset of every row
-        self._pg_off = torch.zeros(R, dtype=torch.int32, device=dev)
-        super().__init__(model, slots, max_len, eos_token_ids=eos_token_ids, pad_token_id=pad_token_id, use_graph=use_graph,
-                         cache=model.new_cache(1, max_len))
-
-    def idle_page(self, j: int) -> int:
-        return self.kv_pages + j
-
-    def _set_table_row(self, j: int, pages) -> None:
-        row = torch.full((self.table_width,), -1, dtype=torch.int32)
-        row[:len(pages)] = torch.tensor(list(pages), dtype=torch.int32)
-        self.table[j].copy_(row.pin_memory(), non_blocking=True)
-
-    def _idle(self, j: int) -> None:
-        super()._idle(j)
-        self._set_table_row(j, [self.idle_page(j)])
-
-    # -- the step: one page-map launch before the layers, then the forward with the paged cache calls ----------------------
-    def _step(self):
-        B = self.slots
-        ops.kv_page_map(self.table, self._mrow[:B], self.pos, self._pg_page[:B], self._pg_off[:B], frozen=self.done)
-        super()._step()
-
-    def _mixed_step(self):
-        ops.kv_page_map(self.table, self._mrow, self._mpos, self._pg_page, self._pg_off, frozen=self.done)
-        super()._mixed_step()
-
-    def _attend(self, li: int, qkv: torch.Tensor) -> torch.Tensor:
-        B = self.slots
-        return self._attend_rows(li, qkv, self._mrope[:B], self._pg_page[:B], self._pg_off[:B])
-
-    def _attend_mixed(self, li: int, qkv: torch.Tensor) -> torch.Tensor:
-        att = self._attend_rows(li, qkv, self._mrope, self._pg_page, self._pg_off)
-        B, nq, hd = self.slots, self.model.config.text_config.num_attention_heads, self.model.language_model.head_dim
-        ops.attention_indexed_paged(qkv[B:, :nq * hd].unsqueeze(0), self.pool_k[li], self.pool_v[li], att[B:].unsqueeze(0), nq,
-                                    hd ** -0.5, self.table, self._mscal[0:1], self._mscal[1:2], self._mscal[2:3])
-        return att
-
-    def _attend_rows(self, li, qkv, rope_pos, page, off) -> torch.Tensor:
-        """RoPE + append of every row of ``qkv`` into its (page, offset), then decode attention of the first ``slots`` rows."""
-        lm, tc = self.model.language_model, self.model.config.text_config
-        nq, nkv, hd = tc.num_attention_heads, tc.num_key_value_heads, lm.head_dim
-        B = self.slots
-        kp, vp = self.pool_k[li], self.pool_v[li]
-        ops.rope_kv_append_map_(qkv, nq, nkv, hd, self.cos, self.sin, rope_pos, kp, vp, page, off)
-        att = torch.empty(qkv.shape[0], nq * hd, dtype=torch.bfloat16, device=qkv.device)
-        ops.attention_paged(qkv[:B, :nq * hd], kp, vp, att[:B], nq, hd ** -0.5, self.table, self.lens)
-        return att
-
-    # -- admission ------------------------------------------------------------------------------------------------------------
-    def admit(self, slot: int, input_ids: torch.Tensor, max_new_tokens: int, temperature: float = 0.0, top_k: int = 0,
-              top_p: float = 1.0, repetition_penalty: float = 1.0, u: Optional[torch.Tensor] = None, past: int = 0,
-              pages=None, **features) -> torch.Tensor:
-        """``SlotDecodeEngine.admit`` into the pages ``pages`` (a list of page ids for positions 0, 64, 128, ...; it must cover
-        S + max_new_tokens positions, and its first ceil(past / 64) pages hold the conversation's first ``past`` positions)."""
-        j = int(slot)
-        S, n = int(input_ids.shape[1]), int(max_new_tokens)
-        pages = list(pages or [])
-        if len(pages) * ops.PAGE < S + n or len(pages) > self.table_width:
-            raise ValueError(f"{len(pages)} pages for a prompt of {S} tokens plus max_new_tokens={n}")
-        if not 0 <= j < self.slots or self.busy[j]:
-            raise ValueError(f"slot {slot} is out of range or busy")
-        self._set_table_row(j, pages)
-        self._pages_dev = torch.tensor(pages, dtype=torch.int32).to(self.pos.device, non_blocking=True)
-        return super().admit(j, input_ids, n, temperature, top_k, top_p, repetition_penalty, u, past=past, **features)
-
-    def _prefill_one(self, j: int, input_ids: torch.Tensor, past: int, features: dict) -> torch.Tensor:
-        """Gather [0, past) into the scratch row, prefill [past, S) there exactly as ``generate(past_key_values=...)`` does, scatter
-        [past, S) into the slot's pages."""
-        from .model import KVCache
-        m, S = self.model, int(input_ids.shape[1])
-        row = self.cache
-        if past:
-            ops.kv_pages_copy(row.k, row.v, self.pool_k, self.pool_v, self._pages_dev, 0, past, to_pages=False)
-            emb = m.prompt_embeds(input_ids, **features)       # embed + splice the whole prompt, prefill only the new suffix
-            out = m.forward(input_ids[:, past:], None, emb[:, past:].contiguous(), past_key_values=KVCache(row.k, row.v, past),
-                            logits_to_keep=1)
-        else:
-            out = m.forward(input_ids, past_key_values=KVCache(row.k, row.v), logits_to_keep=1, **features)
-        ops.kv_pages_copy(row.k, row.v, self.pool_k, self.pool_v, self._pages_dev, past, S, to_pages=True)
-        return out.logits.view(1, -1)
+        kv = _PagedKV(model, int(slots), max_len, kv_pages)
+        self.kv_pages, self.pool_k, self.pool_v = kv.kv_pages, kv.pool_k, kv.pool_v
+        self._setup(model, int(slots), kv, eos_token_ids, pad_token_id, use_graph)
