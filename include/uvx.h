@@ -85,6 +85,7 @@ int uvx_mel_to_timemajor(const float* mel, int64_t N, int n_mels, int64_t T, voi
 enum { UVX_ACT_NONE = 0, UVX_ACT_GELU = 1, UVX_ACT_SWIGLU = 2 };
 enum { UVX_DT_BF16 = 0, UVX_DT_F32 = 1 };
 enum { UVX_TILE_PLAIN = 0, UVX_TILE_ROPE_PAIRS = 1, UVX_TILE_GATE_UP_8 = 8, UVX_TILE_GATE_UP_16 = 16 };   /* uvx_tile_weight interleave */
+enum { UVX_GEMM_W_STATIC = 4 };   /* uvx_gemm_args.flags bit 2 */
 
 typedef struct uvx_gemm_args {
   const void* A;            /* bf16 */
@@ -121,7 +122,12 @@ typedef struct uvx_gemm_args {
   const float* rope_sin;
   const int32_t* rope_positions;
   int64_t rope_rows_per_seq, rope_pos_offset;
-  int32_t flags;            /* bit 1: never take the single-pass form for this call (bit 0 is accepted and ignored)           */
+  int32_t flags;            /* bit 1: never take the single-pass form for this call (bit 0 is accepted and ignored).
+                             * bit 2 (UVX_GEMM_W_STATIC): W is not written by any kernel that may still be running when this call
+                             *   starts - kernels launched with programmatic dependent launch begin before the previous kernel has
+                             *   finished, and its predecessor may be running too.  The call may then start its weight stream before
+                             *   waiting for the previous kernel.  Set it only for weights nothing in the stream writes (frozen
+                             *   pre-tiled images), never where weights change in-stream (adapter merges, training steps).        */
   int32_t w_perm;           /* row order inside the tiles of a w_tiled = 128 image: 0 = plain, 1 = UVX_TILE_ROPE_PAIRS          */
 } uvx_gemm_args;
 
@@ -151,6 +157,12 @@ int uvx_debug_gemm_ws(int enable, int mode, int grid);
  * residual is loaded by TMA ahead of the epilogue.  -1 (default) or > 0 = staged wherever it applies, 0 = register epilogue
  * everywhere.  Never changes the result bits. */
 int uvx_debug_gemm_tma_store(int on);
+/* tuning hook: the split ring.  Calls whose rows one m-tile covers (one batch, <= 256 rows, tiles at most 128 wide, no
+ * thread-block cluster cutting the A box) may stream W through a ring of their own, beside a ring of A boxes that hold only the
+ * rows that exist.  0 = one ring of A + W stages for every call; n >= 2 = split rings with n activation slots (at most 8) for
+ * every such call; -1 (default) = split rings with 5 activation slots where that leaves the W ring deeper than the one ring.
+ * uvx_debug_gemm_stages caps the weight ring.  Never changes the result bits. */
+int uvx_debug_gemm_split_ring(int a_stages);
 /* hooks of tuning knobs the Hopper kernel does not have (phase timestamps, L2 prefetch distance, pipeline isolation): accepted
  * for ABI compatibility, no effect */
 int uvx_debug_gemm_times(void* dev_buf);

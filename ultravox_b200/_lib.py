@@ -62,6 +62,7 @@ SIGNATURES = {
     "uvx_debug_gemm_stages": (C.c_int, [C.c_int]),
     "uvx_debug_gemm_times": (C.c_int, [c_vp]),
     "uvx_debug_gemm_tma_store": (C.c_int, [C.c_int]),
+    "uvx_debug_gemm_split_ring": (C.c_int, [C.c_int]),
     "uvx_debug_gemm_ws": (C.c_int, [C.c_int, C.c_int, C.c_int]),
     "uvx_debug_gemm_ws_times": (C.c_int, [C.c_void_p]),
     "uvx_tile_weight": (C.c_int, [c_vp, c_i64, c_i64, c_i64, c_i32, c_i32, c_vp, c_vp]),

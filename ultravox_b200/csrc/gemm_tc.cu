@@ -51,15 +51,22 @@ struct GemmParams {
   const int32_t* rope_pos;
   int64_t rope_rows_per_seq, rope_pos_offset;
   int rope_cols;
-  int stages;              // ring depth
-  int cm, cn;              // thread-block cluster of cm x cn tiles (1 x 1: no cluster); cm divides m_tiles * a_batch, cn n_tiles
+  int stages;              // ring depth (split ring: depth of the weight ring)
+  int a_stages;            // split ring (0: one ring of A box + W box stages): depth of the separate activation ring
+  int a_box_rows;          // rows of the A box (MT*128, or round8(a_rows) for a split ring)
+  int w_early;             // split ring: the weight lane issues its first ring round before griddepcontrol.wait
+  int cm, cn;           // thread-block cluster of cm x cn tiles (1 x 1: no cluster); cm divides m_tiles * a_batch, cn n_tiles
   int staged_bytes;        // staged epilogue (gemm_wg_kernel<., ., true>): its output tile in shared memory, between the ring and
                            // the barriers (0: register epilogue)
   int r_bcast;             // the residual has batch stride 0: its map (tmR) has no batch dimension
 };
 
 static constexpr int kSmemTotal = 227 * 1024;
-static constexpr int kMaxStages = 8;
+static constexpr int kMaxStages = 8;   // one ring of A + W stages, and the decode form's ring
+static constexpr int kMaxWStages = 16;  // split ring: weight ring (gemm_wg_kernel's full / empty barrier arrays have this many)
+static constexpr int kMaxAStages = 8;   // split ring: activation ring
+static constexpr int kBarBytes = 512;   // gemm_wg_kernel's barriers: 2 x kMaxWStages + 2 + 2 x kMaxAStages mbarriers
+static_assert((2 * kMaxWStages + 2 + 2 * kMaxAStages) * 8 <= kBarBytes, "barrier region");
 static constexpr int kGemmThreads = 384;  // producer warpgroup + two consumer warpgroups
 static constexpr int kPanelBytes = 128 * 128;  // staged output: 128 rows x 128 bytes (64 bf16 / 32 fp32 columns), 128B swizzle
 
@@ -68,7 +75,7 @@ struct WgLayout {
   static constexpr int kABytes = MT * 128 * kBK * 2;
   static constexpr int kWBytes = BN * kBK * 2;  // BN % 8 == 0: a whole number of 1 KB swizzle atoms
   static constexpr int kStageBytes = kABytes + kWBytes;
-  static constexpr int kRingMax = kSmemTotal - 1024 - 256;  // alignment slack + barriers
+  static constexpr int kRingMax = kSmemTotal - 1024 - kBarBytes;  // alignment slack + barriers
   static constexpr int kStages = kRingMax / kStageBytes > kMaxStages ? kMaxStages : kRingMax / kStageBytes;
   static constexpr int kAcc = BN / 2;  // fp32 accumulators per thread and 64-row sub-tile
   static_assert(kStages >= 2, "ring too shallow");
@@ -131,16 +138,31 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);  // 128B-swizzle atoms need 1 KB alignment
-  uint8_t* stage_c = smem + p.stages * L::kStageBytes;                             // staged output tile (1 KB aligned)
-  uint64_t* full_bar = (uint64_t*)(stage_c + p.staged_bytes);
-  uint64_t* empty_bar = full_bar + kMaxStages;
-  uint64_t* res_full = empty_bar + kMaxStages;  // staged: the tile's residual box has landed in stage_c
-  uint64_t* stage_free = res_full + 1;          // staged: the previous tile's TMA store has finished reading stage_c
+  // Ring geometry.  One ring (a_stages == 0): stage s holds the A box at s * kStageBytes and the W box kABytes after it, under
+  // one full and one empty barrier.  Split ring (one m-tile covers the rows of a single batch): an activation ring of a_stages
+  // slots of a_box_rows * 128 bytes, then a weight ring of `stages` slots of kWBytes, each ring with its own barriers and its
+  // own producer lane, so a weight load never waits for an activation slot.  The consumers' m64 MMAs still read MT * 128 rows of an
+  // A slot: rows a_box_rows .. MT * 128 - 1 come from whatever follows the slot (the next A slot, or the weight ring after the
+  // last one - inside the allocation).  Accumulator row r depends only on A row r, so the garbage reaches accumulator rows
+  // >= a_box_rows >= a_rows alone, and every epilogue (plain, SwiGLU, RoPE, split-K partial) skips rows >= a_rows.
+  // (the staged kernel and the 208 / 256-wide tiles - tensor-bound calls - never run it: their loops keep the one ring's code)
+  constexpr bool kSplitRing = !STAGED && BN <= 128;
+  const bool split_ring = kSplitRing && p.a_stages > 0;
+  const int stages = p.stages, a_stages = split_ring ? p.a_stages : stages;
+  const int a_box_bytes = p.a_box_rows * (kBK * 2);
+  const int a_stride = split_ring ? a_box_bytes : L::kStageBytes, w_stride = split_ring ? L::kWBytes : L::kStageBytes;
+  uint8_t* const w_ring = split_ring ? smem + a_stages * a_box_bytes : smem + L::kABytes;
+  uint8_t* stage_c = smem + (split_ring ? a_stages * a_box_bytes + stages * L::kWBytes : stages * L::kStageBytes);  // staged output tile
+  uint64_t* full_bar = (uint64_t*)(stage_c + p.staged_bytes);  // weight ring (one ring: the stage)
+  uint64_t* empty_bar = full_bar + kMaxWStages;
+  uint64_t* res_full = empty_bar + kMaxWStages;  // staged: the tile's residual box has landed in stage_c
+  uint64_t* stage_free = res_full + 1;           // staged: the previous tile's TMA store has finished reading stage_c
+  uint64_t* const a_full = split_ring ? stage_free + 1 : full_bar;  // activation ring (one ring: the stage's barriers)
+  uint64_t* const a_empty = split_ring ? a_full + kMaxAStages : empty_bar;
 
   const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   const int tiles_m_total = p.m_tiles * (int)p.a_batch;
   const int num_kb = (int)((p.K + kBK - 1) / kBK);
-  const int stages = p.stages;
   // Thread-block cluster of cm x cn tiles (rank r = rm * cn + rn), walked in lockstep: the cluster takes cluster units
   // (cluster tile, split) and CTA (rm, rn) computes m-tile gm * cm + rm and n-tile gn * cn + rn of cluster tile (gm, gn) with the
   // split's k range, so every member runs the same k-blocks in the same ring order.  It loads its 1/cn share of the A box and
@@ -156,9 +178,16 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int first_unit = blockIdx.x / csize, unit_step = gridDim.x / csize;
 
   if (threadIdx.x == 0) {
+    // one arrival per consumer warp of every CTA of the cluster on each empty barrier
     for (int s = 0; s < stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 8 * csize);  // one arrival per consumer warp of every CTA of the cluster
+      mbar_init(&empty_bar[s], 8 * csize);
+    }
+    if (split_ring) {
+      for (int s = 0; s < a_stages; ++s) {
+        mbar_init(&a_full[s], 1);
+        mbar_init(&a_empty[s], 8 * csize);
+      }
     }
     if (STAGED) {
       mbar_init(res_full, 1);
@@ -170,23 +199,28 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   // no CTA multicasts into a peer before the peer's barriers are initialised
   if (csize > 1) cluster_sync();
   else __syncthreads();
-  // set-up above overlapped the previous kernel's tail; its outputs are visible after griddepcontrol.wait
-  pdl_wait();
+  // the weight lane of a split ring streams W (or A and W: one ring), the activation lane A
+  const bool w_lane = wg == 0 && tid == 0, a_lane = split_ring && wg == 0 && tid == 32;
+  // set-up above overlapped the previous kernel's tail; its outputs are visible after griddepcontrol.wait.  W no kernel that may
+  // still be running writes (uvx_gemm_args.flags bit 2) is read before it: the weight lane's first ring round.
+  const bool w_early = split_ring && p.w_early && w_lane;
+  if (!w_early) pdl_wait();
 
   if (wg == 0) {
-    // ---- TMA producer (one thread); its warpgroup hands registers to the consumers' accumulators (128 x 40 + 256 x 232
-    // fits the 384 x 168 the CTA was launched with)
+    // ---- TMA producer lanes; their warpgroup hands registers to the consumers' accumulators (128 x 40 + 256 x 232 fits the
+    // 384 x 168 the CTA was launched with)
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-    if (tid == 0) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmW) : "memory");
+    if (w_lane || a_lane) {
+      const bool do_w = w_lane, do_a = split_ring ? a_lane : w_lane;
+      if (do_a) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
+      if (do_w) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmW) : "memory");
       // slices are whole 8-row (1 KB) swizzle atoms; each lands at its own offset of the box in every CTA of the mask
-      const int a_slice = MT * 128 / cn, w_slice = BN / cm;
+      const int a_slice = p.a_box_rows / cn, w_slice = BN / cm;
       const uint16_t row_mask = (uint16_t)(((1u << cn) - 1u) << (rm * cn));
       uint16_t col_mask = 0;
       for (int j = 0; j < cm; ++j) col_mask |= (uint16_t)(1u << (j * cn + rn));
-      int s = 0;
-      uint32_t ph = 0;
+      int s = 0, sa = 0, issued = 0;
+      uint32_t ph = 0, pha = 0;
       for (int unit = first_unit, tile_i = 0; unit < num_units; unit += unit_step, ++tile_i) {
         const int ctile = unit / p.splits, split = unit % p.splits;
         const int tm_idx = (ctile % cluster_tiles_m) * cm + rm;  // consecutive tiles share the W tile
@@ -204,19 +238,31 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         // tile's first k-block is loaded, which those MMAs need.
         const int r_kb = max(kb_begin, kb_end - stages);
         for (int kb = kb_begin; kb < kb_end; ++kb) {
-          mbar_wait(&empty_bar[s], ph ^ 1u);
-          uint8_t* sa = smem + s * L::kStageBytes;
-          // the whole stage lands in every CTA (own slices and the peers'); TMA zero fill counts toward the bytes
-          mbar_expect_tx(&full_bar[s], (uint32_t)L::kStageBytes);
-          uint8_t* da = sa + rn * a_slice * (kBK * 2);
-          if (cn > 1) tma_load_3d_mc(da, &tmA, kb * kBK, m0 + rn * a_slice, b, &full_bar[s], row_mask);
-          else tma_load_3d(da, &tmA, kb * kBK, m0, b, &full_bar[s]);
-          uint8_t* dw = sa + L::kABytes + rm * w_slice * (kBK * 2);
-          const int w0 = p.w_tiled ? 0 : kb * kBK;
-          const int w1 = (p.w_tiled ? wt_base + kb * BN : tn_idx * BN) + rm * w_slice;
-          if (cm > 1) tma_load_2d_mc(dw, &tmW, w0, w1, &full_bar[s], col_mask);
-          else tma_load_2d(dw, &tmW, w0, w1, &full_bar[s]);
+          // the whole box lands in every CTA (own slices and the peers'); TMA zero fill counts toward the bytes.  One ring: the
+          // weight lane loads both boxes of the stage, against one expect_tx of the stage's bytes.
+          if (do_w) {
+            if (w_early && issued++ == stages) pdl_wait();  // after the first ring round
+            mbar_wait(&empty_bar[s], ph ^ 1u);
+            mbar_expect_tx(&full_bar[s], (uint32_t)(split_ring ? L::kWBytes : L::kStageBytes));
+          }
+          if (do_a) {
+            if (split_ring) {
+              mbar_wait(&a_empty[sa], pha ^ 1u);
+              mbar_expect_tx(&a_full[sa], (uint32_t)a_box_bytes);
+            }
+            uint8_t* da = smem + sa * a_stride + rn * a_slice * (kBK * 2);
+            if (cn > 1) tma_load_3d_mc(da, &tmA, kb * kBK, m0 + rn * a_slice, b, &a_full[sa], row_mask);
+            else tma_load_3d(da, &tmA, kb * kBK, m0, b, &a_full[sa]);
+          }
+          if (do_w) {
+            uint8_t* dw = w_ring + s * w_stride + rm * w_slice * (kBK * 2);
+            const int w0 = p.w_tiled ? 0 : kb * kBK;
+            const int w1 = (p.w_tiled ? wt_base + kb * BN : tn_idx * BN) + rm * w_slice;
+            if (cm > 1) tma_load_2d_mc(dw, &tmW, w0, w1, &full_bar[s], col_mask);
+            else tma_load_2d(dw, &tmW, w0, w1, &full_bar[s]);
+          }
           if (++s == stages) { s = 0; ph ^= 1u; }
+          if (++sa == a_stages) { sa = 0; pha ^= 1u; }
           if (STAGED && p.R && kb == r_kb) {
             mbar_wait(stage_free, (uint32_t)(tile_i & 1) ^ 1u);
             const int n0 = tn_idx * BN, panels = (int)min((int64_t)BN, p.N - n0) / 64;
@@ -237,18 +283,18 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int warp = tid >> 5, lane = tid & 31;
   // hand ring slot `slot` back: to this CTA's producer, or to the producers of every CTA of the cluster (each may have
   // multicast a slice into it), one lane per CTA
-  auto release = [&](int slot) {
+  auto release = [&](uint64_t* bar) {
     __syncwarp();
     if (csize == 1) {
-      if (lane == 0) mbar_arrive(&empty_bar[slot]);
+      if (lane == 0) mbar_arrive(bar);
     } else if (lane < csize) {
-      mbar_arrive_cluster(&empty_bar[slot], (uint32_t)lane);
+      mbar_arrive_cluster(bar, (uint32_t)lane);
     }
   };
   // staged epilogue: consumer thread 0 issues the tile's TMA stores and tracks their completion
   auto store_thread = [&]() { return STAGED && threadIdx.x == 128; };
-  int s = 0;
-  uint32_t ph = 0;
+  int s = 0, sa = 0;
+  uint32_t ph = 0, pha = 0;
   for (int unit = first_unit; unit < num_units; unit += unit_step) {
     const int ctile = unit / p.splits, split = unit % p.splits;
     const int tm_idx = (ctile % cluster_tiles_m) * cm + rm;
@@ -260,15 +306,16 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int kb_end = min(num_kb, kb_begin + p.kb_per_split);
 
     float acc[MT][L::kAcc];
-    int prev = -1;
+    int prev = -1, prev_a = -1;
     for (int kb = kb_begin; kb < kb_end; ++kb) {
       mbar_wait(&full_bar[s], ph);
-      const uint32_t sa = smem_u32(smem + s * L::kStageBytes);
-      const uint64_t dw = make_wgmma_desc(sa + L::kABytes);
+      if (split_ring) mbar_wait(&a_full[sa], pha);
+      const uint32_t a_addr = smem_u32(smem + sa * a_stride);
+      const uint64_t dw = make_wgmma_desc(smem_u32(w_ring + s * w_stride));
       wgmma_fence();
 #pragma unroll
       for (int mt = 0; mt < MT; ++mt) {
-        const uint64_t da = make_wgmma_desc(sa + (mt * 128 + c * 64) * (kBK * 2));
+        const uint64_t da = make_wgmma_desc(a_addr + (mt * 128 + c * 64) * (kBK * 2));
 #pragma unroll
         for (int k = 0; k < kBK / 16; ++k)
           Wgmma<BN>::mma(acc[mt], da + (uint64_t)(2 * k), dw + (uint64_t)(2 * k), (kb > kb_begin || k > 0) ? 1u : 0u);
@@ -280,14 +327,20 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         bulk_wait_read0();
         mbar_arrive(stage_free);
       }
-      // one k-block of MMAs stays in flight; the slot read by the previous one is handed back to the producer
+      // one k-block of MMAs stays in flight; the slots read by the previous one are handed back to the producers
       wgmma_wait<1>();
-      if (prev >= 0) release(prev);
+      if (prev >= 0) {
+        release(&empty_bar[prev]);
+        if (split_ring) release(&a_empty[prev_a]);
+      }
       prev = s;
+      prev_a = sa;
       if (++s == stages) { s = 0; ph ^= 1u; }
+      if (++sa == a_stages) { sa = 0; pha ^= 1u; }
     }
     wgmma_wait<0>();
-    release(prev);
+    release(&empty_bar[prev]);
+    if (split_ring) release(&a_empty[prev_a]);
 
     // ---- epilogue from registers: this thread holds rows r0 (+8) of each 64-row sub-tile, columns 8j + 2(lane % 4) (+1)
     const int rq = warp * 16 + (lane >> 2);
@@ -827,6 +880,7 @@ static int num_sms() {
 static int g_gemm_stage_cap = 0;  // tuning only (uvx_debug_gemm_stages): upper bound on the ring depth
 static int g_grid_cap = 0;        // tuning only (uvx_debug_gemm_ws grid): upper bound on the persistent grid
 static int g_tma_store = -1;      // uvx_debug_gemm_tma_store: 0 = register epilogue everywhere, otherwise staged where it applies
+static int g_split_ring = -1;     // uvx_debug_gemm_split_ring: 0 = one ring everywhere, n >= 2 = n activation slots, -1 = default
 
 // after the main kernel: split-K reduce (fused RMSNorm where it applies) or the row norm of a direct epilogue
 static int finish_gemm(const uvx_gemm_args* a, const GemmParams& p, cudaStream_t stream) {
@@ -869,11 +923,27 @@ static int launch_gemm(const uvx_gemm_args* a, int splits, int cm, int cn, cudaS
   const int m_tiles = (int)((a->a_rows + MT * 128 - 1) / (MT * 128));
   const int n_tiles = (int)((a->N + BN - 1) / BN);
   legal_cluster(MT, BN, m_tiles * (int)a->a_batch, n_tiles, &cm, &cn);
+  // Split ring (weight-streaming prefill: one m-tile covers every row of the single batch, and no cluster cuts the A box): the
+  // A box holds only the rows that exist (rounded to a swizzle atom), and A and W get rings of their own.  The weight ring takes
+  // what the activation ring leaves (<2, 128> at M = 201: 5 x 26 KB + 5 x 16 KB, against 4 stages of 32 + 16 KB in one ring).
+  // The A box comes from L2, but its latency still needs a lead of 3 k-blocks (H100 80GB HBM3 at 700 W, gate|up at M = 201:
+  // 123.9 / 116.9 us with 3 / 4 stages of one ring, 102.4 / 101.8 / 103.7 us with 4 / 5 / 6 A slots).  It runs where the W ring
+  // gets deeper than the one ring: at 256 rows the box cannot shrink, 5 A slots leave 4 W slots, and gate|up takes 106.8 us
+  // against 102.1 us in one ring.  Where two m-tiles share the W box through a cluster (q|k|v at 129..256 rows) one ring is
+  // faster too (31.2 us, against 32.4 with 6 A slots).  scripts/prefill_gemm_ab.py measures these; DESIGN §3.
+  const int box_rows = (int)((a->a_rows + 7) / 8 * 8);
+  int split_a = g_split_ring > 0 ? (g_split_ring < kMaxAStages ? g_split_ring : kMaxAStages) : 5;
+  if (split_a < 2) split_a = 2;
+  int split_w = (L::kRingMax - split_a * box_rows * kBK * 2) / L::kWBytes;
+  if (split_w > kMaxWStages) split_w = kMaxWStages;
+  const bool split_ring = BN <= 128 && g_split_ring != 0 && a->a_batch == 1 && m_tiles == 1 && cn == 1 &&
+                          (g_split_ring > 0 || split_w > L::kStages);
+  const int a_box_rows = split_ring ? box_rows : MT * 128;
   CUtensorMap tmA, tmW;
   {
     uint64_t dims[3] = {(uint64_t)a->K, (uint64_t)a->a_rows, (uint64_t)a->a_batch};
     uint64_t st[2] = {(uint64_t)a->a_row_stride * 2, (uint64_t)(a->a_batch > 1 ? a->a_batch_stride : a->a_row_stride) * 2};
-    uint32_t box[3] = {kBK, (uint32_t)(MT * 128 / cn), 1};  // a CTA loads its 1/cn share of the A box
+    uint32_t box[3] = {kBK, (uint32_t)(a_box_rows / cn), 1};  // a CTA loads its 1/cn share of the A box
     int rc = encode_map(&tmA, a->A, 3, dims, st, box, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
     if (rc) return rc;
   }
@@ -931,6 +1001,7 @@ static int launch_gemm(const uvx_gemm_args* a, int splits, int cm, int cn, cudaS
   p.num_tiles = p.m_tiles * (int)a->a_batch * p.n_tiles;
   p.cm = cm;
   p.cn = cn;
+  p.a_box_rows = a_box_rows;
   const int num_kb = (int)((a->K + kBK - 1) / kBK);
   if (a->N % BN != 0) splits = 1;  // ragged column tiles exist only in the direct epilogue
   // split-K needs the caller's workspace: [splits][rows][N] fp32 partial sums
@@ -970,10 +1041,23 @@ static int launch_gemm(const uvx_gemm_args* a, int splits, int cm, int cn, cudaS
     }
     p.staged_bytes = BN / 64 * (p.out_f32 ? 2 : 1) * kPanelBytes;
   }
-  p.stages = (L::kRingMax - p.staged_bytes) / L::kStageBytes;
-  if (p.stages > L::kStages) p.stages = L::kStages;
-  if (g_gemm_stage_cap >= 2 && p.stages > g_gemm_stage_cap) p.stages = g_gemm_stage_cap;
-  const int smem = p.stages * L::kStageBytes + p.staged_bytes + 1024 + 2 * kMaxStages * 8 + 16;
+  int ring_bytes;
+  if (split_ring) {
+    // the MMAs' reads past the last activation slot (rows a_box_rows .. MT * 128 - 1) land in the weight ring
+    const int a_bytes = a_box_rows * kBK * 2;
+    p.a_stages = split_a;
+    p.stages = split_w;
+    if (g_gemm_stage_cap >= 2 && p.stages > g_gemm_stage_cap) p.stages = g_gemm_stage_cap;
+    UVX_REQUIRE(p.stages >= 2 && (MT * 128 - a_box_rows) * kBK * 2 <= p.stages * L::kWBytes, "uvx_gemm_bf16: split ring does not fit");
+    p.w_early = (a->flags & UVX_GEMM_W_STATIC) ? 1 : 0;
+    ring_bytes = p.a_stages * a_bytes + p.stages * L::kWBytes;
+  } else {
+    p.stages = (L::kRingMax - p.staged_bytes) / L::kStageBytes;
+    if (p.stages > L::kStages) p.stages = L::kStages;
+    if (g_gemm_stage_cap >= 2 && p.stages > g_gemm_stage_cap) p.stages = g_gemm_stage_cap;
+    ring_bytes = p.stages * L::kStageBytes;
+  }
+  const int smem = ring_bytes + p.staged_bytes + 1024 + kBarBytes;
   static bool attr_set[2] = {false, false};
   if (!attr_set[staged]) {
     cudaError_t e = staged ? set_smem_attr<MT, BN, true>() : set_smem_attr<MT, BN, false>();
@@ -1193,6 +1277,14 @@ extern "C" int uvx_debug_gemm_cluster(int cm, int cn) {
 // -1 (default) or > 0 = staged wherever it applies.  Never changes the result bits.
 extern "C" int uvx_debug_gemm_tma_store(int on) {
   uvx::g_tma_store = on;
+  return UVX_OK;
+}
+
+// tuning hook: the split weight / activation ring of calls one m-tile covers: 0 = the one ring of A + W stages, n >= 2 = split
+// with n activation slots (at most 8) wherever the shape allows, -1 (default) = split with 5 where the W ring gets deeper than
+// the one ring (launch_gemm).  Never changes the result bits.
+extern "C" int uvx_debug_gemm_split_ring(int a_stages) {
+  uvx::g_split_ring = a_stages;
   return UVX_OK;
 }
 

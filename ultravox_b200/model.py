@@ -484,6 +484,10 @@ class UltravoxModel(nn.Module):
                                         gate_up=ops.TiledWeight(mlp.gate_up_w, gu_rows, swiglu=True) if FUSE_SWIGLU
                                         else ops.TiledWeight(mlp.gate_up_w, gu_rows),
                                         down=ops.TiledWeight(mlp.down_proj.weight, 128) if down_t else None))
+                    # the prefill GEMMs read these images with ops.GEMM_W_STATIC (their weight stream starts before the previous
+                    # kernel ends): every image is complete before the first such call
+                    if not torch.cuda.is_current_stream_capturing():
+                        torch.cuda.current_stream(self.device).synchronize()
                     self._tiled = out
         return self._tiled or None
 
@@ -643,7 +647,7 @@ class UltravoxModel(nn.Module):
             sa, mlp = layer.self_attn, layer.mlp
             tw = tiled[li] if tiled is not None else None
             if tw is not None and tw["qkv"] is not None:
-                ops.linear_tiled(x, tw["qkv"], out=qkv, rope=rope)
+                ops.linear_tiled(x, tw["qkv"], out=qkv, rope=rope, flags=ops.GEMM_W_STATIC)
             else:
                 ops.linear(x, sa.qkv_w, out=qkv, rope=rope, flags=qkv_flags)
             if rope is None:
@@ -660,23 +664,23 @@ class UltravoxModel(nn.Module):
             # o_proj / down_proj write the residual stream AND the RMSNorm the next block reads (fused into split-K's pass 2)
             n1 = (layer.post_attention_layernorm.weight, eps, x) if FUSE_NORM else None
             if tw is not None and tw["o"] is not None:
-                ops.linear_tiled(att, tw["o"], residual=h, out=h, norm=n1)
+                ops.linear_tiled(att, tw["o"], residual=h, out=h, norm=n1, flags=ops.GEMM_W_STATIC)
             else:
                 ops.linear(att, sa.o_proj.weight, residual=h, out=h, norm=n1)
             if not FUSE_NORM:
                 ops.rmsnorm(h, layer.post_attention_layernorm.weight, eps, out=x)
             if fuse_act:
-                ops.linear_tiled(x, tw["gate_up"], out=act, act=ops.ACT_SWIGLU)      # silu(gate) * up straight from the accumulators
+                ops.linear_tiled(x, tw["gate_up"], out=act, act=ops.ACT_SWIGLU, flags=ops.GEMM_W_STATIC)   # silu(gate) * up from the accumulators
             else:
                 if tw is not None:
-                    ops.linear_tiled(x, tw["gate_up"], out=gu)
+                    ops.linear_tiled(x, tw["gate_up"], out=gu, flags=ops.GEMM_W_STATIC)
                 else:
                     ops.linear(x, mlp.gate_up_w, out=gu)
                 ops.swiglu(gu, gate_first=True, out=act)
             nxt = layers[li + 1].input_layernorm.weight if li + 1 < len(layers) else lm.model.norm.weight
             n2 = (nxt, eps, x) if FUSE_NORM else None
             if tw is not None and tw["down"] is not None:
-                ops.linear_tiled(act, tw["down"], residual=h, out=h, norm=n2)
+                ops.linear_tiled(act, tw["down"], residual=h, out=h, norm=n2, flags=ops.GEMM_W_STATIC)
             else:
                 ops.linear(act, mlp.down_proj.weight, residual=h, out=h, norm=n2)
             if not FUSE_NORM:

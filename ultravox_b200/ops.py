@@ -144,13 +144,16 @@ class TiledWeight:
 
 
 ACT_SWIGLU = 2
+GEMM_W_STATIC = 4   # uvx_gemm_args.flags bit 2 (UVX_GEMM_W_STATIC)
 
 
 def linear_tiled(x: torch.Tensor, wt: TiledWeight, out: Optional[torch.Tensor] = None, residual: Optional[torch.Tensor] = None,
-                 act: int = ACT_NONE, norm: Optional[tuple] = None, rope: Optional[tuple] = None) -> torch.Tensor:
+                 act: int = ACT_NONE, norm: Optional[tuple] = None, rope: Optional[tuple] = None, flags: int = 0) -> torch.Tensor:
     """y = x @ W.T (+ residual) over the pre-tiled weight image; ``act=ACT_SWIGLU`` -> y = silu(gate) * up [M, N/2] (needs a
     ``swiglu`` image); ``rope=(cos, sin, positions|None, rows_per_seq, pos_offset, rope_cols)`` rotates the q / k heads in the
-    epilogue (head_dim 128); ``norm`` as in ``linear``."""
+    epilogue (head_dim 128); ``norm`` as in ``linear``.  ``flags=GEMM_W_STATIC`` promises that no kernel still running in the
+    stream writes the image (a frozen image finished before the call), so the weight stream may start before the previous
+    kernel ends."""
     _cuda(x, BF16, "x")
     K = x.shape[-1]
     x2 = x.reshape(-1, K)
@@ -178,6 +181,7 @@ def linear_tiled(x: torch.Tensor, wt: TiledWeight, out: Optional[torch.Tensor] =
         a.norm_w, a.norm_eps, a.norm_out = norm[0].data_ptr(), float(norm[1]), norm[2].data_ptr()
     a.w_tiled = wt.R
     a.w_perm = 1 if wt.rope_pairs else 0
+    a.flags = flags
     if rope is not None:
         cos, sin, positions, rows_per_seq, pos_offset, rope_cols = rope
         a.rope_cos, a.rope_sin, a.rope_positions = cos.data_ptr(), sin.data_ptr(), _p(positions)
