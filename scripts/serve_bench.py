@@ -32,6 +32,16 @@ callback as soon as the previous reply arrives (its prompt: the conversation so 
 Per arm: wall time, tokens per second, TTFT p50 / p90 per turn index (from the turn's submission to its first token), plain
 and mixed step times; the sessions arm also reports the admission gather + scatter of 4096 positions at these widths.
 
+`--workload system-prompt`: 32 requests (`--requests`), each a fixed system prompt (the Llama 3.1 system header, then
+`--prefix-tokens` seeded random text ids, default 1024), then a user turn with one 5 or 10 s clip between 8 and 5 text tokens,
+and the assistant header; budgets 16-256.  Arms (`SlotScheduler(kv_pages=N)`, 8 slots):
+- paged: prefix cache off, so every request prefills its whole prompt (over 256 rows: in chunks inside the decode steps);
+- prefix: `prefix_cache=True`, so requests after the first take the system prompt's full pages from the cache and prefill
+  only the rest.
+Per arm: wall time, tokens per second, TTFT p50 / p90, the prompt rows prefilled, the positions each request took from the
+cache, plain and mixed step counts and times.  After the rounds, one more `prefix` run over four different system prompts
+with a pool too small to keep them all cached shows that eviction serves every request.
+
 Prints the device name and power limit first, then one JSON line per arm."""
 import argparse, json, os, statistics, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -190,6 +200,80 @@ def main_conversations(args, model, cfg):
         print(json.dumps(line), flush=True)
 
 
+# Llama 3.1 chat template ids: <|begin_of_text|><|start_header_id|>system<|end_header_id|>\n\n ... <|eot_id|>, the user header
+# and the assistant header
+SYS_HEAD, EOT = [128000, 128006, 9125, 128007, 271], 128009
+USER_HEAD, ASSISTANT_HEAD = [128006, 882, 128007, 271], [128006, 78191, 128007, 271]
+
+
+def make_system_prompt_requests(cfg, n, prefix_tokens, seed, n_prompts=1):
+    """n requests: one of ``n_prompts`` system prompts, then a user turn with a 5 or 10 s clip; (features, budget) each."""
+    rng = np.random.default_rng(seed)
+    g = torch.Generator().manual_seed(seed)
+    prompts = [SYS_HEAD + torch.randint(0, 128000, (prefix_tokens,), generator=g).tolist() + [EOT] + USER_HEAD
+               for _ in range(n_prompts)]
+    reqs = []
+    for i in range(n):
+        head = prompts[i % n_prompts]
+        wave = torch.from_numpy(rng.standard_normal(int(rng.choice([5, 10])) * SR).astype(np.float32)).cuda()
+        mel = ops.logmel(wave[None], cfg.audio_config.num_mel_bins)
+        tok = -(-mel.shape[-1] // 16)
+        text = torch.randint(0, 128000, (PRE + tok + POST,), generator=g).tolist()
+        ids = torch.tensor([head + text + [EOT] + ASSISTANT_HEAD]).cuda()
+        reqs.append(dict(feats=dict(input_ids=ids, audio_values=mel, audio_token_start_idx=torch.tensor([len(head) + PRE]).cuda(),
+                                    audio_lens=torch.tensor([mel.shape[-1]]).cuda(),
+                                    audio_token_len=torch.tensor([tok], dtype=torch.int32).cuda(),
+                                    audio_batch_size=torch.tensor([1]).cuda()),
+                         budget=int(rng.integers(16, 257))))
+    return reqs
+
+
+def main_system_prompt(args, model, cfg):
+    from ultravox_b200.serving import SlotScheduler, pages_for
+    reqs = make_system_prompt_requests(cfg, args.requests, args.prefix_tokens, args.seed)
+    useful = sum(r["budget"] for r in reqs)
+    rows = sum(r["feats"]["input_ids"].shape[1] for r in reqs)
+    longest = max(r["feats"]["input_ids"].shape[1] + r["budget"] for r in reqs)
+    max_len = pages_for(longest) * ops.PAGE
+    kv_pages = args.kv_pages or 8 * pages_for(max_len) + pages_for(args.prefix_tokens)
+    scheds = {"paged": SlotScheduler(model, slots=8, max_len=max_len, kv_pages=kv_pages),
+              "prefix": SlotScheduler(model, slots=8, max_len=max_len, kv_pages=kv_pages, prefix_cache=True)}
+    warm = [dict(r, budget=16) for r in reqs[:8]]
+    for sched in scheds.values():
+        run_slots(sched, warm)
+    out = {a: [] for a in scheds}
+    for _ in range(args.rounds):
+        for a, sched in scheds.items():
+            out[a].append(run_slots(sched, reqs))
+    for arm, runs in out.items():
+        walls = [r[0] for r in runs]
+        k = walls.index(sorted(walls)[len(walls) // 2])
+        wall, first, step, _, _, split, ids = runs[k]
+        sched = scheds[arm]
+        hits = [sched.cached_tokens.get(i, 0) for i in ids]
+        line = {"bench": f"serve {len(reqs)} requests, {args.prefix_tokens}-token system prompt + 5-10 s clip, 8B + large-v3, "
+                         f"budgets 16-256, greedy, 8 slots", "arm": arm,
+                "wall_s_median": wall, "wall_s_all": [round(w, 3) for w in walls], "useful_tokens": useful,
+                "tokens_per_s": useful / wall, "tokens_per_s_all": [round(useful / w, 1) for w in walls],
+                "ttft_ms_p50": pct(first, 50), "ttft_ms_p90": pct(first, 90),
+                "ttft_ms_p50_all": [round(pct(r[1], 50), 2) for r in runs], "ttft_ms_p90_all": [round(pct(r[1], 90), 2) for r in runs],
+                "prompt_rows": rows, "prefill_rows": rows - sum(hits), "cached_positions": hits,
+                "plain_step_ms_mean": statistics.fmean(split[False]) if split[False] else None, "plain_steps": len(split[False]),
+                "mixed_step_ms_mean": statistics.fmean(split[True]) if split[True] else None, "mixed_steps": len(split[True]),
+                "kv_pages": kv_pages, "max_len": max_len}
+        print(json.dumps(line), flush=True)
+    # eviction: four system prompts, a pool that holds what 3 requests need at once, so cached prompts must make room
+    ev_reqs = make_system_prompt_requests(cfg, 16, args.prefix_tokens, args.seed + 1, n_prompts=4)
+    ev_pages = 3 * max(pages_for(r["feats"]["input_ids"].shape[1] + r["budget"]) for r in ev_reqs)
+    sched = SlotScheduler(model, slots=8, max_len=max_len, kv_pages=ev_pages, prefix_cache=True)
+    wall, first, step, _, _, split, ids = run_slots(sched, ev_reqs)
+    served = sum(i in sched.first_token for i in ids)
+    print(json.dumps({"bench": "prefix cache eviction: 16 requests over 4 system prompts", "arm": "prefix-evict",
+                      "kv_pages": ev_pages, "served": served, "requests": len(ev_reqs), "evicted_pages": sched.pool.evicted,
+                      "cached_positions": [sched.cached_tokens[i] for i in ids], "free_pages_after": sched.free_pages,
+                      "wall_s": wall, "ttft_ms_p50": pct(first, 50)}), flush=True)
+
+
 def collate(batch):
     """Left padding, as the inference collator does: ids padded with 0 on the left, the audio start shifted, mel padded."""
     S = max(r["feats"]["input_ids"].shape[1] for r in batch)
@@ -294,7 +378,7 @@ def run_slots(sched, reqs):
         times = [f] + ends[k:k + r["budget"] - 1]
         gaps.append([b - a for a, b in zip(times, times[1:])])
     split = {m: [t for t, (_, _, x) in zip(step, marks) if x == m] for m in (False, True)}
-    return wall, first, step, (sched.steps - steps0) * eng.slots, gaps, split
+    return wall, first, step, (sched.steps - steps0) * eng.slots, gaps, split, ids
 
 
 def pct(xs, q):
@@ -306,14 +390,15 @@ def main():
     ap.add_argument("--requests", type=int, default=64)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--seed", type=int, default=0)
-    ap.add_argument("--workload", choices=["default", "long", "conversations"], default="default")
+    ap.add_argument("--workload", choices=["default", "long", "conversations", "system-prompt"], default="default")
     ap.add_argument("--arms", default=None, help="default: static,slots (conversations: sessions,slots)")
+    ap.add_argument("--prefix-tokens", type=int, default=1024, help="system-prompt workload: random text ids in the system prompt")
     ap.add_argument("--turns", type=int, default=4)
     ap.add_argument("--kv-pages", type=int, default=None)
     args = ap.parse_args()
     if args.arms is None:
         args.arms = "sessions,slots" if args.workload == "conversations" else "static,slots"
-    if args.workload == "conversations" and "--requests" not in sys.argv:
+    if args.workload in ("conversations", "system-prompt") and "--requests" not in sys.argv:
         args.requests = 32
     arms = args.arms.split(",")
     if args.kv_pages and args.workload != "conversations" and "paged" not in arms:
@@ -327,6 +412,8 @@ def main():
     model = UltravoxModel(cfg, device="cuda").init_random_(seed=42)
     if args.workload == "conversations":
         return main_conversations(args, model, cfg)
+    if args.workload == "system-prompt":
+        return main_system_prompt(args, model, cfg)
     reqs = make_requests(cfg, args.requests, args.seed, args.workload)
     useful = sum(r["budget"] for r in reqs)
     useful_steps = useful - len(reqs)                         # tokens picked by decode steps (the first comes from the prefill)
@@ -360,7 +447,7 @@ def main():
                 "ttft_ms_p50": pct(first, 50), "ttft_ms_p90": pct(first, 90), "row_steps": row_steps,
                 "wasted_row_step_share": 1.0 - useful_steps / row_steps}
         if arm in ("slots", "paged"):
-            gaps, split = runs[k][4:]
+            gaps, split = runs[k][4:6]
             flat, worst = [g for gs in gaps for g in gs], [max(gs) for gs in gaps if gs]
             line.update(gap_ms_p50=pct(flat, 50), gap_ms_p99=pct(flat, 99), max_gap_ms_p50=pct(worst, 50), max_gap_ms_max=max(worst),
                         plain_step_ms_mean=statistics.fmean(split[False]) if split[False] else None, plain_steps=len(split[False]),

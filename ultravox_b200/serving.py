@@ -13,12 +13,14 @@ With ``kv_pages`` the engine is ``engine.PagedSlotDecodeEngine``: the KV cache i
 with exactly what ``generate(past_key_values=...)`` returns for that turn.  At admission a request reserves every page it can
 need (its session's pages count towards that), so decoding never runs out of pages and nothing is pre-empted; a request at the
 head of the queue that cannot get its pages waits for them (FIFO).  ``PagePool`` is that bookkeeping, on the host alone.
+With ``prefix_cache`` requests that open with the same tokens (a system prompt) also share the pages of that prefix, and
+prefill only what follows it.
 """
 from __future__ import annotations
 
 import collections
 import dataclasses
-from typing import Callable, Deque, Dict, List, Optional
+from typing import Callable, Deque, Dict, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -41,19 +43,39 @@ class _Session:
 class PagePool:
     """Host bookkeeping of a pool of ``n_pages`` KV pages shared by requests and sessions (no device state).  A session holds
     the pages of its ``kv_len`` cached positions between turns; a turn (or a request without a session) reserves all the pages
-    it can need at admission and gives back, when it retires, every page beyond what its session keeps."""
+    it can need at admission and gives back, when it retires, every page beyond what its session keeps.
+
+    Pages are reference-counted, so several requests and sessions can hold one page.  The prefix index (used by
+    ``SlotScheduler(prefix_cache=True)``) maps ``(parent, tokens)`` to a page whose K / V hold those 64 token ids right after
+    the chain of pages ending at page ``parent`` (None for the first page).  The parent's page id stands for its whole chain
+    of token ids: eviction takes a page's indexed descendants with it, so an id never names two chains.  Keys are exact tuples,
+    not digests, so no other prompt's K / V can be served.  An indexed page nobody holds is *reclaimable*: it keeps its
+    contents and can still be hit, until a reservation that finds no free page evicts it (least recently released first).
+    A holder of an indexed page holds its whole chain from the first page, so a page nobody holds has no held descendant."""
 
     def __init__(self, n_pages: int):
         if int(n_pages) < 1:
             raise ValueError(f"the pool needs at least one page, got {n_pages}")
         self.n_pages = int(n_pages)
         self._free: List[int] = list(range(self.n_pages))
+        self._refs: List[int] = [0] * self.n_pages
+        self._reclaimable: "collections.OrderedDict[int, None]" = collections.OrderedDict()    # oldest first
+        self._index: Dict[tuple, int] = {}              # (parent page or None, 64 token ids) -> page
+        self._key: Dict[int, tuple] = {}                # indexed page -> its key
+        self._children: Dict[int, set] = {}             # indexed page -> the indexed pages keyed under it
         self._sessions: Dict[int, _Session] = {}
         self._next_sid = 0
+        self.evicted = 0                                # cached pages evicted so far
 
     @property
     def free_pages(self) -> int:
-        return len(self._free)
+        """Pages a reservation can take now: free ones and reclaimable cached ones."""
+        return len(self._free) + len(self._reclaimable)
+
+    @property
+    def cached_pages(self) -> int:
+        """Pages in the prefix index (held or reclaimable)."""
+        return len(self._index)
 
     def session_pages(self) -> int:
         """Pages held by sessions between turns (not by a running turn beyond its session's share)."""
@@ -75,32 +97,102 @@ class PagePool:
         s = self.session(sid)
         if s.busy:
             raise RuntimeError(f"session {sid} has a turn in flight; close it after the turn returns")
-        self._free.extend(s.pages)
+        self._drop(s.pages)
         del self._sessions[sid]
 
-    def reserve(self, positions: int, sid: Optional[int] = None) -> Optional[List[int]]:
-        """The page list of a request that needs ``positions`` positions (its session's pages first), or None (nothing taken)
-        when the pool is short."""
+    def match(self, page_tokens: Sequence[tuple]) -> List[int]:
+        """The indexed pages holding ``page_tokens[0]``, ``page_tokens[1]``, ... (64 token ids each) from position 0 on, as far
+        as they match.  Takes nothing."""
+        chain, parent = [], None
+        for t in page_tokens:
+            p = self._index.get((parent, t))
+            if p is None:
+                break
+            chain.append(p)
+            parent = p
+        return chain
+
+    def reserve(self, positions: int, sid: Optional[int] = None, shared: Sequence[int] = ()) -> Optional[List[int]]:
+        """The page list of a request that needs ``positions`` positions (its session's pages first, or the cached pages
+        ``shared`` from ``match``, then new ones), or None (nothing taken) when the pool is short.  New pages come from the
+        free list first, then by evicting reclaimable cached pages, least recently released first."""
         held = self.session(sid).pages if sid is not None else []
-        extra = pages_for(positions) - len(held)
-        if extra > len(self._free):
+        shared = list(shared)
+        if shared and held:
+            raise ValueError("a session that holds pages extends its own; only its first turn can share cached pages")
+        extra = max(pages_for(positions) - len(held) - len(shared), 0)
+        if extra > self.free_pages - sum(p in self._reclaimable for p in shared):
             return None
-        new = [self._free.pop() for _ in range(max(extra, 0))]
+        for p in shared:                # held first, so the evictions below cannot take them
+            self._acquire(p)
+        new = [self._take() for _ in range(extra)]
+        pages = held + shared + new
         if sid is not None:
-            self._sessions[sid].pages = held + new
-            return list(self._sessions[sid].pages)
-        return new
+            self._sessions[sid].pages = pages
+            return list(pages)
+        return pages
+
+    def register(self, pages: Sequence[int], page_tokens: Sequence[tuple]) -> None:
+        """Indexes ``pages[k]`` under ``page_tokens[k]`` for k = 0, 1, ..., once the holder has written their K / V.  Pages
+        that are already indexed under those tokens (the shared part of ``pages``) are passed; the first key that another page
+        already holds ends the chain, and the rest of ``pages`` stay private (the first registration wins)."""
+        parent = None
+        for p, t in zip(pages, page_tokens):
+            key = (parent, t)
+            if self._key.get(p) != key:
+                if key in self._index or p in self._key:
+                    return
+                if self._refs[p] < 1:
+                    raise ValueError(f"page {p} is not held; only a holder can register it")
+                self._index[key], self._key[p] = p, key
+                if parent is not None:
+                    self._children.setdefault(parent, set()).add(p)
+            parent = p
 
     def release(self, pages: List[int], sid: Optional[int] = None, kv_len: int = 0) -> None:
         """A request retired: without a session its pages go back; with one, the session keeps the pages of its first ``kv_len``
-        positions and the rest go back."""
+        positions and the rest go back.  A page goes back to the free list when nobody holds it, unless it is cached: then it
+        becomes reclaimable."""
         if sid is None:
-            self._free.extend(pages)
+            self._drop(pages)
             return
         s = self.session(sid)
         keep = pages_for(kv_len)
-        self._free.extend(s.pages[keep:])
+        self._drop(s.pages[keep:])
         s.pages, s.kv_len, s.busy = s.pages[:keep], int(kv_len), False
+
+    def _acquire(self, p: int) -> None:
+        if self._refs[p] == 0:
+            del self._reclaimable[p]
+        self._refs[p] += 1
+
+    def _take(self) -> int:
+        if not self._free:
+            self._evict(next(iter(self._reclaimable)))
+        p = self._free.pop()
+        self._refs[p] = 1
+        return p
+
+    def _drop(self, pages: Sequence[int]) -> None:
+        for p in reversed(pages):       # last page first, so a chain's tail is evicted before its head
+            self._refs[p] -= 1
+            if self._refs[p] == 0:
+                if p in self._key:
+                    self._reclaimable[p] = None
+                else:
+                    self._free.append(p)
+
+    def _evict(self, p: int) -> None:
+        """Unindexes reclaimable page ``p`` and its descendants (unreachable without it) and frees them all."""
+        key = self._key.pop(p)
+        del self._index[key]
+        del self._reclaimable[p]
+        if key[0] in self._children:    # not when the parent is being evicted itself
+            self._children[key[0]].discard(p)
+        for c in self._children.pop(p, ()):
+            self._evict(c)
+        self._free.append(p)
+        self.evicted += 1
 
 
 @dataclasses.dataclass
@@ -115,6 +207,7 @@ class _Request:
     penalty: float
     u: Optional[torch.Tensor]
     session: Optional[int] = None
+    prefix: Tuple[tuple, ...] = ()     # token ids of its shareable pages (prefix cache on)
     pages: Optional[List[int]] = None
     past: int = 0
     admitted_at: int = -1
@@ -129,14 +222,27 @@ class SlotScheduler:
     ``kv_pages``: None keeps the contiguous engine (a ``[max_len]`` cache row per slot); an int makes it
     ``PagedSlotDecodeEngine`` with that many shareable 64-position pages, and enables sessions: ``open_session()`` returns a
     session id, ``submit(..., session=sid)`` queues one turn of that conversation (its prompt must extend the conversation so
-    far: the previous turn's prompt, its reply and the new turn's tokens), ``close_session(sid)`` gives its pages back."""
+    far: the previous turn's prompt, its reply and the new turn's tokens), ``close_session(sid)`` gives its pages back.
+
+    ``prefix_cache`` (needs ``kv_pages``): requests that start with the same tokens share the K / V pages of that prefix
+    instead of prefilling it again.  A request without a session, or a session's first turn, registers its *shareable* pages
+    (the full pages before its first audio row) once their K / V are written; a later such request takes the longest matching
+    chain of them, up to its own first audio row and S - 1 positions, and prefills only the rest, as
+    ``generate(past_key_values=...)`` with those pages as the cache.  ``cached_tokens[id]`` is the number of positions a request
+    took from the cache.  Pages nobody holds stay cached until the pool needs them (least recently released first).  Off by
+    default because a hit's bits depend on which earlier request computed the shared K / V: its prefill's row count picked
+    its GEMM tiling, so a request can get different bits than when it prefills its whole prompt."""
 
     def __init__(self, model, slots: int = 8, max_len: int = 2048, eos_token_ids=None, pad_token_id: Optional[int] = None,
-                 sync_every: int = 8, use_graph: bool = True, kv_pages: Optional[int] = None):
+                 sync_every: int = 8, use_graph: bool = True, kv_pages: Optional[int] = None, prefix_cache: bool = False):
         eos = sorted(set([eos_token_ids] if isinstance(eos_token_ids, int) else (eos_token_ids or [])))
         pad = pad_token_id if pad_token_id is not None else (min(eos) if eos else 0)     # generate()'s default
         if int(sync_every) < 1:
             raise ValueError(f"sync_every must be >= 1, got {sync_every}")
+        if prefix_cache and kv_pages is None:
+            raise ValueError("prefix_cache shares KV pages between requests: it needs the paged cache (kv_pages=N)")
+        self.prefix_cache = bool(prefix_cache)
+        self.cached_tokens: Dict[int, int] = {}
         self.model = model
         self.pool: Optional[PagePool] = None
         if kv_pages is None:
@@ -186,7 +292,13 @@ class SlotScheduler:
 
     @property
     def free_pages(self) -> int:
+        """Pages a request can take now (free ones and cached ones nobody holds)."""
         return self._pool().free_pages
+
+    @property
+    def cached_pages(self) -> int:
+        """Pages in the prefix cache, held or not."""
+        return self._pool().cached_pages
 
     def submit(self, features: dict, max_new_tokens: int = 20, do_sample: bool = False, temperature: Optional[float] = None,
                top_k: Optional[int] = None, top_p: Optional[float] = None, repetition_penalty: float = 1.0,
@@ -232,9 +344,17 @@ class SlotScheduler:
         if sampling:
             u = torch.rand(S + n + 1, 1, device=self.engine.pos.device, dtype=torch.float32, generator=generator)
         feats = {k: v for k, v in features.items() if k not in ("input_ids", "attention_mask", "labels")}
+        prefix = ()
+        if self.prefix_cache and (sess is None or sess.kv_len == 0):
+            # audio rows hold the same placeholder id in every request, so only the full pages before the first one can be keyed
+            starts = feats.get("audio_token_start_idx")
+            first = min(S, int(starts.min())) if starts is not None and starts.numel() else S
+            head = ids[0, :first // PAGE * PAGE].tolist()
+            prefix = tuple(tuple(head[i:i + PAGE]) for i in range(0, len(head), PAGE))
         rid = self._next_id
         self._next_id += 1
-        self._queue.append(_Request(rid, ids, feats, n, temp, k_top, p_top, float(repetition_penalty or 1.0), u, session))
+        self._queue.append(_Request(rid, ids, feats, n, temp, k_top, p_top, float(repetition_penalty or 1.0), u, session,
+                                    prefix))
         if sess is not None:
             sess.busy = True
         return rid
@@ -250,24 +370,36 @@ class SlotScheduler:
             head = self._queue[0]
             S = int(head.input_ids.shape[1])
             past = self.pool.session(head.session).kv_len if head.session is not None else 0
+            shared = []
+            if head.prefix:             # at least one row (the last) is prefilled: it gives the first token's logits
+                shared = self.pool.match(head.prefix[:(S - 1) // PAGE])
+                past = PAGE * len(shared)
             long = S - past > PREFILL_ROWS
             if long and self._prefilling is not None:
                 return                  # FIFO: it waits until the prompt in flight has been prefilled
             kw = {}
             if self.pool is not None:
-                pages = self.pool.reserve(S + head.max_new, head.session)
+                pages = self.pool.reserve(S + head.max_new, head.session, shared)
                 if pages is None:
                     return              # FIFO: it waits for pages
                 head.pages, head.past = pages, past
                 kw = dict(past=past, pages=pages)
             r = self._queue.popleft()
+            if self.prefix_cache:
+                self.cached_tokens[r.rid] = PAGE * len(shared)
             feats = {k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in r.features.items()}
             eng.admit(j, r.input_ids, r.max_new, r.temperature, r.top_k, r.top_p, r.penalty, r.u, **kw, **feats)
             r.features, r.u = {}, None
             if long:
                 self._prefilling = (j, r)
             else:
+                self._register(r)       # one stream: a later admission's gather runs after this prefill's scatter
                 self._started(j, r)
+
+    def _register(self, r: _Request) -> None:
+        """The request's prompt K / V are in its pages: its shareable pages join the prefix cache."""
+        if r.prefix:
+            self.pool.register(r.pages, r.prefix)
 
     def _started(self, j: int, r: _Request) -> None:
         """The request's first token has been picked: its budget counts from here."""
@@ -321,6 +453,7 @@ class SlotScheduler:
             if self._prefilling is not None and self.engine.prefilling is None:
                 j, r = self._prefilling
                 self._prefilling = None
+                self._register(r)
                 self._started(j, r)
         return results
 
