@@ -59,6 +59,8 @@ struct GemmParams {
   int staged_bytes;        // staged epilogue (gemm_wg_kernel<., ., true>): its output tile in shared memory, between the ring and
                            // the barriers (0: register epilogue)
   int r_bcast;             // the residual has batch stride 0: its map (tmR) has no batch dimension
+  int w_evict_first;       // W is read once per call (prefill rows): its boxes enter L2 as the first lines to evict, so the
+                           // stream does not flush what is read again (A operand, split-K partials, residual, attention operands)
 };
 
 static constexpr int kSmemTotal = 227 * 1024;
@@ -258,8 +260,15 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             uint8_t* dw = w_ring + s * w_stride + rm * w_slice * (kBK * 2);
             const int w0 = p.w_tiled ? 0 : kb * kBK;
             const int w1 = (p.w_tiled ? wt_base + kb * BN : tn_idx * BN) + rm * w_slice;
-            if (cm > 1) tma_load_2d_mc(dw, &tmW, w0, w1, &full_bar[s], col_mask);
-            else tma_load_2d(dw, &tmW, w0, w1, &full_bar[s]);
+            if (p.w_evict_first) {  // the policy is made at each load: one instruction, no register held across the loop
+              const uint64_t pol = l2_policy_evict_first();
+              if (cm > 1) tma_load_2d_mc_hint(dw, &tmW, w0, w1, &full_bar[s], col_mask, pol);
+              else tma_load_2d_hint(dw, &tmW, w0, w1, &full_bar[s], pol);
+            } else if (cm > 1) {
+              tma_load_2d_mc(dw, &tmW, w0, w1, &full_bar[s], col_mask);
+            } else {
+              tma_load_2d(dw, &tmW, w0, w1, &full_bar[s]);
+            }
           }
           if (++s == stages) { s = 0; ph ^= 1u; }
           if (++sa == a_stages) { sa = 0; pha ^= 1u; }
@@ -1099,6 +1108,8 @@ static int launch_gemm(const uvx_gemm_args* a, int splits, int cm, int cn, cudaS
   int clusters = units < max_units ? units : max_units;
   if (g_grid_cap > 0 && clusters * csize > g_grid_cap) clusters = g_grid_cap / csize > 1 ? g_grid_cap / csize : 1;
   const dim3 grid((unsigned)(clusters * csize));
+  // the weight of a prefill call (one batch, <= 256 rows) is read once per call; the tensor-bound calls keep the default policy
+  p.w_evict_first = a->a_batch == 1 && a->a_rows <= 256 && !staged;
   if (csize > 1)
     launch_k_cluster(gemm_wg_kernel<MT, BN, false>, grid, dim3(kGemmThreads), (size_t)smem, stream, (unsigned)csize, tmA, tmW, tmC, tmR, p);
   else if (staged)

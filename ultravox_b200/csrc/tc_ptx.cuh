@@ -103,6 +103,28 @@ __device__ __forceinline__ void tma_load_2d_mc(void* dst, const CUtensorMap* tm,
       "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
       : "memory");
 }
+// ---- L2 policy of a read-once stream (gemm_tc.cu: the prefill weight stream)
+// an L2 cache policy that marks the lines a load brings in as the first to be evicted
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+  uint64_t pol;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
+__device__ __forceinline__ void tma_load_2d_hint(void* dst, const CUtensorMap* tm, int c0, int c1, uint64_t* bar, uint64_t pol) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;" ::
+          "r"(smem_u32(dst)),
+      "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(pol)
+      : "memory");
+}
+__device__ __forceinline__ void tma_load_2d_mc_hint(void* dst, const CUtensorMap* tm, int c0, int c1, uint64_t* bar, uint16_t mask,
+                                                    uint64_t pol) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint [%0], [%1, {%3, %4}], "
+      "[%2], %5, %6;" ::"r"(smem_u32(dst)),
+      "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask), "l"(pol)
+      : "memory");
+}
 __device__ __forceinline__ void tma_load_3d_mc(void* dst, const CUtensorMap* tm, int c0, int c1, int c2, uint64_t* bar, uint16_t mask) {
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5}], [%2], %6;" ::
