@@ -376,6 +376,27 @@ int uvx_slot_finish(const int64_t* tok, int32_t* done, const int64_t* eos_ids, i
                     int32_t* cur_len, int32_t* n_new, const int32_t* max_new, const int32_t* active, int32_t* pos, int32_t* lens,
                     int32_t* rope_pos, int32_t* n_open, int64_t B, uvx_stream_t stream);
 
+/* Log-probabilities and scores of a decode step, written on the device at an index read from device memory (no host sync, so
+ * they sit inside the captured step).
+ * uvx_token_logprobs  per row b with n_top[b] >= 0 (rows with n_top[b] < 0 are not touched), on the RAW logits row x:
+ *                     lse = m + log(sum exp(x - m)) (m = max x) and, at d = dst[b] (0 <= d < cap, else nothing is written):
+ *                     out_lp[b * cap + d] = x[tok[b]] - lse (torch.log_softmax(x)[tok], the OpenAI-style `logprobs` of the
+ *                     chosen token); for n = min(n_top[b], n_max) > 0, out_ids / out_top[(b * cap + d) * n_max + i], i < n, are
+ *                     the n largest entries by (value desc, index asc) - a tie at the n-th place goes to the lower index, as in
+ *                     uvx_beam_select - with their x - lse (`top_logprobs`); entries i >= n are not written.  0 <= n_max <= 20.
+ *                     One CTA per row with fixed-order reductions: a row's bits depend on its own logits only.
+ * uvx_record_scores   at s = step_idx[0] (nothing when s is outside [0, steps)): raw[s, b, :] = logits[b] (HF's `output_logits`;
+ *                     call it before uvx_repetition_penalty, which rewrites the logits in place) and scores[s, b, :] = HF's
+ *                     processed scores (`output_scores`, hf:generation/utils.py _sample) of the penalised logits: for
+ *                     temperature <= 0 (greedy: HF adds no warper) the row itself, otherwise TemperatureLogitsWarper ->
+ *                     TopKLogitsWarper -> TopPLogitsWarper: x / temperature (IEEE division) on the entries uvx_sample /
+ *                     uvx_sample_top_p draw from with the same temperature, top_k and top_p, -inf elsewhere, so a sampled
+ *                     token always has a finite score.  scores / raw are [steps, B, V] fp32; either may be NULL.  V <= 2^24. */
+int uvx_token_logprobs(const float* logits, int64_t B, int64_t V, const int64_t* tok, const int32_t* n_top, const int32_t* dst,
+                       int64_t cap, int32_t n_max, float* out_lp, int64_t* out_ids, float* out_top, uvx_stream_t stream);
+int uvx_record_scores(const float* logits, int64_t B, int64_t V, float temperature, int32_t top_k, float top_p,
+                      const int32_t* step_idx, int64_t steps, float* scores, float* raw, uvx_stream_t stream);
+
 /* Beam search (hf:generation/utils.py _beam_search, transformers 5.5, and the helpers above it), one decode step as four
  * launches that read every per-step scalar from device memory.  B prompts, nb <= 8 beams each: row r = b * nb + j.
  * uvx_log_softmax   out[r] = log_softmax(in[r]) in fp32 (in == out allowed).  Beam search scores log-probs; the repetition

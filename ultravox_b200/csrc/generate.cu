@@ -76,17 +76,54 @@ __device__ __forceinline__ uint32_t f2key(float f) {  // order-preserving float 
 // seeded torch generator).  sample_kernel<false> is uvx_sample; top_p is read only by sample_kernel<true>.
 constexpr float kMassOne = 1099511627776.f;  // 2^40: fixed-point unit of the top-p mass (sum <= V * 2^40 < 2^64 for V <= 2^24)
 
-// The body is sample_row, shared with uvx_sample_slots: TOP_P = 0 never runs the nucleus pass, 1 always does, 2 does when the
-// row's top_p < 1 (the per-row form of uvx_sample_top_p routing top_p >= 1 to uvx_sample).  The caller's CTA handles one row.
+// The k-th largest f2key of a row (1 <= k <= V) by a 4-pass radix select from the top byte down: afterwards sel_prefix is that
+// key and sel_remaining the number of entries equal to it that rank among the k largest (the rest of the k lie above it).
+// Every thread of the CTA (1024) calls it; hist [256] and the two scalars are the caller's shared memory.
+__device__ __forceinline__ void radix_select_kth(const float* __restrict__ row, int64_t V, uint32_t k_th, uint32_t* hist,
+                                                 uint32_t& sel_prefix, uint32_t& sel_remaining) {
+  const int tid = threadIdx.x;
+  if (tid == 0) { sel_prefix = 0u; sel_remaining = k_th; }
+  for (int pass = 3; pass >= 0; --pass) {
+    if (tid < 256) hist[tid] = 0u;
+    __syncthreads();
+    const uint32_t prefix = sel_prefix;
+    const uint32_t hi_mask = pass == 3 ? 0u : (0xFFFFFFFFu << ((pass + 1) * 8));
+    for (int64_t i = tid; i < V; i += 1024) {
+      const uint32_t k = f2key(row[i]);
+      if ((k & hi_mask) == (prefix & hi_mask)) atomicAdd(&hist[(k >> (pass * 8)) & 255u], 1u);
+    }
+    __syncthreads();
+    if (tid == 0) {
+      uint32_t rem = sel_remaining;
+      int d = 255;
+      for (; d > 0; --d) {
+        if (hist[d] >= rem) break;
+        rem -= hist[d];
+      }
+      sel_prefix = prefix | ((uint32_t)d << (pass * 8));
+      sel_remaining = rem;
+    }
+    __syncthreads();
+  }
+}
+
+// The row maximum (mx) and the key threshold of the set a sampled pick draws from: entries with f2key(x) >= the returned key
+// are kept (top-k, then top-p as below).  Shared by sample_row and uvx_record_scores, so a recorded score is finite exactly
+// where the sampler can pick.  TOP_P = 0 never runs the nucleus pass, 1 always does, 2 does when the row's top_p < 1 (the
+// per-row form of uvx_sample_top_p routing top_p >= 1 to uvx_sample).
+struct ThresholdSmem {  // keep_threshold's shared memory, declared by the caller (sample_row keeps its own declaration order)
+  float* red;                                     // [32]
+  uint32_t* hist;                                 // [256]
+  uint32_t *sel_prefix, *sel_remaining;
+  unsigned long long* mhist;                      // [256]
+  unsigned long long *p_below, *p_target;
+  uint32_t* p_prefix;
+};
+
 template <int TOP_P>
-__device__ __forceinline__ void sample_row(const float* __restrict__ row, int64_t V, float inv_temp, int top_k, float top_p,
-                                           const float* __restrict__ u_all, const int32_t* __restrict__ step_idx, int64_t u_stride,
-                                           int64_t col, int64_t* __restrict__ out_ptr) {
-  __shared__ float red[32];
-  __shared__ uint32_t hist[256];
-  __shared__ uint32_t sel_prefix, sel_remaining;
-  __shared__ float chunk_base[32];
-  __shared__ int win_thread;
+__device__ __forceinline__ uint32_t keep_threshold(const float* __restrict__ row, int64_t V, float inv_temp, int top_k, float top_p,
+                                                   ThresholdSmem sm, float& mx_out) {
+  float* red = sm.red;
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   // ---- max
   float mx = -INFINITY;
@@ -96,33 +133,12 @@ __device__ __forceinline__ void sample_row(const float* __restrict__ row, int64_
   __syncthreads();
   mx = warp_max(red[lane]);
   __syncthreads();
+  mx_out = mx;
   // ---- top-k threshold (keys >= thr_key are kept); top_k <= 0 or >= V keeps everything
   uint32_t thr_key = 0u;
   if (top_k > 0 && (int64_t)top_k < V) {
-    if (tid == 0) { sel_prefix = 0u; sel_remaining = (uint32_t)top_k; }
-    for (int pass = 3; pass >= 0; --pass) {
-      if (tid < 256) hist[tid] = 0u;
-      __syncthreads();
-      const uint32_t prefix = sel_prefix;
-      const uint32_t hi_mask = pass == 3 ? 0u : (0xFFFFFFFFu << ((pass + 1) * 8));
-      for (int64_t i = tid; i < V; i += 1024) {
-        const uint32_t k = f2key(row[i]);
-        if ((k & hi_mask) == (prefix & hi_mask)) atomicAdd(&hist[(k >> (pass * 8)) & 255u], 1u);
-      }
-      __syncthreads();
-      if (tid == 0) {
-        uint32_t rem = sel_remaining;
-        int d = 255;
-        for (; d > 0; --d) {
-          if (hist[d] >= rem) break;
-          rem -= hist[d];
-        }
-        sel_prefix = prefix | ((uint32_t)d << (pass * 8));
-        sel_remaining = rem;
-      }
-      __syncthreads();
-    }
-    thr_key = sel_prefix;
+    radix_select_kth(row, V, (uint32_t)top_k, sm.hist, *sm.sel_prefix, *sm.sel_remaining);
+    thr_key = *sm.sel_prefix;
   }
   if (TOP_P == 1 || (TOP_P == 2 && top_p < 1.f)) {
     // ---- top-p threshold over the top-k survivors (HF TopPLogitsWarper after TopKLogitsWarper): with m_i = exp((x_i - max) / T),
@@ -131,9 +147,10 @@ __device__ __forceinline__ void sample_row(const float* __restrict__ row, int64_
     // carried below the prefix.  Masses are 64-bit fixed point (kMassOne = 1), so the atomics are order-free and the result
     // deterministic; a tie group has one key and is kept or dropped whole.  Entries whose mass rounds to 0 never cross the
     // threshold and are skipped.  target <= total - 1 makes the maximum (mass exactly kMassOne) always kept: top_p = 0 -> argmax.
-    __shared__ unsigned long long mhist[256];
-    __shared__ unsigned long long p_below, p_target;
-    __shared__ uint32_t p_prefix;
+    unsigned long long* mhist = sm.mhist;
+    unsigned long long& p_below = *sm.p_below;
+    unsigned long long& p_target = *sm.p_target;
+    uint32_t& p_prefix = *sm.p_prefix;
     if (tid == 0) { p_prefix = 0u; p_below = 0ull; p_target = 0ull; }
     for (int pass = 3; pass >= 0; --pass) {
       if (tid < 256) mhist[tid] = 0ull;
@@ -209,6 +226,26 @@ __device__ __forceinline__ void sample_row(const float* __restrict__ row, int64_
     }
     thr_key = max(thr_key, p_prefix);
   }
+  return thr_key;
+}
+
+// The body of sample_kernel, shared with uvx_sample_slots (TOP_P as in keep_threshold).  The caller's CTA handles one row.
+template <int TOP_P>
+__device__ __forceinline__ void sample_row(const float* __restrict__ row, int64_t V, float inv_temp, int top_k, float top_p,
+                                           const float* __restrict__ u_all, const int32_t* __restrict__ step_idx, int64_t u_stride,
+                                           int64_t col, int64_t* __restrict__ out_ptr) {
+  __shared__ float red[32];
+  __shared__ uint32_t hist[256];
+  __shared__ uint32_t sel_prefix, sel_remaining;
+  __shared__ float chunk_base[32];
+  __shared__ int win_thread;
+  __shared__ unsigned long long mhist[256];
+  __shared__ unsigned long long p_below, p_target;
+  __shared__ uint32_t p_prefix;
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  float mx;
+  const uint32_t thr_key = keep_threshold<TOP_P>(row, V, inv_temp, top_k, top_p,
+                                                 {red, hist, &sel_prefix, &sel_remaining, mhist, &p_below, &p_target, &p_prefix}, mx);
   // ---- chunk sums
   const int64_t c = (V + 1023) / 1024;
   const int64_t lo = (int64_t)tid * c, hi = lo + c < V ? lo + c : V;
@@ -424,6 +461,150 @@ __global__ void token_finish_kernel(int64_t* __restrict__ tok, int32_t* __restri
     *cur_len = n + 1;
     if (step_idx) *step_idx += 1;
     if (all_done) *all_done = any_open ? 0 : 1;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// Log-probabilities of the decode step, recorded on the device at an index the step state holds, so the step stays one graph.
+constexpr int kLogprobsMax = 20;  // alternatives per token (OpenAI-style top_logprobs <= 20)
+
+// One CTA (1024 threads) per row, skipped when n_top[b] < 0: lse = m + log(sum exp(x - m)) of the raw row, the chosen token's
+// x[tok] - lse, and (n_top[b] > 0) the n_top[b] largest entries by (value desc, index asc) with their x - lse, written at
+// index dst[b] of the row's [cap] (or [cap, n_max]) outputs.  The radix select of the sampler finds the n-th largest key; the
+// keys above it (fewer than n) are gathered in any order, the missing ones are taken from the keys equal to it in index order
+// (thread t owns the chunk [t*c, (t+1)*c), an exclusive scan of the per-chunk counts ranks them), and the n are sorted by
+// rank, as in beam_row_topk_kernel.  Every reduction has a fixed order, so a row's bits depend on its logits alone.
+__global__ void __launch_bounds__(1024, 1) token_logprobs_kernel(const float* logits, int64_t V, const int64_t* tok,
+                                                                 const int32_t* n_top, const int32_t* dst, int64_t cap, int n_max,
+                                                                 float* __restrict__ out_lp, int64_t* __restrict__ out_ids,
+                                                                 float* __restrict__ out_top) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ float red[32];
+  __shared__ uint32_t hist[256];
+  __shared__ uint32_t sel_prefix, sel_remaining;
+  __shared__ int n_gt;
+  __shared__ int scan[32];
+  __shared__ float s_val[kLogprobsMax];
+  __shared__ int64_t s_idx[kLogprobsMax];
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  const int64_t b = blockIdx.x;
+  const int want = n_top[b];
+  const int64_t d = dst[b];
+  if (want < 0 || d < 0 || d >= cap) return;
+  const float* row = logits + b * V;
+  float mx = -INFINITY;
+  for (int64_t i = tid; i < V; i += 1024) mx = fmaxf(mx, row[i]);
+  mx = warp_max(mx);
+  if (lane == 0) red[w] = mx;
+  __syncthreads();
+  mx = warp_max(red[lane]);
+  __syncthreads();
+  float s = 0.f;
+  for (int64_t i = tid; i < V; i += 1024) s += expf(row[i] - mx);
+  s = warp_sum(s);
+  if (lane == 0) red[w] = s;
+  __syncthreads();
+  const float lse = mx + logf(warp_sum(red[lane]));
+  if (tid == 0) {
+    const int64_t t = tok[b];
+    out_lp[b * cap + d] = (t >= 0 && t < V) ? row[t] - lse : NAN;
+  }
+  int64_t kk = want < n_max ? want : n_max;
+  kk = kk < V ? kk : V;
+  const int K = (int)kk;
+  if (K == 0) return;
+  radix_select_kth(row, V, (uint32_t)K, hist, sel_prefix, sel_remaining);
+  const uint32_t thr = sel_prefix;
+  const int need_eq = (int)sel_remaining;  // keys equal to thr to take; K - need_eq keys lie above it
+  if (tid == 0) n_gt = 0;
+  __syncthreads();
+  for (int64_t i = tid; i < V; i += 1024) {
+    const float x = row[i];
+    if (f2key(x) > thr) {
+      const int j = atomicAdd(&n_gt, 1);
+      s_val[j] = x;
+      s_idx[j] = i;
+    }
+  }
+  const int64_t c = (V + 1023) / 1024;
+  const int64_t lo = (int64_t)tid * c, hi = lo + c < V ? lo + c : V;
+  int cnt = 0;
+  for (int64_t i = lo; i < hi; ++i) cnt += f2key(row[i]) == thr;
+  int incl = cnt;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += t;
+  }
+  if (lane == 31) scan[w] = incl;
+  __syncthreads();
+  if (w == 0) {
+    const int v = scan[lane];
+    int sc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, sc, o);
+      if (lane >= o) sc += t;
+    }
+    scan[lane] = sc - v;
+  }
+  __syncthreads();
+  int rank = scan[w] + incl - cnt;
+  const int base = K - need_eq;
+  for (int64_t i = lo; i < hi && rank < need_eq; ++i) {
+    const float x = row[i];
+    if (f2key(x) == thr) {
+      s_val[base + rank] = x;
+      s_idx[base + rank] = i;
+      ++rank;
+    }
+  }
+  __syncthreads();
+  if (tid < K) {
+    const float x = s_val[tid];
+    const int64_t ix = s_idx[tid];
+    int pos = 0;
+    for (int m = 0; m < K; ++m) pos += s_val[m] > x || (s_val[m] == x && s_idx[m] < ix);
+    const int64_t o = (b * cap + d) * n_max + pos;
+    out_ids[o] = ix;
+    out_top[o] = x - lse;
+  }
+}
+
+// One CTA (1024 threads) per row, at step s = step_idx[0] (nothing when s is outside [0, steps)): raw[s, b] = the row as given;
+// scores[s, b] = the row after HF's warpers - a copy when temperature <= 0 (greedy: no warper), else x / temperature (IEEE
+// division, TemperatureLogitsWarper) on the entries keep_threshold keeps (TopKLogitsWarper, TopPLogitsWarper) and -inf on the
+// rest.  Either output may be NULL.
+__global__ void __launch_bounds__(1024, 1) record_scores_kernel(const float* logits, int64_t V, float temperature, float inv_temp,
+                                                                int top_k, float top_p, const int32_t* step_idx, int64_t steps,
+                                                                int64_t B, float* __restrict__ scores, float* __restrict__ raw) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ float red[32];
+  __shared__ uint32_t hist[256];
+  __shared__ uint32_t sel_prefix, sel_remaining;
+  __shared__ unsigned long long mhist[256];
+  __shared__ unsigned long long p_below, p_target;
+  __shared__ uint32_t p_prefix;
+  const int64_t b = blockIdx.x;
+  const int64_t step = *step_idx;
+  if (step < 0 || step >= steps) return;
+  const float* row = logits + b * V;
+  const int64_t o = (step * B + b) * V;
+  if (raw)
+    for (int64_t i = threadIdx.x; i < V; i += 1024) raw[o + i] = row[i];
+  if (!scores) return;
+  if (!(temperature > 0.f)) {
+    for (int64_t i = threadIdx.x; i < V; i += 1024) scores[o + i] = row[i];
+    return;
+  }
+  float mx;
+  const uint32_t thr = keep_threshold<2>(row, V, inv_temp, top_k, top_p,
+                                         {red, hist, &sel_prefix, &sel_remaining, mhist, &p_below, &p_target, &p_prefix}, mx);
+  for (int64_t i = threadIdx.x; i < V; i += 1024) {
+    const float x = row[i];
+    scores[o + i] = f2key(x) >= thr ? x / temperature : -INFINITY;
   }
 }
 
@@ -1013,4 +1194,28 @@ extern "C" int uvx_kv_pages_copy(void* k_row, void* v_row, int64_t row_layer_str
            row_layer_stride / 8, (uint4*)k_pool, (uint4*)v_pool, pool_layer_stride / 8, L, row_elems / 8, pages, p0, p1 - p0,
            (int)to_pages);
   return check_launch("kv_pages_copy_kernel");
+}
+
+extern "C" int uvx_token_logprobs(const float* logits, int64_t B, int64_t V, const int64_t* tok, const int32_t* n_top,
+                                  const int32_t* dst, int64_t cap, int32_t n_max, float* out_lp, int64_t* out_ids, float* out_top,
+                                  uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(logits && tok && n_top && dst && out_lp && B >= 1 && V >= 1 && V <= ((int64_t)1 << 31) - 1 && cap >= 1 &&
+                  n_max >= 0 && n_max <= kLogprobsMax && (n_max == 0 || (out_ids && out_top)),
+              "uvx_token_logprobs: bad arguments (0 <= n_max <= %d)", kLogprobsMax);
+  launch_k(token_logprobs_kernel, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, tok, n_top, dst, cap, (int)n_max,
+           out_lp, out_ids, out_top);
+  return check_launch("token_logprobs_kernel");
+}
+
+extern "C" int uvx_record_scores(const float* logits, int64_t B, int64_t V, float temperature, int32_t top_k, float top_p,
+                                 const int32_t* step_idx, int64_t steps, float* scores, float* raw, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(logits && step_idx && (scores || raw) && B >= 1 && V >= 1 && V <= (int64_t)1 << 24 && steps >= 1 && top_p >= 0.f &&
+                  top_p <= 1.f,
+              "uvx_record_scores: bad arguments");
+  const float t = temperature > 0.f ? temperature : 0.f;
+  launch_k(record_scores_kernel, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, t, t > 0.f ? 1.0f / t : 0.f,
+           (int)top_k, top_p, step_idx, steps, B, scores, raw);
+  return check_launch("record_scores_kernel");
 }

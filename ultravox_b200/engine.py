@@ -8,6 +8,8 @@ multi-GPU inference is independent replicas (SURVEY.md 8e) - no collective.
 """
 from __future__ import annotations
 
+import dataclasses
+import numbers
 from typing import Optional
 
 import torch
@@ -108,6 +110,17 @@ class PrefillEngine:
         self._host_token.copy_(self.token, non_blocking=True)
         torch.cuda.current_stream().synchronize()
         return self._host_token
+
+
+@dataclasses.dataclass
+class TokenLogprobs:
+    """Log-probabilities of a request's generated tokens under the model's raw distribution (log_softmax of the LM-head logits,
+    before the repetition penalty, temperature, top-k and top-p - what OpenAI-style ``logprobs`` report), one entry per new
+    token: ``token_logprobs`` [n] fp32 of the chosen tokens, ``top_ids`` [n, k] int64 / ``top_logprobs`` [n, k] fp32 the k most
+    likely tokens of each step (value descending, lower id first on a tie).  Device tensors."""
+    token_logprobs: torch.Tensor
+    top_ids: torch.Tensor
+    top_logprobs: torch.Tensor
 
 
 class _RowKV:
@@ -365,7 +378,13 @@ class DecodeEngine(_Decoder):
 
     def __init__(self, model: UltravoxModel, batch: int, max_len: int, use_graph: bool = True, cache=None,
                  eos_token_ids=None, pad_token_id: int = 0, temperature: float = 0.0, top_k: int = 0,
-                 repetition_penalty: float = 1.0, generator: Optional[torch.Generator] = None, top_p: Optional[float] = None):
+                 repetition_penalty: float = 1.0, generator: Optional[torch.Generator] = None, top_p: Optional[float] = None,
+                 output_scores: bool = False, output_logits: bool = False, max_new_tokens: Optional[int] = None):
+        """``output_scores`` / ``output_logits``: every pick (the first one, in ``begin``, is step 0) also records HF's processed
+        scores / the raw logits of its rows into ``scores`` / ``raw_logits`` [max_new_tokens, batch, V] fp32, at the device
+        step counter (``uvx_record_scores``).  That is one [batch, V] fp32 tensor per generated token, which is what HF's
+        ``generate(output_scores=True / output_logits=True)`` holds too.  Without them nothing is allocated and the step is
+        unchanged."""
         super().__init__(model, batch, _RowKV(cache if cache is not None else model.new_cache(batch, max_len)), eos_token_ids,
                          pad_token_id, use_graph)
         dev = model.device
@@ -382,6 +401,14 @@ class DecodeEngine(_Decoder):
             # one uniform per (step, stream), drawn up front from the caller's (seedable) generator: the graph reads row step_idx
             self.u = torch.rand(self.max_len + 1, batch, device=dev, dtype=torch.float32, generator=generator)
         self.scratch = torch.empty(batch, self.max_len + 1, dtype=torch.float32, device=dev) if self.penalty != 1.0 else None
+        self.scores = self.raw_logits = None
+        if output_scores or output_logits:
+            steps = int(max_new_tokens or 0)
+            if not 1 <= steps <= self.max_len:
+                raise ValueError(f"recording scores / logits needs max_new_tokens in [1, {self.max_len}], got {max_new_tokens}")
+            shape = (steps, batch, model.language_model.lm_head.weight.shape[0])
+            self.scores = torch.empty(shape, dtype=torch.float32, device=dev) if output_scores else None
+            self.raw_logits = torch.empty(shape, dtype=torch.float32, device=dev) if output_logits else None
 
     # -- state ---------------------------------------------------------------------------------------------
     def begin(self, input_ids: torch.Tensor, first_logits: torch.Tensor, kv_start: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -413,8 +440,14 @@ class DecodeEngine(_Decoder):
     def _pick(self, logits: torch.Tensor):
         """logits [B, V] fp32 -> self.token (+ sequence / EOS / counter bookkeeping), all on the device."""
         self.logits = logits
+        rec = (self.temperature, self.top_k, self.top_p, self.step_idx)
+        raw_first = self.raw_logits is not None and self.penalty != 1.0
+        if raw_first:       # the penalty rewrites the logits in place: take the raw copy before it
+            ops.record_scores(logits, *rec, raw=self.raw_logits)
         if self.penalty != 1.0:
             ops.repetition_penalty_(logits, self.seq, self.cur_len, self.penalty, self.scratch)
+        if self.scores is not None or (self.raw_logits is not None and not raw_first):
+            ops.record_scores(logits, *rec, scores=self.scores, raw=None if raw_first else self.raw_logits)
         tok = self.token.view(-1)
         if self.temperature > 0:
             ops.sample(logits, self.temperature, self.top_k, self.u, self.step_idx, out=tok, top_p=self.top_p)
@@ -567,14 +600,24 @@ class SlotDecodeEngine(_Decoder):
     decode row writes nothing to the cache and picks nothing; after the last chunk its first token is picked from that row's
     logits and the slot becomes active.  One slot prefills at a time.  A chunk's rows are independent of the decode rows
     (every kernel is row-independent at the fixed row count), so a chunked request gets the same bits whatever else is
-    decoding; the decode rows of a mixed step run at 256 rows instead of ``slots`` and are not bit-identical to a plain step."""
+    decoding; the decode rows of a mixed step run at 256 rows instead of ``slots`` and are not bit-identical to a plain step.
+
+    ``max_logprobs`` (0..20) > 0 adds per-token log-probabilities: every pick (the step's, the mixed step's and the one-row
+    admission pick) copies the raw logits rows aside before the penalty and runs ``uvx_token_logprobs`` after the sampler, which
+    writes each row's chosen-token log-prob and its ``n_top[b]`` most likely alternatives at index ``n_new[b]`` of
+    ``lp_token`` [slots, max_len + 1] / ``lp_ids``, ``lp_top`` [slots, max_len + 1, max_logprobs].  A request asks with
+    ``admit(..., logprobs=k)``.  With 0 (the default) nothing is allocated and the step is unchanged."""
 
     def __init__(self, model: UltravoxModel, slots: int, max_len: int, eos_token_ids=None, pad_token_id: int = 0,
-                 use_graph: bool = True, cache=None):
+                 use_graph: bool = True, cache=None, max_logprobs: int = 0):
         kv = _RowKV(cache if cache is not None else model.new_cache(slots, max_len))
-        self._setup(model, int(slots), kv, eos_token_ids, pad_token_id, use_graph)
+        self._setup(model, int(slots), kv, eos_token_ids, pad_token_id, use_graph, max_logprobs)
 
-    def _setup(self, model: UltravoxModel, slots: int, kv, eos_token_ids, pad_token_id: int, use_graph: bool):
+    def _setup(self, model: UltravoxModel, slots: int, kv, eos_token_ids, pad_token_id: int, use_graph: bool, max_logprobs: int = 0):
+        if isinstance(max_logprobs, bool) or not isinstance(max_logprobs, numbers.Integral) or \
+                not 0 <= max_logprobs <= ops.LOGPROBS_MAX:
+            raise ValueError(f"max_logprobs must be an integer in [0, {ops.LOGPROBS_MAX}], got {max_logprobs!r}")
+        self.max_logprobs = int(max_logprobs)
         self.slots = slots
         self.chunk = PREFILL_ROWS - slots
         # mixed-step rows: [0, slots) decode rows, [slots, slots + chunk) prompt-chunk rows.  The host writes the chunk part of
@@ -603,6 +646,13 @@ class SlotDecodeEngine(_Decoder):
         self._chunk_logits = None
         self._prefill: Optional[dict] = None
         self.launches_per_mixed_step = 0
+        if self.max_logprobs:
+            V = model.language_model.lm_head.weight.shape[0]
+            self.n_top = torch.full((slots,), -1, **i32)                # per slot: alternatives asked for, -1 = none
+            self._raw = torch.empty(slots, V, **f32)                    # the picked rows' logits before the penalty
+            self.lp_token = torch.zeros(slots, self.max_len + 1, **f32)
+            self.lp_ids = torch.zeros(slots, self.max_len + 1, self.max_logprobs, dtype=torch.int64, device=dev)
+            self.lp_top = torch.zeros(slots, self.max_len + 1, self.max_logprobs, **f32)
         self.busy = [False] * slots
         for j in range(slots):
             self._idle(j)
@@ -619,6 +669,8 @@ class SlotDecodeEngine(_Decoder):
         self.rope_pos[j] = 0
         self.token[j] = self.pad_id
         self.busy[j] = False
+        if self.max_logprobs:
+            self.n_top[j] = -1
         self.kv.release(j)
 
     def _state(self):
@@ -626,8 +678,13 @@ class SlotDecodeEngine(_Decoder):
 
     def _pick_rows(self, logits: torch.Tensor, r: slice, n_open: torch.Tensor) -> None:
         tok = self.token.view(-1)[r]
+        if self.max_logprobs:
+            raw = self._raw[r]
+            raw.copy_(logits)
         ops.repetition_penalty_slots_(logits, self.seq[r], self.cur_len[r], self.penalties[r], self.active[r], self.scratch[r])
         ops.sample_slots(logits, self.temps[r], self.top_ks[r], self.top_ps[r], self.u[r], self.n_new[r], self.active[r], tok)
+        if self.max_logprobs:       # at n_new, before the finish kernel advances it
+            ops.token_logprobs(raw, tok, self.n_top[r], self.n_new[r], self.lp_token[r], self.lp_ids[r], self.lp_top[r])
         ops.slot_finish(tok, self.done[r], self.eos, self.seq[r], self.cur_len[r], self.n_new[r], self.max_new[r], self.active[r],
                         self.pos[r], self.lens[r], self.rope_pos[r], n_open)
 
@@ -672,6 +729,8 @@ class SlotDecodeEngine(_Decoder):
         if a + n == S:
             self._prefill = None
             self.active[j] = 1
+            if self.max_logprobs:
+                self.n_top[j] = pf["n_top"]
             self._seed(j, S)
             self._mrow[j] = j
             self._pick_rows(self._chunk_logits, slice(j, j + 1), self._admit_open)
@@ -679,7 +738,7 @@ class SlotDecodeEngine(_Decoder):
 
     def admit(self, slot: int, input_ids: torch.Tensor, max_new_tokens: int, temperature: float = 0.0, top_k: int = 0,
               top_p: float = 1.0, repetition_penalty: float = 1.0, u: Optional[torch.Tensor] = None, past: int = 0,
-              pages=None, **features) -> torch.Tensor:
+              pages=None, logprobs: Optional[int] = None, **features) -> torch.Tensor:
         """Prefills one request (``input_ids`` [1, S] plus the processor's audio features, passed to ``model.forward``) at B = 1
         into cache row ``slot``, sets the slot's state and picks its first token from the prefill logits with the slot kernels.
         ``temperature <= 0`` is greedy; a sampled request reads ``u`` (its uniforms, one per step, as ``generate()`` draws them
@@ -693,7 +752,11 @@ class SlotDecodeEngine(_Decoder):
         first ``past`` positions of ``input_ids``, so only the suffix is prefilled, as ``generate(past_key_values=...)`` does; the
         chunked form then starts at ``past`` and is taken when the suffix has more than ``PREFILL_ROWS`` rows.  ``pages``
         (``PagedSlotDecodeEngine`` only): the request's page ids for positions 0, 64, 128, ...; they must cover
-        S + max_new_tokens positions, and the first ceil(past / 64) of them hold the conversation's first ``past`` positions."""
+        S + max_new_tokens positions, and the first ceil(past / 64) of them hold the conversation's first ``past`` positions.
+
+        ``logprobs`` (engines with ``max_logprobs`` > 0): None records nothing, 0 the chosen tokens' log-probs, 1..max_logprobs
+        also that many alternatives per token (``token_logprobs_of``)."""
+        n_top = self.check_logprobs(logprobs)
         j = int(slot)
         if not 0 <= j < self.slots:
             raise ValueError(f"slot {slot} out of range [0, {self.slots})")
@@ -723,7 +786,7 @@ class SlotDecodeEngine(_Decoder):
             embeds = self.model.prompt_embeds(input_ids, **features).view(S, -1)
             if self._mixed_in is None:
                 self._mixed_in = torch.zeros(self.slots + self.chunk, embeds.shape[1], dtype=embeds.dtype, device=dev)
-            self._prefill = dict(slot=j, S=S, done=P, embeds=embeds)
+            self._prefill = dict(slot=j, S=S, done=P, embeds=embeds, n_top=n_top)
             self._mrow[j] = -1          # the slot's idle decode row must not overwrite position 0 of the prompt
         else:
             logits = self.kv.prefill(self.model, j, input_ids, P, features)
@@ -744,8 +807,29 @@ class SlotDecodeEngine(_Decoder):
             self.u[j, :w].copy_(u.reshape(-1)[:w])
         self.busy[j] = True
         if not chunked:
+            if self.max_logprobs:
+                self.n_top[j] = n_top
             self._pick_rows(logits, slice(j, j + 1), self._admit_open)
         return self.token.view(-1)
+
+    def check_logprobs(self, logprobs) -> int:
+        """The slot kernels' n_top of a request's ``logprobs`` argument (None -> -1); ValueError unless it is None or an integer
+        in [0, max_logprobs]."""
+        if logprobs is None:
+            return -1
+        if isinstance(logprobs, bool) or not isinstance(logprobs, numbers.Integral):
+            raise ValueError(f"logprobs must be None or an integer, got {logprobs!r}")
+        if not self.max_logprobs:
+            raise ValueError("this engine records no log-probabilities: create it with max_logprobs > 0")
+        if not 0 <= logprobs <= self.max_logprobs:
+            raise ValueError(f"logprobs must be in [0, max_logprobs = {self.max_logprobs}], got {logprobs}")
+        return int(logprobs)
+
+    def token_logprobs_of(self, slot: int, n: int, k: int) -> TokenLogprobs:
+        """Copies of slot ``slot``'s log-probs of its first ``n`` new tokens with ``k`` alternatives each (read before
+        ``retire``)."""
+        j = int(slot)
+        return TokenLogprobs(self.lp_token[j, :n].clone(), self.lp_ids[j, :n, :k].clone(), self.lp_top[j, :n, :k].clone())
 
     def retire(self, slot: int, length: Optional[int] = None) -> torch.Tensor:
         """The slot's sequence [1, prompt + new tokens] (a copy; ``length`` = its ``cur_len`` if the caller already read it, else
@@ -770,7 +854,7 @@ class PagedSlotDecodeEngine(SlotDecodeEngine):
     (``serving.PagePool``)."""
 
     def __init__(self, model: UltravoxModel, slots: int, max_len: int, kv_pages: int, eos_token_ids=None, pad_token_id: int = 0,
-                 use_graph: bool = True):
+                 use_graph: bool = True, max_logprobs: int = 0):
         kv = _PagedKV(model, int(slots), max_len, kv_pages)
         self.kv_pages, self.pool_k, self.pool_v = kv.kv_pages, kv.pool_k, kv.pool_v
-        self._setup(model, int(slots), kv, eos_token_ids, pad_token_id, use_graph)
+        self._setup(model, int(slots), kv, eos_token_ids, pad_token_id, use_graph, max_logprobs)

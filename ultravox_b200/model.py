@@ -19,7 +19,7 @@ from __future__ import annotations
 
 import dataclasses
 import os
-from typing import Optional
+from typing import Optional, Tuple
 
 import torch
 import torch.nn as nn
@@ -220,10 +220,14 @@ class KVCache:
 @dataclasses.dataclass
 class GenerateOutput:
     """``return_dict_in_generate=True`` result: what the reference's conversation mode reads (ref infer.py:131-148), plus the
-    final beam scores of a beam search asked for with ``output_scores=True`` (HF's ``sequences_scores``)."""
+    final beam scores of a beam search asked for with ``output_scores=True`` (HF's ``sequences_scores``).  Without beams,
+    ``scores`` (``output_scores=True``) and ``logits`` (``output_logits=True``) are HF's: one [B, V] fp32 tensor per generated
+    token, the processed scores the token was picked from and the raw LM-head logits."""
     sequences: torch.Tensor
     past_key_values: Optional[KVCache]
     sequences_scores: Optional[torch.Tensor] = None
+    scores: Optional[Tuple[torch.Tensor, ...]] = None
+    logits: Optional[Tuple[torch.Tensor, ...]] = None
 
 
 # ------------------------------------------------------------------------------------------------ the model
@@ -892,7 +896,7 @@ class UltravoxModel(nn.Module):
                  audio_waveforms: Optional[torch.Tensor] = None, audio_num_frames: Optional[torch.Tensor] = None,
                  audio_pad_frames: Optional[torch.Tensor] = None, use_graph: bool = True, num_beams: int = 1,
                  length_penalty: float = 1.0, early_stopping=False, num_return_sequences: int = 1, output_scores: bool = False,
-                 **kwargs):
+                 output_logits: bool = False, **kwargs):
         """``GenerationMixin.generate`` for this model (ref :398-426; arguments as ``LocalInference._generate`` passes them, ref
         infer.py:309-342).  Returns prompt ids followed by the new tokens.
 
@@ -913,6 +917,14 @@ class UltravoxModel(nn.Module):
         decode step (``engine.DecodeEngine``: GEMV linears, device-side positions / EOS / sequence bookkeeping), so the loop
         has no per-token host synchronisation unless a streamer asks for the token.
 
+        ``output_scores`` / ``output_logits`` with ``return_dict_in_generate=True`` (``num_beams == 1``): ``scores`` and
+        ``logits`` of the result are tuples with one [B, V] fp32 tensor per new token, as HF's ``_sample`` returns them:
+        ``logits[t]`` the raw LM-head output of step t, ``scores[t]`` the distribution the token was picked from - the repetition
+        penalty, then (when sampling) ``TemperatureLogitsWarper`` (x / temperature), ``TopKLogitsWarper`` and
+        ``TopPLogitsWarper`` (-inf outside the kept set).  The step records them on the device into [max_new_tokens, B, V]
+        buffers (``uvx_record_scores``), the memory HF holds for them as well; rows that have finished keep getting entries.
+        ``compute_transition_scores`` turns them into per-token scores.
+
         ``num_beams > 1`` runs beam search as hf:generation/utils.py ``_beam_search`` does (the reference passes the argument
         through to ``language_model.generate``, ref :398-426): log-probs, ``repetition_penalty`` applied to them, the top
         ``max(2, 1 + #EOS) * num_beams`` continuations per prompt, hypotheses scored ``sum log-prob / generated_len **
@@ -932,6 +944,8 @@ class UltravoxModel(nn.Module):
         if not isinstance(num_return_sequences, int) or not 1 <= num_return_sequences <= num_beams:
             raise ValueError(f"num_return_sequences ({num_return_sequences!r}) must be in [1, num_beams = {num_beams}]")
         if num_beams > 1:
+            if output_logits and return_dict_in_generate:
+                raise NotImplementedError("output_logits with beam search is not built (per-step beam scores neither)")
             if do_sample:
                 raise NotImplementedError("beam sampling (num_beams > 1 with do_sample=True) is not built")
             if streamer is not None:
@@ -998,9 +1012,11 @@ class UltravoxModel(nn.Module):
             out = self.forward(input_ids[:, P:], None, inputs_embeds[:, P:].contiguous(), past_key_values=cache, logits_to_keep=1)
         eos = sorted(set([eos_token_id] if isinstance(eos_token_id, int) else (eos_token_id or [])))
         pad_id = pad_token_id if pad_token_id is not None else (min(eos) if eos else 0)
+        want_scores, want_logits = bool(return_dict_in_generate and output_scores), bool(return_dict_in_generate and output_logits)
         eng = DecodeEngine(self, B, cache.capacity, use_graph=use_graph, cache=cache, eos_token_ids=eos, pad_token_id=pad_id,
                            temperature=temp, top_k=k_top, top_p=p_top, repetition_penalty=repetition_penalty or 1.0,
-                           generator=generator)
+                           generator=generator, output_scores=want_scores, output_logits=want_logits,
+                           max_new_tokens=max_new_tokens if want_scores or want_logits else None)
         if streamer is not None:
             streamer.put(input_ids)
         tok = eng.begin(input_ids, out.logits.view(B, -1), kv_start)
@@ -1027,7 +1043,22 @@ class UltravoxModel(nn.Module):
             new = new[:, :n_new]
         cache.length = S + n_new - 1                        # the last new token has not been fed yet
         sequences = torch.cat([input_ids, new], dim=1)
-        return GenerateOutput(sequences, cache) if return_dict_in_generate else sequences
+        if not return_dict_in_generate:
+            return sequences
+        scores = tuple(eng.scores[:n_new].unbind(0)) if want_scores else None
+        logits = tuple(eng.raw_logits[:n_new].unbind(0)) if want_logits else None
+        return GenerateOutput(sequences, cache, scores=scores, logits=logits)
+
+    def compute_transition_scores(self, sequences: torch.Tensor, scores: Tuple[torch.Tensor, ...],
+                                  beam_indices: Optional[torch.Tensor] = None, normalize_logits: bool = False) -> torch.Tensor:
+        """transformers' ``GenerationMixin.compute_transition_scores``: [B, new tokens] scores of the generated tokens from the
+        ``scores`` of ``generate(output_scores=True, return_dict_in_generate=True)`` (``normalize_logits=True``: their log-probs)."""
+        from transformers.generation.utils import GenerationMixin
+        V = self.language_model.lm_head.weight.shape[0]
+        if self.config.get_text_config().vocab_size != V:
+            raise ValueError(f"config.get_text_config().vocab_size = {self.config.get_text_config().vocab_size} but the LM head "
+                             f"has {V} rows")
+        return GenerationMixin.compute_transition_scores(self, sequences, scores, beam_indices, normalize_logits)
 
     def _beam_search(self, input_ids: torch.Tensor, forward_kw: dict, kv_start: Optional[torch.Tensor], max_new_tokens: int,
                      eos_token_id, pad_token_id: Optional[int], num_beams: int, length_penalty: float, early_stopping,

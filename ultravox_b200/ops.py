@@ -949,6 +949,57 @@ def slot_finish(tok: torch.Tensor, done: torch.Tensor, eos_ids: Optional[torch.T
                                 lens.data_ptr(), rope_pos.data_ptr(), n_open.data_ptr(), B, _stream()), "uvx_slot_finish")
 
 
+# ------------------------------------------------------------------------------------------ log-probabilities
+LOGPROBS_MAX = 20   # alternatives per token (kLogprobsMax in generate.cu)
+
+
+def token_logprobs(logits: torch.Tensor, tok: torch.Tensor, n_top: torch.Tensor, dst: torch.Tensor, out_lp: torch.Tensor,
+                   out_ids: Optional[torch.Tensor] = None, out_top: Optional[torch.Tensor] = None) -> None:
+    """``uvx_token_logprobs``: raw logits [B, V] fp32, chosen tokens [B] int64, n_top / dst [B] int32 -> at index dst[b] of
+    row b: out_lp [B, cap] fp32 = log_softmax(logits[b])[tok[b]], out_ids [B, cap, n_max] int64 / out_top [B, cap, n_max] fp32 =
+    the n_top[b] largest entries (value desc, index asc) and their log-probs.  Rows with n_top < 0 are not touched."""
+    _cuda(logits, torch.float32, "logits")
+    if logits.dim() != 2 or not logits.is_contiguous():
+        raise ValueError("logits must be a contiguous [B, V] tensor")
+    B, V = logits.shape
+    _rows(tok, torch.int64, B, "tok"), _rows(n_top, torch.int32, B, "n_top"), _rows(dst, torch.int32, B, "dst")
+    _cuda(out_lp, torch.float32, "out_lp")
+    if out_lp.dim() != 2 or out_lp.shape[0] != B or not out_lp.is_contiguous():
+        raise ValueError(f"out_lp must be a contiguous [{B}, cap] tensor, got {tuple(out_lp.shape)}")
+    cap = out_lp.shape[1]
+    n_max = 0
+    if out_ids is not None or out_top is not None:
+        _cuda(out_ids, torch.int64, "out_ids"), _cuda(out_top, torch.float32, "out_top")
+        n_max = out_ids.shape[-1]
+        for t, name in ((out_ids, "out_ids"), (out_top, "out_top")):
+            if t.shape != (B, cap, n_max) or not t.is_contiguous():
+                raise ValueError(f"{name} must be a contiguous [{B}, {cap}, n_max] tensor, got {tuple(t.shape)}")
+    check(lib().uvx_token_logprobs(logits.data_ptr(), B, V, tok.data_ptr(), n_top.data_ptr(), dst.data_ptr(), cap, n_max,
+                                   out_lp.data_ptr(), _p(out_ids), _p(out_top), _stream()), "uvx_token_logprobs")
+
+
+def record_scores(logits: torch.Tensor, temperature: float, top_k: int, top_p: float, step_idx: torch.Tensor,
+                  scores: Optional[torch.Tensor] = None, raw: Optional[torch.Tensor] = None) -> None:
+    """``uvx_record_scores``: logits [B, V] fp32 -> at step s = step_idx[0] of the [steps, B, V] fp32 buffers, raw[s] = the
+    logits as given and scores[s] = HF's processed scores (temperature <= 0: the logits; else x / temperature on the entries the
+    sampler keeps with top_k / top_p, -inf elsewhere)."""
+    _cuda(logits, torch.float32, "logits"), _cuda(step_idx, torch.int32, "step_idx")
+    if logits.dim() != 2 or not logits.is_contiguous():
+        raise ValueError("logits must be a contiguous [B, V] tensor")
+    B, V = logits.shape
+    steps = None
+    for t, name in ((scores, "scores"), (raw, "raw")):
+        if t is not None:
+            _cuda(t, torch.float32, name)
+            if t.dim() != 3 or t.shape[1:] != (B, V) or not t.is_contiguous() or (steps is not None and t.shape[0] != steps):
+                raise ValueError(f"{name} must be a contiguous [steps, {B}, {V}] tensor, got {tuple(t.shape)}")
+            steps = t.shape[0]
+    if steps is None:
+        raise ValueError("record_scores needs scores, raw or both")
+    check(lib().uvx_record_scores(logits.data_ptr(), B, V, float(temperature), int(top_k or 0), float(top_p), step_idx.data_ptr(),
+                                  steps, _p(scores), _p(raw), _stream()), "uvx_record_scores")
+
+
 # ------------------------------------------------------------------------------------------ beam search
 BEAM_MAX = 8        # beams per prompt (kBeamMax in generate.cu)
 BEAM_MAX_K = 64     # candidates per prompt, max(2, 1 + n_eos) * num_beams

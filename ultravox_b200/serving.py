@@ -24,7 +24,7 @@ from typing import Callable, Deque, Dict, List, Optional, Sequence, Tuple
 
 import torch
 
-from .engine import PREFILL_ROWS, PagedSlotDecodeEngine, SlotDecodeEngine
+from .engine import PREFILL_ROWS, PagedSlotDecodeEngine, SlotDecodeEngine, TokenLogprobs
 
 PAGE = 64       # positions per KV page (ops.PAGE)
 
@@ -212,6 +212,7 @@ class _Request:
     past: int = 0
     admitted_at: int = -1
     first_token: Optional[torch.cuda.Event] = None
+    logprobs: Optional[int] = None     # alternatives per token asked for (None: no log-probs)
 
 
 class SlotScheduler:
@@ -231,10 +232,18 @@ class SlotScheduler:
     ``generate(past_key_values=...)`` with those pages as the cache.  ``cached_tokens[id]`` is the number of positions a request
     took from the cache.  Pages nobody holds stay cached until the pool needs them (least recently released first).  Off by
     default because a hit's bits depend on which earlier request computed the shared K / V: its prefill's row count picked
-    its GEMM tiling, so a request can get different bits than when it prefills its whole prompt."""
+    its GEMM tiling, so a request can get different bits than when it prefills its whole prompt.
+
+    ``max_logprobs`` (0..20): requests may ask for per-token log-probabilities with ``submit(..., logprobs=k)``, k <=
+    ``max_logprobs``.  When such a request finishes, ``logprobs[id]`` holds its ``TokenLogprobs`` (filled before ``on_tokens``
+    is called): the chosen tokens' log-probs and their k most likely alternatives, one entry per new token, under the model's
+    raw distribution - the log_softmax of the logits before the repetition penalty, temperature, top-k and top-p, as
+    OpenAI-style ``logprobs`` report them.  (``generate(output_scores=True)`` gives the processed distribution instead.)  With
+    0, the default, the engine allocates nothing for them and its step is unchanged."""
 
     def __init__(self, model, slots: int = 8, max_len: int = 2048, eos_token_ids=None, pad_token_id: Optional[int] = None,
-                 sync_every: int = 8, use_graph: bool = True, kv_pages: Optional[int] = None, prefix_cache: bool = False):
+                 sync_every: int = 8, use_graph: bool = True, kv_pages: Optional[int] = None, prefix_cache: bool = False,
+                 max_logprobs: int = 0):
         eos = sorted(set([eos_token_ids] if isinstance(eos_token_ids, int) else (eos_token_ids or [])))
         pad = pad_token_id if pad_token_id is not None else (min(eos) if eos else 0)     # generate()'s default
         if int(sync_every) < 1:
@@ -243,13 +252,16 @@ class SlotScheduler:
             raise ValueError("prefix_cache shares KV pages between requests: it needs the paged cache (kv_pages=N)")
         self.prefix_cache = bool(prefix_cache)
         self.cached_tokens: Dict[int, int] = {}
+        self.logprobs: Dict[int, TokenLogprobs] = {}
         self.model = model
         self.pool: Optional[PagePool] = None
+        lp = {} if max_logprobs == 0 else dict(max_logprobs=max_logprobs)     # the engine validates it
         if kv_pages is None:
-            self.engine = SlotDecodeEngine(model, slots, max_len, eos_token_ids=eos, pad_token_id=pad, use_graph=use_graph)
+            self.engine = SlotDecodeEngine(model, slots, max_len, eos_token_ids=eos, pad_token_id=pad, use_graph=use_graph,
+                                           **lp)
         else:
             self.engine = PagedSlotDecodeEngine(model, slots, max_len, int(kv_pages), eos_token_ids=eos, pad_token_id=pad,
-                                                use_graph=use_graph)
+                                                use_graph=use_graph, **lp)
             self.pool = PagePool(int(kv_pages))
         self.sync_every = int(sync_every)
         self.steps = 0
@@ -302,7 +314,8 @@ class SlotScheduler:
 
     def submit(self, features: dict, max_new_tokens: int = 20, do_sample: bool = False, temperature: Optional[float] = None,
                top_k: Optional[int] = None, top_p: Optional[float] = None, repetition_penalty: float = 1.0,
-               generator: Optional[torch.Generator] = None, num_beams: int = 1, session: Optional[int] = None) -> int:
+               generator: Optional[torch.Generator] = None, num_beams: int = 1, session: Optional[int] = None,
+               logprobs: Optional[int] = None) -> int:
         """Queues one request: ``features`` is the processor's output for it (``input_ids`` [1, S] and, for audio, its mel or
         waveform fields).  Arguments and defaults are ``generate()``'s: greedy unless ``do_sample``; sampling defaults to
         temperature 1 and top_k 50; ``top_p`` must lie in [0, 1].  A sampled request draws its uniforms here, as ``generate()``
@@ -310,7 +323,12 @@ class SlotScheduler:
 
         ``session``: a turn of that conversation (``open_session``), served like ``generate(past_key_values=...)`` with the
         conversation's cache: ``input_ids`` must extend the ``session_length(sid)`` positions already cached.  One turn per
-        session may be in flight.  With a paged engine, a request that needs more pages than the pool has raises ValueError."""
+        session may be in flight.  With a paged engine, a request that needs more pages than the pool has raises ValueError.
+
+        ``logprobs``: None records nothing; 0 the log-prob of each chosen token; 1..``max_logprobs`` also that many most likely
+        alternatives per token (``logprobs[id]`` once it has finished).  Anything else raises ValueError."""
+        if logprobs is not None:
+            self.engine.check_logprobs(logprobs)
         if num_beams != 1:
             raise NotImplementedError("beam search is not built into the slot engine; use generate(num_beams=...)")
         if top_p is not None and not 0.0 <= float(top_p) <= 1.0:       # NaN fails too
@@ -354,7 +372,7 @@ class SlotScheduler:
         rid = self._next_id
         self._next_id += 1
         self._queue.append(_Request(rid, ids, feats, n, temp, k_top, p_top, float(repetition_penalty or 1.0), u, session,
-                                    prefix))
+                                    prefix, logprobs=None if logprobs is None else int(logprobs)))
         if sess is not None:
             sess.busy = True
         return rid
@@ -388,6 +406,8 @@ class SlotScheduler:
             if self.prefix_cache:
                 self.cached_tokens[r.rid] = PAGE * len(shared)
             feats = {k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in r.features.items()}
+            if r.logprobs is not None:
+                kw["logprobs"] = r.logprobs
             eng.admit(j, r.input_ids, r.max_new, r.temperature, r.top_k, r.top_p, r.penalty, r.u, **kw, **feats)
             r.features, r.u = {}, None
             if long:
@@ -419,6 +439,8 @@ class SlotScheduler:
             if not int(state[0, j]):
                 continue
             r = self._running.pop(j)
+            if r.logprobs is not None:
+                self.logprobs[r.rid] = eng.token_logprobs_of(j, int(state[1, j]) - int(r.input_ids.shape[1]), r.logprobs)
             seq = eng.retire(j, int(state[1, j]))
             if self.pool is not None:   # the conversation keeps every position but the last token, which has not been fed
                 self.pool.release(r.pages, r.session, int(state[1, j]) - 1)
