@@ -258,6 +258,22 @@ int uvx_attention_paged(const uvx_attn_args* a, const int32_t* table, int64_t ta
 int uvx_attention_indexed_paged(const uvx_attn_args* a, int64_t n_pages, const int32_t* table, int64_t table_stride,
                                 const int32_t* kv_row, const int32_t* past, uvx_stream_t stream);
 
+/* FP8 (e4m3) paged KV pool: the same pool layout with 1-byte elements (strides in elements = bytes; torch.float8_e4m3fn), one fp32
+ * scale for K and one for V per layer, kv_scales [L, 2] (positive, finite), read on the device so captured graphs stay valid.
+ *   quantize   (every write into the pool):  q = cvt.rn.satfinite.e4m3(float(x) / s), IEEE fp32 division.  NaN stays NaN (stored
+ *              as 0x7F whatever its sign); +-Inf and anything beyond +-448 become +-448 (host reference, equal up to the sign of
+ *              NaN: (x.float() / s).clamp(-448, 448).to(float8_e4m3fn)).
+ *   dequantize (every read from the pool):   x = bf16_rn(float(q) * s); after it every kernel does the arithmetic of its bf16 twin.
+ * Bytes 0x7F / 0xFF are NaN: keys outside the key bound never reach O (zero-filled / zeroed as in the bf16 kernels).
+ * uvx_attention_paged_fp8          uvx_attention_paged over an e4m3 pool layer, kv_scale = that layer's [K, V] scales.  Bit-identical
+ *                                  to uvx_attention_paged on a bf16 pool holding the dequantized values.  k_rs / v_rs % 16 == 0.
+ * uvx_attention_indexed_paged_fp8  uvx_attention_indexed_paged over an e4m3 pool layer (bf16 wgmma MMAs on the dequantized tiles);
+ *                                  bit-identical to uvx_attention_indexed_paged on a bf16 pool holding the dequantized values.  */
+int uvx_attention_paged_fp8(const uvx_attn_args* a, const int32_t* table, int64_t table_stride, const float* kv_scale,
+                            uvx_stream_t stream);
+int uvx_attention_indexed_paged_fp8(const uvx_attn_args* a, int64_t n_pages, const int32_t* table, int64_t table_stride,
+                                    const int32_t* kv_row, const int32_t* past, const float* kv_scale, uvx_stream_t stream);
+
 /* RoPE on the q and k sections of a fused [rows, (Hq + 2*Hkv) * D] projection, in place
  * (hf:modeling_llama.py:124-168; cos/sin tables [max_pos, D/2] fp32 built by the host exactly like
  * LlamaRotaryEmbedding incl. llama3 scaling, hf:modeling_rope_utils.py:550-626).
@@ -318,6 +334,13 @@ int uvx_rope_kv_append(void* qkv, int64_t B, int64_t row_stride, int Hq, int Hkv
 int uvx_rope_kv_append_map(void* qkv, int64_t rows, int64_t row_stride, int Hq, int Hkv, int D, const float* cos_tab,
                            const float* sin_tab, const int32_t* rope_positions, void* k_cache, void* v_cache,
                            int64_t cache_batch_stride, const int32_t* cache_row, const int32_t* positions, uvx_stream_t stream);
+/* uvx_rope_kv_append_map into an e4m3 cache (the FP8 paged pool, see uvx_attention_paged_fp8): q / k in qkv get the same bits as
+ * uvx_rope_kv_append_map; the stored k / v are the bf16 rows it would store, quantized with kv_scale[0] / kv_scale[1] (this layer's
+ * K and V scales).  Rows with cache_row[r] < 0 write nothing.                                                                   */
+int uvx_rope_kv_append_map_fp8(void* qkv, int64_t rows, int64_t row_stride, int Hq, int Hkv, int D, const float* cos_tab,
+                               const float* sin_tab, const int32_t* rope_positions, void* k_cache, void* v_cache,
+                               int64_t cache_batch_stride, const int32_t* cache_row, const int32_t* positions, const float* kv_scale,
+                               uvx_stream_t stream);
 /* a[i] += delta (and b[i] += delta when b != NULL): advances the device-side positions / lengths after each step     */
 int uvx_add_i32(int32_t* a, int32_t* b, int64_t n, int32_t delta, uvx_stream_t stream);
 /* prefill counterpart of uvx_kv_append: rows b*S + s of the fused projection -> cache[b, past + s] (k and v sections),
@@ -449,6 +472,12 @@ int uvx_kv_page_map(const int32_t* table, int64_t table_stride, const int32_t* c
 int uvx_kv_pages_copy(void* k_row, void* v_row, int64_t row_layer_stride, void* k_pool, void* v_pool, int64_t pool_layer_stride,
                       int64_t L, int64_t row_elems, const int32_t* pages, int64_t p0, int64_t p1, int32_t to_pages,
                       uvx_stream_t stream);
+/* uvx_kv_pages_copy between a bf16 one-row cache and an e4m3 pool (see uvx_attention_paged_fp8): to_pages = 1 quantizes, 0
+ * dequantizes, with layer l's scales kv_scales[2 l] (K) / kv_scales[2 l + 1] (V).  row_elems and both layer strides % 16 == 0;
+ * nothing outside [p0, p1) is written.                                                                                          */
+int uvx_kv_pages_copy_fp8(void* k_row, void* v_row, int64_t row_layer_stride, void* k_pool, void* v_pool, int64_t pool_layer_stride,
+                          int64_t L, int64_t row_elems, const int32_t* pages, int64_t p0, int64_t p1, int32_t to_pages,
+                          const float* kv_scales, uvx_stream_t stream);
 
 /* Shifted causal-LM cross entropy (hf:loss/loss_utils.py:28-67; called through LlamaForCausalLM.forward(labels=)
  * from ref:ultravox/model/ultravox_model.py:328-334).  logits [B*S, V] fp32 (row_stride elements), labels [B, S]

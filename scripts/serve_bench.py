@@ -42,6 +42,9 @@ Per arm: wall time, tokens per second, TTFT p50 / p90, the prompt rows prefilled
 cache, plain and mixed step counts and times.  After the rounds, one more `prefix` run over four different system prompts
 with a pool too small to keep them all cached shows that eviction serves every request.
 
+`--kv-dtype fp8_e4m3` gives every paged scheduler an FP8 (e4m3) pool, whose pages take half the bytes: compare it with the bf16
+pool at equal pool bytes by doubling `--kv-pages`.
+
 Prints the device name and power limit first, then one JSON line per arm."""
 import argparse, json, os, statistics, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -149,15 +152,21 @@ def run_conversations(sched, convs, sessions):
     return wall, ttft, step, split
 
 
+def kv_dtype(args) -> dict:
+    """The paged schedulers' pool element type (``--kv-dtype``); bf16 is the default and passes nothing."""
+    return {} if args.kv_dtype == "bf16" else dict(kv_cache_dtype=args.kv_dtype)
+
+
 def pages_copy_ms(eng, n=4096, reps=5):
     """Admission gather + scatter of n positions (every layer, K and V) between the one-row scratch and the pool."""
     pages = torch.arange(-(-n // ops.PAGE), dtype=torch.int32, device="cuda") % eng.kv_pages
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    ops.kv_pages_copy(eng.cache.k, eng.cache.v, eng.pool_k, eng.pool_v, pages, 0, n, to_pages=False)
+    sc = dict(kv_scales=eng.kv_scales)
+    ops.kv_pages_copy(eng.cache.k, eng.cache.v, eng.pool_k, eng.pool_v, pages, 0, n, to_pages=False, **sc)
     a.record()
     for _ in range(reps):
-        ops.kv_pages_copy(eng.cache.k, eng.cache.v, eng.pool_k, eng.pool_v, pages, 0, n, to_pages=False)
-        ops.kv_pages_copy(eng.cache.k, eng.cache.v, eng.pool_k, eng.pool_v, pages, 0, n, to_pages=True)
+        ops.kv_pages_copy(eng.cache.k, eng.cache.v, eng.pool_k, eng.pool_v, pages, 0, n, to_pages=False, **sc)
+        ops.kv_pages_copy(eng.cache.k, eng.cache.v, eng.pool_k, eng.pool_v, pages, 0, n, to_pages=True, **sc)
     b.record()
     torch.cuda.synchronize()
     return a.elapsed_time(b) / reps
@@ -172,7 +181,7 @@ def main_conversations(args, model, cfg):
     kv_pages = args.kv_pages or 8 * (-(-max_len // ops.PAGE))
     scheds = {}
     if "sessions" in arms:
-        scheds["sessions"] = (SlotScheduler(model, slots=8, max_len=max_len, kv_pages=kv_pages), True)
+        scheds["sessions"] = (SlotScheduler(model, slots=8, max_len=max_len, kv_pages=kv_pages, **kv_dtype(args)), True)
     if "slots" in arms:
         scheds["slots"] = (SlotScheduler(model, slots=8, max_len=max_len), False)
     warm = [c[:2] for c in convs[:8]]
@@ -195,7 +204,8 @@ def main_conversations(args, model, cfg):
                 "plain_step_ms_mean": statistics.fmean(split[False]) if split[False] else None, "plain_steps": len(split[False]),
                 "mixed_step_ms_mean": statistics.fmean(split[True]) if split[True] else None, "mixed_steps": len(split[True])}
         if arm == "sessions":
-            line["kv_pages"] = kv_pages
+            eng = scheds[arm][0].engine
+            line.update(kv_pages=kv_pages, kv_dtype=args.kv_dtype, pool_bytes=eng.pool_k.nbytes + eng.pool_v.nbytes)
             line["gather_plus_scatter_4096_positions_ms"] = pages_copy_ms(scheds[arm][0].engine)
         print(json.dumps(line), flush=True)
 
@@ -236,8 +246,8 @@ def main_system_prompt(args, model, cfg):
     longest = max(r["feats"]["input_ids"].shape[1] + r["budget"] for r in reqs)
     max_len = pages_for(longest) * ops.PAGE
     kv_pages = args.kv_pages or 8 * pages_for(max_len) + pages_for(args.prefix_tokens)
-    scheds = {"paged": SlotScheduler(model, slots=8, max_len=max_len, kv_pages=kv_pages),
-              "prefix": SlotScheduler(model, slots=8, max_len=max_len, kv_pages=kv_pages, prefix_cache=True)}
+    scheds = {"paged": SlotScheduler(model, slots=8, max_len=max_len, kv_pages=kv_pages, **kv_dtype(args)),
+              "prefix": SlotScheduler(model, slots=8, max_len=max_len, kv_pages=kv_pages, prefix_cache=True, **kv_dtype(args))}
     warm = [dict(r, budget=16) for r in reqs[:8]]
     for sched in scheds.values():
         run_slots(sched, warm)
@@ -260,12 +270,13 @@ def main_system_prompt(args, model, cfg):
                 "prompt_rows": rows, "prefill_rows": rows - sum(hits), "cached_positions": hits,
                 "plain_step_ms_mean": statistics.fmean(split[False]) if split[False] else None, "plain_steps": len(split[False]),
                 "mixed_step_ms_mean": statistics.fmean(split[True]) if split[True] else None, "mixed_steps": len(split[True]),
-                "kv_pages": kv_pages, "max_len": max_len}
+                "kv_pages": kv_pages, "max_len": max_len, "kv_dtype": args.kv_dtype,
+                "pool_bytes": sched.engine.pool_k.nbytes + sched.engine.pool_v.nbytes}
         print(json.dumps(line), flush=True)
     # eviction: four system prompts, a pool that holds what 3 requests need at once, so cached prompts must make room
     ev_reqs = make_system_prompt_requests(cfg, 16, args.prefix_tokens, args.seed + 1, n_prompts=4)
     ev_pages = 3 * max(pages_for(r["feats"]["input_ids"].shape[1] + r["budget"]) for r in ev_reqs)
-    sched = SlotScheduler(model, slots=8, max_len=max_len, kv_pages=ev_pages, prefix_cache=True)
+    sched = SlotScheduler(model, slots=8, max_len=max_len, kv_pages=ev_pages, prefix_cache=True, **kv_dtype(args))
     wall, first, step, _, _, split, ids = run_slots(sched, ev_reqs)
     served = sum(i in sched.first_token for i in ids)
     print(json.dumps({"bench": "prefix cache eviction: 16 requests over 4 system prompts", "arm": "prefix-evict",
@@ -395,6 +406,8 @@ def main():
     ap.add_argument("--prefix-tokens", type=int, default=1024, help="system-prompt workload: random text ids in the system prompt")
     ap.add_argument("--turns", type=int, default=4)
     ap.add_argument("--kv-pages", type=int, default=None)
+    ap.add_argument("--kv-dtype", choices=["bf16", "fp8_e4m3"], default="bf16",
+                    help="element type of the paged pool; fp8_e4m3 pages take half the bytes, so pass twice --kv-pages for equal memory")
     args = ap.parse_args()
     if args.arms is None:
         args.arms = "sessions,slots" if args.workload == "conversations" else "static,slots"
@@ -422,7 +435,7 @@ def main():
     sched = SlotScheduler(model, slots=8, max_len=max_len)
     torch.cuda.synchronize()
     build_s = time.perf_counter() - c0
-    paged = SlotScheduler(model, slots=8, max_len=max_len, kv_pages=args.kv_pages) if "paged" in arms else None
+    paged = SlotScheduler(model, slots=8, max_len=max_len, kv_pages=args.kv_pages, **kv_dtype(args)) if "paged" in arms else None
     warm = [dict(r, budget=16) for r in reqs[:8]]
     if "static" in arms:
         run_static(model, warm)

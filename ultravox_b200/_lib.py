@@ -76,6 +76,9 @@ SIGNATURES = {
     "uvx_attention_indexed_paged": (C.c_int, [C.POINTER(AttnArgs), c_i64, c_vp, c_i64, c_vp, c_vp, c_vp]),
     "uvx_kv_page_map": (C.c_int, [c_vp, c_i64, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp]),
     "uvx_kv_pages_copy": (C.c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp]),
+    "uvx_attention_paged_fp8": (C.c_int, [C.POINTER(AttnArgs), c_vp, c_i64, c_vp, c_vp]),
+    "uvx_attention_indexed_paged_fp8": (C.c_int, [C.POINTER(AttnArgs), c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp]),
+    "uvx_kv_pages_copy_fp8": (C.c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp, c_vp]),
     "uvx_rope": (C.c_int, [c_vp, c_i64, c_i64, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp]),
     "uvx_swiglu": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_i64, C.c_int, c_vp]),
     "uvx_splice_plan": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp]),
@@ -88,6 +91,8 @@ SIGNATURES = {
     "uvx_rope_kv_append": (C.c_int, [c_vp, c_i64, c_i64, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp]),
     "uvx_rope_kv_append_map": (C.c_int, [c_vp, c_i64, c_i64, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp,
                                          c_vp]),
+    "uvx_rope_kv_append_map_fp8": (C.c_int, [c_vp, c_i64, c_i64, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp,
+                                             c_vp, c_vp, c_vp]),
     "uvx_add_i32": (C.c_int, [c_vp, c_vp, c_i64, c_i32, c_vp]),
     "uvx_kv_write": (C.c_int, [c_vp, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_vp]),
     "uvx_repetition_penalty": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_f32, c_vp, c_vp]),

@@ -36,6 +36,14 @@ struct PagedAttnParams : AttnParams {
   int64_t table_stride;
 };
 
+// FP8 pool: k / v address e4m3 bytes (strides in elements = bytes); kv_scale [2] holds this layer's K and V scales.
+struct PagedFp8AttnParams : PagedAttnParams {
+  const float* kv_scale;
+};
+
+template <bool kPaged, bool kFp8>
+using AttnParamsT = std::conditional_t<kFp8, PagedFp8AttnParams, std::conditional_t<kPaged, PagedAttnParams, AttnParams>>;
+
 __device__ __forceinline__ void cp_async16(void* dst, const void* src, bool valid) {
   const uint32_t d = (uint32_t)__cvta_generic_to_shared(dst);
   const int sz = valid ? 16 : 0;
@@ -67,15 +75,21 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&t);
 }
 
-template <int D, bool kPaged = false>
-__global__ void __launch_bounds__(kAThreads) attn_fwd_kernel(const std::conditional_t<kPaged, PagedAttnParams, AttnParams> p) {
+// kFp8 (paged only): the pool is e4m3.  Each key tile's raw bytes are double-buffered by cp.async into a staging area after the
+// bf16 tiles (K then V, [64][D] bytes per stage), and dequantized into one bf16 K / V stage right after the wait; from there on the
+// MMA / softmax loop is the bf16 kernel's.  Rows outside the key bound are zero-filled raw bytes, i.e. +0 after dequantization,
+// exactly as the bf16 kernel zero-fills them.
+template <int D, bool kPaged = false, bool kFp8 = false>
+__global__ void __launch_bounds__(kAThreads) attn_fwd_kernel(const AttnParamsT<kPaged, kFp8> p) {
+  static_assert(!kFp8 || kPaged, "the fp8 form is paged");
   pdl_trigger();
   pdl_wait();
   constexpr int LD = D + 8;  // padded row (bf16 elements): 16-byte aligned, conflict-free ldmatrix
   extern __shared__ __align__(16) uint8_t attn_smem[];
   bf16* sQ = reinterpret_cast<bf16*>(attn_smem);
-  bf16* sK = sQ + kAM * LD;       // 2 stages
-  bf16* sV = sK + 2 * kAN * LD;   // 2 stages
+  bf16* sK = sQ + kAM * LD;       // 2 stages (fp8: 1)
+  bf16* sV = sK + (kFp8 ? 1 : 2) * kAN * LD;
+  uint8_t* sRaw = reinterpret_cast<uint8_t*>(sV + (kFp8 ? 1 : 2) * kAN * LD);   // fp8: 2 stages of K, V bytes
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, t4 = lane & 3;
@@ -97,6 +111,11 @@ __global__ void __launch_bounds__(kAThreads) attn_fwd_kernel(const std::conditio
   const int n_tiles = (kv_end + kAN - 1) / kAN;
 
   constexpr int CH = D / 8;  // 16-byte chunks per row
+  float k_sc = 1.f, v_sc = 1.f;
+  if constexpr (kFp8) {
+    k_sc = p.kv_scale[0];
+    v_sc = p.kv_scale[1];
+  }
   auto load_q = [&]() {
     for (int i = tid; i < kAM * CH; i += kAThreads) {
       const int r = i / CH, c = i % CH;
@@ -108,7 +127,19 @@ __global__ void __launch_bounds__(kAThreads) attn_fwd_kernel(const std::conditio
     const int n0 = tile * kAN;
     bf16* dk = sK + stage * kAN * LD;
     bf16* dv = sV + stage * kAN * LD;
-    if constexpr (kPaged) {
+    if constexpr (kFp8) {
+      const int64_t pg = p.table[(int64_t)b * p.table_stride + tile];
+      const uint8_t* kp = reinterpret_cast<const uint8_t*>(p.k) + pg * p.k_bs + (int64_t)hk * D;
+      const uint8_t* vp = reinterpret_cast<const uint8_t*>(p.v) + pg * p.v_bs + (int64_t)hk * D;
+      uint8_t* rk = sRaw + stage * 2 * kAN * D;
+      for (int i = tid; i < kAN * (D / 16); i += kAThreads) {
+        const int r = i / (D / 16), c = i % (D / 16);
+        const bool ok = (n0 + r) < kv_end;
+        const int64_t row = ok ? r : 0;
+        cp_async16(rk + r * D + c * 16, kp + row * p.k_rs + c * 16, ok);
+        cp_async16(rk + kAN * D + r * D + c * 16, vp + row * p.v_rs + c * 16, ok);
+      }
+    } else if constexpr (kPaged) {
       // the tile is one page: row r of the tile is row r of the page (only tiles below kv_end are ever looked up)
       const int64_t pg = p.table[(int64_t)b * p.table_stride + tile];
       const bf16* kp = kb + pg * p.k_bs;
@@ -150,13 +181,25 @@ __global__ void __launch_bounds__(kAThreads) attn_fwd_kernel(const std::conditio
     cp_async_commit();
     cp_async_wait<1>();
     __syncthreads();
+    if constexpr (kFp8) {        // raw stage -> the bf16 K / V tiles
+      const uint8_t* rk = sRaw + stage * 2 * kAN * D;
+      for (int i = tid; i < 2 * kAN * (D / 16); i += kAThreads) {
+        const int which = i / (kAN * (D / 16)), r = (i / (D / 16)) % kAN, c = i % (D / 16);
+        uint4 lo, hi;
+        e4m3x16_dequant(*reinterpret_cast<const uint4*>(rk + which * kAN * D + r * D + c * 16), which ? v_sc : k_sc, lo, hi);
+        uint4* dst = reinterpret_cast<uint4*>((which ? sV : sK) + r * LD + c * 16);
+        dst[0] = lo;
+        dst[1] = hi;
+      }
+      __syncthreads();
+    }
     if (tile == tile0) {
 #pragma unroll
       for (int kk = 0; kk < D / 16; ++kk)
         ldsm_x4(qf[kk][0], qf[kk][1], qf[kk][2], qf[kk][3], sQ + (warp * 16 + (lane & 15)) * LD + kk * 16 + (lane >> 4) * 8);
     }
-    const bf16* tk = sK + stage * kAN * LD;
-    const bf16* tv = sV + stage * kAN * LD;
+    const bf16* tk = sK + (kFp8 ? 0 : stage) * kAN * LD;
+    const bf16* tv = sV + (kFp8 ? 0 : stage) * kAN * LD;
 
     float s[kAN / 8][4];
 #pragma unroll
@@ -264,24 +307,26 @@ __global__ void __launch_bounds__(kAThreads) attn_fwd_kernel(const std::conditio
   }
 }
 
-template <int D, bool kPaged = false>
-static int launch_attn(const uvx_attn_args* a, cudaStream_t st, const int32_t* table = nullptr, int64_t table_stride = 0) {
+template <int D, bool kPaged = false, bool kFp8 = false>
+static int launch_attn(const uvx_attn_args* a, cudaStream_t st, const int32_t* table = nullptr, int64_t table_stride = 0,
+                       const float* kv_scale = nullptr) {
   constexpr int LD = D + 8;
-  const size_t smem = (size_t)(kAM + 4 * kAN) * LD * 2;
+  const size_t smem = kFp8 ? (size_t)(kAM + 2 * kAN) * LD * 2 + 4 * kAN * D : (size_t)(kAM + 4 * kAN) * LD * 2;
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<D, kPaged>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<D, kPaged, kFp8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) {
       set_error("cudaFuncSetAttribute(attn_fwd_kernel<%d>): %s", D, cudaGetErrorString(e));
       return UVX_ERR_CUDA;
     }
     attr = true;
   }
-  std::conditional_t<kPaged, PagedAttnParams, AttnParams> p;
+  AttnParamsT<kPaged, kFp8> p;
   if constexpr (kPaged) {
     p.table = table;
     p.table_stride = table_stride;
   }
+  if constexpr (kFp8) p.kv_scale = kv_scale;
   p.q = (const bf16*)a->q;
   p.k = (const bf16*)a->k;
   p.v = (const bf16*)a->v;
@@ -299,8 +344,8 @@ static int launch_attn(const uvx_attn_args* a, cudaStream_t st, const int32_t* t
   p.block = a->block;
   p.scale_log2 = a->scale * 1.4426950408889634f;
   dim3 grid((unsigned)((a->Sq + kAM - 1) / kAM), (unsigned)a->Hq, (unsigned)a->B);
-  launch_k(attn_fwd_kernel<D, kPaged>, dim3(grid), dim3(kAThreads), smem, st, p);
-  return check_launch("attn_fwd_kernel");
+  launch_k(attn_fwd_kernel<D, kPaged, kFp8>, dim3(grid), dim3(kAThreads), smem, st, p);
+  return check_launch(kFp8 ? "attn_fwd_kernel (fp8 pool)" : "attn_fwd_kernel");
 }
 
 int launch_attn_wg(const uvx_attn_args* a, cudaStream_t st);  // attention_wg.cu (TMA + wgmma, a tile of queries per head)
@@ -357,6 +402,28 @@ extern "C" int uvx_attention_paged(const uvx_attn_args* a, const int32_t* table,
               "uvx_attention_paged: base pointers must be 16-byte aligned");
   return a->D == 64 ? launch_attn<64, true>(a, (cudaStream_t)stream, table, table_stride)
                     : launch_attn<128, true>(a, (cudaStream_t)stream, table, table_stride);
+}
+
+extern "C" int uvx_attention_paged_fp8(const uvx_attn_args* a, const int32_t* table, int64_t table_stride, const float* kv_scale,
+                                       uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(a && a->q && a->k && a->v && a->o && a->kv_len && table && kv_scale, "uvx_attention_paged_fp8: null pointer");
+  UVX_REQUIRE(a->D == 64 || a->D == 128, "uvx_attention_paged_fp8: head_dim must be 64 or 128 (got %lld)", (long long)a->D);
+  UVX_REQUIRE(a->B >= 1 && a->B < 65536 && a->Hq >= 1 && a->Hq < 65536 && a->Hkv >= 1 && a->Hq % a->Hkv == 0 && a->Sq >= 1 &&
+                  a->Skv >= 1,
+              "uvx_attention_paged_fp8: bad shape");
+  UVX_REQUIRE(table_stride >= (a->Skv + kAN - 1) / kAN,
+              "uvx_attention_paged_fp8: a table row of %lld pages cannot cover Skv = %lld", (long long)table_stride, (long long)a->Skv);
+  UVX_REQUIRE(!a->kv_start && !a->lse && a->block == 0 && (!a->causal || a->Sq == 1),
+              "uvx_attention_paged_fp8: no kv_start, no lse, no block mask, causal only with Sq == 1");
+  UVX_REQUIRE(a->k_bs == (int64_t)kAN * a->k_rs && a->v_bs == (int64_t)kAN * a->v_rs,
+              "uvx_attention_paged_fp8: k_bs / v_bs must be one page of 64 rows");
+  UVX_REQUIRE(a->q_rs % 8 == 0 && a->k_rs % 16 == 0 && a->v_rs % 16 == 0 && a->o_rs % 2 == 0 && a->q_bs % 8 == 0,
+              "uvx_attention_paged_fp8: strides must keep 16-byte alignment");
+  UVX_REQUIRE(((uintptr_t)a->q | (uintptr_t)a->k | (uintptr_t)a->v) % 16 == 0 && (uintptr_t)a->o % 4 == 0,
+              "uvx_attention_paged_fp8: base pointers must be 16-byte aligned");
+  return a->D == 64 ? launch_attn<64, true, true>(a, (cudaStream_t)stream, table, table_stride, kv_scale)
+                    : launch_attn<128, true, true>(a, (cudaStream_t)stream, table, table_stride, kv_scale);
 }
 
 // Whisper-encoder entry over the fused projection: qkv [B*S, row_stride] with head h's q / k / v at columns q_col + 64h,

@@ -35,6 +35,14 @@ struct AttnWgPagedParams : AttnWgParams {
   int64_t table_stride;
 };
 
+// FP8 pool: the K / V tensor maps are uint8 maps over the e4m3 pool layer; kv_scale [2] holds this layer's K and V scales.
+struct AttnWgPagedFp8Params : AttnWgPagedParams {
+  const float* kv_scale;
+};
+
+template <bool kPaged, bool kFp8>
+using AttnWgParamsT = std::conditional_t<kFp8, AttnWgPagedFp8Params, std::conditional_t<kPaged, AttnWgPagedParams, AttnWgParams>>;
+
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 t = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&t);
@@ -56,11 +64,16 @@ struct AttnWgSmem {
 
 // kIndexed: the K / V batch coordinate and the causal shift come from device memory (p.kv_row[b], p.past[b]) instead of b and
 // Skv - Sq, so one captured launch serves whichever cache row and prompt offset the host writes between replays.
-template <int D, bool kIndexed = false, bool kPaged = false>
+// kFp8 (paged only): the pool is e4m3.  Thread 0 double-buffers each page's raw K / V bytes by TMA (one {D, 1, 64, 1} uint8 box
+// each, no swizzle) into the second K / V stage's space; after the wait all threads dequantize them into the first stage's 128B-
+// swizzled bf16 panels - the layout the bf16 TMA boxes give - writing zeros for V rows outside [kv_begin, kv_end), then
+// fence.proxy.async before the MMAs, which are the bf16 kernel's.
+template <int D, bool kIndexed = false, bool kPaged = false, bool kFp8 = false>
 __global__ void __launch_bounds__(128, 1)
 attn_wg_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-               const std::conditional_t<kPaged, AttnWgPagedParams, AttnWgParams> p) {
+               const AttnWgParamsT<kPaged, kFp8> p) {
   static_assert(!kPaged || kIndexed, "the paged form is device-indexed");
+  static_assert(!kFp8 || kPaged, "the fp8 form is paged");
   using L = AttnWgSmem<D>;
   constexpr int P = L::kP;
   pdl_trigger();
@@ -92,7 +105,17 @@ attn_wg_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
   }
   __syncthreads();
   pdl_wait();
+  // fp8: raw bytes of stage s, [64][D] each, in the (unused) second bf16 stage: K at rawK(s), V at rawV(s)
+  auto rawK = [&](int s) { return smem + L::kK + P * kPanel + s * kWK * D; };
+  auto rawV = [&](int s) { return smem + L::kV + P * kPanel + s * kWK * D; };
   auto load_kv = [&](int tile, int stage) {
+    if constexpr (kFp8) {
+      mbar_expect_tx(&full[stage], (uint32_t)(2 * kWK * D));
+      const int pg = p.table[(int64_t)kb * p.table_stride + tile];
+      tma_load_4d(rawK(stage), &tmK, 0, hk, 0, pg, &full[stage]);
+      tma_load_4d(rawV(stage), &tmV, 0, hk, 0, pg, &full[stage]);
+      return;
+    }
     mbar_expect_tx(&full[stage], (uint32_t)(2 * P * kPanel));
     if constexpr (kPaged) {
       // the tile is one whole page (only tiles below kv_end are ever looked up)
@@ -117,6 +140,11 @@ attn_wg_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
     if (n_tiles > tile0) load_kv(tile0, 0);
   }
 
+  float k_sc = 1.f, v_sc = 1.f;
+  if constexpr (kFp8) {
+    k_sc = p.kv_scale[0];
+    v_sc = p.kv_scale[1];
+  }
   float o[D / 2];
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
@@ -131,8 +159,23 @@ attn_wg_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
     if (tid == 0 && tile + 1 < n_tiles) load_kv(tile + 1, stage ^ 1);  // that stage was released at the end of the last iteration
     mbar_wait(&full[stage], (uint32_t)((it >> 1) & 1));
     const int n0 = tile * kWK;
-    uint8_t* vst = smem + L::kV + stage * P * kPanel;
-    if (n0 < kv_begin || n0 + kWK > kv_end) {
+    uint8_t* vst = smem + L::kV + (kFp8 ? 0 : stage) * P * kPanel;
+    if constexpr (kFp8) {
+      // 16 raw bytes (16 elements of row r) -> two 16-byte bf16 chunks j, j + 1 of that row, at chunk (j % 8) ^ (r % 8) of panel j / 8
+      for (int i = tid; i < 2 * kWK * (D / 16); i += 128) {
+        const int which = i / (kWK * (D / 16)), r = (i / (D / 16)) % kWK, c = i % (D / 16);
+        const int key = n0 + r;
+        uint4 lo = make_uint4(0u, 0u, 0u, 0u), hi = lo;
+        if (!which || (key >= kv_begin && key < kv_end))
+          e4m3x16_dequant(*reinterpret_cast<const uint4*>((which ? rawV(stage) : rawK(stage)) + r * D + c * 16), which ? v_sc : k_sc, lo, hi);
+        uint8_t* row = smem + (which ? L::kV : L::kK) + (2 * c / 8) * kPanel + r * 128;
+        const int j = (2 * c) % 8;
+        *reinterpret_cast<uint4*>(row + ((j ^ (r & 7)) << 4)) = lo;
+        *reinterpret_cast<uint4*>(row + (((j + 1) ^ (r & 7)) << 4)) = hi;
+      }
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      __syncthreads();
+    } else if (n0 < kv_begin || n0 + kWK > kv_end) {
       // partly valid tile: zero the V rows outside [kv_begin, kv_end) (whole 128-byte rows: the swizzle permutes within a row)
       for (int i = tid; i < P * kWK * 8; i += 128) {
         const int pn = i / (kWK * 8), r = (i / 8) % kWK, c = i % 8;
@@ -145,7 +188,7 @@ attn_wg_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
 
     // ---- S = Q K^T
     float s[kWK / 2];
-    const uint32_t sK = smem_u32(smem + L::kK + stage * P * kPanel);
+    const uint32_t sK = smem_u32(smem + L::kK + (kFp8 ? 0 : stage) * P * kPanel);
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < D / 16; ++k) {
@@ -240,8 +283,10 @@ attn_wg_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
 typedef CUresult (*AwEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-// [B, S, H, D] view of q / k / v (row stride rs, batch stride bs, heads D elements apart), boxes {64 d, 1 head, 64 rows, 1 batch}
-static int aw_encode(CUtensorMap* tm, const void* base, int64_t D, int64_t H, int64_t S, int64_t B, int64_t rs, int64_t bs) {
+// [B, S, H, D] view of q / k / v (row stride rs, batch stride bs, heads D elements apart), boxes {64 d, 1 head, 64 rows, 1 batch};
+// fp8: a uint8 map with unswizzled {D, 1, 64, 1} boxes
+static int aw_encode(CUtensorMap* tm, const void* base, int64_t D, int64_t H, int64_t S, int64_t B, int64_t rs, int64_t bs,
+                     bool fp8 = false) {
   static AwEncodeFn enc = nullptr;
   if (!enc) {
     void* fp = nullptr;
@@ -252,11 +297,13 @@ static int aw_encode(CUtensorMap* tm, const void* base, int64_t D, int64_t H, in
     }
     enc = (AwEncodeFn)fp;
   }
+  const cuuint64_t es_bytes = fp8 ? 1 : 2;
   cuuint64_t dims[4] = {(cuuint64_t)D, (cuuint64_t)H, (cuuint64_t)S, (cuuint64_t)B};
-  cuuint64_t strides[3] = {(cuuint64_t)D * 2, (cuuint64_t)rs * 2, (cuuint64_t)(B > 1 ? bs : rs * S) * 2};
-  cuuint32_t box[4] = {64, 1, 64, 1}, es[4] = {1, 1, 1, 1};
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  cuuint64_t strides[3] = {(cuuint64_t)D * es_bytes, (cuuint64_t)rs * es_bytes, (cuuint64_t)(B > 1 ? bs : rs * S) * es_bytes};
+  cuuint32_t box[4] = {fp8 ? (cuuint32_t)D : 64u, 1, 64, 1}, es[4] = {1, 1, 1, 1};
+  CUresult r = enc(tm, fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides,
+                   box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, fp8 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("uvx_attention (wgmma): cuTensorMapEncodeTiled failed (%d)", (int)r);
     return UVX_ERR_CUDA;
@@ -275,30 +322,31 @@ bool attn_wg_eligible(const uvx_attn_args* a) {
 }
 
 // kPaged: kv_batch is the pool's page count and the K / V maps cover it as {D, Hkv, 64, n_pages}
-template <int D, bool kIndexed, bool kPaged = false>
+template <int D, bool kIndexed, bool kPaged = false, bool kFp8 = false>
 static int launch_wg(const uvx_attn_args* a, int64_t kv_batch, const int32_t* kv_row, const int32_t* past, cudaStream_t st,
-                     const int32_t* table = nullptr, int64_t table_stride = 0) {
+                     const int32_t* table = nullptr, int64_t table_stride = 0, const float* kv_scale = nullptr) {
   using L = AttnWgSmem<D>;
   CUtensorMap tq, tk, tv;
   const int64_t kv_rows = kPaged ? kWK : a->Skv;
   int rc = aw_encode(&tq, a->q, D, a->Hq, a->Sq, a->B, a->q_rs, a->q_bs);
-  if (!rc) rc = aw_encode(&tk, a->k, D, a->Hkv, kv_rows, kv_batch, a->k_rs, a->k_bs);
-  if (!rc) rc = aw_encode(&tv, a->v, D, a->Hkv, kv_rows, kv_batch, a->v_rs, a->v_bs);
+  if (!rc) rc = aw_encode(&tk, a->k, D, a->Hkv, kv_rows, kv_batch, a->k_rs, a->k_bs, kFp8);
+  if (!rc) rc = aw_encode(&tv, a->v, D, a->Hkv, kv_rows, kv_batch, a->v_rs, a->v_bs, kFp8);
   if (rc) return rc;
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(attn_wg_kernel<D, kIndexed, kPaged>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kBytes);
+    cudaError_t e = cudaFuncSetAttribute(attn_wg_kernel<D, kIndexed, kPaged, kFp8>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kBytes);
     if (e != cudaSuccess) {
       set_error("cudaFuncSetAttribute(attn_wg_kernel<%d>): %s", D, cudaGetErrorString(e));
       return UVX_ERR_CUDA;
     }
     attr = true;
   }
-  std::conditional_t<kPaged, AttnWgPagedParams, AttnWgParams> p;
+  AttnWgParamsT<kPaged, kFp8> p;
   if constexpr (kPaged) {
     p.table = table;
     p.table_stride = table_stride;
   }
+  if constexpr (kFp8) p.kv_scale = kv_scale;
   p.o = (bf16*)a->o;
   p.o_rs = a->o_rs;
   p.o_bs = a->o_bs;
@@ -315,8 +363,8 @@ static int launch_wg(const uvx_attn_args* a, int64_t kv_batch, const int32_t* kv
   p.kv_row = kv_row;
   p.past = past;
   dim3 grid((unsigned)((a->Sq + kWQ - 1) / kWQ), (unsigned)a->Hq, (unsigned)a->B);
-  launch_k(attn_wg_kernel<D, kIndexed, kPaged>, grid, dim3(128), (size_t)L::kBytes, st, tq, tk, tv, p);
-  return check_launch("attn_wg_kernel");
+  launch_k(attn_wg_kernel<D, kIndexed, kPaged, kFp8>, grid, dim3(128), (size_t)L::kBytes, st, tq, tk, tv, p);
+  return check_launch(kFp8 ? "attn_wg_kernel (fp8 pool)" : "attn_wg_kernel");
 }
 
 int launch_attn_wg(const uvx_attn_args* a, cudaStream_t st) {
@@ -364,4 +412,28 @@ extern "C" int uvx_attention_indexed_paged(const uvx_attn_args* a, int64_t n_pag
               "uvx_attention_indexed_paged: base pointers must be 16-byte aligned");
   return a->D == 64 ? launch_wg<64, true, true>(a, n_pages, kv_row, past, (cudaStream_t)stream, table, table_stride)
                     : launch_wg<128, true, true>(a, n_pages, kv_row, past, (cudaStream_t)stream, table, table_stride);
+}
+
+extern "C" int uvx_attention_indexed_paged_fp8(const uvx_attn_args* a, int64_t n_pages, const int32_t* table, int64_t table_stride,
+                                               const int32_t* kv_row, const int32_t* past, const float* kv_scale, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(a && a->q && a->k && a->v && a->o && kv_row && past && a->kv_len && table && kv_scale,
+              "uvx_attention_indexed_paged_fp8: null pointer");
+  UVX_REQUIRE(a->D == 64 || a->D == 128, "uvx_attention_indexed_paged_fp8: head_dim must be 64 or 128 (got %lld)", (long long)a->D);
+  UVX_REQUIRE(a->B >= 1 && a->B < 65536 && a->Hq >= 1 && a->Hq < 65536 && a->Hkv >= 1 && a->Hq % a->Hkv == 0 && a->Sq >= 1 &&
+                  a->Skv >= 1 && n_pages >= 1,
+              "uvx_attention_indexed_paged_fp8: bad shape");
+  UVX_REQUIRE(table_stride >= (a->Skv + kWK - 1) / kWK,
+              "uvx_attention_indexed_paged_fp8: a table row of %lld pages cannot cover Skv = %lld", (long long)table_stride,
+              (long long)a->Skv);
+  UVX_REQUIRE(a->causal == 1 && a->block == 0 && !a->kv_start && !a->lse,
+              "uvx_attention_indexed_paged_fp8: causal, no block mask, no kv_start, no lse");
+  UVX_REQUIRE(a->k_bs == (int64_t)kWK * a->k_rs && a->v_bs == (int64_t)kWK * a->v_rs,
+              "uvx_attention_indexed_paged_fp8: k_bs / v_bs must be one page of 64 rows");
+  UVX_REQUIRE(a->q_rs % 8 == 0 && a->k_rs % 16 == 0 && a->v_rs % 16 == 0 && a->q_bs % 8 == 0 && a->o_rs % 2 == 0,
+              "uvx_attention_indexed_paged_fp8: strides must keep 16-byte alignment");
+  UVX_REQUIRE(((uintptr_t)a->q | (uintptr_t)a->k | (uintptr_t)a->v) % 16 == 0 && (uintptr_t)a->o % 4 == 0,
+              "uvx_attention_indexed_paged_fp8: base pointers must be 16-byte aligned");
+  return a->D == 64 ? launch_wg<64, true, true, true>(a, n_pages, kv_row, past, (cudaStream_t)stream, table, table_stride, kv_scale)
+                    : launch_wg<128, true, true, true>(a, n_pages, kv_row, past, (cudaStream_t)stream, table, table_stride, kv_scale);
 }

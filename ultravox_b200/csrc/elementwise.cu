@@ -1,5 +1,7 @@
 // HBM-bound glue kernels of the hot path: RoPE, SwiGLU, mel re-layout, embedding gather + audio splice.
 // All use 128-bit accesses where the layout allows and are pure index / elementwise work (no tensor cores).
+#include <type_traits>
+
 #include "uvx_common.cuh"
 
 namespace uvx {
@@ -165,14 +167,16 @@ __global__ void kv_append_kernel(const bf16* __restrict__ qkv, int64_t row_strid
 // The two row-local steps between the q|k|v projection and the attention: RoPE on the q and k heads (in place, same arithmetic
 // as rope_kernel) and the append of the rotated k and of v to the static KV cache.  Row b goes to cache row b at positions[b]
 // (kMap = false: the decode step), or to cache row cache_row[b] at positions[b], nowhere when cache_row[b] < 0 (kMap = true:
-// the mixed decode + prompt-chunk step of continuous batching).  q and k are rotated either way.
-template <bool kMap>
+// the mixed decode + prompt-chunk step of continuous batching).  q and k are rotated either way.  KV = uint8_t: the cache is an
+// e4m3 pool (strides in elements = bytes) and the k / v rows are quantized with kv_scale[0] / kv_scale[1] as they are stored.
+template <bool kMap, typename KV = bf16>
 __device__ __forceinline__ void rope_kv_append_body(bf16* __restrict__ qkv, int64_t row_stride, int Hq, int Hkv, int D,
                                                     const float* __restrict__ cos_tab, const float* __restrict__ sin_tab,
-                                                    const int32_t* __restrict__ rope_pos, bf16* __restrict__ k_cache,
-                                                    bf16* __restrict__ v_cache, int64_t cache_batch_stride,
+                                                    const int32_t* __restrict__ rope_pos, KV* __restrict__ k_cache,
+                                                    KV* __restrict__ v_cache, int64_t cache_batch_stride,
                                                     const int32_t* __restrict__ positions, const int32_t* __restrict__ cache_row,
-                                                    int64_t B) {
+                                                    int64_t B, const float* __restrict__ kv_scale = nullptr) {
+  constexpr bool kFp8 = std::is_same<KV, uint8_t>::value;
   const int half = D / 2;
   const int vec_per_head = half / 8;
   const int heads = Hq + 2 * Hkv;
@@ -187,9 +191,17 @@ __device__ __forceinline__ void rope_kv_append_body(bf16* __restrict__ qkv, int6
     const int64_t slot = (int64_t)positions[b];
     if (h >= Hq + Hkv) {   // v head: copy both halves
       if (kMap && crow < 0) continue;
-      bf16* dst = v_cache + crow * cache_batch_stride + slot * kv_width + (int64_t)(h - Hq - Hkv) * D + jv * 8;
-      *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(base);
-      *reinterpret_cast<uint4*>(dst + half) = *reinterpret_cast<const uint4*>(base + half);
+      KV* dst = v_cache + crow * cache_batch_stride + slot * kv_width + (int64_t)(h - Hq - Hkv) * D + jv * 8;
+      if constexpr (kFp8) {
+        float f[8];
+        unpack8(*reinterpret_cast<const bf16x8*>(base), f);
+        *reinterpret_cast<uint2*>(dst) = e4m3x8_quant(f, kv_scale[1]);
+        unpack8(*reinterpret_cast<const bf16x8*>(base + half), f);
+        *reinterpret_cast<uint2*>(dst + half) = e4m3x8_quant(f, kv_scale[1]);
+      } else {
+        *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(base);
+        *reinterpret_cast<uint4*>(dst + half) = *reinterpret_cast<const uint4*>(base + half);
+      }
       continue;
     }
     const int64_t pos = (int64_t)rope_pos[b];
@@ -208,9 +220,17 @@ __device__ __forceinline__ void rope_kv_append_body(bf16* __restrict__ qkv, int6
     *reinterpret_cast<bf16x8*>(base) = p1;
     *reinterpret_cast<bf16x8*>(base + half) = p2;
     if (h >= Hq && (!kMap || crow >= 0)) {         // k head: the rotated row also goes to the cache
-      bf16* dst = k_cache + crow * cache_batch_stride + slot * kv_width + (int64_t)(h - Hq) * D + jv * 8;
-      *reinterpret_cast<bf16x8*>(dst) = p1;
-      *reinterpret_cast<bf16x8*>(dst + half) = p2;
+      KV* dst = k_cache + crow * cache_batch_stride + slot * kv_width + (int64_t)(h - Hq) * D + jv * 8;
+      if constexpr (kFp8) {         // the bf16-rounded rotated values, as the bf16 cache holds them
+        float f[8];
+        unpack8(p1, f);
+        *reinterpret_cast<uint2*>(dst) = e4m3x8_quant(f, kv_scale[0]);
+        unpack8(p2, f);
+        *reinterpret_cast<uint2*>(dst + half) = e4m3x8_quant(f, kv_scale[0]);
+      } else {
+        *reinterpret_cast<bf16x8*>(dst) = p1;
+        *reinterpret_cast<bf16x8*>(dst + half) = p2;
+      }
     }
   }
 }
@@ -234,6 +254,18 @@ __global__ void rope_kv_append_map_kernel(bf16* __restrict__ qkv, int64_t row_st
   pdl_wait();
   rope_kv_append_body<true>(qkv, row_stride, Hq, Hkv, D, cos_tab, sin_tab, rope_pos, k_cache, v_cache, cache_batch_stride, positions,
                             cache_row, B);
+}
+
+__global__ void rope_kv_append_map_fp8_kernel(bf16* __restrict__ qkv, int64_t row_stride, int Hq, int Hkv, int D,
+                                              const float* __restrict__ cos_tab, const float* __restrict__ sin_tab,
+                                              const int32_t* __restrict__ rope_pos, uint8_t* __restrict__ k_cache,
+                                              uint8_t* __restrict__ v_cache, int64_t cache_batch_stride,
+                                              const int32_t* __restrict__ cache_row, const int32_t* __restrict__ positions, int64_t B,
+                                              const float* __restrict__ kv_scale) {
+  pdl_trigger();
+  pdl_wait();
+  rope_kv_append_body<true>(qkv, row_stride, Hq, Hkv, D, cos_tab, sin_tab, rope_pos, k_cache, v_cache, cache_batch_stride, positions,
+                            cache_row, B, kv_scale);
 }
 
 __global__ void add_i32_kernel(int32_t* __restrict__ a, int32_t* __restrict__ b2, int64_t n, int32_t delta) {
@@ -410,6 +442,21 @@ extern "C" int uvx_rope_kv_append_map(void* qkv, int64_t rows, int64_t row_strid
   launch_k(rope_kv_append_map_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, (cudaStream_t)stream, (bf16*)qkv, row_stride,
            Hq, Hkv, D, cos_tab, sin_tab, rope_positions, (bf16*)k_cache, (bf16*)v_cache, cache_batch_stride, cache_row, positions, rows);
   return check_launch("rope_kv_append_map_kernel");
+}
+
+extern "C" int uvx_rope_kv_append_map_fp8(void* qkv, int64_t rows, int64_t row_stride, int Hq, int Hkv, int D, const float* cos_tab,
+                                          const float* sin_tab, const int32_t* rope_positions, void* k_cache, void* v_cache,
+                                          int64_t cache_batch_stride, const int32_t* cache_row, const int32_t* positions,
+                                          const float* kv_scale, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(qkv && cos_tab && sin_tab && rope_positions && k_cache && v_cache && cache_row && positions && kv_scale,
+              "uvx_rope_kv_append_map_fp8: null pointer");
+  UVX_REQUIRE(D % 16 == 0 && row_stride % 8 == 0 && cache_batch_stride % 8 == 0 && rows >= 1, "uvx_rope_kv_append_map_fp8: alignment");
+  const int64_t total = rows * (Hq + 2 * Hkv) * (D / 16);
+  launch_k(rope_kv_append_map_fp8_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, (cudaStream_t)stream, (bf16*)qkv,
+           row_stride, Hq, Hkv, D, cos_tab, sin_tab, rope_positions, (uint8_t*)k_cache, (uint8_t*)v_cache, cache_batch_stride, cache_row,
+           positions, rows, kv_scale);
+  return check_launch("rope_kv_append_map_fp8_kernel");
 }
 
 extern "C" int uvx_add_i32(int32_t* a, int32_t* b, int64_t n, int32_t delta, uvx_stream_t stream) {

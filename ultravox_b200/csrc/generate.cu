@@ -986,11 +986,15 @@ __global__ void kv_page_map_kernel(const int32_t* __restrict__ table, int64_t ta
   off_out[r] = p % kPageRows;
 }
 
-// 16-byte vectors of positions [p0, p1) of every layer, K and V: row cache [L][S_max][row_elems] <-> pool [L][n_pages][64][row_elems]
+// 16-byte vectors of positions [p0, p1) of every layer, K and V: row cache [L][S_max][row_elems] <-> pool [L][n_pages][64][row_elems].
+// kFp8: the pool is e4m3 and a vector is 16 elements (16 pool bytes, 32 row bytes), quantized into the pool / dequantized out of it
+// with layer l's scales kv_scales[2 l] (K), kv_scales[2 l + 1] (V); the strides are then counted in 16-element vectors.
+template <bool kFp8>
 __global__ void __launch_bounds__(256) kv_pages_copy_kernel(uint4* __restrict__ k_row, uint4* __restrict__ v_row, int64_t row_layer_vec,
                                                             uint4* __restrict__ k_pool, uint4* __restrict__ v_pool,
                                                             int64_t pool_layer_vec, int64_t L, int64_t vec,
-                                                            const int32_t* __restrict__ pages, int64_t p0, int64_t n, int to_pages) {
+                                                            const int32_t* __restrict__ pages, int64_t p0, int64_t n, int to_pages,
+                                                            const float* __restrict__ kv_scales) {
   pdl_trigger();
   pdl_wait();
   const int64_t per_layer = n * vec;
@@ -1005,10 +1009,23 @@ __global__ void __launch_bounds__(256) kv_pages_copy_kernel(uint4* __restrict__ 
     const int64_t pi = l * pool_layer_vec + (pg * kPageRows + p % kPageRows) * vec + c;
     uint4* row = which ? v_row : k_row;
     uint4* pool = which ? v_pool : k_pool;
-    if (to_pages)
-      pool[pi] = row[ri];
-    else
-      row[ri] = pool[pi];
+    if constexpr (kFp8) {
+      const float s = kv_scales[2 * l + which];
+      if (to_pages) {
+        float f[16];
+        unpack8(*reinterpret_cast<const bf16x8*>(row + 2 * ri), f);
+        unpack8(*reinterpret_cast<const bf16x8*>(row + 2 * ri + 1), f + 8);
+        const uint2 a = e4m3x8_quant(f, s), b = e4m3x8_quant(f + 8, s);
+        pool[pi] = make_uint4(a.x, a.y, b.x, b.y);
+      } else {
+        e4m3x16_dequant(pool[pi], s, row[2 * ri], row[2 * ri + 1]);
+      }
+    } else {
+      if (to_pages)
+        pool[pi] = row[ri];
+      else
+        row[ri] = pool[pi];
+    }
   }
 }
 
@@ -1190,10 +1207,30 @@ extern "C" int uvx_kv_pages_copy(void* k_row, void* v_row, int64_t row_layer_str
   const int64_t total = 2 * L * (p1 - p0) * (row_elems / 8);
   int64_t blocks = (total + 255) / 256;
   if (blocks > 132 * 16) blocks = 132 * 16;
-  launch_k(kv_pages_copy_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, (uint4*)k_row, (uint4*)v_row,
+  launch_k(kv_pages_copy_kernel<false>, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, (uint4*)k_row, (uint4*)v_row,
            row_layer_stride / 8, (uint4*)k_pool, (uint4*)v_pool, pool_layer_stride / 8, L, row_elems / 8, pages, p0, p1 - p0,
-           (int)to_pages);
+           (int)to_pages, (const float*)nullptr);
   return check_launch("kv_pages_copy_kernel");
+}
+
+extern "C" int uvx_kv_pages_copy_fp8(void* k_row, void* v_row, int64_t row_layer_stride, void* k_pool, void* v_pool,
+                                     int64_t pool_layer_stride, int64_t L, int64_t row_elems, const int32_t* pages, int64_t p0, int64_t p1,
+                                     int32_t to_pages, const float* kv_scales, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(k_row && v_row && k_pool && v_pool && pages && kv_scales && L >= 1, "uvx_kv_pages_copy_fp8: null pointer");
+  UVX_REQUIRE(row_elems >= 16 && row_elems % 16 == 0 && row_layer_stride % 16 == 0 && pool_layer_stride % 16 == 0 && p0 >= 0 &&
+                  p1 >= p0 && p1 * row_elems <= row_layer_stride,
+              "uvx_kv_pages_copy_fp8: bad shape");
+  UVX_REQUIRE(((uintptr_t)k_row | (uintptr_t)v_row | (uintptr_t)k_pool | (uintptr_t)v_pool) % 16 == 0,
+              "uvx_kv_pages_copy_fp8: base pointers must be 16-byte aligned");
+  if (p1 == p0) return UVX_OK;
+  const int64_t total = 2 * L * (p1 - p0) * (row_elems / 16);
+  int64_t blocks = (total + 255) / 256;
+  if (blocks > 132 * 16) blocks = 132 * 16;
+  launch_k(kv_pages_copy_kernel<true>, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, (uint4*)k_row, (uint4*)v_row,
+           row_layer_stride / 16, (uint4*)k_pool, (uint4*)v_pool, pool_layer_stride / 16, L, row_elems / 16, pages, p0, p1 - p0,
+           (int)to_pages, kv_scales);
+  return check_launch("kv_pages_copy_kernel (fp8 pool)");
 }
 
 extern "C" int uvx_token_logprobs(const float* logits, int64_t B, int64_t V, const int64_t* tok, const int32_t* n_top,

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -119,6 +120,32 @@ __device__ __forceinline__ bf16x8 pack8(const float* f) {
 #pragma unroll
   for (int i = 0; i < 4; ++i) p.v[i] = __floats2bfloat162_rn(f[2 * i], f[2 * i + 1]);
   return p;
+}
+
+// ---- FP8 (e4m3) paged KV pool (include/uvx.h): quantize q = cvt.rn.satfinite.e4m3(x / s) with IEEE fp32 division (NaN stays
+// NaN, as 0x7F: the division returns the canonical NaN; +-Inf and |x / s| > 448 become +-448), dequantize
+// x = bf16_rn(float(q) * s).  Element i of a packed group sits in byte i.
+__device__ __forceinline__ uint32_t e4m3x2_quant(float lo, float hi, float s) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(__fdiv_rn(hi, s)), "f"(__fdiv_rn(lo, s)));
+  return r;
+}
+__device__ __forceinline__ uint2 e4m3x8_quant(const float* f, float s) {
+  return make_uint2(e4m3x2_quant(f[0], f[1], s) | e4m3x2_quant(f[2], f[3], s) << 16,
+                    e4m3x2_quant(f[4], f[5], s) | e4m3x2_quant(f[6], f[7], s) << 16);
+}
+// two e4m3 (bytes 0, 1 of q) -> packed bf16x2; e4m3 -> f16 is exact
+__device__ __forceinline__ uint32_t e4m3x2_dequant(uint32_t q, float s) {
+  uint32_t h;
+  asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h) : "h"((uint16_t)q));
+  const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&h));
+  __nv_bfloat162 b = __floats2bfloat162_rn(f.x * s, f.y * s);
+  return *reinterpret_cast<uint32_t*>(&b);
+}
+// 16 e4m3 -> 16 bf16 (lo: elements 0..7, hi: 8..15)
+__device__ __forceinline__ void e4m3x16_dequant(const uint4 q, float s, uint4& lo, uint4& hi) {
+  lo = make_uint4(e4m3x2_dequant(q.x, s), e4m3x2_dequant(q.x >> 16, s), e4m3x2_dequant(q.y, s), e4m3x2_dequant(q.y >> 16, s));
+  hi = make_uint4(e4m3x2_dequant(q.z, s), e4m3x2_dequant(q.z >> 16, s), e4m3x2_dequant(q.w, s), e4m3x2_dequant(q.w >> 16, s));
 }
 
 // streaming 128-bit global load that does not allocate in L1 (weights are read once)

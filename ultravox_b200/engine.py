@@ -168,6 +168,20 @@ class _RowKV:
         pass
 
 
+def check_kv_scales(kv_scales, layers: int) -> torch.Tensor:
+    """The FP8 pool's per-layer K / V scales as a new fp32 [layers, 2] tensor (None: all 1); ValueError unless that shape with
+    positive, finite values.  Always a copy: pages already written must be read back with the scales they were written with,
+    whatever the caller does with its own tensor later."""
+    if kv_scales is None:
+        return torch.ones(layers, 2, dtype=torch.float32)
+    t = torch.as_tensor(kv_scales).to(torch.float32, copy=True)
+    if tuple(t.shape) != (layers, 2):
+        raise ValueError(f"kv_scales must have shape [{layers}, 2] (one K and one V scale per layer), got {tuple(t.shape)}")
+    if not bool((torch.isfinite(t) & (t > 0)).all()):
+        raise ValueError("kv_scales must be positive and finite")
+    return t
+
+
 class _PagedKV:
     """The KV cache as a shared pool of 64-position pages, so a request's K / V can outlive its slot.  K and V are
     ``[L, kv_pages + slots, 64, Hkv, D]``: the ``kv_pages`` shareable pages, then one private idle page per slot (an idle row
@@ -180,19 +194,33 @@ class _PagedKV:
 
     ``cache`` is the one-row admission scratch ``[L, 1, max_len, Hkv, D]``: a prompt prefilled at B = 1 gathers its
     conversation's first ``past`` positions there, is prefilled like ``generate(past_key_values=...)``, and its new positions
-    are scattered into its pages."""
+    are scattered into its pages.
+
+    ``kv_cache_dtype="fp8_e4m3"`` makes the pool ``float8_e4m3fn`` with per-layer K / V scales ``kv_scales`` [L, 2] fp32 on the
+    device (default all 1): every write into the pool (the step's append, the admission scatter) quantizes, every read (both
+    attention kernels, the admission gather into the bf16 scratch) dequantizes, as include/uvx.h states.  This class is the
+    only place that knows the pool's element type."""
 
     keeps_kv = True
 
-    def __init__(self, model: UltravoxModel, slots: int, max_len: int, kv_pages: int):
+    def __init__(self, model: UltravoxModel, slots: int, max_len: int, kv_pages: int, kv_cache_dtype: str = "bf16",
+                 kv_scales: Optional[torch.Tensor] = None):
         lm, tc = model.language_model, model.config.text_config
         dev = model.device
         if int(kv_pages) < 1:
             raise ValueError(f"kv_pages must be >= 1, got {kv_pages}")
+        L, nkv, hd = tc.num_hidden_layers, tc.num_key_value_heads, lm.head_dim
+        dtype = {"bf16": torch.bfloat16, "fp8_e4m3": ops.FP8}.get(kv_cache_dtype)
+        if dtype is None:
+            raise ValueError(f"kv_cache_dtype must be 'bf16' or 'fp8_e4m3', got {kv_cache_dtype!r}")
+        self.kv_scales = None
+        if dtype == ops.FP8:
+            self.kv_scales = check_kv_scales(kv_scales, L).to(dev).contiguous()
+        elif kv_scales is not None:
+            raise ValueError("kv_scales are for kv_cache_dtype='fp8_e4m3'")
         self.kv_pages = int(kv_pages)
         self.table_width = -(-int(max_len) // ops.PAGE)
-        L, nkv, hd = tc.num_hidden_layers, tc.num_key_value_heads, lm.head_dim
-        self.pool_k = torch.empty(L, self.kv_pages + slots, ops.PAGE, nkv, hd, dtype=torch.bfloat16, device=dev)
+        self.pool_k = torch.empty(L, self.kv_pages + slots, ops.PAGE, nkv, hd, dtype=dtype, device=dev)
         self.pool_v = torch.empty_like(self.pool_k)
         self.table = torch.full((slots, self.table_width), -1, dtype=torch.int32, device=dev)
         R = max(slots, PREFILL_ROWS)        # the rows of a mixed step (slots decode rows + PREFILL_ROWS - slots chunk rows)
@@ -209,12 +237,13 @@ class _PagedKV:
         nq, nkv, hd = e.heads
         B, R = e.B, qkv.shape[0]
         kp, vp = self.pool_k[li], self.pool_v[li]
-        ops.rope_kv_append_map_(qkv, nq, nkv, hd, e.cos, e.sin, e._mrope[:R], kp, vp, self.page[:R], self.off[:R])
+        sc = None if self.kv_scales is None else self.kv_scales[li]
+        ops.rope_kv_append_map_(qkv, nq, nkv, hd, e.cos, e.sin, e._mrope[:R], kp, vp, self.page[:R], self.off[:R], kv_scale=sc)
         att = torch.empty(R, nq * hd, dtype=torch.bfloat16, device=qkv.device)
-        ops.attention_paged(qkv[:B, :nq * hd], kp, vp, att[:B], nq, hd ** -0.5, self.table, e.lens)
+        ops.attention_paged(qkv[:B, :nq * hd], kp, vp, att[:B], nq, hd ** -0.5, self.table, e.lens, kv_scale=sc)
         if R > B:
             ops.attention_indexed_paged(qkv[B:, :nq * hd].unsqueeze(0), kp, vp, att[B:].unsqueeze(0), nq, hd ** -0.5, self.table,
-                                        *e._mscal.split(1))
+                                        *e._mscal.split(1), kv_scale=sc)
         return att
 
     def prefill(self, model: UltravoxModel, j: int, input_ids: torch.Tensor, past: int, features: dict) -> torch.Tensor:
@@ -223,13 +252,13 @@ class _PagedKV:
         S = int(input_ids.shape[1])
         row = self.cache
         if past:
-            ops.kv_pages_copy(row.k, row.v, self.pool_k, self.pool_v, self.pages, 0, past, to_pages=False)
+            ops.kv_pages_copy(row.k, row.v, self.pool_k, self.pool_v, self.pages, 0, past, to_pages=False, kv_scales=self.kv_scales)
             emb = model.prompt_embeds(input_ids, **features)       # embed + splice the whole prompt, prefill only the new suffix
             out = model.forward(input_ids[:, past:], None, emb[:, past:].contiguous(), past_key_values=KVCache(row.k, row.v, past),
                                 logits_to_keep=1)
         else:
             out = model.forward(input_ids, past_key_values=KVCache(row.k, row.v), logits_to_keep=1, **features)
-        ops.kv_pages_copy(row.k, row.v, self.pool_k, self.pool_v, self.pages, past, S, to_pages=True)
+        ops.kv_pages_copy(row.k, row.v, self.pool_k, self.pool_v, self.pages, past, S, to_pages=True, kv_scales=self.kv_scales)
         return out.logits.view(1, -1)
 
     def install(self, j: int, S: int, n: int, pages) -> None:
@@ -851,10 +880,13 @@ class PagedSlotDecodeEngine(SlotDecodeEngine):
     ``admit`` takes the request's ``pages``.  A prompt of at most ``PREFILL_ROWS`` new rows is prefilled at B = 1 in the
     one-row scratch ``cache`` ``[L, 1, max_len, Hkv, D]`` and scattered into its pages; longer suffixes go through the mixed
     step from ``past`` on.  Page ownership (which pages a request or a conversation holds) is the caller's bookkeeping
-    (``serving.PagePool``)."""
+    (``serving.PagePool``).
+
+    ``kv_cache_dtype="fp8_e4m3"`` (with ``kv_scales`` [L, 2], default all 1) keeps the pool in e4m3: half the bytes per page
+    (``_PagedKV``).  Every step then computes the bits the bf16 engine would on a pool holding the dequantized values."""
 
     def __init__(self, model: UltravoxModel, slots: int, max_len: int, kv_pages: int, eos_token_ids=None, pad_token_id: int = 0,
-                 use_graph: bool = True, max_logprobs: int = 0):
-        kv = _PagedKV(model, int(slots), max_len, kv_pages)
-        self.kv_pages, self.pool_k, self.pool_v = kv.kv_pages, kv.pool_k, kv.pool_v
+                 use_graph: bool = True, max_logprobs: int = 0, kv_cache_dtype: str = "bf16", kv_scales=None):
+        kv = _PagedKV(model, int(slots), max_len, kv_pages, kv_cache_dtype, kv_scales)
+        self.kv_pages, self.pool_k, self.pool_v, self.kv_scales = kv.kv_pages, kv.pool_k, kv.pool_v, kv.kv_scales
         self._setup(model, int(slots), kv, eos_token_ids, pad_token_id, use_graph, max_logprobs)

@@ -316,11 +316,36 @@ def attention_indexed(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Ten
 
 
 PAGE = 64      # positions per KV page: one key tile of both attention kernels
+FP8 = torch.float8_e4m3fn     # the FP8 paged pool's element type (include/uvx.h: quantize / dequantize contract)
+
+
+def _is_fp8_kv(k: torch.Tensor, v: torch.Tensor, name: str = "k_pool / v_pool") -> bool:
+    """Whether a KV pair is an e4m3 pool (True) or bf16 (False); any other dtype, or a mixed pair, raises UvxError."""
+    _cuda(k, None, name), _cuda(v, None, name)
+    if k.dtype not in (BF16, FP8) or v.dtype != k.dtype:
+        raise _lib.UvxError(f"{name} must both be bfloat16 or both float8_e4m3fn, got {k.dtype} / {v.dtype}")
+    return k.dtype == FP8
+
+
+def _kv_scale(scale: Optional[torch.Tensor], fp8: bool, shape: tuple, name: str) -> Optional[int]:
+    """Device pointer of the fp32 scales an fp8 pool needs (contiguous, ``shape``); a bf16 pool takes none."""
+    if not fp8:
+        if scale is not None:
+            raise ValueError(f"{name} is for a float8_e4m3fn pool; this pool is bfloat16")
+        return None
+    if scale is None:
+        raise ValueError(f"a float8_e4m3fn pool needs {name} {list(shape)} fp32")
+    _cuda(scale, torch.float32, name)
+    if tuple(scale.shape) != tuple(shape) or not scale.is_contiguous():
+        raise ValueError(f"{name} must be a contiguous {list(shape)} fp32 tensor, got {tuple(scale.shape)}")
+    return scale.data_ptr()
 
 
 def _pool(k_pool: torch.Tensor, v_pool: torch.Tensor, table: torch.Tensor):
-    """Checks of a paged pool layer [n_pages, 64, Hkv, D] pair and its table [rows, W] int32; returns (n_pages, Hkv, D, W)."""
-    _cuda(k_pool, BF16, "k_pool"), _cuda(v_pool, BF16, "v_pool"), _cuda(table, torch.int32, "table")
+    """Checks of a paged pool layer [n_pages, 64, Hkv, D] pair (bf16 or e4m3) and its table [rows, W] int32; returns
+    (n_pages, Hkv, D, W, fp8)."""
+    fp8 = _is_fp8_kv(k_pool, v_pool)
+    _cuda(table, torch.int32, "table")
     if k_pool.dim() != 4 or k_pool.shape[1] != PAGE or not k_pool.is_contiguous():
         raise ValueError(f"k_pool must be a contiguous pool layer [n_pages, {PAGE}, Hkv, D], got {tuple(k_pool.shape)}")
     if v_pool.shape != k_pool.shape or not v_pool.is_contiguous():
@@ -328,16 +353,19 @@ def _pool(k_pool: torch.Tensor, v_pool: torch.Tensor, table: torch.Tensor):
     if table.dim() != 2 or table.stride(1) != 1:
         raise ValueError(f"table must be [rows, W] int32 with unit column stride, got {tuple(table.shape)}")
     n_pages, _, Hkv, D = k_pool.shape
-    return n_pages, Hkv, D, table.shape[1]
+    return n_pages, Hkv, D, table.shape[1], fp8
 
 
 def attention_paged(q: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor, out: torch.Tensor, Hq: int, scale: float,
-                    table: torch.Tensor, kv_len: torch.Tensor) -> torch.Tensor:
+                    table: torch.Tensor, kv_len: torch.Tensor, kv_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Decode attention through a page table (``uvx_attention_paged``): q [B, Hq * D] (rows of any stride), one pool layer
     k_pool / v_pool [n_pages, 64, Hkv, D], table [>= B, W] int32 (row b: the pages of batch row b's key tiles), kv_len [B] int32
-    -> out [B, Hq * D].  Row b sees keys [0, kv_len[b]); bit-identical to ``attention`` on a contiguous cache holding them."""
+    -> out [B, Hq * D].  Row b sees keys [0, kv_len[b]); bit-identical to ``attention`` on a contiguous cache holding them.
+    A float8_e4m3fn pool takes ``kv_scale`` [2] fp32 (the layer's K and V scales) and runs ``uvx_attention_paged_fp8``:
+    bit-identical to the bf16 form on the dequantized pool."""
     _cuda(q, BF16, "q"), _cuda(out, BF16, "out")
-    n_pages, Hkv, D, W = _pool(k_pool, v_pool, table)
+    n_pages, Hkv, D, W, fp8 = _pool(k_pool, v_pool, table)
+    sc = _kv_scale(kv_scale, fp8, (2,), "kv_scale")
     B = q.shape[0]
     if q.dim() != 2 or q.shape[1] != Hq * D or q.stride(1) != 1 or out.shape != (B, Hq * D) or out.stride(1) != 1:
         raise ValueError(f"q / out must be [B, {Hq * D}] with unit column stride")
@@ -352,17 +380,24 @@ def attention_paged(q: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor,
     a.kv_len = kv_len.data_ptr()
     a.kv_start = None
     a.causal, a.block, a.scale = 0, 0, float(scale)
-    check(lib().uvx_attention_paged(C.byref(a), table.data_ptr(), table.stride(0), _stream()), "uvx_attention_paged")
+    if fp8:
+        check(lib().uvx_attention_paged_fp8(C.byref(a), table.data_ptr(), table.stride(0), sc, _stream()), "uvx_attention_paged_fp8")
+    else:
+        check(lib().uvx_attention_paged(C.byref(a), table.data_ptr(), table.stride(0), _stream()), "uvx_attention_paged")
     return out
 
 
 def attention_indexed_paged(q: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor, out: torch.Tensor, Hq: int, scale: float,
-                            table: torch.Tensor, kv_row: torch.Tensor, past: torch.Tensor, kv_len: torch.Tensor) -> torch.Tensor:
+                            table: torch.Tensor, kv_row: torch.Tensor, past: torch.Tensor, kv_len: torch.Tensor,
+                            kv_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``attention_indexed`` through a page table (``uvx_attention_indexed_paged``): q [B, Sq, Hq * D], one pool layer
     k_pool / v_pool [n_pages, 64, Hkv, D], table [rows, W] int32; kv_row [B] (a table row) / past / kv_len [B] int32 on the
-    device -> out [B, Sq, Hq * D].  Bit-identical to ``attention_indexed`` on a contiguous cache holding the same keys."""
+    device -> out [B, Sq, Hq * D].  Bit-identical to ``attention_indexed`` on a contiguous cache holding the same keys.
+    A float8_e4m3fn pool takes ``kv_scale`` [2] fp32 and runs ``uvx_attention_indexed_paged_fp8`` (bit-identical to the bf16
+    form on the dequantized pool)."""
     _cuda(q, BF16, "q"), _cuda(out, BF16, "out")
-    n_pages, Hkv, D, W = _pool(k_pool, v_pool, table)
+    n_pages, Hkv, D, W, fp8 = _pool(k_pool, v_pool, table)
+    sc = _kv_scale(kv_scale, fp8, (2,), "kv_scale")
     B, Sq = q.shape[0], q.shape[1]
     if q.shape[2] != Hq * D or q.stride(2) != 1 or out.shape != (B, Sq, Hq * D) or out.stride(2) != 1:
         raise ValueError(f"q / out must be [B, Sq, {Hq * D}] with unit column stride")
@@ -376,8 +411,12 @@ def attention_indexed_paged(q: torch.Tensor, k_pool: torch.Tensor, v_pool: torch
     a.kv_len = kv_len.data_ptr()
     a.kv_start = None
     a.causal, a.block, a.scale = 1, 0, float(scale)
-    check(lib().uvx_attention_indexed_paged(C.byref(a), n_pages, table.data_ptr(), table.stride(0), kv_row.data_ptr(), past.data_ptr(),
-                                            _stream()), "uvx_attention_indexed_paged")
+    if fp8:
+        check(lib().uvx_attention_indexed_paged_fp8(C.byref(a), n_pages, table.data_ptr(), table.stride(0), kv_row.data_ptr(),
+                                                    past.data_ptr(), sc, _stream()), "uvx_attention_indexed_paged_fp8")
+    else:
+        check(lib().uvx_attention_indexed_paged(C.byref(a), n_pages, table.data_ptr(), table.stride(0), kv_row.data_ptr(),
+                                                past.data_ptr(), _stream()), "uvx_attention_indexed_paged")
     return out
 
 
@@ -402,12 +441,15 @@ def kv_page_map(table: torch.Tensor, cache_row: torch.Tensor, pos: torch.Tensor,
 
 
 def kv_pages_copy(k_row: torch.Tensor, v_row: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor, pages: torch.Tensor,
-                  p0: int, p1: int, to_pages: bool) -> None:
+                  p0: int, p1: int, to_pages: bool, kv_scales: Optional[torch.Tensor] = None) -> None:
     """Positions [p0, p1) of every layer, K and V, between a contiguous one-row cache [L, 1, S_max, Hkv, D] and the pool
     [L, n_pages, 64, Hkv, D] (``uvx_kv_pages_copy``): position p lives in page pages[p // 64] (int32 on the device), row p % 64.
-    ``to_pages``: row -> pages (scatter), else pages -> row (gather).  Bit-exact."""
+    ``to_pages``: row -> pages (scatter), else pages -> row (gather).  Bit-exact.  A float8_e4m3fn pool takes ``kv_scales``
+    [L, 2] fp32 (``uvx_kv_pages_copy_fp8``): the scatter quantizes, the gather dequantizes into the bf16 row."""
+    fp8 = _is_fp8_kv(k_pool, v_pool)
+    sc = _kv_scale(kv_scales, fp8, (k_pool.shape[0], 2), "kv_scales")
     for t, name in ((k_row, "k_row"), (v_row, "v_row"), (k_pool, "k_pool"), (v_pool, "v_pool")):
-        _cuda(t, BF16, name)
+        _cuda(t, None if name.endswith("pool") else BF16, name)
         if not t.is_contiguous() or t.dim() != 5:
             raise ValueError(f"{name} must be a contiguous 5-D cache")
     _cuda(pages, torch.int32, "pages")
@@ -418,9 +460,12 @@ def kv_pages_copy(k_row: torch.Tensor, v_row: torch.Tensor, k_pool: torch.Tensor
         raise ValueError(f"k_pool / v_pool must be [{L}, n_pages, {PAGE}, {Hkv}, {D}], got {tuple(k_pool.shape)}")
     if not 0 <= p0 <= p1 <= smax or pages.numel() * PAGE < p1:
         raise ValueError(f"positions [{p0}, {p1}) outside the row ({smax}) or the page list ({pages.numel()} pages)")
-    check(lib().uvx_kv_pages_copy(k_row.data_ptr(), v_row.data_ptr(), smax * Hkv * D, k_pool.data_ptr(), v_pool.data_ptr(),
-                                  k_pool.shape[1] * PAGE * Hkv * D, L, Hkv * D, pages.data_ptr(), int(p0), int(p1), int(bool(to_pages)),
-                                  _stream()), "uvx_kv_pages_copy")
+    args = (k_row.data_ptr(), v_row.data_ptr(), smax * Hkv * D, k_pool.data_ptr(), v_pool.data_ptr(), k_pool.shape[1] * PAGE * Hkv * D, L,
+            Hkv * D, pages.data_ptr(), int(p0), int(p1), int(bool(to_pages)))
+    if fp8:
+        check(lib().uvx_kv_pages_copy_fp8(*args, sc, _stream()), "uvx_kv_pages_copy_fp8")
+    else:
+        check(lib().uvx_kv_pages_copy(*args, _stream()), "uvx_kv_pages_copy")
 
 
 def attention_fused_qkv(qkv: torch.Tensor, B: int, S: int, Hq: int, Hkv: int, D: int, scale: float, causal: bool,
@@ -818,16 +863,22 @@ def rope_kv_append_(qkv: torch.Tensor, Hq: int, Hkv: int, D: int, cos: torch.Ten
 
 def rope_kv_append_map_(qkv: torch.Tensor, Hq: int, Hkv: int, D: int, cos: torch.Tensor, sin: torch.Tensor,
                         rope_positions: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, cache_row: torch.Tensor,
-                        positions: torch.Tensor) -> None:
+                        positions: torch.Tensor, kv_scale: Optional[torch.Tensor] = None) -> None:
     """``rope_kv_append_`` with a per-row map: row r is rotated at rope_positions[r] and appended to cache row cache_row[r] at
-    positions[r], or not appended when cache_row[r] < 0 (all three [rows] int32 on the device)."""
+    positions[r], or not appended when cache_row[r] < 0 (all three [rows] int32 on the device).  A float8_e4m3fn cache (the
+    FP8 paged pool) takes ``kv_scale`` [2] fp32 and stores the k / v rows quantized (``uvx_rope_kv_append_map_fp8``)."""
     _cuda(qkv, BF16, "qkv")
+    fp8 = _is_fp8_kv(k_cache, v_cache, "k_cache / v_cache")
+    sc = _kv_scale(kv_scale, fp8, (2,), "kv_scale")
     R = qkv.shape[0]
     for t, name in ((rope_positions, "rope_positions"), (cache_row, "cache_row"), (positions, "positions")):
         _rows(t, torch.int32, R, name)
-    check(lib().uvx_rope_kv_append_map(qkv.data_ptr(), R, qkv.stride(0), Hq, Hkv, D, cos.data_ptr(), sin.data_ptr(),
-                                       rope_positions.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), k_cache.stride(0),
-                                       cache_row.data_ptr(), positions.data_ptr(), _stream()), "uvx_rope_kv_append_map")
+    args = (qkv.data_ptr(), R, qkv.stride(0), Hq, Hkv, D, cos.data_ptr(), sin.data_ptr(), rope_positions.data_ptr(), k_cache.data_ptr(),
+            v_cache.data_ptr(), k_cache.stride(0), cache_row.data_ptr(), positions.data_ptr())
+    if fp8:
+        check(lib().uvx_rope_kv_append_map_fp8(*args, sc, _stream()), "uvx_rope_kv_append_map_fp8")
+    else:
+        check(lib().uvx_rope_kv_append_map(*args, _stream()), "uvx_rope_kv_append_map")
 
 
 def add_i32_(a: torch.Tensor, b: Optional[torch.Tensor], delta: int) -> None:

@@ -24,7 +24,7 @@ from typing import Callable, Deque, Dict, List, Optional, Sequence, Tuple
 
 import torch
 
-from .engine import PREFILL_ROWS, PagedSlotDecodeEngine, SlotDecodeEngine, TokenLogprobs
+from .engine import PREFILL_ROWS, PagedSlotDecodeEngine, SlotDecodeEngine, TokenLogprobs, check_kv_scales
 
 PAGE = 64       # positions per KV page (ops.PAGE)
 
@@ -239,17 +239,36 @@ class SlotScheduler:
     is called): the chosen tokens' log-probs and their k most likely alternatives, one entry per new token, under the model's
     raw distribution - the log_softmax of the logits before the repetition penalty, temperature, top-k and top-p, as
     OpenAI-style ``logprobs`` report them.  (``generate(output_scores=True)`` gives the processed distribution instead.)  With
-    0, the default, the engine allocates nothing for them and its step is unchanged."""
+    0, the default, the engine allocates nothing for them and its step is unchanged.
+
+    ``kv_cache_dtype`` (needs ``kv_pages`` for ``"fp8_e4m3"``): ``"bf16"`` (the default) or ``"fp8_e4m3"``, a pool of
+    ``float8_e4m3fn`` pages that cost half the bytes of bf16 ones, so the same memory holds twice the positions.
+    ``kv_scales`` [num_hidden_layers, 2] (positive, finite; default all 1) are each layer's K and V scales.  Every K / V value
+    written into the pool is stored as q = e4m3(x / s) (round to nearest even, saturating at +-448, NaN kept) and read back as
+    bf16(q * s).  A step's attention therefore sees the dequantized keys, the row's just-appended key included; a B = 1
+    admission prefills its new suffix over its own bf16 K / V (as ``generate(past_key_values=...)`` with the dequantized past
+    does) and only the pages it writes are quantized.  Sessions, the prefix cache, chunked prefill, sampling, the repetition
+    penalty and log-probs work unchanged."""
 
     def __init__(self, model, slots: int = 8, max_len: int = 2048, eos_token_ids=None, pad_token_id: Optional[int] = None,
                  sync_every: int = 8, use_graph: bool = True, kv_pages: Optional[int] = None, prefix_cache: bool = False,
-                 max_logprobs: int = 0):
+                 max_logprobs: int = 0, kv_cache_dtype: str = "bf16", kv_scales=None):
         eos = sorted(set([eos_token_ids] if isinstance(eos_token_ids, int) else (eos_token_ids or [])))
         pad = pad_token_id if pad_token_id is not None else (min(eos) if eos else 0)     # generate()'s default
         if int(sync_every) < 1:
             raise ValueError(f"sync_every must be >= 1, got {sync_every}")
         if prefix_cache and kv_pages is None:
             raise ValueError("prefix_cache shares KV pages between requests: it needs the paged cache (kv_pages=N)")
+        if kv_cache_dtype not in ("bf16", "fp8_e4m3"):
+            raise ValueError(f"kv_cache_dtype must be 'bf16' or 'fp8_e4m3', got {kv_cache_dtype!r}")
+        kv = {}
+        if kv_cache_dtype == "fp8_e4m3":
+            if kv_pages is None:
+                raise ValueError("kv_cache_dtype='fp8_e4m3' is a paged pool: it needs kv_pages=N")
+            kv = dict(kv_cache_dtype=kv_cache_dtype,
+                      kv_scales=check_kv_scales(kv_scales, model.config.text_config.num_hidden_layers))
+        elif kv_scales is not None:
+            raise ValueError("kv_scales are for kv_cache_dtype='fp8_e4m3'")
         self.prefix_cache = bool(prefix_cache)
         self.cached_tokens: Dict[int, int] = {}
         self.logprobs: Dict[int, TokenLogprobs] = {}
@@ -261,7 +280,7 @@ class SlotScheduler:
                                            **lp)
         else:
             self.engine = PagedSlotDecodeEngine(model, slots, max_len, int(kv_pages), eos_token_ids=eos, pad_token_id=pad,
-                                                use_graph=use_graph, **lp)
+                                                use_graph=use_graph, **lp, **kv)
             self.pool = PagePool(int(kv_pages))
         self.sync_every = int(sync_every)
         self.steps = 0
