@@ -420,6 +420,35 @@ int uvx_token_logprobs(const float* logits, int64_t B, int64_t V, const int64_t*
 int uvx_record_scores(const float* logits, int64_t B, int64_t V, float temperature, int32_t top_k, float top_p,
                       const int32_t* step_idx, int64_t steps, float* scores, float* raw, uvx_stream_t stream);
 
+/* Prompt lookup decoding (ultravox_b200/engine.py LookupDecodeEngine; hf:generation/candidate_generator.py
+ * PromptLookupCandidateGenerator and hf:generation/utils.py _assisted_decoding, transformers 5.5): one decode step feeds k + 1
+ * positions of ONE sequence seq[0:cur_len] (its last token not yet fed) - the last token and up to k drafts - and keeps the
+ * picks that agree with the drafts.  All state is on the device ([1] int32 counters), so the step is one graph.
+ * uvx_lookup_draft           one CTA.  Drafts: for n-gram sizes g = min(n, L - 1) .. 1 (L = cur_len[0]) the leftmost earlier
+ *                            occurrence of seq[L - g, L) followed by at least one token; the continuation seq[e, min(e + k, L))
+ *                            of the first size that has one, cut before its first EOS (an EOS first: no drafts, no further
+ *                            search) and to d <= max_new - n_new[0] - 1 (so n_new + d + 1 <= max_new); none when done[0].
+ *                            Writes tok[0..k] (tok[0] = seq[L - 1], tok[1..d] the drafts, tok[d + 1..k] = seq[L - 1]),
+ *                            n_draft[0] = d, and for row i <= k: pos = rope_pos = L - 1 + i, lens = pen_len = L + i,
+ *                            idx = n_new + i; the drafts also go to seq[L, L + d).  1 <= k <= 31, n >= 1.
+ * uvx_lookup_accept          one warp; nothing once done[0].  m = the number of leading i < d with pick[i] == tok[i + 1]; appends
+ *                            pick[0..m] at seq[cur_len], cur_len and n_new grow by m + 1, done[0] = pick[m] in eos_ids or
+ *                            n_new >= max_new.  With accepted (int32 [steps]): accepted[step[0]] = m (when inside), step[0]++.
+ * uvx_repetition_penalty_rows  uvx_repetition_penalty on row b over seq[b * seq_stride, 0:len[b]] with row b's own scratch
+ *                            [b * scratch_stride, ...]: seq_stride 0 lets the rows share one sequence.
+ * uvx_record_scores_rows     uvx_record_scores with per-row destinations: row b at s = idx[b] of scores / raw [steps, V] fp32
+ *                            (nothing when s is outside [0, steps)).                                                          */
+int uvx_lookup_draft(int64_t* seq, const int32_t* cur_len, const int32_t* n_new, int32_t max_new, int32_t k, int32_t n,
+                     const int64_t* eos_ids, int32_t n_eos, const int32_t* done, int64_t* tok, int32_t* n_draft, int32_t* pos,
+                     int32_t* lens, int32_t* rope_pos, int32_t* pen_len, int32_t* idx, uvx_stream_t stream);
+int uvx_lookup_accept(const int64_t* pick, const int64_t* tok, const int32_t* n_draft, const int64_t* eos_ids, int32_t n_eos,
+                      int64_t* seq, int32_t* cur_len, int32_t* n_new, int32_t max_new, int32_t* step, int32_t* accepted, int32_t steps,
+                      int32_t* done, uvx_stream_t stream);
+int uvx_repetition_penalty_rows(float* logits, int64_t B, int64_t V, const int64_t* seq, int64_t seq_stride, const int32_t* len,
+                                float penalty, float* scratch, int64_t scratch_stride, uvx_stream_t stream);
+int uvx_record_scores_rows(const float* logits, int64_t B, int64_t V, float temperature, int32_t top_k, float top_p,
+                           const int32_t* idx, int64_t steps, float* scores, float* raw, uvx_stream_t stream);
+
 /* Beam search (hf:generation/utils.py _beam_search, transformers 5.5, and the helpers above it), one decode step as four
  * launches that read every per-step scalar from device memory.  B prompts, nb <= 8 beams each: row r = b * nb + j.
  * uvx_log_softmax   out[r] = log_softmax(in[r]) in fp32 (in == out allowed).  Beam search scores log-probs; the repetition

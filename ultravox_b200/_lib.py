@@ -104,6 +104,11 @@ SIGNATURES = {
     "uvx_slot_finish": (C.c_int, [c_vp, c_vp, c_vp, c_i32, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
     "uvx_token_logprobs": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp]),
     "uvx_record_scores": (C.c_int, [c_vp, c_i64, c_i64, c_f32, c_i32, c_f32, c_vp, c_i64, c_vp, c_vp, c_vp]),
+    "uvx_lookup_draft": (C.c_int, [c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                   c_vp]),
+    "uvx_lookup_accept": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp, c_vp]),
+    "uvx_repetition_penalty_rows": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_f32, c_vp, c_i64, c_vp]),
+    "uvx_record_scores_rows": (C.c_int, [c_vp, c_i64, c_i64, c_f32, c_i32, c_f32, c_vp, c_i64, c_vp, c_vp, c_vp]),
     "uvx_log_softmax": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_vp]),
     "uvx_beam_select": (C.c_int, [c_vp, c_i64, c_i32, c_i64, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "uvx_beam_update": (C.c_int, [c_vp, c_vp, c_i64, c_i32, c_i32, c_i64, c_vp, c_i32, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp,

@@ -8,6 +8,9 @@
 //   uvx_token_finish        EOS / pad bookkeeping of the finished rows, append to `sequences`, advance positions
 //   uvx_sample_slots        continuous batching: per-row greedy / sampled pick with each row's own settings and uniform
 //   uvx_repetition_penalty_slots   the repetition penalty with each row's own penalty and length
+//   uvx_repetition_penalty_rows    the repetition penalty with each row's own length and scratch (rows may share a sequence)
+//   uvx_lookup_draft        prompt lookup: n-gram search over the sequence, the k + 1 fed tokens and their positions
+//   uvx_lookup_accept       prompt lookup: the picks that agree with the drafts, appended; counters, budget / EOS, the log
 //   uvx_slot_finish         per-row append / budget / EOS bookkeeping; finished and idle rows stay frozen
 //   uvx_log_softmax         beam search scores: log_softmax over each logits row (hf:generation/utils.py _beam_search)
 //   uvx_beam_select         the top K of (log-prob + running beam score) over each prompt's nb * V continuations
@@ -369,21 +372,9 @@ __global__ void __launch_bounds__(1024, 1) sample_slots_kernel(const float* logi
   sample_row<2>(row, V, __frcp_rn(t), top_k[b], top_p[b], u + b * u_stride, n_new + b, 1, 0, out + b);
 }
 
-// One CTA per row: uvx_repetition_penalty's rule with the row's own penalty over seq[b, 0:cur_len[b]]; inactive rows and
-// penalty 1 are skipped.
-__global__ void __launch_bounds__(1024) rep_penalty_slots_kernel(float* logits, int64_t V, const int64_t* seq, int64_t seq_stride,
-                                                                 const int32_t* cur_len, const float* penalty, const int32_t* active,
-                                                                 float* __restrict__ scratch) {
-  pdl_trigger();
-  pdl_wait();
-  const int64_t b = blockIdx.x;
-  if (!active[b]) return;
-  const float pen = penalty[b];
-  if (pen == 1.f) return;
-  const int n = cur_len[b];
-  float* row = logits + b * V;
-  const int64_t* sq = seq + b * seq_stride;
-  float* sc = scratch + b * seq_stride;
+// uvx_repetition_penalty's rule on one row (the caller's CTA) with penalty pen over sq[0:n], staging the original scores in
+// sc[0:n].  The body of rep_penalty_slots_kernel and rep_penalty_rows_kernel.
+__device__ __forceinline__ void penalty_row(float* row, int64_t V, const int64_t* sq, float* __restrict__ sc, int n, float pen) {
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     const int64_t t = sq[i];
     sc[i] = (t >= 0 && t < V) ? row[t] : 0.f;
@@ -396,6 +387,31 @@ __global__ void __launch_bounds__(1024) rep_penalty_slots_kernel(float* logits, 
       row[t] = x < 0.f ? x * pen : x / pen;
     }
   }
+}
+
+// One CTA per row: uvx_repetition_penalty's rule with the row's own penalty over seq[b, 0:cur_len[b]]; inactive rows and
+// penalty 1 are skipped.
+__global__ void __launch_bounds__(1024) rep_penalty_slots_kernel(float* logits, int64_t V, const int64_t* seq, int64_t seq_stride,
+                                                                 const int32_t* cur_len, const float* penalty, const int32_t* active,
+                                                                 float* __restrict__ scratch) {
+  pdl_trigger();
+  pdl_wait();
+  const int64_t b = blockIdx.x;
+  if (!active[b]) return;
+  const float pen = penalty[b];
+  if (pen == 1.f) return;
+  penalty_row(logits + b * V, V, seq + b * seq_stride, scratch + b * seq_stride, cur_len[b], pen);
+}
+
+// One CTA per row: the penalty over seq[b * seq_stride, 0:len[b]] with per-row scratch, so rows may share one sequence
+// (seq_stride 0: prompt lookup checks k + 1 positions of one sequence, row i over its first len[i] tokens).
+__global__ void __launch_bounds__(1024) rep_penalty_rows_kernel(float* logits, int64_t V, const int64_t* seq, int64_t seq_stride,
+                                                                const int32_t* len, float penalty, float* __restrict__ scratch,
+                                                                int64_t scratch_stride) {
+  pdl_trigger();
+  pdl_wait();
+  const int64_t b = blockIdx.x;
+  penalty_row(logits + b * V, V, seq + b * seq_stride, scratch + b * scratch_stride, len[b], penalty);
 }
 
 // One CTA: for each active, unfinished row append tok at seq[b, cur_len[b]], advance cur_len / n_new, finish on an EOS id or
@@ -576,6 +592,8 @@ __global__ void __launch_bounds__(1024, 1) token_logprobs_kernel(const float* lo
 // scores[s, b] = the row after HF's warpers - a copy when temperature <= 0 (greedy: no warper), else x / temperature (IEEE
 // division, TemperatureLogitsWarper) on the entries keep_threshold keeps (TopKLogitsWarper, TopPLogitsWarper) and -inf on the
 // rest.  Either output may be NULL.
+// kRows (uvx_record_scores_rows): per-row destinations instead, row b at index s = step_idx[b] of [steps, V] buffers.
+template <bool kRows>
 __global__ void __launch_bounds__(1024, 1) record_scores_kernel(const float* logits, int64_t V, float temperature, float inv_temp,
                                                                 int top_k, float top_p, const int32_t* step_idx, int64_t steps,
                                                                 int64_t B, float* __restrict__ scores, float* __restrict__ raw) {
@@ -588,10 +606,10 @@ __global__ void __launch_bounds__(1024, 1) record_scores_kernel(const float* log
   __shared__ unsigned long long p_below, p_target;
   __shared__ uint32_t p_prefix;
   const int64_t b = blockIdx.x;
-  const int64_t step = *step_idx;
+  const int64_t step = kRows ? step_idx[b] : *step_idx;
   if (step < 0 || step >= steps) return;
   const float* row = logits + b * V;
-  const int64_t o = (step * B + b) * V;
+  const int64_t o = kRows ? step * V : (step * B + b) * V;
   if (raw)
     for (int64_t i = threadIdx.x; i < V; i += 1024) raw[o + i] = row[i];
   if (!scores) return;
@@ -605,6 +623,121 @@ __global__ void __launch_bounds__(1024, 1) record_scores_kernel(const float* log
   for (int64_t i = threadIdx.x; i < V; i += 1024) {
     const float x = row[i];
     scores[o + i] = f2key(x) >= thr ? x / temperature : -INFINITY;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// Prompt lookup (hf:generation/candidate_generator.py PromptLookupCandidateGenerator, transformers 5.5): one decode step checks
+// k drafted positions of one sequence besides the fed token.  The sequence seq[0:cur_len] is the prompt plus the tokens
+// generated so far; its last token has not been fed yet.
+constexpr int kLookupMaxK = 31;  // drafts per step: k + 1 rows within the decode-form GEMM's 32
+
+// One CTA (1024 threads).  For every continuation start e in [1, L) (L = cur_len), m(e) = the number of tokens, at most
+// min(n, L - 1), that agree going back from e - 1 and from L - 1.  HF tries n-gram sizes from min(n, L - 1) down and takes
+// the leftmost earlier occurrence with a non-empty continuation, so the winner is the largest size g with a match (the block
+// maximum of m) at the smallest e with m(e) >= g (a block minimum).  Drafts: seq[e, min(e + k, L)), cut before the first EOS
+// and to the budget (n_new + d + 1 <= max_new); none when done.  Writes the k + 1 fed tokens (row 0 the last token, rows 1..d
+// the drafts, later rows the last token again), d, each row's cache position / key count / RoPE position (L - 1 + i, L + i,
+// L - 1 + i), penalty length L + i and record index n_new + i, and the drafts into seq[L, L + d).
+__global__ void __launch_bounds__(1024) lookup_draft_kernel(int64_t* seq, const int32_t* cur_len, const int32_t* n_new, int max_new,
+                                                            int k, int n, const int64_t* __restrict__ eos, int n_eos,
+                                                            const int32_t* done, int64_t* tok, int32_t* n_draft, int32_t* pos,
+                                                            int32_t* lens, int32_t* rope_pos, int32_t* pen_len, int32_t* idx) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ int red[32];
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  const int L = *cur_len, nn = *n_new;
+  const int room = max_new - nn - 1;
+  const int nmax = min(n, L - 1);
+  const bool search = !*done && room > 0 && nmax > 0;
+  const int64_t* tail = seq + L - 1;  // tail[-j] is the j-th token from the end
+  int best = 0;
+  if (search) {
+    for (int e = tid + 1; e < L; e += 1024) {
+      const int cap = min(nmax, e);
+      int j = 0;
+      while (j < cap && seq[e - 1 - j] == tail[-j]) ++j;
+      best = max(best, j);
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, o));
+  if (lane == 0) red[w] = best;
+  __syncthreads();
+  int g = red[lane];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) g = max(g, __shfl_xor_sync(0xffffffffu, g, o));
+  __syncthreads();
+  int first = INT_MAX;
+  if (g > 0) {
+    for (int e = tid + g; e < L; e += 1024) {
+      int j = 0;
+      while (j < g && seq[e - 1 - j] == tail[-j]) ++j;
+      if (j == g) { first = e; break; }
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) first = min(first, __shfl_xor_sync(0xffffffffu, first, o));
+  if (lane == 0) red[w] = first;
+  __syncthreads();
+  if (w != 0) return;
+  first = red[lane];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) first = min(first, __shfl_xor_sync(0xffffffffu, first, o));
+  int d = 0;
+  if (g > 0) d = min(min(k, L - first), room);
+  int64_t t = 0;
+  bool stop = false;
+  if (lane < d) {
+    t = seq[first + lane];
+    for (int i = 0; i < n_eos; ++i) stop |= t == eos[i];
+  }
+  const unsigned hit = __ballot_sync(0xffffffffu, stop);
+  if (hit) d = __ffs(hit) - 1;  // drafts end before the first EOS; an EOS first means no drafts (HF looks no further)
+  if (lane < d) seq[L + lane] = t;
+  const int64_t last = *tail;
+  const int64_t tok_in = __shfl_up_sync(0xffffffffu, t, 1);  // lane i feeds draft i - 1
+  if (lane <= k) {
+    tok[lane] = (lane >= 1 && lane <= d) ? tok_in : last;
+    pos[lane] = L - 1 + lane;
+    lens[lane] = L + lane;
+    rope_pos[lane] = L - 1 + lane;
+    pen_len[lane] = L + lane;
+    idx[lane] = nn + lane;
+  }
+  if (lane == 0) *n_draft = d;
+}
+
+// One warp.  n_matches = the leading picks that equal the drafts (pick[i] == tok[i + 1], i < d), the valid tokens are
+// pick[0 : n_matches + 1] (HF _assisted_decoding): appended at seq[cur_len], cur_len and n_new advance by their count, done when
+// the last is an EOS (drafts hold none, so only the last can be) or n_new reaches max_new.  accepted[step] = n_matches and step
+// advances (when accepted is given).  Nothing happens once done.
+__global__ void __launch_bounds__(32) lookup_accept_kernel(const int64_t* pick, const int64_t* tok, const int32_t* n_draft,
+                                                           const int64_t* __restrict__ eos, int n_eos, int64_t* seq, int32_t* cur_len,
+                                                           int32_t* n_new, int max_new, int32_t* step, int32_t* accepted, int steps,
+                                                           int32_t* done) {
+  pdl_trigger();
+  pdl_wait();
+  if (*done) return;
+  const int lane = threadIdx.x;
+  const int d = *n_draft;
+  const bool miss = lane >= d || pick[lane] != tok[lane + 1];
+  const int m = __ffs(__ballot_sync(0xffffffffu, miss)) - 1;  // d <= 31: lane d always misses
+  const int L = *cur_len, nn = *n_new;
+  if (lane <= m) seq[L + lane] = pick[lane];
+  if (lane == 0) {
+    const int64_t t = pick[m];
+    int fin = nn + m + 1 >= max_new;
+    for (int i = 0; i < n_eos; ++i) fin |= t == eos[i];
+    *cur_len = L + m + 1;
+    *n_new = nn + m + 1;
+    *done = fin;
+    if (accepted) {
+      const int s = *step;
+      if (s >= 0 && s < steps) accepted[s] = m;
+      *step = s + 1;
+    }
   }
 }
 
@@ -1098,6 +1231,42 @@ extern "C" int uvx_repetition_penalty_slots(float* logits, int64_t B, int64_t V,
   return check_launch("rep_penalty_slots_kernel");
 }
 
+extern "C" int uvx_repetition_penalty_rows(float* logits, int64_t B, int64_t V, const int64_t* seq, int64_t seq_stride,
+                                           const int32_t* len, float penalty, float* scratch, int64_t scratch_stride,
+                                           uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(logits && seq && len && scratch && B >= 1 && V >= 1 && penalty > 0.f && seq_stride >= 0 && scratch_stride >= 0 &&
+                  (B == 1 || scratch_stride > 0),
+              "uvx_repetition_penalty_rows: bad arguments");
+  launch_k(rep_penalty_rows_kernel, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, seq, seq_stride, len, penalty,
+           scratch, scratch_stride);
+  return check_launch("rep_penalty_rows_kernel");
+}
+
+extern "C" int uvx_lookup_draft(int64_t* seq, const int32_t* cur_len, const int32_t* n_new, int32_t max_new, int32_t k, int32_t n,
+                                const int64_t* eos_ids, int32_t n_eos, const int32_t* done, int64_t* tok, int32_t* n_draft,
+                                int32_t* pos, int32_t* lens, int32_t* rope_pos, int32_t* pen_len, int32_t* idx, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(seq && cur_len && n_new && done && tok && n_draft && pos && lens && rope_pos && pen_len && idx &&
+                  (n_eos == 0 || eos_ids) && n_eos >= 0 && max_new >= 1 && k >= 1 && k <= kLookupMaxK && n >= 1,
+              "uvx_lookup_draft: bad arguments (1 <= k <= %d, n >= 1, max_new >= 1)", kLookupMaxK);
+  launch_k(lookup_draft_kernel, dim3(1), dim3(1024), 0, (cudaStream_t)stream, seq, cur_len, n_new, (int)max_new, (int)k, (int)n,
+           eos_ids, (int)n_eos, done, tok, n_draft, pos, lens, rope_pos, pen_len, idx);
+  return check_launch("lookup_draft_kernel");
+}
+
+extern "C" int uvx_lookup_accept(const int64_t* pick, const int64_t* tok, const int32_t* n_draft, const int64_t* eos_ids, int32_t n_eos,
+                                 int64_t* seq, int32_t* cur_len, int32_t* n_new, int32_t max_new, int32_t* step, int32_t* accepted,
+                                 int32_t steps, int32_t* done, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(pick && tok && n_draft && seq && cur_len && n_new && done && (n_eos == 0 || eos_ids) && n_eos >= 0 && max_new >= 1 &&
+                  (!accepted || (step && steps >= 0)),
+              "uvx_lookup_accept: bad arguments");
+  launch_k(lookup_accept_kernel, dim3(1), dim3(32), 0, (cudaStream_t)stream, pick, tok, n_draft, eos_ids, (int)n_eos, seq, cur_len,
+           n_new, (int)max_new, step, accepted, (int)steps, done);
+  return check_launch("lookup_accept_kernel");
+}
+
 extern "C" int uvx_slot_finish(const int64_t* tok, int32_t* done, const int64_t* eos_ids, int32_t n_eos, int64_t* seq,
                                int64_t seq_stride, int32_t* cur_len, int32_t* n_new, const int32_t* max_new, const int32_t* active,
                                int32_t* pos, int32_t* lens, int32_t* rope_pos, int32_t* n_open, int64_t B, uvx_stream_t stream) {
@@ -1252,7 +1421,19 @@ extern "C" int uvx_record_scores(const float* logits, int64_t B, int64_t V, floa
                   top_p <= 1.f,
               "uvx_record_scores: bad arguments");
   const float t = temperature > 0.f ? temperature : 0.f;
-  launch_k(record_scores_kernel, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, t, t > 0.f ? 1.0f / t : 0.f,
+  launch_k(record_scores_kernel<false>, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, t, t > 0.f ? 1.0f / t : 0.f,
            (int)top_k, top_p, step_idx, steps, B, scores, raw);
   return check_launch("record_scores_kernel");
+}
+
+extern "C" int uvx_record_scores_rows(const float* logits, int64_t B, int64_t V, float temperature, int32_t top_k, float top_p,
+                                      const int32_t* idx, int64_t steps, float* scores, float* raw, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(logits && idx && (scores || raw) && B >= 1 && V >= 1 && V <= (int64_t)1 << 24 && steps >= 1 && top_p >= 0.f &&
+                  top_p <= 1.f,
+              "uvx_record_scores_rows: bad arguments");
+  const float t = temperature > 0.f ? temperature : 0.f;
+  launch_k(record_scores_kernel<true>, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, t, t > 0.f ? 1.0f / t : 0.f,
+           (int)top_k, top_p, idx, steps, B, scores, raw);
+  return check_launch("record_scores_rows_kernel");
 }

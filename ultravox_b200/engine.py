@@ -489,6 +489,135 @@ class DecodeEngine(_Decoder):
         return [self.pos, self.lens, self.rope_pos, self.token, self.cur_len, self.step_idx, self.done, self.all_done]
 
 
+class _SeqKV(_RowKV):
+    """The KV cache of ONE sequence, ``cache`` [L, 1, S_max, Hkv, D], fed by several rows of a step that are consecutive
+    positions of it (prompt lookup): row i appends its K / V at ``pos[i]`` of the one cache row and attends to its first
+    ``lens[i]`` positions, through a K / V batch stride of 0.  The append writes every row before the attention reads, so row i
+    sees the positions rows 0..i-1 wrote in the same step, as a plain decode step of its own would have."""
+
+    def attend(self, e: "_Decoder", li: int, qkv: torch.Tensor) -> torch.Tensor:
+        nq, nkv, hd = e.heads
+        R = qkv.shape[0]
+        kc, vc = self.cache.k[li], self.cache.v[li]
+        smax = kc.shape[1]
+        ops.rope_kv_append_(qkv, nq, nkv, hd, e.cos, e.sin, e.rope_pos, kc.expand(R, -1, -1, -1), vc.expand(R, -1, -1, -1), e.pos)
+        att = torch.empty(R, nq * hd, dtype=torch.bfloat16, device=qkv.device)
+        rs = qkv.stride(0)
+        ops.attention(qkv.data_ptr(), kc.data_ptr(), vc.data_ptr(), att, R, nq, nkv, 1, smax, hd,
+                      (rs, rs, nkv * hd, 0, nkv * hd, 0, nq * hd, nq * hd), hd ** -0.5, False, e.lens, 0, None)
+        return att
+
+
+class LookupDecodeEngine(_Decoder):
+    """Prompt lookup decoding of one sequence (hf:generation/utils.py ``_assisted_decoding`` with
+    hf:generation/candidate_generator.py ``PromptLookupCandidateGenerator``, transformers 5.5).  Every step is one CUDA graph
+    replay over k + 1 rows: ``uvx_lookup_draft`` drafts up to k tokens from the sequence's own earlier n-grams and feeds the
+    last token followed by the drafts, the forward runs the k + 1 rows as positions of the one cache row (``_SeqKV``; the
+    linears on the decode-form GEMM, whose output rows do not depend on each other), each row is picked exactly as plain
+    decoding picks that position (penalty over the sequence up to it, uniform and score index n_new + i), and
+    ``uvx_lookup_accept`` keeps the picks that agree with the drafts plus one.  So the tokens are those of ``DecodeEngine``
+    for the same call, sampled ones included; a step yields 1 to k + 1 of them.
+
+    ``cache`` needs S + max_new_tokens + k positions: the last check writes up to k positions past the budget.  ``accepted``
+    [max_new_tokens] int32 logs each step's accepted draft count (``step_idx`` steps so far); ``cur_len`` / ``n_new`` /
+    ``done`` are the device counters the host reads."""
+
+    def __init__(self, model: UltravoxModel, prompt_len: int, max_new_tokens: int, num_tokens: int, ngram: int = 2,
+                 use_graph: bool = True, cache=None, eos_token_ids=None, pad_token_id: int = 0, temperature: float = 0.0,
+                 top_k: int = 0, top_p: Optional[float] = None, repetition_penalty: float = 1.0,
+                 generator: Optional[torch.Generator] = None, output_scores: bool = False, output_logits: bool = False,
+                 uniforms: Optional[int] = None):
+        """``uniforms``: how many uniforms to draw when sampling, default S + max_new_tokens + 1 - the count ``DecodeEngine``
+        draws (its cache capacity + 1) for the same call, so that a seeded ``generator`` gives the same tokens."""
+        k, n, S, N = int(num_tokens), int(ngram), int(prompt_len), int(max_new_tokens)
+        if not 1 <= k <= ops.LOOKUP_MAX_K:
+            raise ValueError(f"prompt_lookup_num_tokens must be in [1, {ops.LOOKUP_MAX_K}], got {num_tokens}")
+        if n < 1:
+            raise ValueError(f"max_matching_ngram_size must be >= 1, got {ngram}")
+        if N < 1 or S < 1:
+            raise ValueError(f"need a prompt and max_new_tokens >= 1, got S = {S}, max_new_tokens = {N}")
+        need = S + N + k
+        if cache is None:
+            cache = model.new_cache(1, need)
+        if cache.k.shape[1] != 1 or cache.capacity < need:
+            raise ValueError(f"the cache must be one row of at least {need} positions, got {tuple(cache.k.shape[1:3])}")
+        super().__init__(model, k + 1, _SeqKV(cache), eos_token_ids, pad_token_id, use_graph)
+        dev = model.device
+        i32 = dict(dtype=torch.int32, device=dev)
+        self.k, self.ngram, self.prompt_len, self.max_new = k, n, S, N
+        self.seq = torch.zeros(self.max_len + 1, dtype=torch.int64, device=dev)       # the one sequence
+        self.cur_len = torch.zeros(1, **i32)
+        self.n_new = torch.zeros(1, **i32)
+        self.step_idx = torch.zeros(1, **i32)
+        self.done = torch.zeros(1, **i32)
+        self.n_draft = torch.zeros(1, **i32)
+        self.accepted = torch.zeros(N, **i32)
+        self.pen_len = torch.zeros(k + 1, **i32)
+        self.idx = torch.zeros(k + 1, **i32)
+        self.pick = torch.zeros(k + 1, dtype=torch.int64, device=dev)
+        self.temperature, self.top_k = float(temperature or 0.0), int(top_k or 0)
+        self.top_p = 1.0 if top_p is None else float(top_p)
+        if not 0.0 <= self.top_p <= 1.0:
+            raise ValueError(f"top_p must be in [0, 1], got {top_p}")
+        self.penalty = float(repetition_penalty or 1.0)
+        self.u = None
+        if self.temperature > 0:
+            # the uniforms DecodeEngine draws for this call (one per new token), padded for the rows past the budget: row i of a
+            # step reads u[n_new + i] through uvx_sample's (step, row) indexing at a row stride of 1
+            u = torch.rand(int(uniforms or S + N + 1), 1, device=dev, dtype=torch.float32, generator=generator)
+            self.u = torch.cat([u, torch.zeros(k + 1, 1, device=dev, dtype=torch.float32)])
+        self.scratch = torch.empty(k + 1, self.max_len + 1, dtype=torch.float32, device=dev) if self.penalty != 1.0 else None
+        V = model.language_model.lm_head.weight.shape[0]
+        self.scores = torch.empty(N, 1, V, dtype=torch.float32, device=dev) if output_scores else None
+        self.raw_logits = torch.empty(N, 1, V, dtype=torch.float32, device=dev) if output_logits else None
+
+    def begin(self, input_ids: torch.Tensor, first_logits: torch.Tensor) -> None:
+        """After the prompt input_ids [1, S] has been prefilled into the cache: seeds the sequence and the counters and picks the
+        first new token from ``first_logits`` [1, V] fp32 (one row, no drafts)."""
+        S = self.prompt_len
+        if tuple(input_ids.shape) != (1, S):
+            raise ValueError(f"input_ids must be [1, {S}], got {tuple(input_ids.shape)}")
+        self.seq[:S].copy_(input_ids[0])
+        self.cur_len.fill_(S)
+        for t in (self.n_new, self.step_idx, self.done, self.n_draft, self.accepted, self.idx):
+            t.zero_()
+        self.pen_len.fill_(S)
+        self._pick(first_logits.contiguous(), log=False)
+
+    def _pick(self, logits: torch.Tensor, log: bool = True) -> None:
+        """logits [R, V] fp32 of rows 0..R-1 (R = 1: the first token) -> picks, then the accepted tokens and the counters."""
+        R = logits.shape[0]
+        self.logits = logits
+        idx = self.idx[:R]
+        rec = (self.temperature, self.top_k, self.top_p, idx)
+        scores = None if self.scores is None else self.scores.view(self.max_new, -1)
+        raw = None if self.raw_logits is None else self.raw_logits.view(self.max_new, -1)
+        raw_first = raw is not None and self.penalty != 1.0
+        if raw_first:       # the penalty rewrites the logits in place: take the raw copy before it
+            ops.record_scores_rows(logits, *rec, raw=raw)
+        if self.penalty != 1.0:
+            ops.repetition_penalty_rows_(logits, self.seq.view(1, -1).expand(R, -1), self.pen_len[:R], self.penalty,
+                                         self.scratch[:R])
+        if scores is not None or (raw is not None and not raw_first):
+            ops.record_scores_rows(logits, *rec, scores=scores, raw=None if raw_first else raw)
+        pick = self.pick[:R]
+        if self.temperature > 0:
+            ops.sample(logits, self.temperature, self.top_k, self.u, self.n_new, out=pick, top_p=self.top_p)
+        else:
+            ops.argmax(logits, out=pick)
+        ops.lookup_accept(pick, self.token.view(-1)[:R], self.n_draft, self.eos, self.seq, self.cur_len, self.n_new, self.max_new,
+                          self.done, self.step_idx if log else None, self.accepted if log else None)
+
+    def _step(self):
+        ops.lookup_draft(self.seq, self.cur_len, self.n_new, self.max_new, self.k, self.ngram, self.eos, self.done,
+                         self.token.view(-1), self.n_draft, self.pos, self.lens, self.rope_pos, self.pen_len, self.idx)
+        self._pick(self._forward())
+
+    def _state(self):
+        return [self.pos, self.lens, self.rope_pos, self.token, self.cur_len, self.n_new, self.step_idx, self.done, self.n_draft,
+                self.pen_len, self.idx, self.pick]
+
+
 class BeamDecodeEngine(DecodeEngine):
     """Beam search over ``batch`` prompts with ``num_beams`` beams each (row b * num_beams + j), as
     hf:generation/utils.py ``_beam_search``: the forward of ``DecodeEngine._step`` runs unchanged over the batch * num_beams

@@ -896,7 +896,8 @@ class UltravoxModel(nn.Module):
                  audio_waveforms: Optional[torch.Tensor] = None, audio_num_frames: Optional[torch.Tensor] = None,
                  audio_pad_frames: Optional[torch.Tensor] = None, use_graph: bool = True, num_beams: int = 1,
                  length_penalty: float = 1.0, early_stopping=False, num_return_sequences: int = 1, output_scores: bool = False,
-                 output_logits: bool = False, **kwargs):
+                 output_logits: bool = False, prompt_lookup_num_tokens: Optional[int] = None,
+                 max_matching_ngram_size: Optional[int] = None, **kwargs):
         """``GenerationMixin.generate`` for this model (ref :398-426; arguments as ``LocalInference._generate`` passes them, ref
         infer.py:309-342).  Returns prompt ids followed by the new tokens.
 
@@ -934,11 +935,29 @@ class UltravoxModel(nn.Module):
         ``pad_token_id`` (or the first EOS id when that is unset or 0).  With ``return_dict_in_generate=True`` and
         ``output_scores=True`` their scores are in ``sequences_scores``; ``past_key_values`` is None, because the cache rows
         belong to the running beams, not to the returned hypotheses.  Not built: beam sampling (``do_sample=True``), a
-        streamer, conversation KV reuse and per-step ``scores`` / ``beam_indices``."""
+        streamer, conversation KV reuse and per-step ``scores`` / ``beam_indices``.
+
+        ``prompt_lookup_num_tokens=k`` (1..31; None: off) decodes by prompt lookup, as transformers' ``generate`` with the same
+        argument (``PromptLookupCandidateGenerator`` + ``_assisted_decoding``): each step drafts up to k tokens that followed
+        the sequence's last n-gram (``max_matching_ngram_size``, default 2) where it occurred earlier in the prompt or the reply,
+        and checks them in one replay over k + 1 positions (``engine.LookupDecodeEngine``), keeping the drafts that agree with
+        the model's own picks plus one more token.  The tokens are exactly those of plain decoding - greedy or sampled with the
+        same ``generator`` - with every option above except beams; only the number of weight passes changes.  It pays when the
+        reply repeats earlier text (quoted turns, names, numbers, structured output); a step costs about as much as one
+        plain step of k + 1 streams, so with nothing to look up it is slower than plain decoding.  Batch size 1 only
+        (``ValueError`` otherwise, as HF; also for ``num_beams > 1`` or k / n out of range); a padded prompt raises
+        ``NotImplementedError``.  The streamer gets the prompt, the first token, then one ``put`` per step with the tokens that
+        step accepted.  Unlike HF, drafts are not filtered through the logits processors (which never changes the tokens) and
+        never run past ``max_new_tokens``, so the output never has more than ``max_new_tokens`` new tokens.  After the call
+        ``self.lookup_stats`` holds the drafts each step accepted (``accepted``), the step count and the graph bookkeeping."""
         from .engine import DecodeEngine
         unknown = [k for k, v in kwargs.items() if isinstance(v, torch.Tensor)]
         if unknown:
             raise TypeError(f"generate() got unexpected tensor arguments {unknown}")
+        lookup = prompt_lookup_num_tokens is not None
+        if lookup:
+            k_look, n_look = self._check_lookup(input_ids, attention_mask, num_beams, prompt_lookup_num_tokens,
+                                                max_matching_ngram_size)
         if not isinstance(num_beams, int) or not 1 <= num_beams <= ops.BEAM_MAX:
             raise ValueError(f"num_beams must be an integer in [1, {ops.BEAM_MAX}], got {num_beams!r}")
         if not isinstance(num_return_sequences, int) or not 1 <= num_return_sequences <= num_beams:
@@ -988,8 +1007,9 @@ class UltravoxModel(nn.Module):
             return seqs
         has_wave = audio_waveforms is not None and len(audio_waveforms) > 0
         has_mel = audio_values is not None and len(audio_values) > 0
+        extra = k_look if lookup else 0     # the last lookup step writes up to k positions past the budget
         if past_key_values is None:
-            cache = self.new_cache(B, S + max_new_tokens)
+            cache = self.new_cache(B, S + max_new_tokens + extra)
             out = self.forward(input_ids, audio_values, inputs_embeds, None, attention_mask, audio_token_start_idx, audio_lens,
                                audio_token_len, audio_batch_size, cache, logits_to_keep=1, position_ids=position_ids,
                                audio_waveforms=audio_waveforms, audio_num_frames=audio_num_frames, audio_pad_frames=audio_pad_frames)
@@ -998,7 +1018,8 @@ class UltravoxModel(nn.Module):
             if not (0 <= P < S) or past_key_values.k.shape[1] != B:
                 raise ValueError(f"past_key_values holds {P} positions for batch {past_key_values.k.shape[1]}; the prompt has "
                                  f"{S} tokens for batch {B} - it must extend the cached prefix")
-            cache = past_key_values.grown(S + max_new_tokens)
+            plain_cap = max(past_key_values.capacity, S + max_new_tokens)      # the cache plain decoding would use
+            cache = past_key_values.grown(S + max_new_tokens + extra)
             if inputs_embeds is None:                       # embed + splice the whole prompt, prefill only the new suffix
                 if has_wave:
                     tm = self.mel_chunks_from_waveforms(audio_waveforms, audio_num_frames, audio_pad_frames=audio_pad_frames)
@@ -1013,6 +1034,11 @@ class UltravoxModel(nn.Module):
         eos = sorted(set([eos_token_id] if isinstance(eos_token_id, int) else (eos_token_id or [])))
         pad_id = pad_token_id if pad_token_id is not None else (min(eos) if eos else 0)
         want_scores, want_logits = bool(return_dict_in_generate and output_scores), bool(return_dict_in_generate and output_logits)
+        if lookup:
+            return self._lookup_decode(input_ids, out.logits.view(1, -1), cache, k_look, n_look, max_new_tokens, eos, pad_id,
+                                       temp, k_top, p_top, repetition_penalty or 1.0, generator, want_scores, want_logits, streamer,
+                                       use_graph, (S + max_new_tokens if past_key_values is None else plain_cap) + 1,
+                                       return_dict_in_generate)
         eng = DecodeEngine(self, B, cache.capacity, use_graph=use_graph, cache=cache, eos_token_ids=eos, pad_token_id=pad_id,
                            temperature=temp, top_k=k_top, top_p=p_top, repetition_penalty=repetition_penalty or 1.0,
                            generator=generator, output_scores=want_scores, output_logits=want_logits,
@@ -1044,6 +1070,65 @@ class UltravoxModel(nn.Module):
         cache.length = S + n_new - 1                        # the last new token has not been fed yet
         sequences = torch.cat([input_ids, new], dim=1)
         if not return_dict_in_generate:
+            return sequences
+        scores = tuple(eng.scores[:n_new].unbind(0)) if want_scores else None
+        logits = tuple(eng.raw_logits[:n_new].unbind(0)) if want_logits else None
+        return GenerateOutput(sequences, cache, scores=scores, logits=logits)
+
+    @staticmethod
+    def _check_lookup(input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor], num_beams: int, k, n):
+        """``generate``'s argument checks for prompt lookup -> (k, n)."""
+        if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= ops.LOOKUP_MAX_K:
+            raise ValueError(f"prompt_lookup_num_tokens must be an integer in [1, {ops.LOOKUP_MAX_K}] (k + 1 rows of the decode "
+                             f"step), got {k!r}")
+        n = 2 if n is None else n
+        if isinstance(n, bool) or not isinstance(n, int) or n < 1:
+            raise ValueError(f"max_matching_ngram_size must be an integer >= 1, got {n!r}")
+        if input_ids.dim() != 2 or input_ids.shape[0] != 1:
+            raise ValueError("assisted generate is only supported for batch_size = 1")
+        if num_beams > 1:
+            raise ValueError("prompt lookup decoding does not combine with beam search (num_beams must be 1)")
+        if attention_mask is not None and not bool(attention_mask.to(torch.bool).all()):
+            raise NotImplementedError("prompt lookup decoding of a padded prompt is not built")
+        return k, n
+
+    def _lookup_decode(self, input_ids: torch.Tensor, first_logits: torch.Tensor, cache: KVCache, k: int, n: int,
+                       max_new_tokens: int, eos, pad_id: int, temp: float, k_top: int, p_top: float, penalty: float, generator,
+                       want_scores: bool, want_logits: bool, streamer, use_graph: bool, uniforms: int, return_dict: bool):
+        """``generate``'s prompt-lookup loop after the prefill of ``input_ids`` [1, S] into ``cache``."""
+        from .engine import LookupDecodeEngine
+        S = int(input_ids.shape[1])
+        eng = LookupDecodeEngine(self, S, max_new_tokens, k, n, use_graph=use_graph, cache=cache, eos_token_ids=eos,
+                                 pad_token_id=pad_id, temperature=temp, top_k=k_top, top_p=p_top, repetition_penalty=penalty,
+                                 generator=generator, output_scores=want_scores, output_logits=want_logits, uniforms=uniforms)
+        if streamer is not None:
+            streamer.put(input_ids)
+        eng.begin(input_ids, first_logits)
+        steps, emitted = 0, S
+        sync_every = 8          # without a streamer the host looks at the done flag every few steps only
+        while True:
+            if streamer is not None:
+                cur, done = torch.cat([eng.cur_len, eng.done]).tolist()
+                if cur > emitted:           # the tokens this step accepted
+                    streamer.put(eng.seq[emitted:cur].view(1, -1).clone())
+                    emitted = cur
+                if done:
+                    break
+            if steps >= max_new_tokens - 1:     # every step yields at least one token
+                break
+            if streamer is None and steps % sync_every == 0 and bool(int(eng.done)):
+                break
+            eng.step()
+            steps += 1
+        if streamer is not None:
+            streamer.end()
+        n_new, n_steps = torch.cat([eng.n_new, eng.step_idx]).tolist()
+        # the last call's per-step accepted draft counts and graph bookkeeping (what a user tunes k and n by)
+        self.lookup_stats = dict(accepted=eng.accepted[:n_steps].tolist(), steps=n_steps, captures=eng.captures,
+                                 launches_per_step=eng.launches_per_step)
+        cache.length = S + n_new - 1                        # the last new token has not been fed yet
+        sequences = torch.cat([input_ids, eng.seq[S:S + n_new].view(1, -1)], dim=1)
+        if not return_dict:
             return sequences
         scores = tuple(eng.scores[:n_new].unbind(0)) if want_scores else None
         logits = tuple(eng.raw_logits[:n_new].unbind(0)) if want_logits else None

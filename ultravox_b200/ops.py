@@ -1051,6 +1051,112 @@ def record_scores(logits: torch.Tensor, temperature: float, top_k: int, top_p: f
                                   steps, _p(scores), _p(raw), _stream()), "uvx_record_scores")
 
 
+def record_scores_rows(logits: torch.Tensor, temperature: float, top_k: int, top_p: float, idx: torch.Tensor,
+                       scores: Optional[torch.Tensor] = None, raw: Optional[torch.Tensor] = None) -> None:
+    """``uvx_record_scores_rows``: ``record_scores`` with per-row destinations - row b of logits [B, V] fp32 goes to index
+    s = idx[b] ([B] int32) of the [steps, V] fp32 buffers (nothing when s is outside [0, steps))."""
+    _cuda(logits, torch.float32, "logits")
+    if logits.dim() != 2 or not logits.is_contiguous():
+        raise ValueError("logits must be a contiguous [B, V] tensor")
+    B, V = logits.shape
+    _rows(idx, torch.int32, B, "idx")
+    steps = None
+    for t, name in ((scores, "scores"), (raw, "raw")):
+        if t is not None:
+            _cuda(t, torch.float32, name)
+            if t.dim() != 2 or t.shape[1] != V or not t.is_contiguous() or (steps is not None and t.shape[0] != steps):
+                raise ValueError(f"{name} must be a contiguous [steps, {V}] tensor, got {tuple(t.shape)}")
+            steps = t.shape[0]
+    if steps is None:
+        raise ValueError("record_scores_rows needs scores, raw or both")
+    check(lib().uvx_record_scores_rows(logits.data_ptr(), B, V, float(temperature), int(top_k or 0), float(top_p), idx.data_ptr(),
+                                       steps, _p(scores), _p(raw), _stream()), "uvx_record_scores_rows")
+
+
+# ------------------------------------------------------------------------------------------ prompt lookup
+LOOKUP_MAX_K = 31   # drafts per step (kLookupMaxK in generate.cu): k + 1 rows within the decode-form GEMM's 32
+
+
+def repetition_penalty_rows_(logits: torch.Tensor, seq: torch.Tensor, lens: torch.Tensor, penalty: float,
+                             scratch: torch.Tensor) -> torch.Tensor:
+    """``uvx_repetition_penalty_rows``: HF's repetition penalty on row b of logits [B, V] fp32 over seq[b, :lens[b]], in place.
+    seq [B, W] int64 with unit column stride and any row stride (0: the rows share one sequence, e.g. ``s.expand(B, -1)``),
+    lens [B] int32, scratch fp32 [B, >= W] with its own rows."""
+    _cuda(logits, torch.float32, "logits")
+    if logits.dim() != 2 or not logits.is_contiguous():
+        raise ValueError("logits must be a contiguous [B, V] tensor")
+    B, V = logits.shape
+    _seq_rows(seq, torch.int64, B, "seq"), _rows(lens, torch.int32, B, "lens"), _seq_rows(scratch, torch.float32, B, "scratch")
+    if scratch.shape[1] < seq.shape[1] or (B > 1 and scratch.stride(0) < scratch.shape[1]):
+        raise ValueError("scratch must have its own row of at least seq.shape[1] entries per row")
+    if not float(penalty) > 0.0:
+        raise ValueError(f"penalty must be > 0, got {penalty}")
+    check(lib().uvx_repetition_penalty_rows(logits.data_ptr(), B, V, seq.data_ptr(), seq.stride(0), lens.data_ptr(), float(penalty),
+                                            scratch.data_ptr(), scratch.stride(0), _stream()), "uvx_repetition_penalty_rows")
+    return logits
+
+
+def lookup_draft(seq: torch.Tensor, cur_len: torch.Tensor, n_new: torch.Tensor, max_new: int, k: int, n: int,
+                 eos_ids: Optional[torch.Tensor], done: torch.Tensor, tok: torch.Tensor, n_draft: torch.Tensor, pos: torch.Tensor,
+                 lens: torch.Tensor, rope_pos: torch.Tensor, pen_len: torch.Tensor, idx: torch.Tensor) -> None:
+    """``uvx_lookup_draft`` (include/uvx.h): prompt-lookup drafts for the sequence seq [W] int64 (its first cur_len[0] tokens)
+    -> the k + 1 fed tokens tok [k + 1] int64, n_draft [1], the per-row pos / lens / rope_pos / pen_len / idx [k + 1] int32, and
+    the drafts into seq[cur_len : cur_len + n_draft].  cur_len / n_new / done are [1] int32 device counters."""
+    if not 1 <= int(k) <= LOOKUP_MAX_K:
+        raise ValueError(f"k must be in [1, {LOOKUP_MAX_K}], got {k}")
+    if int(n) < 1:
+        raise ValueError(f"n must be >= 1, got {n}")
+    if int(max_new) < 1:
+        raise ValueError(f"max_new must be >= 1, got {max_new}")
+    _cuda(seq, torch.int64, "seq")
+    if seq.dim() != 1 or not seq.is_contiguous():
+        raise ValueError("seq must be a contiguous [W] tensor")
+    R = int(k) + 1
+    for t, name in ((cur_len, "cur_len"), (n_new, "n_new"), (done, "done"), (n_draft, "n_draft")):
+        _rows(t, torch.int32, 1, name)
+    _rows(tok, torch.int64, R, "tok")
+    for t, name in ((pos, "pos"), (lens, "lens"), (rope_pos, "rope_pos"), (pen_len, "pen_len"), (idx, "idx")):
+        _rows(t, torch.int32, R, name)
+    if eos_ids is not None:
+        _cuda(eos_ids, torch.int64, "eos_ids")
+    check(lib().uvx_lookup_draft(seq.data_ptr(), cur_len.data_ptr(), n_new.data_ptr(), int(max_new), int(k), int(n), _p(eos_ids),
+                                 0 if eos_ids is None else eos_ids.numel(), done.data_ptr(), tok.data_ptr(), n_draft.data_ptr(),
+                                 pos.data_ptr(), lens.data_ptr(), rope_pos.data_ptr(), pen_len.data_ptr(), idx.data_ptr(), _stream()),
+          "uvx_lookup_draft")
+
+
+def lookup_accept(pick: torch.Tensor, tok: torch.Tensor, n_draft: torch.Tensor, eos_ids: Optional[torch.Tensor], seq: torch.Tensor,
+                  cur_len: torch.Tensor, n_new: torch.Tensor, max_new: int, done: torch.Tensor, step: Optional[torch.Tensor] = None,
+                  accepted: Optional[torch.Tensor] = None) -> None:
+    """``uvx_lookup_accept`` (include/uvx.h): picks [R] int64 of the rows that fed tok [R] int64 (R >= n_draft[0] + 1) -> the
+    agreeing prefix plus one token appended to seq [W] int64 at cur_len[0]; cur_len / n_new / done [1] int32 advance.  With
+    ``accepted`` ([steps] int32) and ``step`` ([1] int32) the step's accepted draft count is logged at step[0]."""
+    R = pick.numel()
+    if not 1 <= R <= LOOKUP_MAX_K + 1:
+        raise ValueError(f"pick must hold 1..{LOOKUP_MAX_K + 1} rows, got {R}")
+    _rows(pick, torch.int64, R, "pick"), _rows(tok, torch.int64, R, "tok")
+    _cuda(seq, torch.int64, "seq")
+    if seq.dim() != 1 or not seq.is_contiguous():
+        raise ValueError("seq must be a contiguous [W] tensor")
+    for t, name in ((n_draft, "n_draft"), (cur_len, "cur_len"), (n_new, "n_new"), (done, "done")):
+        _rows(t, torch.int32, 1, name)
+    if (step is None) != (accepted is None):
+        raise ValueError("step and accepted go together")
+    if accepted is not None:
+        _rows(step, torch.int32, 1, "step")
+        _cuda(accepted, torch.int32, "accepted")
+        if accepted.dim() != 1 or not accepted.is_contiguous():
+            raise ValueError("accepted must be a contiguous [steps] tensor")
+    if int(max_new) < 1:
+        raise ValueError(f"max_new must be >= 1, got {max_new}")
+    if eos_ids is not None:
+        _cuda(eos_ids, torch.int64, "eos_ids")
+    check(lib().uvx_lookup_accept(pick.data_ptr(), tok.data_ptr(), n_draft.data_ptr(), _p(eos_ids),
+                                  0 if eos_ids is None else eos_ids.numel(), seq.data_ptr(), cur_len.data_ptr(), n_new.data_ptr(),
+                                  int(max_new), _p(step), _p(accepted), 0 if accepted is None else accepted.numel(), done.data_ptr(),
+                                  _stream()), "uvx_lookup_accept")
+
+
 # ------------------------------------------------------------------------------------------ beam search
 BEAM_MAX = 8        # beams per prompt (kBeamMax in generate.cu)
 BEAM_MAX_K = 64     # candidates per prompt, max(2, 1 + n_eos) * num_beams
