@@ -507,6 +507,20 @@ int uvx_kv_pages_copy(void* k_row, void* v_row, int64_t row_layer_stride, void* 
 int uvx_kv_pages_copy_fp8(void* k_row, void* v_row, int64_t row_layer_stride, void* k_pool, void* v_pool, int64_t pool_layer_stride,
                           int64_t L, int64_t row_elems, const int32_t* pages, int64_t p0, int64_t p1, int32_t to_pages,
                           const float* kv_scales, uvx_stream_t stream);
+/* uvx_kv_pages_move  whole pages between two pools, byte for byte, every layer, K and V, one launch: page src_pages[j] of the
+ *                    source -> page dst_pages[j] of the destination for j < n (both lists int32 on the device; the caller keeps
+ *                    the ids inside each pool and the destination ids distinct).  Layer l of a pool starts at
+ *                    l * *_layer_stride bytes, page p at p * page_bytes within it; nothing else is written.  The element type
+ *                    is not read (a bf16 and an e4m3 pool move alike; an e4m3 pool's scales do not change).  Exception to
+ *                    the DEVICE-pointer convention: each of the four bases may instead be pinned / registered host memory
+ *                    mapped at the same address (the SMs read / write it over PCIe, no staging buffer); anything else (a
+ *                    pageable host pointer) returns UVX_ERR_ARG before any launch (cudaPointerGetAttributes).  16-byte
+ *                    aligned bases, page_bytes and layer strides % 16 == 0, n >= 0 (0 launches nothing).  Not meant for
+ *                    graph capture: the serving scheduler calls it between replays, on the stream of every other kernel
+ *                    that touches either pool.                                                                            */
+int uvx_kv_pages_move(const void* src_k, const void* src_v, int64_t src_layer_stride, void* dst_k, void* dst_v,
+                      int64_t dst_layer_stride, int64_t L, int64_t page_bytes, const int32_t* src_pages, const int32_t* dst_pages,
+                      int64_t n, uvx_stream_t stream);
 
 /* Shifted causal-LM cross entropy (hf:loss/loss_utils.py:28-67; called through LlamaForCausalLM.forward(labels=)
  * from ref:ultravox/model/ultravox_model.py:328-334).  logits [B*S, V] fp32 (row_stride elements), labels [B, S]

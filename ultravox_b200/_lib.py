@@ -79,6 +79,7 @@ SIGNATURES = {
     "uvx_attention_paged_fp8": (C.c_int, [C.POINTER(AttnArgs), c_vp, c_i64, c_vp, c_vp]),
     "uvx_attention_indexed_paged_fp8": (C.c_int, [C.POINTER(AttnArgs), c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp]),
     "uvx_kv_pages_copy_fp8": (C.c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp, c_vp]),
+    "uvx_kv_pages_move": (C.c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_vp, c_vp, c_i64, c_vp]),
     "uvx_rope": (C.c_int, [c_vp, c_i64, c_i64, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp]),
     "uvx_swiglu": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_i64, C.c_int, c_vp]),
     "uvx_splice_plan": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp]),

@@ -18,6 +18,7 @@
 //   uvx_kv_reorder          in-place gather of the KV cache rows by parent beam (and the prefill broadcast to the beams)
 //   uvx_kv_page_map         paged KV cache: (table row, position) of each step row -> (page, offset) for the mapped RoPE + append
 //   uvx_kv_pages_copy       paged KV cache: positions of a contiguous one-row cache <-> their pages, all layers, K and V
+//   uvx_kv_pages_move       paged KV cache: whole pages between two pools (device <-> pinned host), all layers, K and V, raw bytes
 #include "uvx_common.cuh"
 
 namespace uvx {
@@ -1162,6 +1163,29 @@ __global__ void __launch_bounds__(256) kv_pages_copy_kernel(uint4* __restrict__ 
   }
 }
 
+// Whole pages between two pools [L][pages][page_vec] of 16-byte vectors, every layer, K and V: page src_pages[j] of the source
+// -> page dst_pages[j] of the destination for j < n, raw bytes.  Either pool may be mapped pinned host memory (read / written over
+// PCIe through its UVA address); the page lists are on the device.
+__global__ void __launch_bounds__(256) kv_pages_move_kernel(const uint4* __restrict__ src_k, const uint4* __restrict__ src_v,
+                                                            int64_t src_layer_vec, uint4* __restrict__ dst_k, uint4* __restrict__ dst_v,
+                                                            int64_t dst_layer_vec, int64_t L, int64_t page_vec,
+                                                            const int32_t* __restrict__ src_pages, const int32_t* __restrict__ dst_pages,
+                                                            int64_t n) {
+  pdl_trigger();
+  pdl_wait();
+  const int64_t per_layer = n * page_vec;
+  const int64_t total = 2 * L * per_layer;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int which = (int)(i / (L * per_layer));
+    const int64_t rem = i % (L * per_layer);
+    const int64_t l = rem / per_layer, e = rem % per_layer;
+    const int64_t j = e / page_vec, c = e % page_vec;
+    const uint4* src = which ? src_v : src_k;
+    uint4* dst = which ? dst_v : dst_k;
+    dst[l * dst_layer_vec + (int64_t)dst_pages[j] * page_vec + c] = src[l * src_layer_vec + (int64_t)src_pages[j] * page_vec + c];
+  }
+}
+
 }  // namespace uvx
 
 extern "C" int uvx_kv_write(const void* qkv, int64_t row_stride, int64_t k_col, int64_t v_col, int64_t kv_width, void* k_cache,
@@ -1400,6 +1424,40 @@ extern "C" int uvx_kv_pages_copy_fp8(void* k_row, void* v_row, int64_t row_layer
            row_layer_stride / 16, (uint4*)k_pool, (uint4*)v_pool, pool_layer_stride / 16, L, row_elems / 16, pages, p0, p1 - p0,
            (int)to_pages, kv_scales);
   return check_launch("kv_pages_copy_kernel (fp8 pool)");
+}
+
+// Whether the kernel can dereference `p` as it is: device memory, or host memory that is pinned / registered and mapped at the
+// same address (UVA).  A pageable host pointer (cudaMemoryTypeUnregistered) is refused.
+static bool kv_move_addressable(const void* p) {
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    (void)cudaGetLastError();
+    return false;
+  }
+  if (a.type == cudaMemoryTypeDevice) return true;
+  return a.type == cudaMemoryTypeHost && a.devicePointer == p;
+}
+
+extern "C" int uvx_kv_pages_move(const void* src_k, const void* src_v, int64_t src_layer_stride, void* dst_k, void* dst_v,
+                                 int64_t dst_layer_stride, int64_t L, int64_t page_bytes, const int32_t* src_pages,
+                                 const int32_t* dst_pages, int64_t n, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(src_k && src_v && dst_k && dst_v && src_pages && dst_pages, "uvx_kv_pages_move: null pointer");
+  UVX_REQUIRE(L >= 1 && n >= 0 && page_bytes >= 16 && page_bytes % 16 == 0 && src_layer_stride % 16 == 0 && dst_layer_stride % 16 == 0,
+              "uvx_kv_pages_move: bad shape (L >= 1, n >= 0, page_bytes and layer strides multiples of 16 bytes)");
+  UVX_REQUIRE(((uintptr_t)src_k | (uintptr_t)src_v | (uintptr_t)dst_k | (uintptr_t)dst_v) % 16 == 0,
+              "uvx_kv_pages_move: base pointers must be 16-byte aligned");
+  const void* bases[4] = {src_k, src_v, dst_k, dst_v};
+  for (const void* p : bases)
+    UVX_REQUIRE(kv_move_addressable(p),
+                "uvx_kv_pages_move: %p is neither device memory nor pinned host memory mapped into the device's address space", p);
+  if (n == 0) return UVX_OK;
+  const int64_t total = 2 * L * n * (page_bytes / 16);
+  int64_t blocks = (total + 255) / 256;
+  if (blocks > 132 * 16) blocks = 132 * 16;
+  launch_k(kv_pages_move_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, (const uint4*)src_k, (const uint4*)src_v,
+           src_layer_stride / 16, (uint4*)dst_k, (uint4*)dst_v, dst_layer_stride / 16, L, page_bytes / 16, src_pages, dst_pages, n);
+  return check_launch("kv_pages_move_kernel");
 }
 
 extern "C" int uvx_token_logprobs(const float* logits, int64_t B, int64_t V, const int64_t* tok, const int32_t* n_top,

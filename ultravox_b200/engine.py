@@ -199,12 +199,20 @@ class _PagedKV:
     ``kv_cache_dtype="fp8_e4m3"`` makes the pool ``float8_e4m3fn`` with per-layer K / V scales ``kv_scales`` [L, 2] fp32 on the
     device (default all 1): every write into the pool (the step's append, the admission scatter) quantizes, every read (both
     attention kernels, the admission gather into the bf16 scratch) dequantizes, as include/uvx.h states.  This class is the
-    only place that knows the pool's element type."""
+    only place that knows the pool's element type.
+
+    ``host_kv_pages`` > 0 adds a second tier: ``host_k`` / ``host_v`` ``[L, host_kv_pages, 64, Hkv, D]`` in pinned host memory,
+    the device pool's dtype, allocated once here.  ``swap_out(dev_pages, host_pages)`` / ``swap_in(host_pages, dev_pages)`` move
+    whole pages between the tiers with one ``uvx_kv_pages_move`` launch on the current stream, the SMs reading or writing the
+    host pages over PCIe; an e4m3 page moves as its bytes, under the same per-layer scales.  Nothing waits on the host.  That is
+    correct as long as every kernel that touches either tier runs on one stream (the scheduler's): a page freed by a move and
+    taken by the next move, admission or step is then written only after the move has read it.  With 0 (the default) nothing is
+    allocated."""
 
     keeps_kv = True
 
     def __init__(self, model: UltravoxModel, slots: int, max_len: int, kv_pages: int, kv_cache_dtype: str = "bf16",
-                 kv_scales: Optional[torch.Tensor] = None):
+                 kv_scales: Optional[torch.Tensor] = None, host_kv_pages: int = 0):
         lm, tc = model.language_model, model.config.text_config
         dev = model.device
         if int(kv_pages) < 1:
@@ -228,6 +236,34 @@ class _PagedKV:
         self.off = torch.zeros(R, dtype=torch.int32, device=dev)
         self.cache = model.new_cache(1, max_len)
         self.pages = None                   # the admitted request's pages on the device
+        if isinstance(host_kv_pages, bool) or not isinstance(host_kv_pages, numbers.Integral) or host_kv_pages < 0:
+            raise ValueError(f"host_kv_pages must be an integer >= 0, got {host_kv_pages!r}")
+        self.host_kv_pages = int(host_kv_pages)
+        self.host_k = self.host_v = None
+        if self.host_kv_pages:
+            self.host_k = torch.empty(L, self.host_kv_pages, ops.PAGE, nkv, hd, dtype=dtype, pin_memory=True)
+            self.host_v = torch.empty(self.host_k.shape, dtype=dtype, pin_memory=True)
+
+    def swap_out(self, dev_pages, host_pages) -> None:
+        """Device page dev_pages[j] -> host page host_pages[j], every layer, K and V (stream-ordered, no sync)."""
+        self._move(self.pool_k, self.pool_v, dev_pages, self.kv_pages, self.host_k, self.host_v, host_pages, self.host_kv_pages)
+
+    def swap_in(self, host_pages, dev_pages) -> None:
+        """Host page host_pages[j] -> device page dev_pages[j], every layer, K and V (stream-ordered, no sync)."""
+        self._move(self.host_k, self.host_v, host_pages, self.host_kv_pages, self.pool_k, self.pool_v, dev_pages, self.kv_pages)
+
+    def _move(self, sk, sv, src, n_src, dk, dv, dst, n_dst) -> None:
+        src, dst = [int(p) for p in src], [int(p) for p in dst]
+        if not self.host_kv_pages:
+            raise ValueError("no host tier: create the engine with host_kv_pages > 0")
+        if len(src) != len(dst) or len(set(dst)) != len(dst) or not all(0 <= p < n_src for p in src) or \
+                not all(0 <= p < n_dst for p in dst):
+            raise ValueError(f"bad page lists for a move: {src} -> {dst}")
+        if not src:
+            return
+        # one pinned buffer per move (the host allocator keeps it until its copy has run)
+        lists = torch.tensor(src + dst, dtype=torch.int32).pin_memory().to(self.table.device, non_blocking=True)
+        ops.kv_pages_move(sk, sv, dk, dv, lists[:len(src)], lists[len(src):])
 
     def map_rows(self, e: "_Decoder", R: int) -> None:
         ops.kv_page_map(self.table, e._mrow[:R], e._mpos[:R], self.page[:R], self.off[:R], frozen=e.done)
@@ -1012,10 +1048,15 @@ class PagedSlotDecodeEngine(SlotDecodeEngine):
     (``serving.PagePool``).
 
     ``kv_cache_dtype="fp8_e4m3"`` (with ``kv_scales`` [L, 2], default all 1) keeps the pool in e4m3: half the bytes per page
-    (``_PagedKV``).  Every step then computes the bits the bf16 engine would on a pool holding the dequantized values."""
+    (``_PagedKV``).  Every step then computes the bits the bf16 engine would on a pool holding the dequantized values.
+
+    ``host_kv_pages`` > 0 adds ``host_kv_pages`` pinned host pages (``host_k`` / ``host_v``) and ``swap_out`` / ``swap_in``,
+    which move whole pages between them and the device pool between replays (``_PagedKV``)."""
 
     def __init__(self, model: UltravoxModel, slots: int, max_len: int, kv_pages: int, eos_token_ids=None, pad_token_id: int = 0,
-                 use_graph: bool = True, max_logprobs: int = 0, kv_cache_dtype: str = "bf16", kv_scales=None):
-        kv = _PagedKV(model, int(slots), max_len, kv_pages, kv_cache_dtype, kv_scales)
+                 use_graph: bool = True, max_logprobs: int = 0, kv_cache_dtype: str = "bf16", kv_scales=None, host_kv_pages: int = 0):
+        kv = _PagedKV(model, int(slots), max_len, kv_pages, kv_cache_dtype, kv_scales, host_kv_pages)
         self.kv_pages, self.pool_k, self.pool_v, self.kv_scales = kv.kv_pages, kv.pool_k, kv.pool_v, kv.kv_scales
+        self.host_kv_pages, self.host_k, self.host_v = kv.host_kv_pages, kv.host_k, kv.host_v
+        self.swap_out, self.swap_in = kv.swap_out, kv.swap_in
         self._setup(model, int(slots), kv, eos_token_ids, pad_token_id, use_graph, max_logprobs)

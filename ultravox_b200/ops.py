@@ -468,6 +468,31 @@ def kv_pages_copy(k_row: torch.Tensor, v_row: torch.Tensor, k_pool: torch.Tensor
         check(lib().uvx_kv_pages_copy(*args, _stream()), "uvx_kv_pages_copy")
 
 
+def kv_pages_move(src_k: torch.Tensor, src_v: torch.Tensor, dst_k: torch.Tensor, dst_v: torch.Tensor, src_pages: torch.Tensor,
+                  dst_pages: torch.Tensor) -> None:
+    """Whole pages, every layer, K and V, byte for byte, from the pool ``src_k`` / ``src_v`` [L, n_src, 64, Hkv, D] to ``dst_k`` /
+    ``dst_v`` [L, n_dst, 64, Hkv, D] of the same dtype (bf16 or float8_e4m3fn; an e4m3 pool's scales do not change): page
+    src_pages[j] -> page dst_pages[j] (``uvx_kv_pages_move``).  Either pool may be a pinned CPU tensor, which the kernel reads or
+    writes over PCIe; a pageable one raises UvxError and nothing is launched.  The page lists are int32 on the device and are
+    not range-checked here (that would need a sync): the caller keeps them inside the pools, destinations distinct."""
+    if src_v.dtype != src_k.dtype or dst_k.dtype != src_k.dtype or dst_v.dtype != src_k.dtype or src_k.dtype not in (BF16, FP8):
+        raise _lib.UvxError(f"the four pools must share one dtype, bfloat16 or float8_e4m3fn; got {src_k.dtype} / {src_v.dtype} -> "
+                            f"{dst_k.dtype} / {dst_v.dtype}")
+    for t, name in ((src_k, "src_k"), (src_v, "src_v"), (dst_k, "dst_k"), (dst_v, "dst_v")):
+        if not t.is_contiguous() or t.dim() != 5 or t.shape[2] != PAGE:
+            raise ValueError(f"{name} must be a contiguous pool [L, n_pages, {PAGE}, Hkv, D], got {tuple(t.shape)}")
+    if src_v.shape != src_k.shape or dst_v.shape != dst_k.shape or src_k.shape[0] != dst_k.shape[0] or \
+            src_k.shape[2:] != dst_k.shape[2:]:
+        raise ValueError(f"pools of different layers or page shapes: {tuple(src_k.shape)} -> {tuple(dst_k.shape)}")
+    n = src_pages.numel()
+    _rows(src_pages, torch.int32, n, "src_pages")
+    _rows(dst_pages, torch.int32, n, "dst_pages")
+    page_bytes = src_k[0, 0].numel() * src_k.element_size()
+    check(lib().uvx_kv_pages_move(src_k.data_ptr(), src_v.data_ptr(), src_k.shape[1] * page_bytes, dst_k.data_ptr(),
+                                  dst_v.data_ptr(), dst_k.shape[1] * page_bytes, src_k.shape[0], page_bytes, src_pages.data_ptr(),
+                                  dst_pages.data_ptr(), n, _stream()), "uvx_kv_pages_move")
+
+
 def attention_fused_qkv(qkv: torch.Tensor, B: int, S: int, Hq: int, Hkv: int, D: int, scale: float, causal: bool,
                         kv_len: Optional[torch.Tensor] = None, block: int = 0,
                         out: Optional[torch.Tensor] = None, kv_start: Optional[torch.Tensor] = None) -> torch.Tensor:

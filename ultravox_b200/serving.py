@@ -14,12 +14,15 @@ with exactly what ``generate(past_key_values=...)`` returns for that turn.  At a
 need (its session's pages count towards that), so decoding never runs out of pages and nothing is pre-empted; a request at the
 head of the queue that cannot get its pages waits for them (FIFO).  ``PagePool`` is that bookkeeping, on the host alone.
 With ``prefix_cache`` requests that open with the same tokens (a system prompt) also share the pages of that prefix, and
-prefill only what follows it.
+prefill only what follows it.  With ``host_kv_pages`` the pool gets a second tier in pinned host memory: when the head of the
+queue cannot get its pages, idle sessions (no turn queued or running) are swapped out to it, least recently used first, and a
+swapped-out session's pages come back at its next turn's admission.  Running requests are never swapped.
 """
 from __future__ import annotations
 
 import collections
 import dataclasses
+import numbers
 from typing import Callable, Deque, Dict, List, Optional, Sequence, Tuple
 
 import torch
@@ -38,6 +41,8 @@ class _Session:
     pages: List[int]
     kv_len: int = 0             # positions of the conversation held in its pages
     busy: bool = False          # a turn is queued or running
+    host: List[int] = dataclasses.field(default_factory=list)      # swapped out: the host pages of its kv_len positions
+    last_used: int = -1         # when its last turn retired (swap-outs take the least recently used first)
 
 
 class PagePool:
@@ -51,12 +56,22 @@ class PagePool:
     of token ids: eviction takes a page's indexed descendants with it, so an id never names two chains.  Keys are exact tuples,
     not digests, so no other prompt's K / V can be served.  An indexed page nobody holds is *reclaimable*: it keeps its
     contents and can still be hit, until a reservation that finds no free page evicts it (least recently released first).
-    A holder of an indexed page holds its whole chain from the first page, so a page nobody holds has no held descendant."""
+    A holder of an indexed page holds its whole chain from the first page, so a page nobody holds has no held descendant.
 
-    def __init__(self, n_pages: int):
+    ``host_pages`` > 0 adds a host tier of that many pages.  A session then lives on exactly one side: on the device, holding
+    device pages as above, or on the host (``swap_out``), holding ``pages_for(kv_len)`` host pages of its own and no device
+    pages.  Its next reservation takes every page new and gives the host pages back (``reserve``).  ``swap_candidates`` is the
+    policy that picks sessions to swap out."""
+
+    def __init__(self, n_pages: int, host_pages: int = 0):
         if int(n_pages) < 1:
             raise ValueError(f"the pool needs at least one page, got {n_pages}")
+        if int(host_pages) < 0:
+            raise ValueError(f"the host tier cannot have {host_pages} pages")
         self.n_pages = int(n_pages)
+        self.host_pages = int(host_pages)
+        self._host_free: List[int] = list(range(self.host_pages))
+        self._clock = 0                                 # counts retired session turns (LRU)
         self._free: List[int] = list(range(self.n_pages))
         self._refs: List[int] = [0] * self.n_pages
         self._reclaimable: "collections.OrderedDict[int, None]" = collections.OrderedDict()    # oldest first
@@ -76,6 +91,11 @@ class PagePool:
     def cached_pages(self) -> int:
         """Pages in the prefix index (held or reclaimable)."""
         return len(self._index)
+
+    @property
+    def host_free_pages(self) -> int:
+        """Host pages not holding a swapped-out session."""
+        return len(self._host_free)
 
     def session_pages(self) -> int:
         """Pages held by sessions between turns (not by a running turn beyond its session's share)."""
@@ -98,6 +118,7 @@ class PagePool:
         if s.busy:
             raise RuntimeError(f"session {sid} has a turn in flight; close it after the turn returns")
         self._drop(s.pages)
+        self._host_free.extend(s.host)
         del self._sessions[sid]
 
     def match(self, page_tokens: Sequence[tuple]) -> List[int]:
@@ -115,22 +136,73 @@ class PagePool:
     def reserve(self, positions: int, sid: Optional[int] = None, shared: Sequence[int] = ()) -> Optional[List[int]]:
         """The page list of a request that needs ``positions`` positions (its session's pages first, or the cached pages
         ``shared`` from ``match``, then new ones), or None (nothing taken) when the pool is short.  New pages come from the
-        free list first, then by evicting reclaimable cached pages, least recently released first."""
+        free list first, then by evicting reclaimable cached pages, least recently released first.
+
+        A session on the host holds no device pages, so all of its pages are new; the reservation brings it back to the
+        device and frees its host pages.  The caller reads ``session(sid).host`` first and copies those host pages into the
+        first ``len(host)`` pages returned before anything else on the stream can write them."""
         held = self.session(sid).pages if sid is not None else []
         shared = list(shared)
         if shared and held:
             raise ValueError("a session that holds pages extends its own; only its first turn can share cached pages")
-        extra = max(pages_for(positions) - len(held) - len(shared), 0)
-        if extra > self.free_pages - sum(p in self._reclaimable for p in shared):
+        if self.shortfall(positions, sid, shared):
             return None
+        extra = max(pages_for(positions) - len(held) - len(shared), 0)
         for p in shared:                # held first, so the evictions below cannot take them
             self._acquire(p)
         new = [self._take() for _ in range(extra)]
         pages = held + shared + new
         if sid is not None:
-            self._sessions[sid].pages = pages
+            s = self._sessions[sid]
+            s.pages = pages
+            self._host_free.extend(s.host)
+            s.host = []
             return list(pages)
         return pages
+
+    def shortfall(self, positions: int, sid: Optional[int] = None, shared: Sequence[int] = ()) -> int:
+        """How many more device pages ``reserve(positions, sid, shared)`` needs than it can take now (0: it succeeds)."""
+        held = self.session(sid).pages if sid is not None else []
+        extra = max(pages_for(positions) - len(held) - len(shared), 0)
+        return max(extra - (self.free_pages - sum(p in self._reclaimable for p in shared)), 0)
+
+    def swap_candidates(self, need: int, exclude: Optional[int] = None, keep: Sequence[int] = ()) -> Optional[List[int]]:
+        """The idle sessions to swap out so that ``need`` more device pages become free, or None when no choice does (then
+        nothing should move).  Idle means on the device, no turn queued or running and at least one page held; ``exclude``
+        (the waiting request's own session) is never picked.  Sessions are taken least recently used first until the pages
+        their swap-out would free - those nobody else holds, other than the pages in ``keep`` (the waiting request's cached
+        prefix, which it takes itself) - cover ``need``; None if they never do, or if the host tier cannot hold them all."""
+        idle = sorted((s.last_used, sid) for sid, s in self._sessions.items() if sid != exclude and not s.busy and s.pages)
+        keep, refs = set(keep), {}
+        chosen, freed, host = [], 0, 0
+        for _, sid in idle:
+            pages = self._sessions[sid].pages
+            host += len(pages)
+            if host > len(self._host_free):
+                return None
+            chosen.append(sid)
+            for p in pages:
+                refs[p] = refs.get(p, self._refs[p]) - 1
+                freed += refs[p] == 0 and p not in keep
+            if freed >= need:
+                return chosen
+        return None
+
+    def swap_out(self, sid: int) -> Tuple[List[int], List[int]]:
+        """Moves an idle session to the host tier: returns (its device pages, the host pages they must be copied to), and
+        drops its device references (shared pages stay with their other holders or become reclaimable).  The caller launches
+        that copy before anything else on the stream can write those device pages.  ([], []) if it holds no device pages."""
+        s = self.session(sid)
+        if s.busy:
+            raise ValueError(f"session {sid} has a turn in flight; only idle sessions are swapped out")
+        if not s.pages:
+            return [], []
+        if len(s.pages) > len(self._host_free):
+            raise ValueError(f"session {sid} holds {len(s.pages)} pages; the host tier has {len(self._host_free)} free")
+        dev, host = s.pages, [self._host_free.pop() for _ in s.pages]
+        self._drop(dev)
+        s.pages, s.host = [], host
+        return dev, host
 
     def register(self, pages: Sequence[int], page_tokens: Sequence[tuple]) -> None:
         """Indexes ``pages[k]`` under ``page_tokens[k]`` for k = 0, 1, ..., once the holder has written their K / V.  Pages
@@ -160,6 +232,7 @@ class PagePool:
         keep = pages_for(kv_len)
         self._drop(s.pages[keep:])
         s.pages, s.kv_len, s.busy = s.pages[:keep], int(kv_len), False
+        s.last_used, self._clock = self._clock, self._clock + 1
 
     def _acquire(self, p: int) -> None:
         if self._refs[p] == 0:
@@ -248,11 +321,25 @@ class SlotScheduler:
     bf16(q * s).  A step's attention therefore sees the dequantized keys, the row's just-appended key included; a B = 1
     admission prefills its new suffix over its own bf16 K / V (as ``generate(past_key_values=...)`` with the dequantized past
     does) and only the pages it writes are quantized.  Sessions, the prefix cache, chunked prefill, sampling, the repetition
-    penalty and log-probs work unchanged."""
+    penalty and log-probs work unchanged.
+
+    ``host_kv_pages`` (needs ``kv_pages``; default 0, none): that many pages of pinned host memory (same page size and dtype as
+    the pool) form a second tier for idle sessions - conversations with no turn queued or running.  When the request at the
+    head of the queue cannot get its pages from free or reclaimable cached ones, idle sessions other than its own are swapped
+    out, least recently used first (by when their last turn retired): all of their pages, shared prefix pages included, are
+    copied to host pages and their device references dropped.  That happens only if the device pages it would free cover what
+    the head lacks and the host tier has room; otherwise nothing moves and the head waits as before.  A swapped-out session's
+    next turn reserves every page new, its first ``pages_for(kv_len)`` pages are copied back from the host before its suffix
+    is prefilled, and its host pages are freed: the restored pages are private (no longer shared with the prefix cache).  The
+    bits of every turn are those of the same workload on a pool large enough never to swap.  ``offload_session(sid)`` swaps a
+    session out on request, ``session_on_host(sid)`` tells where it is, ``host_free_pages`` counts the free host pages and
+    ``swapped_out_pages`` / ``swapped_in_pages`` the pages moved so far.  Each move is one ``uvx_kv_pages_move`` launch on the
+    scheduler's stream (the SMs read or write the host pages over PCIe) between decode steps; it pauses the other slots for
+    its duration, as an admission's prefill does.  Running requests are never swapped."""
 
     def __init__(self, model, slots: int = 8, max_len: int = 2048, eos_token_ids=None, pad_token_id: Optional[int] = None,
                  sync_every: int = 8, use_graph: bool = True, kv_pages: Optional[int] = None, prefix_cache: bool = False,
-                 max_logprobs: int = 0, kv_cache_dtype: str = "bf16", kv_scales=None):
+                 max_logprobs: int = 0, kv_cache_dtype: str = "bf16", kv_scales=None, host_kv_pages: int = 0):
         eos = sorted(set([eos_token_ids] if isinstance(eos_token_ids, int) else (eos_token_ids or [])))
         pad = pad_token_id if pad_token_id is not None else (min(eos) if eos else 0)     # generate()'s default
         if int(sync_every) < 1:
@@ -261,6 +348,10 @@ class SlotScheduler:
             raise ValueError("prefix_cache shares KV pages between requests: it needs the paged cache (kv_pages=N)")
         if kv_cache_dtype not in ("bf16", "fp8_e4m3"):
             raise ValueError(f"kv_cache_dtype must be 'bf16' or 'fp8_e4m3', got {kv_cache_dtype!r}")
+        if isinstance(host_kv_pages, bool) or not isinstance(host_kv_pages, numbers.Integral) or host_kv_pages < 0:
+            raise ValueError(f"host_kv_pages must be an integer >= 0, got {host_kv_pages!r}")
+        if host_kv_pages and kv_pages is None:
+            raise ValueError("host_kv_pages swaps sessions' KV pages to the host: it needs the paged cache (kv_pages=N)")
         kv = {}
         if kv_cache_dtype == "fp8_e4m3":
             if kv_pages is None:
@@ -275,13 +366,17 @@ class SlotScheduler:
         self.model = model
         self.pool: Optional[PagePool] = None
         lp = {} if max_logprobs == 0 else dict(max_logprobs=max_logprobs)     # the engine validates it
+        if host_kv_pages:
+            kv["host_kv_pages"] = int(host_kv_pages)
         if kv_pages is None:
             self.engine = SlotDecodeEngine(model, slots, max_len, eos_token_ids=eos, pad_token_id=pad, use_graph=use_graph,
                                            **lp)
         else:
             self.engine = PagedSlotDecodeEngine(model, slots, max_len, int(kv_pages), eos_token_ids=eos, pad_token_id=pad,
                                                 use_graph=use_graph, **lp, **kv)
-            self.pool = PagePool(int(kv_pages))
+            self.pool = PagePool(int(kv_pages), int(host_kv_pages))
+        self.swapped_out_pages = 0
+        self.swapped_in_pages = 0
         self.sync_every = int(sync_every)
         self.steps = 0
         self.first_token: Dict[int, torch.cuda.Event] = {}
@@ -317,6 +412,27 @@ class SlotScheduler:
             raise RuntimeError(f"session {sid} has a turn in flight; close it after the turn returns")
         self._pool().close_session(sid)
 
+    def offload_session(self, sid: int) -> None:
+        """Swaps an idle session's pages out to the host tier now (a no-op if it is there already or holds no pages); its next
+        turn brings them back.  ValueError without a host tier, while a turn of it is queued or running, or when the host tier
+        has too few free pages."""
+        s = self._session(sid)
+        if not self.pool.host_pages:
+            raise ValueError("offload_session needs a host tier: SlotScheduler(..., kv_pages=N, host_kv_pages=M)")
+        if s.busy:
+            raise ValueError(f"session {sid} has a turn in flight; only idle sessions are swapped out")
+        self._swap_out(sid)
+
+    def session_on_host(self, sid: int) -> bool:
+        """Whether the session's pages are on the host tier (swapped out) rather than in the device pool."""
+        return bool(self._session(sid).host)
+
+    def _swap_out(self, sid: int) -> None:
+        dev, host = self.pool.swap_out(sid)
+        if dev:                         # launched before any later admission or step can write the freed device pages
+            self.engine.swap_out(dev, host)
+            self.swapped_out_pages += len(dev)
+
     def session_length(self, sid: int) -> int:
         """Positions of the conversation held in its KV pages: the last turn's sequence minus its last token (not fed yet)."""
         return self._session(sid).kv_len
@@ -330,6 +446,11 @@ class SlotScheduler:
     def cached_pages(self) -> int:
         """Pages in the prefix cache, held or not."""
         return self._pool().cached_pages
+
+    @property
+    def host_free_pages(self) -> int:
+        """Pages of the host tier not holding a swapped-out session."""
+        return self._pool().host_free_pages
 
     def submit(self, features: dict, max_new_tokens: int = 20, do_sample: bool = False, temperature: Optional[float] = None,
                top_k: Optional[int] = None, top_p: Optional[float] = None, repetition_penalty: float = 1.0,
@@ -416,9 +537,18 @@ class SlotScheduler:
                 return                  # FIFO: it waits until the prompt in flight has been prefilled
             kw = {}
             if self.pool is not None:
-                pages = self.pool.reserve(S + head.max_new, head.session, shared)
+                need = S + head.max_new
+                short = self.pool.shortfall(need, head.session, shared) if self.pool.host_pages else 0
+                if short:               # after free and reclaimable pages, before waiting: swap idle sessions out
+                    for sid in self.pool.swap_candidates(short, head.session, shared) or ():
+                        self._swap_out(sid)
+                restore = self.pool.session(head.session).host if head.session is not None else []
+                pages = self.pool.reserve(need, head.session, shared)
                 if pages is None:
                     return              # FIFO: it waits for pages
+                if restore:             # before the prefill reads them; the freed host pages are rewritten only after this
+                    self.engine.swap_in(restore, pages[:len(restore)])
+                    self.swapped_in_pages += len(restore)
                 head.pages, head.past = pages, past
                 kw = dict(past=past, pages=pages)
             r = self._queue.popleft()
@@ -480,8 +610,11 @@ class SlotScheduler:
             if self._queue and not self._running and self._prefilling is None:
                 head = self._queue[0]
                 need = pages_for(int(head.input_ids.shape[1]) + head.max_new)
+                tier = ""
+                if self.pool.host_pages:
+                    tier = f" and the host tier has {self.pool.host_free_pages} of {self.pool.host_pages} pages free"
                 raise RuntimeError(f"request {head.rid} needs {need} KV pages but only {self.pool.free_pages} of "
-                                   f"{self.pool.n_pages} are free: open sessions hold {self.pool.session_pages()}; close some")
+                                   f"{self.pool.n_pages} are free: open sessions hold {self.pool.session_pages()}{tier}; close some")
             due = any(self._budget_spent(r) for r in self._running.values())
             if due or self.steps - self._last_poll >= self.sync_every:
                 self._last_poll = self.steps
