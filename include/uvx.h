@@ -274,6 +274,20 @@ int uvx_attention_paged_fp8(const uvx_attn_args* a, const int32_t* table, int64_
 int uvx_attention_indexed_paged_fp8(const uvx_attn_args* a, int64_t n_pages, const int32_t* table, int64_t table_stride,
                                     const int32_t* kv_row, const int32_t* past, const float* kv_scale, uvx_stream_t stream);
 
+/* Row-mapped decode attention (the prompt-lookup slot step, ultravox_b200/engine.py SlotDecodeEngine): several query rows read
+ * the keys of one slot.  Query row b (a->B rows, Sq = 1) reads cache row kv_row[b] (int32 [B], read on the device) instead of
+ * row b, and the keys [0, kv_len[b]) of it; everything else is the unmapped call on the mma.sync kernel, so each row is bit-identical
+ * to uvx_attention / uvx_attention_paged / uvx_attention_paged_fp8 of that row against that cache row.  Requires a->kv_len,
+ * Sq = 1, kv_start = NULL, lse = NULL, block = 0; kv_row[b] must address a row that exists (a->k + kv_row[b] * k_bs, or a table row).
+ * uvx_attention_rows            contiguous cache [rows, S_max, Hkv, D] through the strides of a.
+ * uvx_attention_paged_rows      uvx_attention_paged with table row kv_row[b].
+ * uvx_attention_paged_fp8_rows  uvx_attention_paged_fp8 with table row kv_row[b].                                             */
+int uvx_attention_rows(const uvx_attn_args* a, const int32_t* kv_row, uvx_stream_t stream);
+int uvx_attention_paged_rows(const uvx_attn_args* a, const int32_t* table, int64_t table_stride, const int32_t* kv_row,
+                             uvx_stream_t stream);
+int uvx_attention_paged_fp8_rows(const uvx_attn_args* a, const int32_t* table, int64_t table_stride, const float* kv_scale,
+                                 const int32_t* kv_row, uvx_stream_t stream);
+
 /* RoPE on the q and k sections of a fused [rows, (Hq + 2*Hkv) * D] projection, in place
  * (hf:modeling_llama.py:124-168; cos/sin tables [max_pos, D/2] fp32 built by the host exactly like
  * LlamaRotaryEmbedding incl. llama3 scaling, hf:modeling_rope_utils.py:550-626).
@@ -448,6 +462,49 @@ int uvx_repetition_penalty_rows(float* logits, int64_t B, int64_t V, const int64
                                 float penalty, float* scratch, int64_t scratch_stride, uvx_stream_t stream);
 int uvx_record_scores_rows(const float* logits, int64_t B, int64_t V, float temperature, int32_t top_k, float top_p,
                            const int32_t* idx, int64_t steps, float* scores, float* raw, uvx_stream_t stream);
+
+/* Prompt lookup inside the slot step (ultravox_b200/engine.py SlotDecodeEngine with prompt_lookup_num_tokens = K): slot s owns
+ * the R = slots * (K + 1) step rows r = s * (K + 1) + i, i <= K.  Per-slot arrays are [slots]; per-row arrays are [R]; seq is
+ * [slots, seq_stride] int64.
+ * uvx_lookup_draft_slots       one CTA per slot: the drafts of uvx_lookup_draft on seq[s, 0:cur_len[s]] with k[s] (<= K, 0 = none),
+ *                              n[s], n_new[s], max_new[s] - searched only when active[s], !done[s] and !prefilling[s] - written to
+ *                              seq[s, L, L + d) and n_draft[s] = d.  Row 0 of the slot feeds tok = token[s] at row_pos / row_lens /
+ *                              row_rope = pos[s] / lens[s] / rope_pos[s] (the slot's row of a plain step); row i in 1..d feeds
+ *                              draft i - 1 at pos[s] + i, lens[s] + i, rope_pos[s] + i; rows past d feed token[s] at row 0's values.
+ *                              pen_len = L + i and idx = n_new[s] + i for rows i <= d, idx = -1 past them; row_slot = s;
+ *                              cache_row = s for rows 1..d and for row 0 unless the slot is done or prefilling, else -1 (no
+ *                              K / V write).  1 <= K <= 31.
+ * uvx_lookup_accept_slots      for each active slot that is not done: uvx_lookup_accept's m over its rows (pick[r], tok[r + 1])
+ *                              appended at seq[s, cur_len[s]]; cur_len / n_new += m + 1; done = the last pick is an EOS id or
+ *                              n_new >= max_new; pos / lens / rope_pos += m + 1 while the slot stays open (m when it finishes) - what
+ *                              m + 1 uvx_slot_finish calls leave; token[s] = the last pick; accepted[s] += m.  Done and inactive
+ *                              slots are untouched.  n_open[0] = active slots still open.  One warp per slot.
+ * uvx_sample_rows              uvx_sample_slots per row r with slot s = row_slot[r]'s temperature / top_k / top_p, active[s] and the
+ *                              uniform u[s * u_stride + row_idx[r]]; rows with row_idx[r] < 0 or an inactive slot are not written.
+ *                              Bit for bit the pick uvx_sample_slots makes for slot s with n_new[s] = row_idx[r].
+ * uvx_repetition_penalty_rows_map  uvx_repetition_penalty_slots per row r with slot s = row_slot[r]'s penalty and active flag over
+ *                              seq[s, 0:row_len[r]], scratch [R, seq_stride] fp32 (row r's own); rows with row_idx[r] < 0 skipped.
+ * uvx_token_logprobs_rows      uvx_token_logprobs per row r with n_top[s], s = row_slot[r], written to slot s's outputs
+ *                              (out_lp[s * cap + dst[r]], ...); dst[r] < 0 writes nothing.                                      */
+int uvx_lookup_draft_slots(int64_t* seq, int64_t seq_stride, const int64_t* token, const int32_t* cur_len, const int32_t* n_new,
+                           const int32_t* max_new, const int32_t* k, const int32_t* n, const int32_t* done, const int32_t* active,
+                           const int32_t* prefilling, const int32_t* pos, const int32_t* lens, const int32_t* rope_pos, int64_t slots,
+                           int32_t K, const int64_t* eos_ids, int32_t n_eos, int64_t* tok, int32_t* n_draft, int32_t* row_pos,
+                           int32_t* row_lens, int32_t* row_rope, int32_t* pen_len, int32_t* idx, int32_t* row_slot,
+                           int32_t* cache_row, uvx_stream_t stream);
+int uvx_lookup_accept_slots(const int64_t* pick, const int64_t* tok, const int32_t* n_draft, int64_t slots, int32_t K,
+                            const int64_t* eos_ids, int32_t n_eos, int64_t* seq, int64_t seq_stride, int64_t* token, int32_t* done,
+                            int32_t* cur_len, int32_t* n_new, const int32_t* max_new, const int32_t* active, int32_t* pos,
+                            int32_t* lens, int32_t* rope_pos, int32_t* accepted, int32_t* n_open, uvx_stream_t stream);
+int uvx_sample_rows(const float* logits, int64_t R, int64_t V, const float* temperature, const int32_t* top_k, const float* top_p,
+                    const float* u, int64_t u_stride, const int32_t* active, const int32_t* row_slot, const int32_t* row_idx,
+                    int64_t* out_idx, uvx_stream_t stream);
+int uvx_repetition_penalty_rows_map(float* logits, int64_t R, int64_t V, const int64_t* seq, int64_t seq_stride, const float* penalty,
+                                    const int32_t* active, const int32_t* row_slot, const int32_t* row_len, const int32_t* row_idx,
+                                    float* scratch, uvx_stream_t stream);
+int uvx_token_logprobs_rows(const float* logits, int64_t R, int64_t V, const int64_t* tok, const int32_t* n_top,
+                            const int32_t* row_slot, const int32_t* dst, int64_t cap, int32_t n_max, float* out_lp, int64_t* out_ids,
+                            float* out_top, uvx_stream_t stream);
 
 /* Beam search (hf:generation/utils.py _beam_search, transformers 5.5, and the helpers above it), one decode step as four
  * launches that read every per-step scalar from device memory.  B prompts, nb <= 8 beams each: row r = b * nb + j.

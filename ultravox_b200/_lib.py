@@ -110,6 +110,16 @@ SIGNATURES = {
     "uvx_lookup_accept": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp, c_vp]),
     "uvx_repetition_penalty_rows": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_f32, c_vp, c_i64, c_vp]),
     "uvx_record_scores_rows": (C.c_int, [c_vp, c_i64, c_i64, c_f32, c_i32, c_f32, c_vp, c_i64, c_vp, c_vp, c_vp]),
+    "uvx_lookup_draft_slots": (C.c_int, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64,
+                                         c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "uvx_lookup_accept_slots": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_i32, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                          c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "uvx_sample_rows": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "uvx_repetition_penalty_rows_map": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "uvx_token_logprobs_rows": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp]),
+    "uvx_attention_rows": (C.c_int, [C.POINTER(AttnArgs), c_vp, c_vp]),
+    "uvx_attention_paged_rows": (C.c_int, [C.POINTER(AttnArgs), c_vp, c_i64, c_vp, c_vp]),
+    "uvx_attention_paged_fp8_rows": (C.c_int, [C.POINTER(AttnArgs), c_vp, c_i64, c_vp, c_vp, c_vp]),
     "uvx_log_softmax": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_vp]),
     "uvx_beam_select": (C.c_int, [c_vp, c_i64, c_i32, c_i64, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "uvx_beam_update": (C.c_int, [c_vp, c_vp, c_i64, c_i32, c_i32, c_i64, c_vp, c_i32, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp,

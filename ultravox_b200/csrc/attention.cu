@@ -23,6 +23,7 @@ struct AttnParams {
   int64_t q_rs, q_bs, k_rs, k_bs, v_rs, v_bs, o_rs, o_bs;
   const int32_t* kv_len;
   const int32_t* kv_start;  // optional [B]: keys before it are masked (left-padded batches)
+  const int32_t* kv_row;    // optional [B]: query row b reads cache row (paged: table row) kv_row[b] instead of b
   float* lse;  // optional [B, Hq, Sq]: natural-log sum-exp of the scaled scores (for the backward)
   int Sq, Skv, group, Hq;  // group = Hq / Hkv
   int causal, block;
@@ -96,9 +97,10 @@ __global__ void __launch_bounds__(kAThreads) attn_fwd_kernel(const AttnParamsT<k
   const int m0 = blockIdx.x * kAM;
   const int h = blockIdx.y, b = blockIdx.z;
   const int hk = h / p.group;
+  const int kvb = p.kv_row ? p.kv_row[b] : b;  // the cache / table row of query row b
   const bf16* qb = p.q + (int64_t)b * p.q_bs + (int64_t)h * D;
-  const bf16* kb = p.k + (kPaged ? 0 : (int64_t)b * p.k_bs) + (int64_t)hk * D;
-  const bf16* vb = p.v + (kPaged ? 0 : (int64_t)b * p.v_bs) + (int64_t)hk * D;
+  const bf16* kb = p.k + (kPaged ? 0 : (int64_t)kvb * p.k_bs) + (int64_t)hk * D;
+  const bf16* vb = p.v + (kPaged ? 0 : (int64_t)kvb * p.v_bs) + (int64_t)hk * D;
 
   int kv_end = p.Skv;
   if (p.kv_len) kv_end = min(kv_end, max(p.kv_len[b], 0));
@@ -128,7 +130,7 @@ __global__ void __launch_bounds__(kAThreads) attn_fwd_kernel(const AttnParamsT<k
     bf16* dk = sK + stage * kAN * LD;
     bf16* dv = sV + stage * kAN * LD;
     if constexpr (kFp8) {
-      const int64_t pg = p.table[(int64_t)b * p.table_stride + tile];
+      const int64_t pg = p.table[(int64_t)kvb * p.table_stride + tile];
       const uint8_t* kp = reinterpret_cast<const uint8_t*>(p.k) + pg * p.k_bs + (int64_t)hk * D;
       const uint8_t* vp = reinterpret_cast<const uint8_t*>(p.v) + pg * p.v_bs + (int64_t)hk * D;
       uint8_t* rk = sRaw + stage * 2 * kAN * D;
@@ -141,7 +143,7 @@ __global__ void __launch_bounds__(kAThreads) attn_fwd_kernel(const AttnParamsT<k
       }
     } else if constexpr (kPaged) {
       // the tile is one page: row r of the tile is row r of the page (only tiles below kv_end are ever looked up)
-      const int64_t pg = p.table[(int64_t)b * p.table_stride + tile];
+      const int64_t pg = p.table[(int64_t)kvb * p.table_stride + tile];
       const bf16* kp = kb + pg * p.k_bs;
       const bf16* vp = vb + pg * p.v_bs;
       for (int i = tid; i < kAN * CH; i += kAThreads) {
@@ -309,7 +311,7 @@ __global__ void __launch_bounds__(kAThreads) attn_fwd_kernel(const AttnParamsT<k
 
 template <int D, bool kPaged = false, bool kFp8 = false>
 static int launch_attn(const uvx_attn_args* a, cudaStream_t st, const int32_t* table = nullptr, int64_t table_stride = 0,
-                       const float* kv_scale = nullptr) {
+                       const float* kv_scale = nullptr, const int32_t* kv_row = nullptr) {
   constexpr int LD = D + 8;
   const size_t smem = kFp8 ? (size_t)(kAM + 2 * kAN) * LD * 2 + 4 * kAN * D : (size_t)(kAM + 4 * kAN) * LD * 2;
   static bool attr = false;
@@ -335,6 +337,7 @@ static int launch_attn(const uvx_attn_args* a, cudaStream_t st, const int32_t* t
   p.v_rs = a->v_rs; p.v_bs = a->v_bs; p.o_rs = a->o_rs; p.o_bs = a->o_bs;
   p.kv_len = a->kv_len;
   p.kv_start = a->kv_start;
+  p.kv_row = kv_row;
   p.lse = a->lse;
   p.Hq = (int)a->Hq;
   p.Sq = (int)a->Sq;
@@ -361,18 +364,54 @@ extern "C" int uvx_debug_attn_tc(int on) {
   return UVX_OK;
 }
 
-extern "C" int uvx_attention(const uvx_attn_args* a, uvx_stream_t stream) {
-  using namespace uvx;
-  UVX_REQUIRE(a && a->q && a->k && a->v && a->o, "uvx_attention: null pointer");
-  UVX_REQUIRE(a->D == 64 || a->D == 128, "uvx_attention: head_dim must be 64 or 128 (got %lld)", (long long)a->D);
-  UVX_REQUIRE(a->B >= 1 && a->Hq >= 1 && a->Hkv >= 1 && a->Hq % a->Hkv == 0 && a->Sq >= 1 && a->Skv >= 1,
-              "uvx_attention: bad shape");
-  UVX_REQUIRE(a->B < 65536 && a->Hq < 65536, "uvx_attention: grid too large");
+namespace uvx {
+
+static int check_attn(const uvx_attn_args* a, const char* name) {
+  UVX_REQUIRE(a && a->q && a->k && a->v && a->o, "%s: null pointer", name);
+  UVX_REQUIRE(a->D == 64 || a->D == 128, "%s: head_dim must be 64 or 128 (got %lld)", name, (long long)a->D);
+  UVX_REQUIRE(a->B >= 1 && a->Hq >= 1 && a->Hkv >= 1 && a->Hq % a->Hkv == 0 && a->Sq >= 1 && a->Skv >= 1, "%s: bad shape", name);
+  UVX_REQUIRE(a->B < 65536 && a->Hq < 65536, "%s: grid too large", name);
   UVX_REQUIRE(a->q_rs % 8 == 0 && a->k_rs % 8 == 0 && a->v_rs % 8 == 0 && a->o_rs % 2 == 0 && a->q_bs % 8 == 0 &&
                   a->k_bs % 8 == 0 && a->v_bs % 8 == 0,
-              "uvx_attention: strides must keep 16-byte alignment");
+              "%s: strides must keep 16-byte alignment", name);
   UVX_REQUIRE(((uintptr_t)a->q | (uintptr_t)a->k | (uintptr_t)a->v) % 16 == 0 && (uintptr_t)a->o % 4 == 0,
-              "uvx_attention: base pointers must be 16-byte aligned");
+              "%s: base pointers must be 16-byte aligned", name);
+  return UVX_OK;
+}
+
+// The paged forms' checks (fp8: e4m3 pool, k_rs / v_rs % 16).
+static int check_attn_paged(const uvx_attn_args* a, const int32_t* table, int64_t table_stride, bool fp8, const char* name) {
+  UVX_REQUIRE(a && a->q && a->k && a->v && a->o && a->kv_len && table, "%s: null pointer", name);
+  UVX_REQUIRE(a->D == 64 || a->D == 128, "%s: head_dim must be 64 or 128 (got %lld)", name, (long long)a->D);
+  UVX_REQUIRE(a->B >= 1 && a->B < 65536 && a->Hq >= 1 && a->Hq < 65536 && a->Hkv >= 1 && a->Hq % a->Hkv == 0 && a->Sq >= 1 &&
+                  a->Skv >= 1,
+              "%s: bad shape", name);
+  UVX_REQUIRE(table_stride >= (a->Skv + kAN - 1) / kAN, "%s: a table row of %lld pages cannot cover Skv = %lld", name,
+              (long long)table_stride, (long long)a->Skv);
+  UVX_REQUIRE(!a->kv_start && !a->lse && a->block == 0 && (!a->causal || a->Sq == 1),
+              "%s: no kv_start, no lse, no block mask, causal only with Sq == 1", name);
+  UVX_REQUIRE(a->k_bs == (int64_t)kAN * a->k_rs && a->v_bs == (int64_t)kAN * a->v_rs, "%s: k_bs / v_bs must be one page of 64 rows",
+              name);
+  const int64_t kal = fp8 ? 16 : 8;
+  UVX_REQUIRE(a->q_rs % 8 == 0 && a->k_rs % kal == 0 && a->v_rs % kal == 0 && a->o_rs % 2 == 0 && a->q_bs % 8 == 0,
+              "%s: strides must keep 16-byte alignment", name);
+  UVX_REQUIRE(((uintptr_t)a->q | (uintptr_t)a->k | (uintptr_t)a->v) % 16 == 0 && (uintptr_t)a->o % 4 == 0,
+              "%s: base pointers must be 16-byte aligned", name);
+  return UVX_OK;
+}
+
+// The row-mapped forms are decode calls: one query per row, keys bounded by kv_len only.
+static int check_rows(const uvx_attn_args* a, const int32_t* kv_row, const char* name) {
+  UVX_REQUIRE(a && kv_row && a->kv_len && a->Sq == 1 && !a->kv_start && !a->lse && a->block == 0,
+              "%s: needs kv_row and kv_len, Sq = 1, no kv_start, no lse, no block mask", name);
+  return UVX_OK;
+}
+
+}  // namespace uvx
+
+extern "C" int uvx_attention(const uvx_attn_args* a, uvx_stream_t stream) {
+  using namespace uvx;
+  if (int e = check_attn(a, "uvx_attention")) return e;
   if (g_attn_wg < 0) {
     const char* e = getenv("UVX_ATTN_TC");
     g_attn_wg = e ? atoi(e) : 1;
@@ -383,47 +422,47 @@ extern "C" int uvx_attention(const uvx_attn_args* a, uvx_stream_t stream) {
   return a->D == 64 ? launch_attn<64>(a, (cudaStream_t)stream) : launch_attn<128>(a, (cudaStream_t)stream);
 }
 
+extern "C" int uvx_attention_rows(const uvx_attn_args* a, const int32_t* kv_row, uvx_stream_t stream) {
+  using namespace uvx;
+  if (int e = check_rows(a, kv_row, "uvx_attention_rows")) return e;
+  if (int e = check_attn(a, "uvx_attention_rows")) return e;
+  return a->D == 64 ? launch_attn<64>(a, (cudaStream_t)stream, nullptr, 0, nullptr, kv_row)
+                    : launch_attn<128>(a, (cudaStream_t)stream, nullptr, 0, nullptr, kv_row);
+}
+
 extern "C" int uvx_attention_paged(const uvx_attn_args* a, const int32_t* table, int64_t table_stride, uvx_stream_t stream) {
   using namespace uvx;
-  UVX_REQUIRE(a && a->q && a->k && a->v && a->o && a->kv_len && table, "uvx_attention_paged: null pointer");
-  UVX_REQUIRE(a->D == 64 || a->D == 128, "uvx_attention_paged: head_dim must be 64 or 128 (got %lld)", (long long)a->D);
-  UVX_REQUIRE(a->B >= 1 && a->B < 65536 && a->Hq >= 1 && a->Hq < 65536 && a->Hkv >= 1 && a->Hq % a->Hkv == 0 && a->Sq >= 1 &&
-                  a->Skv >= 1,
-              "uvx_attention_paged: bad shape");
-  UVX_REQUIRE(table_stride >= (a->Skv + kAN - 1) / kAN, "uvx_attention_paged: a table row of %lld pages cannot cover Skv = %lld",
-              (long long)table_stride, (long long)a->Skv);
-  UVX_REQUIRE(!a->kv_start && !a->lse && a->block == 0 && (!a->causal || a->Sq == 1),
-              "uvx_attention_paged: no kv_start, no lse, no block mask, causal only with Sq == 1");
-  UVX_REQUIRE(a->k_bs == (int64_t)kAN * a->k_rs && a->v_bs == (int64_t)kAN * a->v_rs,
-              "uvx_attention_paged: k_bs / v_bs must be one page of 64 rows");
-  UVX_REQUIRE(a->q_rs % 8 == 0 && a->k_rs % 8 == 0 && a->v_rs % 8 == 0 && a->o_rs % 2 == 0 && a->q_bs % 8 == 0,
-              "uvx_attention_paged: strides must keep 16-byte alignment");
-  UVX_REQUIRE(((uintptr_t)a->q | (uintptr_t)a->k | (uintptr_t)a->v) % 16 == 0 && (uintptr_t)a->o % 4 == 0,
-              "uvx_attention_paged: base pointers must be 16-byte aligned");
+  if (int e = check_attn_paged(a, table, table_stride, false, "uvx_attention_paged")) return e;
   return a->D == 64 ? launch_attn<64, true>(a, (cudaStream_t)stream, table, table_stride)
                     : launch_attn<128, true>(a, (cudaStream_t)stream, table, table_stride);
+}
+
+extern "C" int uvx_attention_paged_rows(const uvx_attn_args* a, const int32_t* table, int64_t table_stride, const int32_t* kv_row,
+                                        uvx_stream_t stream) {
+  using namespace uvx;
+  if (int e = check_rows(a, kv_row, "uvx_attention_paged_rows")) return e;
+  if (int e = check_attn_paged(a, table, table_stride, false, "uvx_attention_paged_rows")) return e;
+  return a->D == 64 ? launch_attn<64, true>(a, (cudaStream_t)stream, table, table_stride, nullptr, kv_row)
+                    : launch_attn<128, true>(a, (cudaStream_t)stream, table, table_stride, nullptr, kv_row);
 }
 
 extern "C" int uvx_attention_paged_fp8(const uvx_attn_args* a, const int32_t* table, int64_t table_stride, const float* kv_scale,
                                        uvx_stream_t stream) {
   using namespace uvx;
-  UVX_REQUIRE(a && a->q && a->k && a->v && a->o && a->kv_len && table && kv_scale, "uvx_attention_paged_fp8: null pointer");
-  UVX_REQUIRE(a->D == 64 || a->D == 128, "uvx_attention_paged_fp8: head_dim must be 64 or 128 (got %lld)", (long long)a->D);
-  UVX_REQUIRE(a->B >= 1 && a->B < 65536 && a->Hq >= 1 && a->Hq < 65536 && a->Hkv >= 1 && a->Hq % a->Hkv == 0 && a->Sq >= 1 &&
-                  a->Skv >= 1,
-              "uvx_attention_paged_fp8: bad shape");
-  UVX_REQUIRE(table_stride >= (a->Skv + kAN - 1) / kAN,
-              "uvx_attention_paged_fp8: a table row of %lld pages cannot cover Skv = %lld", (long long)table_stride, (long long)a->Skv);
-  UVX_REQUIRE(!a->kv_start && !a->lse && a->block == 0 && (!a->causal || a->Sq == 1),
-              "uvx_attention_paged_fp8: no kv_start, no lse, no block mask, causal only with Sq == 1");
-  UVX_REQUIRE(a->k_bs == (int64_t)kAN * a->k_rs && a->v_bs == (int64_t)kAN * a->v_rs,
-              "uvx_attention_paged_fp8: k_bs / v_bs must be one page of 64 rows");
-  UVX_REQUIRE(a->q_rs % 8 == 0 && a->k_rs % 16 == 0 && a->v_rs % 16 == 0 && a->o_rs % 2 == 0 && a->q_bs % 8 == 0,
-              "uvx_attention_paged_fp8: strides must keep 16-byte alignment");
-  UVX_REQUIRE(((uintptr_t)a->q | (uintptr_t)a->k | (uintptr_t)a->v) % 16 == 0 && (uintptr_t)a->o % 4 == 0,
-              "uvx_attention_paged_fp8: base pointers must be 16-byte aligned");
+  UVX_REQUIRE(kv_scale, "uvx_attention_paged_fp8: null pointer");
+  if (int e = check_attn_paged(a, table, table_stride, true, "uvx_attention_paged_fp8")) return e;
   return a->D == 64 ? launch_attn<64, true, true>(a, (cudaStream_t)stream, table, table_stride, kv_scale)
                     : launch_attn<128, true, true>(a, (cudaStream_t)stream, table, table_stride, kv_scale);
+}
+
+extern "C" int uvx_attention_paged_fp8_rows(const uvx_attn_args* a, const int32_t* table, int64_t table_stride, const float* kv_scale,
+                                            const int32_t* kv_row, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(kv_scale, "uvx_attention_paged_fp8_rows: null pointer");
+  if (int e = check_rows(a, kv_row, "uvx_attention_paged_fp8_rows")) return e;
+  if (int e = check_attn_paged(a, table, table_stride, true, "uvx_attention_paged_fp8_rows")) return e;
+  return a->D == 64 ? launch_attn<64, true, true>(a, (cudaStream_t)stream, table, table_stride, kv_scale, kv_row)
+                    : launch_attn<128, true, true>(a, (cudaStream_t)stream, table, table_stride, kv_scale, kv_row);
 }
 
 // Whisper-encoder entry over the fused projection: qkv [B*S, row_stride] with head h's q / k / v at columns q_col + 64h,

@@ -356,21 +356,25 @@ __device__ __forceinline__ void argmax_row(const float* row, int64_t V, int64_t*
 
 // One CTA per row: inactive rows are left alone; temperature <= 0 takes the argmax, otherwise sample_row with the row's own
 // settings and the uniform u[row * u_stride + n_new[row]].
+// Row-mapped form (row_slot != NULL, uvx_sample_rows): row b takes slot s = row_slot[b]'s settings and the uniform
+// u[s * u_stride + row_idx[b]]; rows with row_idx[b] < 0 are left alone.
 __global__ void __launch_bounds__(1024, 1) sample_slots_kernel(const float* logits, int64_t V, const float* temperature,
                                                                const int32_t* top_k, const float* top_p, const float* u,
                                                                int64_t u_stride, const int32_t* n_new, const int32_t* active,
-                                                               int64_t* out) {
+                                                               int64_t* out, const int32_t* row_slot, const int32_t* row_idx) {
   pdl_trigger();
   pdl_wait();
   const int64_t b = blockIdx.x;
-  if (!active[b]) return;
-  const float t = temperature[b];
+  const int64_t s = row_slot ? row_slot[b] : b;
+  const int32_t* step = row_slot ? row_idx + b : n_new + s;
+  if (!active[s] || *step < 0) return;
+  const float t = temperature[s];
   const float* row = logits + b * V;
   if (!(t > 0.f)) {
     argmax_row(row, V, out + b);
     return;
   }
-  sample_row<2>(row, V, __frcp_rn(t), top_k[b], top_p[b], u + b * u_stride, n_new + b, 1, 0, out + b);
+  sample_row<2>(row, V, __frcp_rn(t), top_k[s], top_p[s], u + s * u_stride, step, 1, 0, out + b);
 }
 
 // uvx_repetition_penalty's rule on one row (the caller's CTA) with penalty pen over sq[0:n], staging the original scores in
@@ -392,16 +396,20 @@ __device__ __forceinline__ void penalty_row(float* row, int64_t V, const int64_t
 
 // One CTA per row: uvx_repetition_penalty's rule with the row's own penalty over seq[b, 0:cur_len[b]]; inactive rows and
 // penalty 1 are skipped.
+// Row-mapped form (row_slot != NULL, uvx_repetition_penalty_rows_map): row b takes slot s = row_slot[b]'s penalty over
+// seq[s, 0:row_len[b]] with its own scratch row b; rows with row_idx[b] < 0 are skipped.
 __global__ void __launch_bounds__(1024) rep_penalty_slots_kernel(float* logits, int64_t V, const int64_t* seq, int64_t seq_stride,
                                                                  const int32_t* cur_len, const float* penalty, const int32_t* active,
-                                                                 float* __restrict__ scratch) {
+                                                                 float* __restrict__ scratch, const int32_t* row_slot,
+                                                                 const int32_t* row_len, const int32_t* row_idx) {
   pdl_trigger();
   pdl_wait();
   const int64_t b = blockIdx.x;
-  if (!active[b]) return;
-  const float pen = penalty[b];
+  const int64_t s = row_slot ? row_slot[b] : b;
+  if (!active[s] || (row_slot && row_idx[b] < 0)) return;
+  const float pen = penalty[s];
   if (pen == 1.f) return;
-  penalty_row(logits + b * V, V, seq + b * seq_stride, scratch + b * seq_stride, cur_len[b], pen);
+  penalty_row(logits + b * V, V, seq + s * seq_stride, scratch + b * seq_stride, row_slot ? row_len[b] : cur_len[s], pen);
 }
 
 // One CTA per row: the penalty over seq[b * seq_stride, 0:len[b]] with per-row scratch, so rows may share one sequence
@@ -491,10 +499,12 @@ constexpr int kLogprobsMax = 20;  // alternatives per token (OpenAI-style top_lo
 // keys above it (fewer than n) are gathered in any order, the missing ones are taken from the keys equal to it in index order
 // (thread t owns the chunk [t*c, (t+1)*c), an exclusive scan of the per-chunk counts ranks them), and the n are sorted by
 // rank, as in beam_row_topk_kernel.  Every reduction has a fixed order, so a row's bits depend on its logits alone.
+// Row-mapped form (row_slot != NULL, uvx_token_logprobs_rows): row b takes slot s = row_slot[b]'s n_top[s] and writes slot s's
+// outputs at index dst[b].
 __global__ void __launch_bounds__(1024, 1) token_logprobs_kernel(const float* logits, int64_t V, const int64_t* tok,
                                                                  const int32_t* n_top, const int32_t* dst, int64_t cap, int n_max,
                                                                  float* __restrict__ out_lp, int64_t* __restrict__ out_ids,
-                                                                 float* __restrict__ out_top) {
+                                                                 float* __restrict__ out_top, const int32_t* row_slot) {
   pdl_trigger();
   pdl_wait();
   __shared__ float red[32];
@@ -506,7 +516,8 @@ __global__ void __launch_bounds__(1024, 1) token_logprobs_kernel(const float* lo
   __shared__ int64_t s_idx[kLogprobsMax];
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const int64_t b = blockIdx.x;
-  const int want = n_top[b];
+  const int64_t so = row_slot ? row_slot[b] : b;  // the output row
+  const int want = n_top[so];
   const int64_t d = dst[b];
   if (want < 0 || d < 0 || d >= cap) return;
   const float* row = logits + b * V;
@@ -525,7 +536,7 @@ __global__ void __launch_bounds__(1024, 1) token_logprobs_kernel(const float* lo
   const float lse = mx + logf(warp_sum(red[lane]));
   if (tid == 0) {
     const int64_t t = tok[b];
-    out_lp[b * cap + d] = (t >= 0 && t < V) ? row[t] - lse : NAN;
+    out_lp[so * cap + d] = (t >= 0 && t < V) ? row[t] - lse : NAN;
   }
   int64_t kk = want < n_max ? want : n_max;
   kk = kk < V ? kk : V;
@@ -583,7 +594,7 @@ __global__ void __launch_bounds__(1024, 1) token_logprobs_kernel(const float* lo
     const int64_t ix = s_idx[tid];
     int pos = 0;
     for (int m = 0; m < K; ++m) pos += s_val[m] > x || (s_val[m] == x && s_idx[m] < ix);
-    const int64_t o = (b * cap + d) * n_max + pos;
+    const int64_t o = (so * cap + d) * n_max + pos;
     out_ids[o] = ix;
     out_top[o] = x - lse;
   }
@@ -633,25 +644,13 @@ __global__ void __launch_bounds__(1024, 1) record_scores_kernel(const float* log
 // generated so far; its last token has not been fed yet.
 constexpr int kLookupMaxK = 31;  // drafts per step: k + 1 rows within the decode-form GEMM's 32
 
-// One CTA (1024 threads).  For every continuation start e in [1, L) (L = cur_len), m(e) = the number of tokens, at most
-// min(n, L - 1), that agree going back from e - 1 and from L - 1.  HF tries n-gram sizes from min(n, L - 1) down and takes
-// the leftmost earlier occurrence with a non-empty continuation, so the winner is the largest size g with a match (the block
-// maximum of m) at the smallest e with m(e) >= g (a block minimum).  Drafts: seq[e, min(e + k, L)), cut before the first EOS
-// and to the budget (n_new + d + 1 <= max_new); none when done.  Writes the k + 1 fed tokens (row 0 the last token, rows 1..d
-// the drafts, later rows the last token again), d, each row's cache position / key count / RoPE position (L - 1 + i, L + i,
-// L - 1 + i), penalty length L + i and record index n_new + i, and the drafts into seq[L, L + d).
-__global__ void __launch_bounds__(1024) lookup_draft_kernel(int64_t* seq, const int32_t* cur_len, const int32_t* n_new, int max_new,
-                                                            int k, int n, const int64_t* __restrict__ eos, int n_eos,
-                                                            const int32_t* done, int64_t* tok, int32_t* n_draft, int32_t* pos,
-                                                            int32_t* lens, int32_t* rope_pos, int32_t* pen_len, int32_t* idx) {
-  pdl_trigger();
-  pdl_wait();
-  __shared__ int red[32];
+// The search and the cut, shared by lookup_draft_kernel and lookup_draft_slots_kernel (the rule is stated above
+// lookup_draft_kernel): the whole CTA (1024 threads) searches seq[0:L] when `search`; returns true in warp 0 only, with d = the
+// draft count (<= min(k, room)) and, in lanes < d, t = draft lane.  Needs room > 0 and min(n, L - 1) > 0 when searching.
+__device__ __forceinline__ bool lookup_find(const int64_t* seq, int L, int k, int n, int room, bool search,
+                                            const int64_t* __restrict__ eos, int n_eos, int* red, int& d, int64_t& t) {
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  const int L = *cur_len, nn = *n_new;
-  const int room = max_new - nn - 1;
   const int nmax = min(n, L - 1);
-  const bool search = !*done && room > 0 && nmax > 0;
   const int64_t* tail = seq + L - 1;  // tail[-j] is the j-th token from the end
   int best = 0;
   if (search) {
@@ -682,13 +681,13 @@ __global__ void __launch_bounds__(1024) lookup_draft_kernel(int64_t* seq, const 
   for (int o = 16; o > 0; o >>= 1) first = min(first, __shfl_xor_sync(0xffffffffu, first, o));
   if (lane == 0) red[w] = first;
   __syncthreads();
-  if (w != 0) return;
+  if (w != 0) return false;
   first = red[lane];
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) first = min(first, __shfl_xor_sync(0xffffffffu, first, o));
-  int d = 0;
+  d = 0;
   if (g > 0) d = min(min(k, L - first), room);
-  int64_t t = 0;
+  t = 0;
   bool stop = false;
   if (lane < d) {
     t = seq[first + lane];
@@ -696,8 +695,32 @@ __global__ void __launch_bounds__(1024) lookup_draft_kernel(int64_t* seq, const 
   }
   const unsigned hit = __ballot_sync(0xffffffffu, stop);
   if (hit) d = __ffs(hit) - 1;  // drafts end before the first EOS; an EOS first means no drafts (HF looks no further)
+  return true;
+}
+
+// One CTA (1024 threads).  For every continuation start e in [1, L) (L = cur_len), m(e) = the number of tokens, at most
+// min(n, L - 1), that agree going back from e - 1 and from L - 1.  HF tries n-gram sizes from min(n, L - 1) down and takes
+// the leftmost earlier occurrence with a non-empty continuation, so the winner is the largest size g with a match (the block
+// maximum of m) at the smallest e with m(e) >= g (a block minimum).  Drafts: seq[e, min(e + k, L)), cut before the first EOS
+// and to the budget (n_new + d + 1 <= max_new); none when done.  Writes the k + 1 fed tokens (row 0 the last token, rows 1..d
+// the drafts, later rows the last token again), d, each row's cache position / key count / RoPE position (L - 1 + i, L + i,
+// L - 1 + i), penalty length L + i and record index n_new + i, and the drafts into seq[L, L + d).
+__global__ void __launch_bounds__(1024) lookup_draft_kernel(int64_t* seq, const int32_t* cur_len, const int32_t* n_new, int max_new,
+                                                            int k, int n, const int64_t* __restrict__ eos, int n_eos,
+                                                            const int32_t* done, int64_t* tok, int32_t* n_draft, int32_t* pos,
+                                                            int32_t* lens, int32_t* rope_pos, int32_t* pen_len, int32_t* idx) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ int red[32];
+  const int lane = threadIdx.x & 31;
+  const int L = *cur_len, nn = *n_new;
+  const int room = max_new - nn - 1;
+  const bool search = !*done && room > 0 && min(n, L - 1) > 0;
+  int d;
+  int64_t t;
+  if (!lookup_find(seq, L, k, n, room, search, eos, n_eos, red, d, t)) return;
   if (lane < d) seq[L + lane] = t;
-  const int64_t last = *tail;
+  const int64_t last = seq[L - 1];
   const int64_t tok_in = __shfl_up_sync(0xffffffffu, t, 1);  // lane i feeds draft i - 1
   if (lane <= k) {
     tok[lane] = (lane >= 1 && lane <= d) ? tok_in : last;
@@ -708,6 +731,21 @@ __global__ void __launch_bounds__(1024) lookup_draft_kernel(int64_t* seq, const 
     idx[lane] = nn + lane;
   }
   if (lane == 0) *n_draft = d;
+}
+
+// One warp: the count m of leading picks that equal the drafts; pick[0 : m + 1] are appended at seq[L] (lanes <= m), and
+// whether the last of them finishes the sequence (an EOS id or the budget) is returned.  Shared by lookup_accept_kernel and
+// lookup_accept_slots_kernel.
+__device__ __forceinline__ int lookup_match(const int64_t* pick, const int64_t* tok, int d, const int64_t* __restrict__ eos, int n_eos,
+                                            int64_t* seq, int L, int nn, int max_new, int& fin) {
+  const int lane = threadIdx.x & 31;
+  const bool miss = lane >= d || pick[lane] != tok[lane + 1];
+  const int m = __ffs(__ballot_sync(0xffffffffu, miss)) - 1;  // d <= 31: lane d always misses
+  if (lane <= m) seq[L + lane] = pick[lane];
+  const int64_t t = pick[m];
+  fin = nn + m + 1 >= max_new;
+  for (int i = 0; i < n_eos; ++i) fin |= t == eos[i];
+  return m;
 }
 
 // One warp.  n_matches = the leading picks that equal the drafts (pick[i] == tok[i + 1], i < d), the valid tokens are
@@ -722,15 +760,10 @@ __global__ void __launch_bounds__(32) lookup_accept_kernel(const int64_t* pick, 
   pdl_wait();
   if (*done) return;
   const int lane = threadIdx.x;
-  const int d = *n_draft;
-  const bool miss = lane >= d || pick[lane] != tok[lane + 1];
-  const int m = __ffs(__ballot_sync(0xffffffffu, miss)) - 1;  // d <= 31: lane d always misses
   const int L = *cur_len, nn = *n_new;
-  if (lane <= m) seq[L + lane] = pick[lane];
+  int fin;
+  const int m = lookup_match(pick, tok, *n_draft, eos, n_eos, seq, L, nn, max_new, fin);
   if (lane == 0) {
-    const int64_t t = pick[m];
-    int fin = nn + m + 1 >= max_new;
-    for (int i = 0; i < n_eos; ++i) fin |= t == eos[i];
     *cur_len = L + m + 1;
     *n_new = nn + m + 1;
     *done = fin;
@@ -740,6 +773,90 @@ __global__ void __launch_bounds__(32) lookup_accept_kernel(const int64_t* pick, 
       *step = s + 1;
     }
   }
+}
+
+// Prompt lookup inside the slot step (SlotDecodeEngine's lookup step): slot s owns rows s * (K + 1) + i, i <= K.
+// One CTA (1024 threads) per slot: lookup_find over seq[s, 0:cur_len[s]] with the slot's own k[s] (<= K), n[s] and budget,
+// when the slot is active, not done, not prefilling and k[s] > 0.  Row 0 feeds token[s] at the slot's pos / lens / rope_pos
+// (what a plain step feeds), draft row i <= d feeds draft i - 1 at pos + i, lens + i, rope_pos + i; rows past the drafts feed
+// token[s] with row 0's positions.  pen_len = cur_len + i and idx = n_new + i for row 0 and the drafts, idx = -1 past them;
+// row_slot = s; cache_row = s for row 0 (-1 when the slot is done or prefilling) and the drafts, -1 past them.
+__global__ void __launch_bounds__(1024) lookup_draft_slots_kernel(int64_t* seq, int64_t seq_stride, const int64_t* token,
+                                                                  const int32_t* cur_len, const int32_t* n_new,
+                                                                  const int32_t* max_new, const int32_t* k_slot, const int32_t* n_slot,
+                                                                  const int32_t* done, const int32_t* active, const int32_t* prefilling,
+                                                                  const int32_t* pos, const int32_t* lens, const int32_t* rope_pos,
+                                                                  int K, const int64_t* __restrict__ eos, int n_eos, int64_t* tok,
+                                                                  int32_t* n_draft, int32_t* row_pos, int32_t* row_lens,
+                                                                  int32_t* row_rope, int32_t* pen_len, int32_t* idx,
+                                                                  int32_t* row_slot, int32_t* cache_row) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ int red[32];
+  const int lane = threadIdx.x & 31;
+  const int s = blockIdx.x;
+  int64_t* sq = seq + (int64_t)s * seq_stride;
+  const bool open = active[s] && !done[s] && !prefilling[s];
+  const int L = cur_len[s], nn = n_new[s], ks = min(k_slot[s], K), ns = n_slot[s];
+  const int room = max_new[s] - nn - 1;
+  const bool search = open && ks > 0 && ns > 0 && room > 0 && min(ns, L - 1) > 0;
+  int d;
+  int64_t t;
+  if (!lookup_find(sq, L, ks, ns, room, search, eos, n_eos, red, d, t)) return;
+  if (lane < d) sq[L + lane] = t;
+  const int64_t tok_in = __shfl_up_sync(0xffffffffu, t, 1);  // lane i feeds draft i - 1
+  if (lane <= K) {
+    const int r = s * (K + 1) + lane;
+    const bool real = lane <= d;
+    const int i = real ? lane : 0;
+    tok[r] = (lane >= 1 && lane <= d) ? tok_in : token[s];
+    row_pos[r] = pos[s] + i;
+    row_lens[r] = lens[s] + i;
+    row_rope[r] = rope_pos[s] + i;
+    pen_len[r] = L + i;
+    idx[r] = real ? nn + lane : -1;
+    row_slot[r] = s;
+    cache_row[r] = real && (lane > 0 || (!done[s] && !prefilling[s])) ? s : -1;
+  }
+  if (lane == 0) n_draft[s] = d;
+}
+
+// Warp w of one CTA takes slots w, w + warps, ...: for each active slot that is not done, lookup_match over its rows, then
+// uvx_slot_finish's bookkeeping for the m + 1 tokens - cur_len / n_new += m + 1, done = the last is an EOS id or the budget is
+// reached, pos / lens / rope_pos += m + 1 while the slot stays open (m when it finishes: only the last token can finish it) -
+// token[s] = the last pick (fed next), accepted[s] += m.  n_open[0] = active slots still open.
+__global__ void lookup_accept_slots_kernel(const int64_t* pick, const int64_t* tok, const int32_t* n_draft, int K,
+                                           const int64_t* __restrict__ eos, int n_eos, int64_t* seq, int64_t seq_stride,
+                                           int64_t* token, int32_t* done, int32_t* cur_len, int32_t* n_new, const int32_t* max_new,
+                                           const int32_t* active, int32_t* pos, int32_t* lens, int32_t* rope_pos,
+                                           int32_t* accepted, int32_t* n_open, int slots) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ int open;
+  if (threadIdx.x == 0) open = 0;
+  __syncthreads();
+  const int lane = threadIdx.x & 31, warps = blockDim.x >> 5;
+  for (int s = threadIdx.x >> 5; s < slots; s += warps) {
+    if (!active[s] || done[s]) continue;
+    const int64_t r0 = (int64_t)s * (K + 1);
+    const int L = cur_len[s], nn = n_new[s];
+    int fin;
+    const int m = lookup_match(pick + r0, tok + r0, n_draft[s], eos, n_eos, seq + s * seq_stride, L, nn, max_new[s], fin);
+    if (lane == 0) {
+      cur_len[s] = L + m + 1;
+      n_new[s] = nn + m + 1;
+      done[s] = fin;
+      token[s] = pick[r0 + m];
+      accepted[s] += m;
+      const int bump = fin ? m : m + 1;
+      pos[s] += bump;
+      lens[s] += bump;
+      rope_pos[s] += bump;
+      if (!fin) atomicAdd(&open, 1);
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) *n_open = open;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -1240,7 +1357,7 @@ extern "C" int uvx_sample_slots(const float* logits, int64_t B, int64_t V, const
                   V <= (int64_t)1 << 24 && u_stride >= 0,
               "uvx_sample_slots: bad arguments");
   launch_k(sample_slots_kernel, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, temperature, top_k, top_p, u,
-           u_stride, n_new, active, out_idx);
+           u_stride, n_new, active, out_idx, (const int32_t*)nullptr, (const int32_t*)nullptr);
   return check_launch("sample_slots_kernel");
 }
 
@@ -1251,7 +1368,7 @@ extern "C" int uvx_repetition_penalty_slots(float* logits, int64_t B, int64_t V,
   UVX_REQUIRE(logits && seq && cur_len && penalty && active && scratch && B >= 1 && V >= 1,
               "uvx_repetition_penalty_slots: bad arguments");
   launch_k(rep_penalty_slots_kernel, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, seq, seq_stride, cur_len,
-           penalty, active, scratch);
+           penalty, active, scratch, (const int32_t*)nullptr, (const int32_t*)nullptr, (const int32_t*)nullptr);
   return check_launch("rep_penalty_slots_kernel");
 }
 
@@ -1289,6 +1406,64 @@ extern "C" int uvx_lookup_accept(const int64_t* pick, const int64_t* tok, const 
   launch_k(lookup_accept_kernel, dim3(1), dim3(32), 0, (cudaStream_t)stream, pick, tok, n_draft, eos_ids, (int)n_eos, seq, cur_len,
            n_new, (int)max_new, step, accepted, (int)steps, done);
   return check_launch("lookup_accept_kernel");
+}
+
+extern "C" int uvx_lookup_draft_slots(int64_t* seq, int64_t seq_stride, const int64_t* token, const int32_t* cur_len,
+                                      const int32_t* n_new, const int32_t* max_new, const int32_t* k, const int32_t* n,
+                                      const int32_t* done, const int32_t* active, const int32_t* prefilling, const int32_t* pos,
+                                      const int32_t* lens, const int32_t* rope_pos, int64_t slots, int32_t K, const int64_t* eos_ids,
+                                      int32_t n_eos, int64_t* tok, int32_t* n_draft, int32_t* row_pos, int32_t* row_lens,
+                                      int32_t* row_rope, int32_t* pen_len, int32_t* idx, int32_t* row_slot, int32_t* cache_row,
+                                      uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(seq && token && cur_len && n_new && max_new && k && n && done && active && prefilling && pos && lens && rope_pos && tok &&
+                  n_draft && row_pos && row_lens && row_rope && pen_len && idx && row_slot && cache_row && (n_eos == 0 || eos_ids) &&
+                  n_eos >= 0 && slots >= 1 && slots < 65536 && K >= 1 && K <= kLookupMaxK && seq_stride >= 1,
+              "uvx_lookup_draft_slots: bad arguments (1 <= K <= %d)", kLookupMaxK);
+  launch_k(lookup_draft_slots_kernel, dim3((unsigned)slots), dim3(1024), 0, (cudaStream_t)stream, seq, seq_stride, token, cur_len,
+           n_new, max_new, k, n, done, active, prefilling, pos, lens, rope_pos, (int)K, eos_ids, (int)n_eos, tok, n_draft, row_pos,
+           row_lens, row_rope, pen_len, idx, row_slot, cache_row);
+  return check_launch("lookup_draft_slots_kernel");
+}
+
+extern "C" int uvx_lookup_accept_slots(const int64_t* pick, const int64_t* tok, const int32_t* n_draft, int64_t slots, int32_t K,
+                                       const int64_t* eos_ids, int32_t n_eos, int64_t* seq, int64_t seq_stride, int64_t* token,
+                                       int32_t* done, int32_t* cur_len, int32_t* n_new, const int32_t* max_new, const int32_t* active,
+                                       int32_t* pos, int32_t* lens, int32_t* rope_pos, int32_t* accepted, int32_t* n_open,
+                                       uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(pick && tok && n_draft && seq && token && done && cur_len && n_new && max_new && active && pos && lens && rope_pos &&
+                  accepted && n_open && (n_eos == 0 || eos_ids) && n_eos >= 0 && slots >= 1 && slots < 65536 && K >= 1 &&
+                  K <= kLookupMaxK,
+              "uvx_lookup_accept_slots: bad arguments (1 <= K <= %d)", kLookupMaxK);
+  const int warps = slots < 32 ? (int)slots : 32;
+  launch_k(lookup_accept_slots_kernel, dim3(1), dim3(32 * warps), 0, (cudaStream_t)stream, pick, tok, n_draft, (int)K, eos_ids,
+           (int)n_eos, seq, seq_stride, token, done, cur_len, n_new, max_new, active, pos, lens, rope_pos, accepted, n_open, (int)slots);
+  return check_launch("lookup_accept_slots_kernel");
+}
+
+extern "C" int uvx_sample_rows(const float* logits, int64_t R, int64_t V, const float* temperature, const int32_t* top_k,
+                               const float* top_p, const float* u, int64_t u_stride, const int32_t* active, const int32_t* row_slot,
+                               const int32_t* row_idx, int64_t* out_idx, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(logits && temperature && top_k && top_p && u && active && row_slot && row_idx && out_idx && R >= 1 && R < 65536 &&
+                  V >= 1 && V <= (int64_t)1 << 24 && u_stride >= 0,
+              "uvx_sample_rows: bad arguments");
+  launch_k(sample_slots_kernel, dim3((unsigned)R), dim3(1024), 0, (cudaStream_t)stream, logits, V, temperature, top_k, top_p, u,
+           u_stride, (const int32_t*)nullptr, active, out_idx, row_slot, row_idx);
+  return check_launch("sample_slots_kernel (rows)");
+}
+
+extern "C" int uvx_repetition_penalty_rows_map(float* logits, int64_t R, int64_t V, const int64_t* seq, int64_t seq_stride,
+                                               const float* penalty, const int32_t* active, const int32_t* row_slot,
+                                               const int32_t* row_len, const int32_t* row_idx, float* scratch, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(logits && seq && penalty && active && row_slot && row_len && row_idx && scratch && R >= 1 && R < 65536 && V >= 1 &&
+                  seq_stride >= 1,
+              "uvx_repetition_penalty_rows_map: bad arguments");
+  launch_k(rep_penalty_slots_kernel, dim3((unsigned)R), dim3(1024), 0, (cudaStream_t)stream, logits, V, seq, seq_stride,
+           (const int32_t*)nullptr, penalty, active, scratch, row_slot, row_len, row_idx);
+  return check_launch("rep_penalty_slots_kernel (rows)");
 }
 
 extern "C" int uvx_slot_finish(const int64_t* tok, int32_t* done, const int64_t* eos_ids, int32_t n_eos, int64_t* seq,
@@ -1468,8 +1643,20 @@ extern "C" int uvx_token_logprobs(const float* logits, int64_t B, int64_t V, con
                   n_max >= 0 && n_max <= kLogprobsMax && (n_max == 0 || (out_ids && out_top)),
               "uvx_token_logprobs: bad arguments (0 <= n_max <= %d)", kLogprobsMax);
   launch_k(token_logprobs_kernel, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, tok, n_top, dst, cap, (int)n_max,
-           out_lp, out_ids, out_top);
+           out_lp, out_ids, out_top, (const int32_t*)nullptr);
   return check_launch("token_logprobs_kernel");
+}
+
+extern "C" int uvx_token_logprobs_rows(const float* logits, int64_t R, int64_t V, const int64_t* tok, const int32_t* n_top,
+                                       const int32_t* row_slot, const int32_t* dst, int64_t cap, int32_t n_max, float* out_lp,
+                                       int64_t* out_ids, float* out_top, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(logits && tok && n_top && row_slot && dst && out_lp && R >= 1 && R < 65536 && V >= 1 && V <= ((int64_t)1 << 31) - 1 &&
+                  cap >= 1 && n_max >= 0 && n_max <= kLogprobsMax && (n_max == 0 || (out_ids && out_top)),
+              "uvx_token_logprobs_rows: bad arguments (0 <= n_max <= %d)", kLogprobsMax);
+  launch_k(token_logprobs_kernel, dim3((unsigned)R), dim3(1024), 0, (cudaStream_t)stream, logits, V, tok, n_top, dst, cap, (int)n_max,
+           out_lp, out_ids, out_top, row_slot);
+  return check_launch("token_logprobs_kernel (rows)");
 }
 
 extern "C" int uvx_record_scores(const float* logits, int64_t B, int64_t V, float temperature, int32_t top_k, float top_p,

@@ -131,27 +131,33 @@ class _RowKV:
     def __init__(self, cache: KVCache):
         self.cache = cache
 
-    def map_rows(self, e: "_Decoder", R: int) -> None:
-        """Before the embedding of a step over R rows: a row's cache row is its own (or ``_mrow``'s), nothing to map."""
+    def map_rows(self, e: "_Decoder", R: int, mode: str) -> None:
+        """Before the embedding of a step over R rows: a row's cache row is its own (or ``_mrow``'s / ``_lk_wrow``'s), nothing
+        to map."""
 
-    def attend(self, e: "_Decoder", li: int, qkv: torch.Tensor) -> torch.Tensor:
+    def attend(self, e: "_Decoder", li: int, qkv: torch.Tensor, mode: str) -> torch.Tensor:
         """The cache-touching calls of layer ``li`` of a step over the R rows of ``qkv``: RoPE on q / k + the KV append, then
-        attention of the B decode rows over their cache rows and, in a mixed step (R > B), of the chunk rows over the prefilling
-        slot's row -> [R, Hq * D].  A plain step appends row b at ``pos[b]`` of cache row b, a mixed step through ``_mrow``."""
+        attention -> [R, Hq * D].  ``mode`` "plain": row b appends at ``pos[b]`` of cache row b and attends to it; "mixed": the
+        B decode rows as in a plain step, the chunk rows appended through ``_mrow`` and attending to the prefilling slot's row;
+        "lookup" (``SlotDecodeEngine``'s lookup step): row r appends through ``_lk_wrow`` / ``_lk_pos`` and attends to cache row
+        ``_lk_slot[r]``, so a slot's draft rows see the positions its earlier rows appended in the same step."""
         nq, nkv, hd = e.heads
         B, R = e.B, qkv.shape[0]
         kc, vc = self.cache.k[li], self.cache.v[li]
         smax = kc.shape[1]
-        if R == B:
+        att = torch.empty(R, nq * hd, dtype=torch.bfloat16, device=qkv.device)
+        if mode == "lookup":
+            ops.rope_kv_append_map_(qkv, nq, nkv, hd, e.cos, e.sin, e._lk_rope, kc, vc, e._lk_wrow, e._lk_pos)
+            return ops.attention_rows(qkv[:, :nq * hd], kc, vc, att, nq, hd ** -0.5, e._lk_lens, e._lk_slot)
+        if mode == "plain":
             ops.rope_kv_append_(qkv, nq, nkv, hd, e.cos, e.sin, e.rope_pos, kc, vc, e.pos)
         else:
             ops.rope_kv_append_map_(qkv, nq, nkv, hd, e.cos, e.sin, e._mrope, kc, vc, e._mrow, e._mpos)
-        att = torch.empty(R, nq * hd, dtype=torch.bfloat16, device=qkv.device)
         rs = qkv.stride(0)
         ops.attention(qkv.data_ptr(), kc.data_ptr(), vc.data_ptr(), att, B, nq, nkv, 1, smax, hd,
                       (rs, rs, nkv * hd, smax * nkv * hd, nkv * hd, smax * nkv * hd, nq * hd, nq * hd), hd ** -0.5, False,
                       e.lens, 0, e.kv_start)
-        if R > B:
+        if mode == "mixed":
             ops.attention_indexed(qkv[B:, :nq * hd].unsqueeze(0), kc, vc, att[B:].unsqueeze(0), nq, hd ** -0.5, *e._mscal.split(1))
         return att
 
@@ -180,6 +186,20 @@ def check_kv_scales(kv_scales, layers: int) -> torch.Tensor:
     if not bool((torch.isfinite(t) & (t > 0)).all()):
         raise ValueError("kv_scales must be positive and finite")
     return t
+
+
+def check_lookup_k(slots: int, k) -> int:
+    """The engine-wide draft maximum K of ``prompt_lookup_num_tokens`` (None -> 0, off); ValueError unless None or an integer
+    in [1, LOOKUP_MAX_K] with slots * (K + 1) <= PREFILL_ROWS."""
+    if k is None:
+        return 0
+    if isinstance(k, bool) or not isinstance(k, numbers.Integral) or not 1 <= k <= ops.LOOKUP_MAX_K:
+        raise ValueError(f"prompt_lookup_num_tokens must be an integer in [1, {ops.LOOKUP_MAX_K}] (k + 1 rows of the decode "
+                         f"step), got {k!r}")
+    if slots * (int(k) + 1) > PREFILL_ROWS:
+        raise ValueError(f"{slots} slots x (prompt_lookup_num_tokens = {k} + 1) = {slots * (int(k) + 1)} rows per step; at most "
+                         f"{PREFILL_ROWS}")
+    return int(k)
 
 
 class _PagedKV:
@@ -265,19 +285,26 @@ class _PagedKV:
         lists = torch.tensor(src + dst, dtype=torch.int32).pin_memory().to(self.table.device, non_blocking=True)
         ops.kv_pages_move(sk, sv, dk, dv, lists[:len(src)], lists[len(src):])
 
-    def map_rows(self, e: "_Decoder", R: int) -> None:
-        ops.kv_page_map(self.table, e._mrow[:R], e._mpos[:R], self.page[:R], self.off[:R], frozen=e.done)
+    def map_rows(self, e: "_Decoder", R: int, mode: str) -> None:
+        if mode == "lookup":        # done and prefilling slots already map to -1 (uvx_lookup_draft_slots)
+            ops.kv_page_map(self.table, e._lk_wrow, e._lk_pos, self.page[:R], self.off[:R])
+        else:
+            ops.kv_page_map(self.table, e._mrow[:R], e._mpos[:R], self.page[:R], self.off[:R], frozen=e.done)
 
-    def attend(self, e: "_Decoder", li: int, qkv: torch.Tensor) -> torch.Tensor:
+    def attend(self, e: "_Decoder", li: int, qkv: torch.Tensor, mode: str) -> torch.Tensor:
         """``_RowKV.attend`` through the page map and the table: every row appends at its (page, offset)."""
         nq, nkv, hd = e.heads
         B, R = e.B, qkv.shape[0]
         kp, vp = self.pool_k[li], self.pool_v[li]
         sc = None if self.kv_scales is None else self.kv_scales[li]
-        ops.rope_kv_append_map_(qkv, nq, nkv, hd, e.cos, e.sin, e._mrope[:R], kp, vp, self.page[:R], self.off[:R], kv_scale=sc)
+        rope = e._lk_rope if mode == "lookup" else e._mrope[:R]
+        ops.rope_kv_append_map_(qkv, nq, nkv, hd, e.cos, e.sin, rope, kp, vp, self.page[:R], self.off[:R], kv_scale=sc)
         att = torch.empty(R, nq * hd, dtype=torch.bfloat16, device=qkv.device)
+        if mode == "lookup":
+            return ops.attention_paged(qkv[:, :nq * hd], kp, vp, att, nq, hd ** -0.5, self.table, e._lk_lens, kv_scale=sc,
+                                       kv_row=e._lk_slot)
         ops.attention_paged(qkv[:B, :nq * hd], kp, vp, att[:B], nq, hd ** -0.5, self.table, e.lens, kv_scale=sc)
-        if R > B:
+        if mode == "mixed":
             ops.attention_indexed_paged(qkv[B:, :nq * hd].unsqueeze(0), kp, vp, att[B:].unsqueeze(0), nq, hd ** -0.5, self.table,
                                         *e._mscal.split(1), kv_scale=sc)
         return att
@@ -355,21 +382,26 @@ class _Decoder:
         self.rope_pos[rows] = (S - 1) - pad
 
     # -- one step ------------------------------------------------------------------------------------------
-    def _forward(self, mixed_in: Optional[torch.Tensor] = None, head_rows: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def _forward(self, mixed_in: Optional[torch.Tensor] = None, head_rows: Optional[torch.Tensor] = None,
+                 lookup: bool = False) -> torch.Tensor:
         """Embedding -> layers -> final norm -> LM head of a step -> fp32 logits.  A plain step (``mixed_in`` None) feeds the B
         rows of ``token``.  A mixed step feeds ``mixed_in`` [R, D]: the token embedding is written into its first B rows, the
-        prompt-chunk rows follow, and the LM head runs over rows ``head_rows`` only."""
+        prompt-chunk rows follow, and the LM head runs over rows ``head_rows`` only.  A lookup step (``lookup``,
+        ``SlotDecodeEngine``) feeds the R rows of ``_lk_tok``."""
         m = self.model
         lm, tc = m.language_model, m.config.text_config
         B = self.B
+        mode = "lookup" if lookup else ("plain" if mixed_in is None else "mixed")
+        tokens = self._lk_tok if lookup else self.token
+        R = tokens.shape[0] if mixed_in is None else mixed_in.shape[0]
         # one stream: matrix-vector kernels (fp32 FMAs on the CUDA cores keep up with the weight stream) with RMSNorm / SwiGLU fused
         # into their prologues; more streams: the tensor-core GEMM (at B = 8 the FMA work per weight byte is 8x and the GEMV is
         # instruction-bound)
-        one = mixed_in is None and B <= GEMV_MAX_B
+        one = mode == "plain" and B <= GEMV_MAX_B
         eps = tc.rms_norm_eps
-        self.kv.map_rows(self, B if mixed_in is None else mixed_in.shape[0])
+        self.kv.map_rows(self, R, mode)
         if mixed_in is None:
-            h = ops.embed_splice(self.token, lm.model.embed_tokens.weight, None, None).view(B, tc.hidden_size)
+            h = ops.embed_splice(tokens, lm.model.embed_tokens.weight, None, None).view(R, tc.hidden_size)
         else:
             h = mixed_in
             ops.embed_splice(self.token, lm.model.embed_tokens.weight, None, None, out=h[:B])
@@ -379,7 +411,7 @@ class _Decoder:
                 qkv = ops.gemv(h, sa.qkv_w, norm=(layer.input_layernorm.weight, eps))
             else:
                 qkv = ops.linear(ops.rmsnorm(h, layer.input_layernorm.weight, eps), sa.qkv_w)
-            att = self.kv.attend(self, li, qkv)
+            att = self.kv.attend(self, li, qkv, mode)
             if one:
                 h = ops.gemv(att, sa.o_proj.weight, residual=h)
                 gu = ops.gemv(h, mlp.gate_up_w, norm=(layer.post_attention_layernorm.weight, eps))
@@ -531,7 +563,7 @@ class _SeqKV(_RowKV):
     ``lens[i]`` positions, through a K / V batch stride of 0.  The append writes every row before the attention reads, so row i
     sees the positions rows 0..i-1 wrote in the same step, as a plain decode step of its own would have."""
 
-    def attend(self, e: "_Decoder", li: int, qkv: torch.Tensor) -> torch.Tensor:
+    def attend(self, e: "_Decoder", li: int, qkv: torch.Tensor, mode: str) -> torch.Tensor:
         nq, nkv, hd = e.heads
         R = qkv.shape[0]
         kc, vc = self.cache.k[li], self.cache.v[li]
@@ -800,17 +832,33 @@ class SlotDecodeEngine(_Decoder):
     admission pick) copies the raw logits rows aside before the penalty and runs ``uvx_token_logprobs`` after the sampler, which
     writes each row's chosen-token log-prob and its ``n_top[b]`` most likely alternatives at index ``n_new[b]`` of
     ``lp_token`` [slots, max_len + 1] / ``lp_ids``, ``lp_top`` [slots, max_len + 1, max_logprobs].  A request asks with
-    ``admit(..., logprobs=k)``.  With 0 (the default) nothing is allocated and the step is unchanged."""
+    ``admit(..., logprobs=k)``.  With 0 (the default) nothing is allocated and the step is unchanged.
+
+    ``prompt_lookup_num_tokens`` = K (1..31, with slots * (K + 1) <= ``PREFILL_ROWS``) adds prompt lookup decoding: a request
+    admitted with ``lookup=(k, n)``, 1 <= k <= K, drafts up to k tokens per step from its own earlier n-grams
+    (``uvx_lookup_draft``'s rule, capped so it never passes its budget) and keeps the picks that agree plus one, so its tokens
+    are those of plain slot decoding and a step yields 1 to k + 1 of them.  While no chunked prompt is in flight and some
+    active slot has k > 0, ``step`` replays a third graph, the lookup step (captured on first use), over R = slots * (K + 1)
+    rows, slot s owning rows s * (K + 1) + i: ``uvx_lookup_draft_slots`` lays out the rows, the forward runs them with the
+    row-mapped RoPE + append and attention (a slot's rows all read its cache row; rows past its drafts write nothing), the
+    row-mapped penalty / sampler / log-prob kernels pick each row as plain decoding would pick that position, and
+    ``uvx_lookup_accept_slots`` appends the accepted tokens and leaves every counter as ``uvx_slot_finish`` would.  So the
+    plain and the mixed step can follow any lookup step.  ``accepted`` [slots] int32 counts each request's accepted drafts.
+    The linears of a lookup step run at R rows: a request's bits are those of a plain engine of R slots (the decode-form GEMM
+    keeps rows independent at a fixed row count).  None (the default) allocates and captures nothing."""
 
     def __init__(self, model: UltravoxModel, slots: int, max_len: int, eos_token_ids=None, pad_token_id: int = 0,
-                 use_graph: bool = True, cache=None, max_logprobs: int = 0):
+                 use_graph: bool = True, cache=None, max_logprobs: int = 0, prompt_lookup_num_tokens: Optional[int] = None):
+        check_lookup_k(int(slots), prompt_lookup_num_tokens)      # before the cache is allocated
         kv = _RowKV(cache if cache is not None else model.new_cache(slots, max_len))
-        self._setup(model, int(slots), kv, eos_token_ids, pad_token_id, use_graph, max_logprobs)
+        self._setup(model, int(slots), kv, eos_token_ids, pad_token_id, use_graph, max_logprobs, prompt_lookup_num_tokens)
 
-    def _setup(self, model: UltravoxModel, slots: int, kv, eos_token_ids, pad_token_id: int, use_graph: bool, max_logprobs: int = 0):
+    def _setup(self, model: UltravoxModel, slots: int, kv, eos_token_ids, pad_token_id: int, use_graph: bool, max_logprobs: int = 0,
+               lookup_k: Optional[int] = None):
         if isinstance(max_logprobs, bool) or not isinstance(max_logprobs, numbers.Integral) or \
                 not 0 <= max_logprobs <= ops.LOGPROBS_MAX:
             raise ValueError(f"max_logprobs must be an integer in [0, {ops.LOGPROBS_MAX}], got {max_logprobs!r}")
+        self.K = check_lookup_k(slots, lookup_k)
         self.max_logprobs = int(max_logprobs)
         self.slots = slots
         self.chunk = PREFILL_ROWS - slots
@@ -847,6 +895,28 @@ class SlotDecodeEngine(_Decoder):
             self.lp_token = torch.zeros(slots, self.max_len + 1, **f32)
             self.lp_ids = torch.zeros(slots, self.max_len + 1, self.max_logprobs, dtype=torch.int64, device=dev)
             self.lp_top = torch.zeros(slots, self.max_len + 1, self.max_logprobs, **f32)
+        self._lookup_graph = None
+        self.launches_per_lookup_step = 0
+        # host copy of lk_k: the host picks the graph of each step from it without a sync.  It is cleared at retirement, so a
+        # slot that has finished on the device but is not retired yet (up to the scheduler's sync_every steps) keeps the lookup
+        # step running even when no open slot drafts: the same tokens, at the R-row step's cost for that window
+        self._slot_k = [0] * slots
+        if self.K:
+            R = slots * (self.K + 1)
+            self.lk_k = torch.zeros(slots, **i32)      # per slot: drafts per step (0: none) and n-gram size
+            self.lk_n = torch.full((slots,), 2, **i32)
+            self.accepted = torch.zeros(slots, **i32)
+            self.n_draft = torch.zeros(slots, **i32)
+            # the prefilling mask of uvx_lookup_draft_slots: set while a slot's prompt is chunked, but step() only replays the
+            # lookup step when no prompt is in flight, so it is all zero whenever the lookup step runs
+            self._pf = torch.zeros(slots, **i32)
+            self._lk_tok = torch.zeros(R, 1, dtype=torch.int64, device=dev)
+            self._lk_pick = torch.zeros(R, dtype=torch.int64, device=dev)
+            self._lk_pos, self._lk_lens, self._lk_rope, self._lk_pen, self._lk_idx, self._lk_slot, self._lk_wrow = (
+                torch.zeros(R, **i32) for _ in range(7))
+            self._lk_scratch = torch.empty(R, self.max_len + 1, **f32)
+            if self.max_logprobs:
+                self._lk_raw = torch.empty(R, model.language_model.lm_head.weight.shape[0], **f32)
         self.busy = [False] * slots
         for j in range(slots):
             self._idle(j)
@@ -865,10 +935,35 @@ class SlotDecodeEngine(_Decoder):
         self.busy[j] = False
         if self.max_logprobs:
             self.n_top[j] = -1
+        if self.K:
+            self.lk_k[j] = 0
+            self._slot_k[j] = 0
         self.kv.release(j)
 
     def _state(self):
-        return [self.pos, self.lens, self.rope_pos, self.token, self.cur_len, self.n_new, self.done, self.n_open]
+        lk = [self.accepted, self.n_draft] if self.K else []
+        return [self.pos, self.lens, self.rope_pos, self.token, self.cur_len, self.n_new, self.done, self.n_open] + lk
+
+    def _lookup_step(self):
+        """The lookup step: drafts and row layout, the forward over R rows, the row-mapped pick, the accept."""
+        R = self._lk_tok.shape[0]
+        ops.lookup_draft_slots(self.seq, self.token.view(-1), self.cur_len, self.n_new, self.max_new, self.lk_k, self.lk_n, self.done,
+                               self.active, self._pf, self.pos, self.lens, self.rope_pos, self.K, self.eos, self._lk_tok.view(-1),
+                               self.n_draft, self._lk_pos, self._lk_lens, self._lk_rope, self._lk_pen, self._lk_idx, self._lk_slot,
+                               self._lk_wrow)
+        logits = self._forward(lookup=True)
+        self.logits = logits
+        rows = (self._lk_slot, self._lk_idx)
+        if self.max_logprobs:
+            self._lk_raw.copy_(logits)
+        ops.repetition_penalty_rows_map_(logits, self.seq, self.penalties, self.active, self._lk_slot, self._lk_pen, self._lk_idx,
+                                         self._lk_scratch[:R])
+        ops.sample_rows(logits, self.temps, self.top_ks, self.top_ps, self.u, self.active, *rows, self._lk_pick)
+        if self.max_logprobs:       # at n_new + i, before the accept advances n_new; rows past the drafts (idx -1) record nothing
+            ops.token_logprobs_rows(self._lk_raw, self._lk_pick, self.n_top, *rows, self.lp_token, self.lp_ids, self.lp_top)
+        ops.lookup_accept_slots(self._lk_pick, self._lk_tok.view(-1), self.n_draft, self.K, self.eos, self.seq, self.token.view(-1),
+                                self.done, self.cur_len, self.n_new, self.max_new, self.active, self.pos, self.lens, self.rope_pos,
+                                self.accepted, self.n_open)
 
     def _pick_rows(self, logits: torch.Tensor, r: slice, n_open: torch.Tensor) -> None:
         tok = self.token.view(-1)[r]
@@ -899,6 +994,14 @@ class SlotDecodeEngine(_Decoder):
     def step(self) -> torch.Tensor:
         """A plain decode step, or a mixed step while a chunked prompt is pending (whose last chunk activates its slot)."""
         pf = self._prefill
+        if pf is None and any(self._slot_k):
+            if not self.use_graph:
+                self._lookup_step()
+            else:
+                if self._lookup_graph is None:
+                    self._lookup_graph, self.launches_per_lookup_step = self._capture(self._lookup_step)
+                self._lookup_graph.replay()
+            return self.token
         if pf is None:
             return super().step()
         j, S, a, C, B = pf["slot"], pf["S"], pf["done"], self.chunk, self.slots
@@ -923,6 +1026,8 @@ class SlotDecodeEngine(_Decoder):
         if a + n == S:
             self._prefill = None
             self.active[j] = 1
+            if self.K:
+                self._pf[j] = 0
             if self.max_logprobs:
                 self.n_top[j] = pf["n_top"]
             self._seed(j, S)
@@ -932,7 +1037,7 @@ class SlotDecodeEngine(_Decoder):
 
     def admit(self, slot: int, input_ids: torch.Tensor, max_new_tokens: int, temperature: float = 0.0, top_k: int = 0,
               top_p: float = 1.0, repetition_penalty: float = 1.0, u: Optional[torch.Tensor] = None, past: int = 0,
-              pages=None, logprobs: Optional[int] = None, **features) -> torch.Tensor:
+              pages=None, logprobs: Optional[int] = None, lookup: Optional[tuple] = None, **features) -> torch.Tensor:
         """Prefills one request (``input_ids`` [1, S] plus the processor's audio features, passed to ``model.forward``) at B = 1
         into cache row ``slot``, sets the slot's state and picks its first token from the prefill logits with the slot kernels.
         ``temperature <= 0`` is greedy; a sampled request reads ``u`` (its uniforms, one per step, as ``generate()`` draws them
@@ -949,8 +1054,16 @@ class SlotDecodeEngine(_Decoder):
         S + max_new_tokens positions, and the first ceil(past / 64) of them hold the conversation's first ``past`` positions.
 
         ``logprobs`` (engines with ``max_logprobs`` > 0): None records nothing, 0 the chosen tokens' log-probs, 1..max_logprobs
-        also that many alternatives per token (``token_logprobs_of``)."""
+        also that many alternatives per token (``token_logprobs_of``).
+
+        ``lookup`` (engines with ``prompt_lookup_num_tokens`` = K): (k, n) with 0 <= k <= K drafts per step from n-grams of up
+        to n >= 1 tokens; None or k = 0 drafts nothing."""
         n_top = self.check_logprobs(logprobs)
+        lk, ln = (0, 2) if lookup is None else (int(lookup[0]), int(lookup[1]))
+        if lookup is not None and not self.K:
+            raise ValueError("this engine has no prompt lookup: create it with prompt_lookup_num_tokens = K")
+        if not 0 <= lk <= self.K or ln < 1:
+            raise ValueError(f"lookup = {lookup!r}: need 0 <= k <= {self.K} and n >= 1")
         j = int(slot)
         if not 0 <= j < self.slots:
             raise ValueError(f"slot {slot} out of range [0, {self.slots})")
@@ -982,6 +1095,8 @@ class SlotDecodeEngine(_Decoder):
                 self._mixed_in = torch.zeros(self.slots + self.chunk, embeds.shape[1], dtype=embeds.dtype, device=dev)
             self._prefill = dict(slot=j, S=S, done=P, embeds=embeds, n_top=n_top)
             self._mrow[j] = -1          # the slot's idle decode row must not overwrite position 0 of the prompt
+            if self.K:
+                self._pf[j] = 1
         else:
             logits = self.kv.prefill(self.model, j, input_ids, P, features)
         self.seq[j, :S].copy_(input_ids[0])
@@ -1000,6 +1115,9 @@ class SlotDecodeEngine(_Decoder):
             w = min(u.numel(), self.max_len + 1)
             self.u[j, :w].copy_(u.reshape(-1)[:w])
         self.busy[j] = True
+        if self.K:
+            self.lk_k[j], self.lk_n[j], self.accepted[j] = lk, ln, 0
+            self._slot_k[j] = lk
         if not chunked:
             if self.max_logprobs:
                 self.n_top[j] = n_top
@@ -1054,9 +1172,11 @@ class PagedSlotDecodeEngine(SlotDecodeEngine):
     which move whole pages between them and the device pool between replays (``_PagedKV``)."""
 
     def __init__(self, model: UltravoxModel, slots: int, max_len: int, kv_pages: int, eos_token_ids=None, pad_token_id: int = 0,
-                 use_graph: bool = True, max_logprobs: int = 0, kv_cache_dtype: str = "bf16", kv_scales=None, host_kv_pages: int = 0):
+                 use_graph: bool = True, max_logprobs: int = 0, kv_cache_dtype: str = "bf16", kv_scales=None, host_kv_pages: int = 0,
+                 prompt_lookup_num_tokens: Optional[int] = None):
+        check_lookup_k(int(slots), prompt_lookup_num_tokens)      # before the pool is allocated
         kv = _PagedKV(model, int(slots), max_len, kv_pages, kv_cache_dtype, kv_scales, host_kv_pages)
         self.kv_pages, self.pool_k, self.pool_v, self.kv_scales = kv.kv_pages, kv.pool_k, kv.pool_v, kv.kv_scales
         self.host_kv_pages, self.host_k, self.host_v = kv.host_kv_pages, kv.host_k, kv.host_v
         self.swap_out, self.swap_in = kv.swap_out, kv.swap_in
-        self._setup(model, int(slots), kv, eos_token_ids, pad_token_id, use_graph, max_logprobs)
+        self._setup(model, int(slots), kv, eos_token_ids, pad_token_id, use_graph, max_logprobs, prompt_lookup_num_tokens)

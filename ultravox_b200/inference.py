@@ -244,12 +244,15 @@ class LocalInference(VoiceInference):
 
     @torch.inference_mode()
     def infer_many(self, samples: List[VoiceSample], max_tokens: Optional[int] = None, temperature: Optional[float] = None,
-                   slots: int = 8, max_len: Optional[int] = None) -> List[VoiceOutput]:
+                   slots: int = 8, max_len: Optional[int] = None,
+                   prompt_lookup_num_tokens: Optional[int] = None) -> List[VoiceOutput]:
         """Serves independent samples through ``slots`` continuous-batching slots (``serving.SlotScheduler``): a finished reply
         frees its slot for the next sample at once, instead of a static batch decoding until its longest reply ends.  Same
         data processing, terminators and sampling rule as ``infer``; each result is what ``infer`` gives for that sample alone
         (no conversation mode, like ``infer_batch``).  Results come back in input order.  ``max_len`` is the slot capacity in
-        positions (default: the longest prompt plus ``max_tokens``); a sample that does not fit raises ``ValueError``."""
+        positions (default: the longest prompt plus ``max_tokens``); a sample that does not fit raises ``ValueError``.
+        ``prompt_lookup_num_tokens`` turns on prompt lookup decoding in the slots (``SlotScheduler``): the same replies, in fewer
+        steps where a reply repeats its prompt."""
         assert not self.conversation_mode
         from .serving import SlotScheduler
         feats = [self._dataproc(s) for s in samples]
@@ -259,7 +262,8 @@ class LocalInference(VoiceInference):
         need = max(int(f["input_ids"].shape[1]) for f in feats) + max_new
         if max_len is not None and need > max_len:
             raise ValueError(f"a sample needs {need} positions (prompt + max_tokens); the slots hold {max_len}")
-        sched = SlotScheduler(self.model, slots=slots, max_len=max_len or need, eos_token_ids=self._terminators())
+        sched = SlotScheduler(self.model, slots=slots, max_len=max_len or need, eos_token_ids=self._terminators(),
+                              prompt_lookup_num_tokens=prompt_lookup_num_tokens)
         do_sample = temperature is not None and temperature > 0
         ids = [sched.submit(f, max_new_tokens=max_new, do_sample=do_sample, temperature=temperature if do_sample else None)
                for f in feats]

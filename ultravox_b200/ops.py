@@ -356,22 +356,51 @@ def _pool(k_pool: torch.Tensor, v_pool: torch.Tensor, table: torch.Tensor):
     return n_pages, Hkv, D, table.shape[1], fp8
 
 
+def attention_rows(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, out: torch.Tensor, Hq: int, scale: float,
+                   kv_len: torch.Tensor, kv_row: torch.Tensor) -> torch.Tensor:
+    """Row-mapped decode attention (``uvx_attention_rows``): q [R, Hq * D] (rows of any stride), one cache layer k_cache /
+    v_cache [rows, S_max, Hkv, D] (contiguous), kv_len / kv_row [R] int32 -> out [R, Hq * D].  Row r sees keys [0, kv_len[r]) of
+    cache row kv_row[r]; bit-identical to ``attention`` of that row against that cache row."""
+    _cuda(q, BF16, "q"), _cuda(k_cache, BF16, "k_cache"), _cuda(v_cache, BF16, "v_cache"), _cuda(out, BF16, "out")
+    R = q.shape[0]
+    rows, smax, Hkv, D = k_cache.shape
+    if q.dim() != 2 or q.shape[1] != Hq * D or q.stride(1) != 1 or out.shape != (R, Hq * D) or out.stride(1) != 1:
+        raise ValueError(f"q / out must be [R, {Hq * D}] with unit column stride")
+    if v_cache.shape != k_cache.shape or not k_cache.is_contiguous() or not v_cache.is_contiguous():
+        raise ValueError("k_cache / v_cache must be contiguous [rows, S_max, Hkv, D] of the same shape")
+    _rows(kv_len, torch.int32, R, "kv_len"), _rows(kv_row, torch.int32, R, "kv_row")
+    a = AttnArgs()
+    a.q, a.k, a.v, a.o = q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), out.data_ptr()
+    a.B, a.Hq, a.Hkv, a.Sq, a.Skv, a.D = R, Hq, Hkv, 1, smax, D
+    (a.q_rs, a.q_bs, a.k_rs, a.k_bs, a.v_rs, a.v_bs, a.o_rs, a.o_bs) = (q.stride(0), q.stride(0), Hkv * D, smax * Hkv * D, Hkv * D,
+                                                                        smax * Hkv * D, out.stride(0), out.stride(0))
+    a.kv_len = kv_len.data_ptr()
+    a.kv_start = None
+    a.causal, a.block, a.scale = 0, 0, float(scale)
+    check(lib().uvx_attention_rows(C.byref(a), kv_row.data_ptr(), _stream()), "uvx_attention_rows")
+    return out
+
+
 def attention_paged(q: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor, out: torch.Tensor, Hq: int, scale: float,
-                    table: torch.Tensor, kv_len: torch.Tensor, kv_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
+                    table: torch.Tensor, kv_len: torch.Tensor, kv_scale: Optional[torch.Tensor] = None,
+                    kv_row: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Decode attention through a page table (``uvx_attention_paged``): q [B, Hq * D] (rows of any stride), one pool layer
     k_pool / v_pool [n_pages, 64, Hkv, D], table [>= B, W] int32 (row b: the pages of batch row b's key tiles), kv_len [B] int32
     -> out [B, Hq * D].  Row b sees keys [0, kv_len[b]); bit-identical to ``attention`` on a contiguous cache holding them.
     A float8_e4m3fn pool takes ``kv_scale`` [2] fp32 (the layer's K and V scales) and runs ``uvx_attention_paged_fp8``:
-    bit-identical to the bf16 form on the dequantized pool."""
+    bit-identical to the bf16 form on the dequantized pool.  ``kv_row`` [B] int32 (``uvx_attention_paged_rows`` /
+    ``_fp8_rows``): row b reads table row kv_row[b] instead of b."""
     _cuda(q, BF16, "q"), _cuda(out, BF16, "out")
     n_pages, Hkv, D, W, fp8 = _pool(k_pool, v_pool, table)
     sc = _kv_scale(kv_scale, fp8, (2,), "kv_scale")
     B = q.shape[0]
     if q.dim() != 2 or q.shape[1] != Hq * D or q.stride(1) != 1 or out.shape != (B, Hq * D) or out.stride(1) != 1:
         raise ValueError(f"q / out must be [B, {Hq * D}] with unit column stride")
-    if table.shape[0] < B:
+    if kv_row is None and table.shape[0] < B:
         raise ValueError(f"table has {table.shape[0]} rows for {B} batch rows")
     _rows(kv_len, torch.int32, B, "kv_len")
+    if kv_row is not None:
+        _rows(kv_row, torch.int32, B, "kv_row")
     a = AttnArgs()
     a.q, a.k, a.v, a.o = q.data_ptr(), k_pool.data_ptr(), v_pool.data_ptr(), out.data_ptr()
     a.B, a.Hq, a.Hkv, a.Sq, a.Skv, a.D = B, Hq, Hkv, 1, W * PAGE, D
@@ -380,7 +409,13 @@ def attention_paged(q: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor,
     a.kv_len = kv_len.data_ptr()
     a.kv_start = None
     a.causal, a.block, a.scale = 0, 0, float(scale)
-    if fp8:
+    if kv_row is not None and fp8:
+        check(lib().uvx_attention_paged_fp8_rows(C.byref(a), table.data_ptr(), table.stride(0), sc, kv_row.data_ptr(), _stream()),
+              "uvx_attention_paged_fp8_rows")
+    elif kv_row is not None:
+        check(lib().uvx_attention_paged_rows(C.byref(a), table.data_ptr(), table.stride(0), kv_row.data_ptr(), _stream()),
+              "uvx_attention_paged_rows")
+    elif fp8:
         check(lib().uvx_attention_paged_fp8(C.byref(a), table.data_ptr(), table.stride(0), sc, _stream()), "uvx_attention_paged_fp8")
     else:
         check(lib().uvx_attention_paged(C.byref(a), table.data_ptr(), table.stride(0), _stream()), "uvx_attention_paged")
@@ -1180,6 +1215,129 @@ def lookup_accept(pick: torch.Tensor, tok: torch.Tensor, n_draft: torch.Tensor, 
                                   0 if eos_ids is None else eos_ids.numel(), seq.data_ptr(), cur_len.data_ptr(), n_new.data_ptr(),
                                   int(max_new), _p(step), _p(accepted), 0 if accepted is None else accepted.numel(), done.data_ptr(),
                                   _stream()), "uvx_lookup_accept")
+
+
+# ------------------------------------------------------------------------------------------ prompt lookup in slots
+def lookup_draft_slots(seq: torch.Tensor, token: torch.Tensor, cur_len: torch.Tensor, n_new: torch.Tensor, max_new: torch.Tensor,
+                       k: torch.Tensor, n: torch.Tensor, done: torch.Tensor, active: torch.Tensor, prefilling: torch.Tensor,
+                       pos: torch.Tensor, lens: torch.Tensor, rope_pos: torch.Tensor, K: int, eos_ids: Optional[torch.Tensor],
+                       tok: torch.Tensor, n_draft: torch.Tensor, row_pos: torch.Tensor, row_lens: torch.Tensor, row_rope: torch.Tensor,
+                       pen_len: torch.Tensor, idx: torch.Tensor, row_slot: torch.Tensor, cache_row: torch.Tensor) -> None:
+    """``uvx_lookup_draft_slots`` (include/uvx.h): the drafts of every slot and the R = slots * (K + 1) rows of a lookup step.
+    seq [slots, W] int64, token [slots] int64 and the other per-slot arrays [slots] int32 in; tok [R] int64, n_draft [slots],
+    row_pos / row_lens / row_rope / pen_len / idx / row_slot / cache_row [R] int32 out."""
+    S = cur_len.shape[0]
+    if not 1 <= int(K) <= LOOKUP_MAX_K:
+        raise ValueError(f"K must be in [1, {LOOKUP_MAX_K}], got {K}")
+    R = S * (int(K) + 1)
+    _seq_rows(seq, torch.int64, S, "seq"), _rows(token, torch.int64, S, "token")
+    for t, name in ((cur_len, "cur_len"), (n_new, "n_new"), (max_new, "max_new"), (k, "k"), (n, "n"), (done, "done"),
+                    (active, "active"), (prefilling, "prefilling"), (pos, "pos"), (lens, "lens"), (rope_pos, "rope_pos"),
+                    (n_draft, "n_draft")):
+        _rows(t, torch.int32, S, name)
+    _rows(tok, torch.int64, R, "tok")
+    for t, name in ((row_pos, "row_pos"), (row_lens, "row_lens"), (row_rope, "row_rope"), (pen_len, "pen_len"), (idx, "idx"),
+                    (row_slot, "row_slot"), (cache_row, "cache_row")):
+        _rows(t, torch.int32, R, name)
+    if eos_ids is not None:
+        _cuda(eos_ids, torch.int64, "eos_ids")
+    check(lib().uvx_lookup_draft_slots(seq.data_ptr(), seq.stride(0), token.data_ptr(), cur_len.data_ptr(), n_new.data_ptr(),
+                                       max_new.data_ptr(), k.data_ptr(), n.data_ptr(), done.data_ptr(), active.data_ptr(),
+                                       prefilling.data_ptr(), pos.data_ptr(), lens.data_ptr(), rope_pos.data_ptr(), S, int(K),
+                                       _p(eos_ids), 0 if eos_ids is None else eos_ids.numel(), tok.data_ptr(), n_draft.data_ptr(),
+                                       row_pos.data_ptr(), row_lens.data_ptr(), row_rope.data_ptr(), pen_len.data_ptr(), idx.data_ptr(),
+                                       row_slot.data_ptr(), cache_row.data_ptr(), _stream()), "uvx_lookup_draft_slots")
+
+
+def lookup_accept_slots(pick: torch.Tensor, tok: torch.Tensor, n_draft: torch.Tensor, K: int, eos_ids: Optional[torch.Tensor],
+                        seq: torch.Tensor, token: torch.Tensor, done: torch.Tensor, cur_len: torch.Tensor, n_new: torch.Tensor,
+                        max_new: torch.Tensor, active: torch.Tensor, pos: torch.Tensor, lens: torch.Tensor, rope_pos: torch.Tensor,
+                        accepted: torch.Tensor, n_open: torch.Tensor) -> None:
+    """``uvx_lookup_accept_slots`` (include/uvx.h): picks [R] int64 of the rows that fed tok [R] -> each open slot's agreeing
+    drafts plus one token appended to seq [slots, W] int64 with ``uvx_slot_finish``'s bookkeeping; accepted [slots] += m."""
+    S = cur_len.shape[0]
+    if not 1 <= int(K) <= LOOKUP_MAX_K:
+        raise ValueError(f"K must be in [1, {LOOKUP_MAX_K}], got {K}")
+    R = S * (int(K) + 1)
+    _rows(pick, torch.int64, R, "pick"), _rows(tok, torch.int64, R, "tok")
+    _seq_rows(seq, torch.int64, S, "seq"), _rows(token, torch.int64, S, "token")
+    for t, name in ((n_draft, "n_draft"), (done, "done"), (cur_len, "cur_len"), (n_new, "n_new"), (max_new, "max_new"),
+                    (active, "active"), (pos, "pos"), (lens, "lens"), (rope_pos, "rope_pos"), (accepted, "accepted")):
+        _rows(t, torch.int32, S, name)
+    _rows(n_open, torch.int32, 1, "n_open")
+    if eos_ids is not None:
+        _cuda(eos_ids, torch.int64, "eos_ids")
+    check(lib().uvx_lookup_accept_slots(pick.data_ptr(), tok.data_ptr(), n_draft.data_ptr(), S, int(K), _p(eos_ids),
+                                        0 if eos_ids is None else eos_ids.numel(), seq.data_ptr(), seq.stride(0), token.data_ptr(),
+                                        done.data_ptr(), cur_len.data_ptr(), n_new.data_ptr(), max_new.data_ptr(), active.data_ptr(),
+                                        pos.data_ptr(), lens.data_ptr(), rope_pos.data_ptr(), accepted.data_ptr(), n_open.data_ptr(),
+                                        _stream()), "uvx_lookup_accept_slots")
+
+
+def sample_rows(logits: torch.Tensor, temperature: torch.Tensor, top_k: torch.Tensor, top_p: torch.Tensor, u: torch.Tensor,
+                active: torch.Tensor, row_slot: torch.Tensor, row_idx: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """``uvx_sample_rows``: ``sample_slots`` per row r of logits [R, V] with slot row_slot[r]'s settings (per-slot arrays [slots],
+    u [slots, W]) and its uniform at row_idx[r] -> out [R] int64 (rows with row_idx < 0 or an inactive slot untouched)."""
+    _cuda(logits, torch.float32, "logits")
+    if logits.dim() != 2 or not logits.is_contiguous():
+        raise ValueError("logits must be a contiguous [R, V] tensor")
+    R, V = logits.shape
+    S = temperature.shape[0]
+    _rows(temperature, torch.float32, S, "temperature"), _rows(top_k, torch.int32, S, "top_k"), _rows(top_p, torch.float32, S, "top_p")
+    _rows(active, torch.int32, S, "active"), _seq_rows(u, torch.float32, S, "u")
+    _rows(row_slot, torch.int32, R, "row_slot"), _rows(row_idx, torch.int32, R, "row_idx"), _rows(out, torch.int64, R, "out")
+    check(lib().uvx_sample_rows(logits.data_ptr(), R, V, temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), u.data_ptr(),
+                                u.stride(0), active.data_ptr(), row_slot.data_ptr(), row_idx.data_ptr(), out.data_ptr(), _stream()),
+          "uvx_sample_rows")
+    return out
+
+
+def repetition_penalty_rows_map_(logits: torch.Tensor, seq: torch.Tensor, penalty: torch.Tensor, active: torch.Tensor,
+                                 row_slot: torch.Tensor, row_len: torch.Tensor, row_idx: torch.Tensor,
+                                 scratch: torch.Tensor) -> torch.Tensor:
+    """``uvx_repetition_penalty_rows_map``: HF's repetition penalty on row r of logits [R, V] fp32 with slot s = row_slot[r]'s
+    penalty over seq[s, :row_len[r]] (seq [slots, W] int64), in place; scratch fp32 [R, >= W] sharing seq's row stride."""
+    _cuda(logits, torch.float32, "logits")
+    if logits.dim() != 2 or not logits.is_contiguous():
+        raise ValueError("logits must be a contiguous [R, V] tensor")
+    R, V = logits.shape
+    S = penalty.shape[0]
+    _seq_rows(seq, torch.int64, S, "seq"), _rows(penalty, torch.float32, S, "penalty"), _rows(active, torch.int32, S, "active")
+    for t, name in ((row_slot, "row_slot"), (row_len, "row_len"), (row_idx, "row_idx")):
+        _rows(t, torch.int32, R, name)
+    _seq_rows(scratch, torch.float32, R, "scratch")
+    if scratch.stride(0) != seq.stride(0) or scratch.shape[1] < seq.shape[1]:
+        raise ValueError("scratch and seq must share a row stride")
+    check(lib().uvx_repetition_penalty_rows_map(logits.data_ptr(), R, V, seq.data_ptr(), seq.stride(0), penalty.data_ptr(),
+                                                active.data_ptr(), row_slot.data_ptr(), row_len.data_ptr(), row_idx.data_ptr(),
+                                                scratch.data_ptr(), _stream()), "uvx_repetition_penalty_rows_map")
+    return logits
+
+
+def token_logprobs_rows(logits: torch.Tensor, tok: torch.Tensor, n_top: torch.Tensor, row_slot: torch.Tensor, dst: torch.Tensor,
+                        out_lp: torch.Tensor, out_ids: Optional[torch.Tensor] = None, out_top: Optional[torch.Tensor] = None) -> None:
+    """``uvx_token_logprobs_rows``: ``token_logprobs`` per row r of logits [R, V] with slot s = row_slot[r]'s n_top[s], written to
+    slot s's outputs (out_lp [slots, cap], out_ids / out_top [slots, cap, n_max]) at index dst[r] (< 0: nothing)."""
+    _cuda(logits, torch.float32, "logits")
+    if logits.dim() != 2 or not logits.is_contiguous():
+        raise ValueError("logits must be a contiguous [R, V] tensor")
+    R, V = logits.shape
+    S = n_top.shape[0]
+    _rows(tok, torch.int64, R, "tok"), _rows(n_top, torch.int32, S, "n_top"), _rows(row_slot, torch.int32, R, "row_slot")
+    _rows(dst, torch.int32, R, "dst")
+    _cuda(out_lp, torch.float32, "out_lp")
+    if out_lp.dim() != 2 or out_lp.shape[0] != S or not out_lp.is_contiguous():
+        raise ValueError(f"out_lp must be a contiguous [{S}, cap] tensor, got {tuple(out_lp.shape)}")
+    cap = out_lp.shape[1]
+    n_max = 0
+    if out_ids is not None or out_top is not None:
+        _cuda(out_ids, torch.int64, "out_ids"), _cuda(out_top, torch.float32, "out_top")
+        n_max = out_ids.shape[-1]
+        for t, name in ((out_ids, "out_ids"), (out_top, "out_top")):
+            if t.shape != (S, cap, n_max) or not t.is_contiguous():
+                raise ValueError(f"{name} must be a contiguous [{S}, {cap}, n_max] tensor, got {tuple(t.shape)}")
+    check(lib().uvx_token_logprobs_rows(logits.data_ptr(), R, V, tok.data_ptr(), n_top.data_ptr(), row_slot.data_ptr(), dst.data_ptr(),
+                                        cap, n_max, out_lp.data_ptr(), _p(out_ids), _p(out_top), _stream()), "uvx_token_logprobs_rows")
 
 
 # ------------------------------------------------------------------------------------------ beam search

@@ -27,7 +27,9 @@ from typing import Callable, Deque, Dict, List, Optional, Sequence, Tuple
 
 import torch
 
-from .engine import PREFILL_ROWS, PagedSlotDecodeEngine, SlotDecodeEngine, TokenLogprobs, check_kv_scales
+from . import ops
+from .engine import (PREFILL_ROWS, PagedSlotDecodeEngine, SlotDecodeEngine, TokenLogprobs, check_kv_scales,
+                     check_lookup_k)
 
 PAGE = 64       # positions per KV page (ops.PAGE)
 
@@ -286,6 +288,7 @@ class _Request:
     admitted_at: int = -1
     first_token: Optional[torch.cuda.Event] = None
     logprobs: Optional[int] = None     # alternatives per token asked for (None: no log-probs)
+    lookup: Optional[tuple] = None     # (k, n) of prompt lookup (None: the engine has none)
 
 
 class SlotScheduler:
@@ -335,11 +338,21 @@ class SlotScheduler:
     session out on request, ``session_on_host(sid)`` tells where it is, ``host_free_pages`` counts the free host pages and
     ``swapped_out_pages`` / ``swapped_in_pages`` the pages moved so far.  Each move is one ``uvx_kv_pages_move`` launch on the
     scheduler's stream (the SMs read or write the host pages over PCIe) between decode steps; it pauses the other slots for
-    its duration, as an admission's prefill does.  Running requests are never swapped."""
+    its duration, as an admission's prefill does.  Running requests are never swapped.
+
+    ``prompt_lookup_num_tokens`` = K (None, the default: off): prompt lookup decoding inside the slot step, up to K drafted
+    tokens per slot per step (1 <= K <= 31 and slots * (K + 1) <= 256 rows, else ValueError).  ``submit(...,
+    prompt_lookup_num_tokens=k, max_matching_ngram_size=n)`` sets a request's k (None: K, 0: no drafts) and n (None: 2), with
+    ``generate()``'s meanings.  A request's tokens, log-probs and kept K / V are those plain slot decoding gives it; a step
+    yields 1 to k + 1 of them.  Drafts are taken from the request's own prompt and reply (the leftmost earlier match of its
+    last n-gram, sizes n down to 1), so they pay off where a reply repeats its input.  ``accepted_drafts[id]`` is the number
+    of drafted tokens the request accepted, filled when it finishes.  While a chunked prompt is in flight every slot decodes
+    one token per step; the lookup step's linears run at slots * (K + 1) rows (DESIGN.md §6 has their cost)."""
 
     def __init__(self, model, slots: int = 8, max_len: int = 2048, eos_token_ids=None, pad_token_id: Optional[int] = None,
                  sync_every: int = 8, use_graph: bool = True, kv_pages: Optional[int] = None, prefix_cache: bool = False,
-                 max_logprobs: int = 0, kv_cache_dtype: str = "bf16", kv_scales=None, host_kv_pages: int = 0):
+                 max_logprobs: int = 0, kv_cache_dtype: str = "bf16", kv_scales=None, host_kv_pages: int = 0,
+                 prompt_lookup_num_tokens: Optional[int] = None):
         eos = sorted(set([eos_token_ids] if isinstance(eos_token_ids, int) else (eos_token_ids or [])))
         pad = pad_token_id if pad_token_id is not None else (min(eos) if eos else 0)     # generate()'s default
         if int(sync_every) < 1:
@@ -366,6 +379,10 @@ class SlotScheduler:
         self.model = model
         self.pool: Optional[PagePool] = None
         lp = {} if max_logprobs == 0 else dict(max_logprobs=max_logprobs)     # the engine validates it
+        self.lookup_k = check_lookup_k(int(slots), prompt_lookup_num_tokens)     # 0: off
+        if self.lookup_k:
+            lp["prompt_lookup_num_tokens"] = self.lookup_k
+        self.accepted_drafts: Dict[int, int] = {}
         if host_kv_pages:
             kv["host_kv_pages"] = int(host_kv_pages)
         if kv_pages is None:
@@ -455,7 +472,8 @@ class SlotScheduler:
     def submit(self, features: dict, max_new_tokens: int = 20, do_sample: bool = False, temperature: Optional[float] = None,
                top_k: Optional[int] = None, top_p: Optional[float] = None, repetition_penalty: float = 1.0,
                generator: Optional[torch.Generator] = None, num_beams: int = 1, session: Optional[int] = None,
-               logprobs: Optional[int] = None) -> int:
+               logprobs: Optional[int] = None, prompt_lookup_num_tokens: Optional[int] = None,
+               max_matching_ngram_size: Optional[int] = None) -> int:
         """Queues one request: ``features`` is the processor's output for it (``input_ids`` [1, S] and, for audio, its mel or
         waveform fields).  Arguments and defaults are ``generate()``'s: greedy unless ``do_sample``; sampling defaults to
         temperature 1 and top_k 50; ``top_p`` must lie in [0, 1].  A sampled request draws its uniforms here, as ``generate()``
@@ -466,9 +484,13 @@ class SlotScheduler:
         session may be in flight.  With a paged engine, a request that needs more pages than the pool has raises ValueError.
 
         ``logprobs``: None records nothing; 0 the log-prob of each chosen token; 1..``max_logprobs`` also that many most likely
-        alternatives per token (``logprobs[id]`` once it has finished).  Anything else raises ValueError."""
+        alternatives per token (``logprobs[id]`` once it has finished).  Anything else raises ValueError.
+
+        ``prompt_lookup_num_tokens`` / ``max_matching_ngram_size`` (a scheduler built with ``prompt_lookup_num_tokens``): the
+        request's drafts per step, None for the scheduler's K, 0 for none, at most K; its n-gram size, None for 2."""
         if logprobs is not None:
             self.engine.check_logprobs(logprobs)
+        lookup = self._check_lookup(prompt_lookup_num_tokens, max_matching_ngram_size)
         if num_beams != 1:
             raise NotImplementedError("beam search is not built into the slot engine; use generate(num_beams=...)")
         if top_p is not None and not 0.0 <= float(top_p) <= 1.0:       # NaN fails too
@@ -512,10 +534,28 @@ class SlotScheduler:
         rid = self._next_id
         self._next_id += 1
         self._queue.append(_Request(rid, ids, feats, n, temp, k_top, p_top, float(repetition_penalty or 1.0), u, session,
-                                    prefix, logprobs=None if logprobs is None else int(logprobs)))
+                                    prefix, logprobs=None if logprobs is None else int(logprobs), lookup=lookup))
         if sess is not None:
             sess.busy = True
         return rid
+
+    def _check_lookup(self, k, n) -> Optional[tuple]:
+        """A request's (k, n) of prompt lookup (None when the engine has none), with ``generate()``'s checks."""
+        K = self.lookup_k
+        if not K:
+            if k is not None or n is not None:
+                raise ValueError("prompt lookup is set per scheduler: SlotScheduler(..., prompt_lookup_num_tokens=K)")
+            return None
+        k = K if k is None else k
+        if isinstance(k, bool) or not isinstance(k, int) or not 0 <= k <= ops.LOOKUP_MAX_K:
+            raise ValueError(f"prompt_lookup_num_tokens must be an integer in [1, {ops.LOOKUP_MAX_K}] (k + 1 rows of the decode "
+                             f"step), or 0 for no drafts, got {k!r}")
+        if k > K:
+            raise ValueError(f"prompt_lookup_num_tokens = {k} exceeds the scheduler's prompt_lookup_num_tokens = {K}")
+        n = 2 if n is None else n
+        if isinstance(n, bool) or not isinstance(n, int) or n < 1:
+            raise ValueError(f"max_matching_ngram_size must be an integer >= 1, got {n!r}")
+        return k, n
 
     def _admit(self) -> None:
         eng = self.engine
@@ -557,6 +597,8 @@ class SlotScheduler:
             feats = {k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in r.features.items()}
             if r.logprobs is not None:
                 kw["logprobs"] = r.logprobs
+            if r.lookup is not None:
+                kw["lookup"] = r.lookup
             eng.admit(j, r.input_ids, r.max_new, r.temperature, r.top_k, r.top_p, r.penalty, r.u, **kw, **feats)
             r.features, r.u = {}, None
             if long:
@@ -582,12 +624,14 @@ class SlotScheduler:
         eng = self.engine
         if int(eng.n_open) >= len(self._running) and not any(self._budget_spent(r) for r in self._running.values()):
             return 0                    # n_open counts the slots still open after the last step: nothing finished
-        state = torch.stack([eng.done, eng.cur_len]).cpu()
+        state = torch.stack([eng.done, eng.cur_len] + ([eng.accepted] if self.lookup_k else [])).cpu()
         freed = 0
         for j in sorted(self._running):
             if not int(state[0, j]):
                 continue
             r = self._running.pop(j)
+            if self.lookup_k:
+                self.accepted_drafts[r.rid] = int(state[2, j])
             if r.logprobs is not None:
                 self.logprobs[r.rid] = eng.token_logprobs_of(j, int(state[1, j]) - int(r.input_ids.shape[1]), r.logprobs)
             seq = eng.retire(j, int(state[1, j]))
