@@ -506,6 +506,44 @@ int uvx_token_logprobs_rows(const float* logits, int64_t R, int64_t V, const int
                             const int32_t* row_slot, const int32_t* dst, int64_t cap, int32_t n_max, float* out_lp, int64_t* out_ids,
                             float* out_top, uvx_stream_t stream);
 
+/* Token constraints (hf:generation/logits_process.py SequenceBias -> NoRepeatNGram -> NoBadWords -> MinLength / MinNewTokens
+ * -> SuppressTokens -> SuppressTokensAtBegin, transformers 5.5), one launch in place on fp32 logits rows, run BEFORE the
+ * repetition penalty: every processor but the sequence bias adds or sets -inf, which the penalty maps to itself (NaN and +inf
+ * too), so the result equals HF's up to the sign of zero (HF adds its all-row bias tensor, +0 where no entry matches, to every
+ * column, which turns a -0.0 score into +0.0; here only the tokens with entries are written).  A setting is cfg int32[4] = (n, min_len, begin_len, n_ent) plus a packed table of n_ent
+ * entries: entry j is the ids ids[end[j - 1] .. end[j]) (end[-1] = 0, at least one id), int64 ids, int32 end, fp32 bias[j] and
+ * int32 kind[j] (UVX_CK_*).  Its last id is its target token t; the others are the prefix that the last ids of the sequence
+ * must equal for the entry to match (an entry longer than L never matches).  All entries of one t are consecutive, in HF's
+ * order: sequence-bias entries (the single-token one first, then dict order), bad words, sets.  Per row with sequence seq[0:L]:
+ *   x[t] = ((x[t] + sum of matching UVX_CK_BIAS) + sum of matching UVX_CK_BAD), each sum in fp32 from 0 and added only when t
+ *          has entries of that kind; then x[t] = -inf if a matching entry is UVX_CK_SUPPRESS, UVX_CK_BEGIN with L == begin_len,
+ *          or UVX_CK_MIN_LEN with L < min_len;
+ *   then (n >= 1 and L + 1 >= n) x[seq[e]] = -inf for every e in [n - 1, L) with seq[e - n + 1 .. e - 1] == seq[L - n + 1 .. L - 1].
+ * seq is never read at or past L.  Every form runs 1024 threads per row.
+ * uvx_logits_constraints           B rows, row b over seq[b * seq_stride, 0:cur_len[0]], one setting.
+ * uvx_logits_constraints_slots     active rows b over seq[b, 0:cur_len[b]] with setting b (cfg + 4 b, table at b * tab_stride).
+ * uvx_logits_constraints_rows      row b over seq[b * seq_stride, 0:len[b]] (seq_stride 0: one shared sequence), one setting.
+ * uvx_logits_constraints_rows_map  row r of slot s = row_slot[r] (active[s], row_idx[r] >= 0; others untouched) over
+ *                                  seq[s, 0:row_len[r]] with setting s.                                                          */
+#define UVX_CK_BIAS 0      /* sequence_bias: add */
+#define UVX_CK_BAD 1       /* bad_words_ids: add (bias -inf) */
+#define UVX_CK_SUPPRESS 2  /* suppress_tokens: set -inf */
+#define UVX_CK_BEGIN 3     /* begin_suppress_tokens: set -inf when L == begin_len */
+#define UVX_CK_MIN_LEN 4   /* EOS under min_length / min_new_tokens: set -inf when L < min_len */
+int uvx_logits_constraints(float* logits, int64_t B, int64_t V, const int64_t* seq, int64_t seq_stride, const int32_t* cur_len,
+                           const int32_t* cfg, const int64_t* ids, const int32_t* end, const float* bias, const int32_t* kind,
+                           uvx_stream_t stream);
+int uvx_logits_constraints_slots(float* logits, int64_t B, int64_t V, const int64_t* seq, int64_t seq_stride, const int32_t* cur_len,
+                                 const int32_t* active, const int32_t* cfg, const int64_t* ids, const int32_t* end, const float* bias,
+                                 const int32_t* kind, int64_t tab_stride, uvx_stream_t stream);
+int uvx_logits_constraints_rows(float* logits, int64_t R, int64_t V, const int64_t* seq, int64_t seq_stride, const int32_t* len,
+                                const int32_t* cfg, const int64_t* ids, const int32_t* end, const float* bias, const int32_t* kind,
+                                uvx_stream_t stream);
+int uvx_logits_constraints_rows_map(float* logits, int64_t R, int64_t V, const int64_t* seq, int64_t seq_stride,
+                                    const int32_t* active, const int32_t* row_slot, const int32_t* row_len, const int32_t* row_idx,
+                                    const int32_t* cfg, const int64_t* ids, const int32_t* end, const float* bias, const int32_t* kind,
+                                    int64_t tab_stride, uvx_stream_t stream);
+
 /* Beam search (hf:generation/utils.py _beam_search, transformers 5.5, and the helpers above it), one decode step as four
  * launches that read every per-step scalar from device memory.  B prompts, nb <= 8 beams each: row r = b * nb + j.
  * uvx_log_softmax   out[r] = log_softmax(in[r]) in fp32 (in == out allowed).  Beam search scores log-probs; the repetition

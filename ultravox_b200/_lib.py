@@ -117,6 +117,12 @@ SIGNATURES = {
     "uvx_sample_rows": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "uvx_repetition_penalty_rows_map": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "uvx_token_logprobs_rows": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp]),
+    "uvx_logits_constraints": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "uvx_logits_constraints_slots": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64,
+                                               c_vp]),
+    "uvx_logits_constraints_rows": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "uvx_logits_constraints_rows_map": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                                  c_vp, c_i64, c_vp]),
     "uvx_attention_rows": (C.c_int, [C.POINTER(AttnArgs), c_vp, c_vp]),
     "uvx_attention_paged_rows": (C.c_int, [C.POINTER(AttnArgs), c_vp, c_i64, c_vp, c_vp]),
     "uvx_attention_paged_fp8_rows": (C.c_int, [C.POINTER(AttnArgs), c_vp, c_i64, c_vp, c_vp, c_vp]),

@@ -9,6 +9,8 @@
 //   uvx_sample_slots        continuous batching: per-row greedy / sampled pick with each row's own settings and uniform
 //   uvx_repetition_penalty_slots   the repetition penalty with each row's own penalty and length
 //   uvx_repetition_penalty_rows    the repetition penalty with each row's own length and scratch (rows may share a sequence)
+//   uvx_logits_constraints  sequence bias, n-gram ban, bad words, min length, suppression (hf:generation/logits_process.py),
+//                           before the penalty; _slots / _rows / _rows_map with the penalty's per-row forms
 //   uvx_lookup_draft        prompt lookup: n-gram search over the sequence, the k + 1 fed tokens and their positions
 //   uvx_lookup_accept       prompt lookup: the picks that agree with the drafts, appended; counters, budget / EOS, the log
 //   uvx_slot_finish         per-row append / budget / EOS bookkeeping; finished and idle rows stay frozen
@@ -421,6 +423,66 @@ __global__ void __launch_bounds__(1024) rep_penalty_rows_kernel(float* logits, i
   pdl_wait();
   const int64_t b = blockIdx.x;
   penalty_row(logits + b * V, V, seq + b * seq_stride, scratch + b * scratch_stride, len[b], penalty);
+}
+
+// Token constraints of one row (the caller's CTA) with sequence sq[0:L] and one setting: cfg = (no_repeat_ngram_size n, min
+// length, begin length, entry count) and the packed table (include/uvx.h: entry j is ids[end[j - 1] .. end[j]), its last id the
+// target token; a token's entries are consecutive, in HF's order).  Phase 1: one thread per token group adds its matching
+// sequence-bias entries (one fp32 sum), then its matching bad-word entries (a second sum), then applies the sets.  Phase 2 (after
+// a barrier, so no logit is written by both phases at once): the n-gram bans, threads striding over the end positions e.
+__device__ __forceinline__ void constrain_row(float* row, int64_t V, const int64_t* sq, int L, const int32_t* cfg,
+                                              const int64_t* ids, const int32_t* end, const float* bias, const int32_t* kind) {
+  const int n = cfg[0], min_len = cfg[1], begin_len = cfg[2], n_ent = cfg[3];
+  for (int e = threadIdx.x; e < n_ent; e += blockDim.x) {
+    const int64_t t = ids[end[e] - 1];
+    if ((e > 0 && ids[end[e - 1] - 1] == t) || t < 0 || t >= V) continue;     // not its group's head
+    float sb = 0.f, bw = 0.f;
+    bool has_sb = false, has_bw = false, set = false;
+    for (int j = e; j < n_ent; ++j) {
+      const int lo = j ? end[j - 1] : 0, hi = end[j];
+      if (ids[hi - 1] != t) break;
+      const int k = kind[j], len = hi - lo;
+      has_sb |= k == UVX_CK_BIAS;
+      has_bw |= k == UVX_CK_BAD;
+      if (len > L) continue;                  // longer than the sequence: skipped, as HF does
+      bool match = true;
+      for (int i = len - 2; i >= 0 && match; --i) match = sq[L - len + 1 + i] == ids[lo + i];
+      if (!match) continue;
+      if (k == UVX_CK_BIAS) sb += bias[j];
+      else if (k == UVX_CK_BAD) bw += bias[j];
+      else set |= k == UVX_CK_SUPPRESS || (k == UVX_CK_BEGIN && L == begin_len) || (k == UVX_CK_MIN_LEN && L < min_len);
+    }
+    float x = row[t];
+    if (has_sb) x = x + sb;
+    if (has_bw) x = x + bw;
+    row[t] = set ? -INFINITY : x;
+  }
+  if (n < 1 || L + 1 < n) return;             // HF bans nothing while cur_len + 1 < n
+  __syncthreads();
+  for (int e = n - 1 + threadIdx.x; e < L; e += blockDim.x) {
+    bool match = true;
+    for (int i = 1; i < n && match; ++i) match = sq[e - i] == sq[L - i];
+    const int64_t t = sq[e];
+    if (match && t >= 0 && t < V) row[t] = -INFINITY;
+  }
+}
+
+// One CTA per row b.  Slot s = row_slot ? row_slot[b] : b reads seq + s * seq_stride; its length is len[b * len_stride]; setting
+// c = per_slot ? s : 0 (cfg + 4 c, the table at c * tab_stride).  Rows of an inactive slot (active given) or with row_idx[b] < 0
+// (row_idx given) are skipped.  uvx_logits_constraints / _slots / _rows / _rows_map are the four argument patterns.
+__global__ void __launch_bounds__(1024) logits_constraints_kernel(float* logits, int64_t V, const int64_t* seq, int64_t seq_stride,
+                                                                  const int32_t* len, int64_t len_stride, const int32_t* active,
+                                                                  const int32_t* row_slot, const int32_t* row_idx, const int32_t* cfg,
+                                                                  int per_slot, const int64_t* ids, const int32_t* end,
+                                                                  const float* bias, const int32_t* kind, int64_t tab_stride) {
+  pdl_trigger();
+  pdl_wait();
+  const int64_t b = blockIdx.x;
+  const int64_t s = row_slot ? row_slot[b] : b;
+  if ((active && !active[s]) || (row_idx && row_idx[b] < 0)) return;
+  const int64_t c = per_slot ? s : 0;
+  const int64_t o = c * tab_stride;
+  constrain_row(logits + b * V, V, seq + s * seq_stride, len[b * len_stride], cfg + 4 * c, ids + o, end + o, bias + o, kind + o);
 }
 
 // One CTA: for each active, unfinished row append tok at seq[b, cur_len[b]], advance cur_len / n_new, finish on an EOS id or
@@ -1464,6 +1526,56 @@ extern "C" int uvx_repetition_penalty_rows_map(float* logits, int64_t R, int64_t
   launch_k(rep_penalty_slots_kernel, dim3((unsigned)R), dim3(1024), 0, (cudaStream_t)stream, logits, V, seq, seq_stride,
            (const int32_t*)nullptr, penalty, active, scratch, row_slot, row_len, row_idx);
   return check_launch("rep_penalty_slots_kernel (rows)");
+}
+
+extern "C" int uvx_logits_constraints(float* logits, int64_t B, int64_t V, const int64_t* seq, int64_t seq_stride,
+                                      const int32_t* cur_len, const int32_t* cfg, const int64_t* ids, const int32_t* end,
+                                      const float* bias, const int32_t* kind, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(logits && seq && cur_len && cfg && ids && end && bias && kind &&B >= 1 && B < 65536 && V >= 1 && seq_stride >= 0,
+              "uvx_logits_constraints: bad arguments");
+  launch_k(logits_constraints_kernel, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, seq, seq_stride, cur_len,
+           (int64_t)0, (const int32_t*)nullptr, (const int32_t*)nullptr, (const int32_t*)nullptr, cfg, 0, ids, end, bias, kind,
+           (int64_t)0);
+  return check_launch("logits_constraints_kernel");
+}
+
+extern "C" int uvx_logits_constraints_slots(float* logits, int64_t B, int64_t V, const int64_t* seq, int64_t seq_stride,
+                                            const int32_t* cur_len, const int32_t* active, const int32_t* cfg, const int64_t* ids,
+                                            const int32_t* end, const float* bias, const int32_t* kind, int64_t tab_stride,
+                                            uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(logits && seq && cur_len && active && cfg && ids && end && bias && kind &&B >= 1 && B < 65536 && V >= 1 &&
+                  seq_stride >= 1 && tab_stride >= 1,
+              "uvx_logits_constraints_slots: bad arguments");
+  launch_k(logits_constraints_kernel, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, seq, seq_stride, cur_len,
+           (int64_t)1, active, (const int32_t*)nullptr, (const int32_t*)nullptr, cfg, 1, ids, end, bias, kind, tab_stride);
+  return check_launch("logits_constraints_kernel (slots)");
+}
+
+extern "C" int uvx_logits_constraints_rows(float* logits, int64_t R, int64_t V, const int64_t* seq, int64_t seq_stride,
+                                           const int32_t* len, const int32_t* cfg, const int64_t* ids, const int32_t* end,
+                                           const float* bias, const int32_t* kind, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(logits && seq && len && cfg && ids && end && bias && kind &&R >= 1 && R < 65536 && V >= 1 && seq_stride >= 0,
+              "uvx_logits_constraints_rows: bad arguments");
+  launch_k(logits_constraints_kernel, dim3((unsigned)R), dim3(1024), 0, (cudaStream_t)stream, logits, V, seq, seq_stride, len,
+           (int64_t)1, (const int32_t*)nullptr, (const int32_t*)nullptr, (const int32_t*)nullptr, cfg, 0, ids, end, bias, kind,
+           (int64_t)0);
+  return check_launch("logits_constraints_kernel (rows)");
+}
+
+extern "C" int uvx_logits_constraints_rows_map(float* logits, int64_t R, int64_t V, const int64_t* seq, int64_t seq_stride,
+                                               const int32_t* active, const int32_t* row_slot, const int32_t* row_len,
+                                               const int32_t* row_idx, const int32_t* cfg, const int64_t* ids, const int32_t* end,
+                                               const float* bias, const int32_t* kind, int64_t tab_stride, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(logits && seq && active && row_slot && row_len && row_idx && cfg && ids && end && bias && kind &&R >= 1 && R < 65536 &&
+                  V >= 1 && seq_stride >= 1 && tab_stride >= 1,
+              "uvx_logits_constraints_rows_map: bad arguments");
+  launch_k(logits_constraints_kernel, dim3((unsigned)R), dim3(1024), 0, (cudaStream_t)stream, logits, V, seq, seq_stride, row_len,
+           (int64_t)1, active, row_slot, row_idx, cfg, 1, ids, end, bias, kind, tab_stride);
+  return check_launch("logits_constraints_kernel (rows_map)");
 }
 
 extern "C" int uvx_slot_finish(const int64_t* tok, int32_t* done, const int64_t* eos_ids, int32_t n_eos, int64_t* seq,

@@ -202,6 +202,15 @@ def check_lookup_k(slots: int, k) -> int:
     return int(k)
 
 
+def check_constraint_tokens(n) -> Optional[int]:
+    """The slot engines' ``max_constraint_tokens`` (None: off); ValueError unless None or an integer >= 0."""
+    if n is None:
+        return None
+    if isinstance(n, bool) or not isinstance(n, numbers.Integral) or n < 0:
+        raise ValueError(f"max_constraint_tokens must be None or an integer >= 0, got {n!r}")
+    return int(n)
+
+
 class _PagedKV:
     """The KV cache as a shared pool of 64-position pages, so a request's K / V can outlive its slot.  K and V are
     ``[L, kv_pages + slots, 64, Hkv, D]``: the ``kv_pages`` shareable pages, then one private idle page per slot (an idle row
@@ -476,12 +485,16 @@ class DecodeEngine(_Decoder):
     def __init__(self, model: UltravoxModel, batch: int, max_len: int, use_graph: bool = True, cache=None,
                  eos_token_ids=None, pad_token_id: int = 0, temperature: float = 0.0, top_k: int = 0,
                  repetition_penalty: float = 1.0, generator: Optional[torch.Generator] = None, top_p: Optional[float] = None,
-                 output_scores: bool = False, output_logits: bool = False, max_new_tokens: Optional[int] = None):
+                 output_scores: bool = False, output_logits: bool = False, max_new_tokens: Optional[int] = None,
+                 constraints=None):
         """``output_scores`` / ``output_logits``: every pick (the first one, in ``begin``, is step 0) also records HF's processed
         scores / the raw logits of its rows into ``scores`` / ``raw_logits`` [max_new_tokens, batch, V] fp32, at the device
         step counter (``uvx_record_scores``).  That is one [batch, V] fp32 tensor per generated token, which is what HF's
         ``generate(output_scores=True / output_logits=True)`` holds too.  Without them nothing is allocated and the step is
-        unchanged."""
+        unchanged.
+
+        ``constraints`` (``constraints.LogitsConstraints``): every pick first runs ``uvx_logits_constraints`` over the rows'
+        sequences, before the repetition penalty.  None (the default): nothing is allocated and the step is unchanged."""
         super().__init__(model, batch, _RowKV(cache if cache is not None else model.new_cache(batch, max_len)), eos_token_ids,
                          pad_token_id, use_graph)
         dev = model.device
@@ -506,6 +519,7 @@ class DecodeEngine(_Decoder):
             shape = (steps, batch, model.language_model.lm_head.weight.shape[0])
             self.scores = torch.empty(shape, dtype=torch.float32, device=dev) if output_scores else None
             self.raw_logits = torch.empty(shape, dtype=torch.float32, device=dev) if output_logits else None
+        self.constraints = None if constraints is None else constraints.device_tables(dev)
 
     # -- state ---------------------------------------------------------------------------------------------
     def begin(self, input_ids: torch.Tensor, first_logits: torch.Tensor, kv_start: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -538,9 +552,11 @@ class DecodeEngine(_Decoder):
         """logits [B, V] fp32 -> self.token (+ sequence / EOS / counter bookkeeping), all on the device."""
         self.logits = logits
         rec = (self.temperature, self.top_k, self.top_p, self.step_idx)
-        raw_first = self.raw_logits is not None and self.penalty != 1.0
-        if raw_first:       # the penalty rewrites the logits in place: take the raw copy before it
+        raw_first = self.raw_logits is not None and (self.penalty != 1.0 or self.constraints is not None)
+        if raw_first:       # the constraints and the penalty rewrite the logits in place: take the raw copy before them
             ops.record_scores(logits, *rec, raw=self.raw_logits)
+        if self.constraints is not None:
+            ops.logits_constraints_(logits, self.seq, self.cur_len, self.constraints)
         if self.penalty != 1.0:
             ops.repetition_penalty_(logits, self.seq, self.cur_len, self.penalty, self.scratch)
         if self.scores is not None or (self.raw_logits is not None and not raw_first):
@@ -594,9 +610,10 @@ class LookupDecodeEngine(_Decoder):
                  use_graph: bool = True, cache=None, eos_token_ids=None, pad_token_id: int = 0, temperature: float = 0.0,
                  top_k: int = 0, top_p: Optional[float] = None, repetition_penalty: float = 1.0,
                  generator: Optional[torch.Generator] = None, output_scores: bool = False, output_logits: bool = False,
-                 uniforms: Optional[int] = None):
+                 uniforms: Optional[int] = None, constraints=None):
         """``uniforms``: how many uniforms to draw when sampling, default S + max_new_tokens + 1 - the count ``DecodeEngine``
-        draws (its cache capacity + 1) for the same call, so that a seeded ``generator`` gives the same tokens."""
+        draws (its cache capacity + 1) for the same call, so that a seeded ``generator`` gives the same tokens.
+        ``constraints``: as ``DecodeEngine``'s, row i over the sequence up to its position (``uvx_logits_constraints_rows``)."""
         k, n, S, N = int(num_tokens), int(ngram), int(prompt_len), int(max_new_tokens)
         if not 1 <= k <= ops.LOOKUP_MAX_K:
             raise ValueError(f"prompt_lookup_num_tokens must be in [1, {ops.LOOKUP_MAX_K}], got {num_tokens}")
@@ -638,6 +655,7 @@ class LookupDecodeEngine(_Decoder):
         V = model.language_model.lm_head.weight.shape[0]
         self.scores = torch.empty(N, 1, V, dtype=torch.float32, device=dev) if output_scores else None
         self.raw_logits = torch.empty(N, 1, V, dtype=torch.float32, device=dev) if output_logits else None
+        self.constraints = None if constraints is None else constraints.device_tables(dev)
 
     def begin(self, input_ids: torch.Tensor, first_logits: torch.Tensor) -> None:
         """After the prompt input_ids [1, S] has been prefilled into the cache: seeds the sequence and the counters and picks the
@@ -660,9 +678,11 @@ class LookupDecodeEngine(_Decoder):
         rec = (self.temperature, self.top_k, self.top_p, idx)
         scores = None if self.scores is None else self.scores.view(self.max_new, -1)
         raw = None if self.raw_logits is None else self.raw_logits.view(self.max_new, -1)
-        raw_first = raw is not None and self.penalty != 1.0
-        if raw_first:       # the penalty rewrites the logits in place: take the raw copy before it
+        raw_first = raw is not None and (self.penalty != 1.0 or self.constraints is not None)
+        if raw_first:       # the constraints and the penalty rewrite the logits in place: take the raw copy before them
             ops.record_scores_rows(logits, *rec, raw=raw)
+        if self.constraints is not None:
+            ops.logits_constraints_rows_(logits, self.seq.view(1, -1).expand(R, -1), self.pen_len[:R], self.constraints)
         if self.penalty != 1.0:
             ops.repetition_penalty_rows_(logits, self.seq.view(1, -1).expand(R, -1), self.pen_len[:R], self.penalty,
                                          self.scratch[:R])
@@ -689,14 +709,16 @@ class LookupDecodeEngine(_Decoder):
 class BeamDecodeEngine(DecodeEngine):
     """Beam search over ``batch`` prompts with ``num_beams`` beams each (row b * num_beams + j), as
     hf:generation/utils.py ``_beam_search``: the forward of ``DecodeEngine._step`` runs unchanged over the batch * num_beams
-    rows, and the pick becomes log_softmax -> repetition penalty on the log-probs -> top-K continuations per prompt ->
-    running beams / finished pool / early-stop heuristic -> KV cache rows gathered by parent beam, all on the device, so a
+    rows, and the pick becomes log_softmax -> token constraints (if any) -> repetition penalty on the log-probs -> top-K
+    continuations per prompt -> running beams / finished pool / early-stop heuristic -> KV cache rows gathered by parent beam,
+    all on the device, so a
     step is still one CUDA graph replay.  ``all_done`` is HF's loop condition (negated); ``logprobs`` holds the last step's
     processed log-probs [batch * num_beams, V] and ``logits`` the raw ones.  The cache must have batch * num_beams rows with
     each prompt prefilled into row b * num_beams (``begin`` broadcasts it to the other beams)."""
 
     def __init__(self, model: UltravoxModel, batch: int, num_beams: int, max_len: int, max_new_tokens: int, use_graph: bool = True,
-                 cache=None, eos_token_ids=None, length_penalty: float = 1.0, early_stopping=False, repetition_penalty: float = 1.0):
+                 cache=None, eos_token_ids=None, length_penalty: float = 1.0, early_stopping=False, repetition_penalty: float = 1.0,
+                 constraints=None):
         nb = int(num_beams)
         if not 1 <= nb <= ops.BEAM_MAX:
             raise ValueError(f"num_beams must be in [1, {ops.BEAM_MAX}], got {num_beams}")
@@ -704,7 +726,7 @@ class BeamDecodeEngine(DecodeEngine):
             raise ValueError(f"early_stopping must be True, False or 'never', got {early_stopping!r}")
         eos_list = [eos_token_ids] if isinstance(eos_token_ids, int) else list(eos_token_ids or [])
         super().__init__(model, batch * nb, max_len, use_graph=use_graph, cache=cache, eos_token_ids=eos_list,
-                         repetition_penalty=repetition_penalty)
+                         repetition_penalty=repetition_penalty, constraints=constraints)
         dev = model.device
         R = batch * nb
         self.prompts, self.nb = batch, nb
@@ -777,6 +799,8 @@ class BeamDecodeEngine(DecodeEngine):
         """logits [batch * nb, V] fp32 -> the next running beams in ``token`` / ``seq``, the pool, the cache rows reordered."""
         self.logits = logits
         lp = ops.log_softmax(logits, out=self.logprobs)
+        if self.constraints is not None:        # HF applies the processors to each running beam's log-probs
+            ops.logits_constraints_(lp, self.seq, self.cur_len, self.constraints)
         if self.penalty != 1.0:
             ops.repetition_penalty_(lp, self.seq, self.cur_len, self.penalty, self.scratch)
         s, i = ops.beam_select(lp, self.run_score, self.nb, self.K, scratch=self.row_buf, out=self.cand)
@@ -845,19 +869,29 @@ class SlotDecodeEngine(_Decoder):
     ``uvx_lookup_accept_slots`` appends the accepted tokens and leaves every counter as ``uvx_slot_finish`` would.  So the
     plain and the mixed step can follow any lookup step.  ``accepted`` [slots] int32 counts each request's accepted drafts.
     The linears of a lookup step run at R rows: a request's bits are those of a plain engine of R slots (the decode-form GEMM
-    keeps rows independent at a fixed row count).  None (the default) allocates and captures nothing."""
+    keeps rows independent at a fixed row count).  None (the default) allocates and captures nothing.
+
+    ``max_constraint_tokens`` = N (None, the default: off) adds the token constraints of ``generate()``
+    (``constraints.LogitsConstraints``) per slot: settings ``ck_cfg`` [slots, 4] and a table of N ids per slot (``ck_ids``,
+    ``ck_end``, ``ck_bias``, ``ck_kind`` [slots, max(N, 1)]), written by ``admit(..., constraints=...)`` between replays and
+    cleared when the slot goes idle.  Every pick (the plain, mixed and lookup steps' and the admission pick) then runs
+    ``uvx_logits_constraints_slots`` (``_rows_map`` in the lookup step) after the raw copy for log-probs and before the penalty.
+    None allocates nothing and launches nothing: the steps are unchanged."""
 
     def __init__(self, model: UltravoxModel, slots: int, max_len: int, eos_token_ids=None, pad_token_id: int = 0,
-                 use_graph: bool = True, cache=None, max_logprobs: int = 0, prompt_lookup_num_tokens: Optional[int] = None):
+                 use_graph: bool = True, cache=None, max_logprobs: int = 0, prompt_lookup_num_tokens: Optional[int] = None,
+                 max_constraint_tokens: Optional[int] = None):
         check_lookup_k(int(slots), prompt_lookup_num_tokens)      # before the cache is allocated
         kv = _RowKV(cache if cache is not None else model.new_cache(slots, max_len))
-        self._setup(model, int(slots), kv, eos_token_ids, pad_token_id, use_graph, max_logprobs, prompt_lookup_num_tokens)
+        self._setup(model, int(slots), kv, eos_token_ids, pad_token_id, use_graph, max_logprobs, prompt_lookup_num_tokens,
+                    max_constraint_tokens)
 
     def _setup(self, model: UltravoxModel, slots: int, kv, eos_token_ids, pad_token_id: int, use_graph: bool, max_logprobs: int = 0,
-               lookup_k: Optional[int] = None):
+               lookup_k: Optional[int] = None, max_constraint_tokens: Optional[int] = None):
         if isinstance(max_logprobs, bool) or not isinstance(max_logprobs, numbers.Integral) or \
                 not 0 <= max_logprobs <= ops.LOGPROBS_MAX:
             raise ValueError(f"max_logprobs must be an integer in [0, {ops.LOGPROBS_MAX}], got {max_logprobs!r}")
+        self.max_constraint_tokens = check_constraint_tokens(max_constraint_tokens)
         self.K = check_lookup_k(slots, lookup_k)
         self.max_logprobs = int(max_logprobs)
         self.slots = slots
@@ -917,6 +951,14 @@ class SlotDecodeEngine(_Decoder):
             self._lk_scratch = torch.empty(R, self.max_len + 1, **f32)
             if self.max_logprobs:
                 self._lk_raw = torch.empty(R, model.language_model.lm_head.weight.shape[0], **f32)
+        self.ck = None
+        if self.max_constraint_tokens is not None:
+            T = max(self.max_constraint_tokens, 1)
+            self.ck_cfg = torch.zeros(slots, 4, **i32)
+            self.ck_ids = torch.zeros(slots, T, dtype=torch.int64, device=dev)
+            self.ck_end, self.ck_kind = torch.zeros(slots, T, **i32), torch.zeros(slots, T, **i32)
+            self.ck_bias = torch.zeros(slots, T, **f32)
+            self.ck = (self.ck_cfg, self.ck_ids, self.ck_end, self.ck_bias, self.ck_kind)
         self.busy = [False] * slots
         for j in range(slots):
             self._idle(j)
@@ -938,6 +980,8 @@ class SlotDecodeEngine(_Decoder):
         if self.K:
             self.lk_k[j] = 0
             self._slot_k[j] = 0
+        if self.ck is not None:
+            self.ck_cfg[j] = 0          # no n-gram size and no entries: the kernel leaves the row alone
         self.kv.release(j)
 
     def _state(self):
@@ -956,6 +1000,8 @@ class SlotDecodeEngine(_Decoder):
         rows = (self._lk_slot, self._lk_idx)
         if self.max_logprobs:
             self._lk_raw.copy_(logits)
+        if self.ck is not None:
+            ops.logits_constraints_rows_map_(logits, self.seq, self.active, self._lk_slot, self._lk_pen, self._lk_idx, self.ck)
         ops.repetition_penalty_rows_map_(logits, self.seq, self.penalties, self.active, self._lk_slot, self._lk_pen, self._lk_idx,
                                          self._lk_scratch[:R])
         ops.sample_rows(logits, self.temps, self.top_ks, self.top_ps, self.u, self.active, *rows, self._lk_pick)
@@ -970,6 +1016,8 @@ class SlotDecodeEngine(_Decoder):
         if self.max_logprobs:
             raw = self._raw[r]
             raw.copy_(logits)
+        if self.ck is not None:
+            ops.logits_constraints_slots_(logits, self.seq[r], self.cur_len[r], self.active[r], tuple(t[r] for t in self.ck))
         ops.repetition_penalty_slots_(logits, self.seq[r], self.cur_len[r], self.penalties[r], self.active[r], self.scratch[r])
         ops.sample_slots(logits, self.temps[r], self.top_ks[r], self.top_ps[r], self.u[r], self.n_new[r], self.active[r], tok)
         if self.max_logprobs:       # at n_new, before the finish kernel advances it
@@ -1037,7 +1085,8 @@ class SlotDecodeEngine(_Decoder):
 
     def admit(self, slot: int, input_ids: torch.Tensor, max_new_tokens: int, temperature: float = 0.0, top_k: int = 0,
               top_p: float = 1.0, repetition_penalty: float = 1.0, u: Optional[torch.Tensor] = None, past: int = 0,
-              pages=None, logprobs: Optional[int] = None, lookup: Optional[tuple] = None, **features) -> torch.Tensor:
+              pages=None, logprobs: Optional[int] = None, lookup: Optional[tuple] = None, constraints=None,
+              **features) -> torch.Tensor:
         """Prefills one request (``input_ids`` [1, S] plus the processor's audio features, passed to ``model.forward``) at B = 1
         into cache row ``slot``, sets the slot's state and picks its first token from the prefill logits with the slot kernels.
         ``temperature <= 0`` is greedy; a sampled request reads ``u`` (its uniforms, one per step, as ``generate()`` draws them
@@ -1057,8 +1106,12 @@ class SlotDecodeEngine(_Decoder):
         also that many alternatives per token (``token_logprobs_of``).
 
         ``lookup`` (engines with ``prompt_lookup_num_tokens`` = K): (k, n) with 0 <= k <= K drafts per step from n-grams of up
-        to n >= 1 tokens; None or k = 0 drafts nothing."""
+        to n >= 1 tokens; None or k = 0 drafts nothing.
+
+        ``constraints`` (engines with ``max_constraint_tokens`` = N): the request's ``constraints.LogitsConstraints`` (built
+        with its whole prompt's length), at most N ids; None: no constraints."""
         n_top = self.check_logprobs(logprobs)
+        ck_rows = self.check_constraints(constraints)
         lk, ln = (0, 2) if lookup is None else (int(lookup[0]), int(lookup[1]))
         if lookup is not None and not self.K:
             raise ValueError("this engine has no prompt lookup: create it with prompt_lookup_num_tokens = K")
@@ -1118,11 +1171,29 @@ class SlotDecodeEngine(_Decoder):
         if self.K:
             self.lk_k[j], self.lk_n[j], self.accepted[j] = lk, ln, 0
             self._slot_k[j] = lk
+        if self.ck is not None:
+            if ck_rows is None:
+                self.ck_cfg[j] = 0
+            else:
+                for t, a in zip(self.ck, ck_rows):
+                    t[j].copy_(torch.from_numpy(a))
         if not chunked:
             if self.max_logprobs:
                 self.n_top[j] = n_top
             self._pick_rows(logits, slice(j, j + 1), self._admit_open)
         return self.token.view(-1)
+
+    def check_constraints(self, constraints):
+        """A request's constraint tables at this engine's width (None for None); ValueError when the engine has no constraints or
+        the request needs more than ``max_constraint_tokens`` ids."""
+        if constraints is None:
+            return None
+        if self.ck is None:
+            raise ValueError("this engine has no token constraints: create it with max_constraint_tokens = N")
+        if constraints.n_ids > self.max_constraint_tokens:
+            raise ValueError(f"the request's constraints need a table of {constraints.n_ids} ids; max_constraint_tokens = "
+                             f"{self.max_constraint_tokens}")
+        return constraints.tables(self.ck_ids.shape[1])
 
     def check_logprobs(self, logprobs) -> int:
         """The slot kernels' n_top of a request's ``logprobs`` argument (None -> -1); ValueError unless it is None or an integer
@@ -1173,10 +1244,11 @@ class PagedSlotDecodeEngine(SlotDecodeEngine):
 
     def __init__(self, model: UltravoxModel, slots: int, max_len: int, kv_pages: int, eos_token_ids=None, pad_token_id: int = 0,
                  use_graph: bool = True, max_logprobs: int = 0, kv_cache_dtype: str = "bf16", kv_scales=None, host_kv_pages: int = 0,
-                 prompt_lookup_num_tokens: Optional[int] = None):
+                 prompt_lookup_num_tokens: Optional[int] = None, max_constraint_tokens: Optional[int] = None):
         check_lookup_k(int(slots), prompt_lookup_num_tokens)      # before the pool is allocated
         kv = _PagedKV(model, int(slots), max_len, kv_pages, kv_cache_dtype, kv_scales, host_kv_pages)
         self.kv_pages, self.pool_k, self.pool_v, self.kv_scales = kv.kv_pages, kv.pool_k, kv.pool_v, kv.kv_scales
         self.host_kv_pages, self.host_k, self.host_v = kv.host_kv_pages, kv.host_k, kv.host_v
         self.swap_out, self.swap_in = kv.swap_out, kv.swap_in
-        self._setup(model, int(slots), kv, eos_token_ids, pad_token_id, use_graph, max_logprobs, prompt_lookup_num_tokens)
+        self._setup(model, int(slots), kv, eos_token_ids, pad_token_id, use_graph, max_logprobs, prompt_lookup_num_tokens,
+                    max_constraint_tokens)

@@ -897,7 +897,9 @@ class UltravoxModel(nn.Module):
                  audio_pad_frames: Optional[torch.Tensor] = None, use_graph: bool = True, num_beams: int = 1,
                  length_penalty: float = 1.0, early_stopping=False, num_return_sequences: int = 1, output_scores: bool = False,
                  output_logits: bool = False, prompt_lookup_num_tokens: Optional[int] = None,
-                 max_matching_ngram_size: Optional[int] = None, **kwargs):
+                 max_matching_ngram_size: Optional[int] = None, no_repeat_ngram_size: Optional[int] = None,
+                 bad_words_ids=None, sequence_bias=None, min_length: Optional[int] = None, min_new_tokens: Optional[int] = None,
+                 suppress_tokens=None, begin_suppress_tokens=None, **kwargs):
         """``GenerationMixin.generate`` for this model (ref :398-426; arguments as ``LocalInference._generate`` passes them, ref
         infer.py:309-342).  Returns prompt ids followed by the new tokens.
 
@@ -949,7 +951,23 @@ class UltravoxModel(nn.Module):
         ``NotImplementedError``.  The streamer gets the prompt, the first token, then one ``put`` per step with the tokens that
         step accepted.  Unlike HF, drafts are not filtered through the logits processors (which never changes the tokens) and
         never run past ``max_new_tokens``, so the output never has more than ``max_new_tokens`` new tokens.  After the call
-        ``self.lookup_stats`` holds the drafts each step accepted (``accepted``), the step count and the graph bookkeeping."""
+        ``self.lookup_stats`` holds the drafts each step accepted (``accepted``), the step count and the graph bookkeeping.
+
+        Token constraints, with transformers 5.5's meanings and checks (``ValueError`` where its processors' constructors raise,
+        and for ids outside the vocabulary in ``sequence_bias`` / ``bad_words_ids``).  Each applies to the whole sequence so far:
+        the prompt (earlier turns, padding and audio placeholder ids included) followed by the new tokens.
+        ``no_repeat_ngram_size=n``: no n-gram occurs twice (the next token may not complete an n-gram already in the sequence).
+        ``sequence_bias`` (``[[ids], float]`` list or ``{tuple: float}`` dict): a bias added to the last token of each sequence
+        whose other tokens end the sequence so far (single tokens always).  ``bad_words_ids``: the same with -inf, except that
+        an EOS id alone is never banned.  ``min_length`` / ``min_new_tokens``: EOS is banned while the sequence / the reply is
+        shorter (``min_new_tokens`` wins when both are given; nothing happens without EOS ids).  ``suppress_tokens`` are banned
+        at every step, ``begin_suppress_tokens`` at the first new token.  HF's order holds: sequence bias, repetition penalty,
+        n-gram ban, bad words, minimum length, suppression, then temperature / top-k / top-p.  One kernel
+        (``uvx_logits_constraints``) applies them inside the captured step before the penalty, which gives HF's scores (up to the
+        sign of a zero score: HF's bias processors turn -0.0 into +0.0 in every column).
+        They work with greedy and sampled decoding, padded batches, conversation turns, the streamer, prompt lookup and beams
+        (on the log-probs, as HF); ``output_scores`` then holds the constrained scores and ``output_logits`` the raw ones."""
+        from .constraints import LogitsConstraints
         from .engine import DecodeEngine
         unknown = [k for k, v in kwargs.items() if isinstance(v, torch.Tensor)]
         if unknown:
@@ -982,6 +1000,9 @@ class UltravoxModel(nn.Module):
         dev = self.device
         input_ids = input_ids.to(dev)
         B, S = input_ids.shape
+        eos = sorted(set([eos_token_id] if isinstance(eos_token_id, int) else (eos_token_id or [])))
+        cons = LogitsConstraints.build(self.language_model.lm_head.weight.shape[0], eos, S, no_repeat_ngram_size, bad_words_ids,
+                                       sequence_bias, min_length, min_new_tokens, suppress_tokens, begin_suppress_tokens)
         # left-padded batches (ref infer.py:155-180 batches prompts with padding_side="left"): keys in the padding are masked
         # for the whole generation and RoPE positions count real tokens only (hf:generation/utils.py:707-729)
         kv_start = None
@@ -1001,7 +1022,7 @@ class UltravoxModel(nn.Module):
                                 audio_batch_size=audio_batch_size, position_ids=position_ids, audio_waveforms=audio_waveforms,
                                 audio_num_frames=audio_num_frames, audio_pad_frames=audio_pad_frames),
                 kv_start, max_new_tokens, eos_token_id, pad_token_id, num_beams, length_penalty, early_stopping,
-                num_return_sequences, repetition_penalty or 1.0, use_graph)
+                num_return_sequences, repetition_penalty or 1.0, use_graph, constraints=cons)
             if return_dict_in_generate:
                 return GenerateOutput(seqs, None, scores if output_scores else None)
             return seqs
@@ -1031,18 +1052,17 @@ class UltravoxModel(nn.Module):
                 else:
                     inputs_embeds = ops.embed_splice(input_ids, self.language_model.model.embed_tokens.weight, None, None)
             out = self.forward(input_ids[:, P:], None, inputs_embeds[:, P:].contiguous(), past_key_values=cache, logits_to_keep=1)
-        eos = sorted(set([eos_token_id] if isinstance(eos_token_id, int) else (eos_token_id or [])))
         pad_id = pad_token_id if pad_token_id is not None else (min(eos) if eos else 0)
         want_scores, want_logits = bool(return_dict_in_generate and output_scores), bool(return_dict_in_generate and output_logits)
         if lookup:
             return self._lookup_decode(input_ids, out.logits.view(1, -1), cache, k_look, n_look, max_new_tokens, eos, pad_id,
                                        temp, k_top, p_top, repetition_penalty or 1.0, generator, want_scores, want_logits, streamer,
                                        use_graph, (S + max_new_tokens if past_key_values is None else plain_cap) + 1,
-                                       return_dict_in_generate)
+                                       return_dict_in_generate, cons)
         eng = DecodeEngine(self, B, cache.capacity, use_graph=use_graph, cache=cache, eos_token_ids=eos, pad_token_id=pad_id,
                            temperature=temp, top_k=k_top, top_p=p_top, repetition_penalty=repetition_penalty or 1.0,
                            generator=generator, output_scores=want_scores, output_logits=want_logits,
-                           max_new_tokens=max_new_tokens if want_scores or want_logits else None)
+                           max_new_tokens=max_new_tokens if want_scores or want_logits else None, constraints=cons)
         if streamer is not None:
             streamer.put(input_ids)
         tok = eng.begin(input_ids, out.logits.view(B, -1), kv_start)
@@ -1094,13 +1114,15 @@ class UltravoxModel(nn.Module):
 
     def _lookup_decode(self, input_ids: torch.Tensor, first_logits: torch.Tensor, cache: KVCache, k: int, n: int,
                        max_new_tokens: int, eos, pad_id: int, temp: float, k_top: int, p_top: float, penalty: float, generator,
-                       want_scores: bool, want_logits: bool, streamer, use_graph: bool, uniforms: int, return_dict: bool):
+                       want_scores: bool, want_logits: bool, streamer, use_graph: bool, uniforms: int, return_dict: bool,
+                       constraints=None):
         """``generate``'s prompt-lookup loop after the prefill of ``input_ids`` [1, S] into ``cache``."""
         from .engine import LookupDecodeEngine
         S = int(input_ids.shape[1])
         eng = LookupDecodeEngine(self, S, max_new_tokens, k, n, use_graph=use_graph, cache=cache, eos_token_ids=eos,
                                  pad_token_id=pad_id, temperature=temp, top_k=k_top, top_p=p_top, repetition_penalty=penalty,
-                                 generator=generator, output_scores=want_scores, output_logits=want_logits, uniforms=uniforms)
+                                 generator=generator, output_scores=want_scores, output_logits=want_logits, uniforms=uniforms,
+                                 constraints=constraints)
         if streamer is not None:
             streamer.put(input_ids)
         eng.begin(input_ids, first_logits)
@@ -1147,7 +1169,7 @@ class UltravoxModel(nn.Module):
 
     def _beam_search(self, input_ids: torch.Tensor, forward_kw: dict, kv_start: Optional[torch.Tensor], max_new_tokens: int,
                      eos_token_id, pad_token_id: Optional[int], num_beams: int, length_penalty: float, early_stopping,
-                     num_return_sequences: int, repetition_penalty: float, use_graph: bool, step_hook=None):
+                     num_return_sequences: int, repetition_penalty: float, use_graph: bool, step_hook=None, constraints=None):
         """``generate``'s beam branch -> (sequences [B * num_return_sequences, S + longest], their scores).  The B prompts are
         prefilled once into cache rows b * num_beams (a view of the [L, B * num_beams, S_max, ...] cache as B rows of
         num_beams * S_max positions).  ``step_hook(engine)``, if given, runs after every beam step (the host then checks
@@ -1166,7 +1188,7 @@ class UltravoxModel(nn.Module):
                            fk.pop("audio_batch_size"), prompt_rows, logits_to_keep=1, **fk)
         eng = BeamDecodeEngine(self, B, num_beams, cache.capacity, max_new_tokens, use_graph=use_graph, cache=cache,
                                eos_token_ids=eos_list, length_penalty=length_penalty, early_stopping=early_stopping,
-                               repetition_penalty=repetition_penalty)
+                               repetition_penalty=repetition_penalty, constraints=constraints)
         eng.begin(input_ids, out.logits.view(B, -1), kv_start)
         n_new = 1
         sync_every = 8          # the host looks at the device's done flag every few steps only

@@ -1156,6 +1156,80 @@ def repetition_penalty_rows_(logits: torch.Tensor, seq: torch.Tensor, lens: torc
     return logits
 
 
+def _constraint_table(table, settings: Optional[int]):
+    """(cfg, ids, end, bias, kind) of ``constraints.LogitsConstraints.tables``: one setting (``settings`` None: cfg [4], the
+    rest [T]) or ``settings`` of them (cfg [settings, 4], the rest [settings, T]), contiguous -> (pointers, T)."""
+    cfg, ids, end, bias, kind = table
+    lead = () if settings is None else (settings,)
+    _cuda(cfg, torch.int32, "cfg")
+    if tuple(cfg.shape) != lead + (4,) or not cfg.is_contiguous():
+        raise ValueError(f"cfg must be a contiguous {lead + (4,)} tensor, got {tuple(cfg.shape)}")
+    T = ids.shape[-1]
+    for t, dt, name in ((ids, torch.int64, "ids"), (end, torch.int32, "end"), (bias, torch.float32, "bias"),
+                        (kind, torch.int32, "kind")):
+        _cuda(t, dt, name)
+        if tuple(t.shape) != lead + (T,) or not t.is_contiguous() or T < 1:
+            raise ValueError(f"{name} must be a contiguous {lead + (T,)} tensor (T >= 1), got {tuple(t.shape)}")
+    return (cfg.data_ptr(), ids.data_ptr(), end.data_ptr(), bias.data_ptr(), kind.data_ptr()), T
+
+
+def _logits_rows(logits: torch.Tensor):
+    _cuda(logits, torch.float32, "logits")
+    if logits.dim() != 2 or not logits.is_contiguous():
+        raise ValueError("logits must be a contiguous [B, V] tensor")
+    return logits.shape
+
+
+def logits_constraints_(logits: torch.Tensor, seq: torch.Tensor, cur_len: torch.Tensor, table) -> torch.Tensor:
+    """``uvx_logits_constraints``: the token constraints of one setting ``table`` on every row b of logits [B, V] fp32 over
+    seq[b, :cur_len[0]], in place (before the repetition penalty)."""
+    B, V = _logits_rows(logits)
+    _seq_rows(seq, torch.int64, B, "seq"), _rows(cur_len, torch.int32, 1, "cur_len")
+    p, _ = _constraint_table(table, None)
+    check(lib().uvx_logits_constraints(logits.data_ptr(), B, V, seq.data_ptr(), seq.stride(0), cur_len.data_ptr(), *p, _stream()),
+          "uvx_logits_constraints")
+    return logits
+
+
+def logits_constraints_slots_(logits: torch.Tensor, seq: torch.Tensor, cur_len: torch.Tensor, active: torch.Tensor,
+                              table) -> torch.Tensor:
+    """``uvx_logits_constraints_slots``: active row b with its own setting b of ``table`` (cfg [B, 4], the rest [B, T]) over
+    seq[b, :cur_len[b]], in place."""
+    B, V = _logits_rows(logits)
+    _seq_rows(seq, torch.int64, B, "seq"), _rows(cur_len, torch.int32, B, "cur_len"), _rows(active, torch.int32, B, "active")
+    p, T = _constraint_table(table, B)
+    check(lib().uvx_logits_constraints_slots(logits.data_ptr(), B, V, seq.data_ptr(), seq.stride(0), cur_len.data_ptr(),
+                                             active.data_ptr(), *p, T, _stream()), "uvx_logits_constraints_slots")
+    return logits
+
+
+def logits_constraints_rows_(logits: torch.Tensor, seq: torch.Tensor, lens: torch.Tensor, table) -> torch.Tensor:
+    """``uvx_logits_constraints_rows``: one setting on row b over seq[b, :lens[b]] (seq's row stride may be 0: one shared
+    sequence), in place."""
+    R, V = _logits_rows(logits)
+    _seq_rows(seq, torch.int64, R, "seq"), _rows(lens, torch.int32, R, "lens")
+    p, _ = _constraint_table(table, None)
+    check(lib().uvx_logits_constraints_rows(logits.data_ptr(), R, V, seq.data_ptr(), seq.stride(0), lens.data_ptr(), *p, _stream()),
+          "uvx_logits_constraints_rows")
+    return logits
+
+
+def logits_constraints_rows_map_(logits: torch.Tensor, seq: torch.Tensor, active: torch.Tensor, row_slot: torch.Tensor,
+                                 row_len: torch.Tensor, row_idx: torch.Tensor, table) -> torch.Tensor:
+    """``uvx_logits_constraints_rows_map``: row r with slot s = row_slot[r]'s setting over seq[s, :row_len[r]]; rows of inactive
+    slots or with row_idx[r] < 0 untouched.  seq [slots, W], active [slots], table of ``slots`` settings, row arrays [R]."""
+    R, V = _logits_rows(logits)
+    S = seq.shape[0]
+    _seq_rows(seq, torch.int64, S, "seq"), _rows(active, torch.int32, S, "active")
+    for t, name in ((row_slot, "row_slot"), (row_len, "row_len"), (row_idx, "row_idx")):
+        _rows(t, torch.int32, R, name)
+    p, T = _constraint_table(table, S)
+    check(lib().uvx_logits_constraints_rows_map(logits.data_ptr(), R, V, seq.data_ptr(), seq.stride(0), active.data_ptr(),
+                                                row_slot.data_ptr(), row_len.data_ptr(), row_idx.data_ptr(), *p, T, _stream()),
+          "uvx_logits_constraints_rows_map")
+    return logits
+
+
 def lookup_draft(seq: torch.Tensor, cur_len: torch.Tensor, n_new: torch.Tensor, max_new: int, k: int, n: int,
                  eos_ids: Optional[torch.Tensor], done: torch.Tensor, tok: torch.Tensor, n_draft: torch.Tensor, pos: torch.Tensor,
                  lens: torch.Tensor, rope_pos: torch.Tensor, pen_len: torch.Tensor, idx: torch.Tensor) -> None:

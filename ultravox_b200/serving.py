@@ -28,6 +28,7 @@ from typing import Callable, Deque, Dict, List, Optional, Sequence, Tuple
 import torch
 
 from . import ops
+from .constraints import LogitsConstraints
 from .engine import (PREFILL_ROWS, PagedSlotDecodeEngine, SlotDecodeEngine, TokenLogprobs, check_kv_scales,
                      check_lookup_k)
 
@@ -289,6 +290,7 @@ class _Request:
     first_token: Optional[torch.cuda.Event] = None
     logprobs: Optional[int] = None     # alternatives per token asked for (None: no log-probs)
     lookup: Optional[tuple] = None     # (k, n) of prompt lookup (None: the engine has none)
+    constraints: Optional[LogitsConstraints] = None
 
 
 class SlotScheduler:
@@ -347,12 +349,20 @@ class SlotScheduler:
     yields 1 to k + 1 of them.  Drafts are taken from the request's own prompt and reply (the leftmost earlier match of its
     last n-gram, sizes n down to 1), so they pay off where a reply repeats its input.  ``accepted_drafts[id]`` is the number
     of drafted tokens the request accepted, filled when it finishes.  While a chunked prompt is in flight every slot decodes
-    one token per step; the lookup step's linears run at slots * (K + 1) rows (DESIGN.md §6 has their cost)."""
+    one token per step; the lookup step's linears run at slots * (K + 1) rows (DESIGN.md §6 has their cost).
+
+    ``max_constraint_tokens`` = N (None, the default: off): requests may take ``generate()``'s token constraints,
+    ``submit(..., no_repeat_ngram_size=, min_new_tokens=, min_length=, bad_words_ids=, sequence_bias=, suppress_tokens=,
+    begin_suppress_tokens=)``, with its meanings and checks, over the request's whole sequence (a session turn's prompt holds
+    the conversation so far).  A request's packed table may hold up to N token ids (each entry's ids; EOS ids count once per
+    entry under ``min_*``).  Each slot's settings live in device arrays, so the steps stay captured once; the constraints run
+    inside every pick, before the penalty, and a request's tokens are those ``generate()`` gives it alone with the same
+    options.  With None the engine allocates nothing for them and its steps are unchanged."""
 
     def __init__(self, model, slots: int = 8, max_len: int = 2048, eos_token_ids=None, pad_token_id: Optional[int] = None,
                  sync_every: int = 8, use_graph: bool = True, kv_pages: Optional[int] = None, prefix_cache: bool = False,
                  max_logprobs: int = 0, kv_cache_dtype: str = "bf16", kv_scales=None, host_kv_pages: int = 0,
-                 prompt_lookup_num_tokens: Optional[int] = None):
+                 prompt_lookup_num_tokens: Optional[int] = None, max_constraint_tokens: Optional[int] = None):
         eos = sorted(set([eos_token_ids] if isinstance(eos_token_ids, int) else (eos_token_ids or [])))
         pad = pad_token_id if pad_token_id is not None else (min(eos) if eos else 0)     # generate()'s default
         if int(sync_every) < 1:
@@ -382,6 +392,9 @@ class SlotScheduler:
         self.lookup_k = check_lookup_k(int(slots), prompt_lookup_num_tokens)     # 0: off
         if self.lookup_k:
             lp["prompt_lookup_num_tokens"] = self.lookup_k
+        if max_constraint_tokens is not None:
+            lp["max_constraint_tokens"] = max_constraint_tokens       # the engine validates it
+        self._eos = eos
         self.accepted_drafts: Dict[int, int] = {}
         if host_kv_pages:
             kv["host_kv_pages"] = int(host_kv_pages)
@@ -473,7 +486,9 @@ class SlotScheduler:
                top_k: Optional[int] = None, top_p: Optional[float] = None, repetition_penalty: float = 1.0,
                generator: Optional[torch.Generator] = None, num_beams: int = 1, session: Optional[int] = None,
                logprobs: Optional[int] = None, prompt_lookup_num_tokens: Optional[int] = None,
-               max_matching_ngram_size: Optional[int] = None) -> int:
+               max_matching_ngram_size: Optional[int] = None, no_repeat_ngram_size: Optional[int] = None,
+               min_new_tokens: Optional[int] = None, min_length: Optional[int] = None, bad_words_ids=None, sequence_bias=None,
+               suppress_tokens=None, begin_suppress_tokens=None) -> int:
         """Queues one request: ``features`` is the processor's output for it (``input_ids`` [1, S] and, for audio, its mel or
         waveform fields).  Arguments and defaults are ``generate()``'s: greedy unless ``do_sample``; sampling defaults to
         temperature 1 and top_k 50; ``top_p`` must lie in [0, 1].  A sampled request draws its uniforms here, as ``generate()``
@@ -487,7 +502,12 @@ class SlotScheduler:
         alternatives per token (``logprobs[id]`` once it has finished).  Anything else raises ValueError.
 
         ``prompt_lookup_num_tokens`` / ``max_matching_ngram_size`` (a scheduler built with ``prompt_lookup_num_tokens``): the
-        request's drafts per step, None for the scheduler's K, 0 for none, at most K; its n-gram size, None for 2."""
+        request's drafts per step, None for the scheduler's K, 0 for none, at most K; its n-gram size, None for 2.
+
+        ``no_repeat_ngram_size``, ``min_new_tokens``, ``min_length``, ``bad_words_ids``, ``sequence_bias``, ``suppress_tokens``,
+        ``begin_suppress_tokens`` (a scheduler built with ``max_constraint_tokens``): ``generate()``'s token constraints and
+        checks.  ValueError when the scheduler has no constraints or the request's table needs more than
+        ``max_constraint_tokens`` ids."""
         if logprobs is not None:
             self.engine.check_logprobs(logprobs)
         lookup = self._check_lookup(prompt_lookup_num_tokens, max_matching_ngram_size)
@@ -502,6 +522,14 @@ class SlotScheduler:
         if am is not None and not bool(am.to(torch.bool).all()):
             raise NotImplementedError("a single request has no padding; its attention_mask must be all ones")
         S, n = int(ids.shape[1]), int(max_new_tokens)
+        ck_args = (no_repeat_ngram_size, bad_words_ids, sequence_bias, min_length, min_new_tokens, suppress_tokens,
+                   begin_suppress_tokens)
+        cons = None
+        if any(a is not None for a in ck_args):
+            if self.engine.max_constraint_tokens is None:
+                raise ValueError("token constraints need a table per slot: SlotScheduler(..., max_constraint_tokens=N)")
+            cons = LogitsConstraints.build(self.model.language_model.lm_head.weight.shape[0], self._eos, S, *ck_args)
+            self.engine.check_constraints(cons)
         if n < 1:
             raise ValueError(f"max_new_tokens must be >= 1, got {max_new_tokens}")
         if S + n > self.capacity:
@@ -534,7 +562,8 @@ class SlotScheduler:
         rid = self._next_id
         self._next_id += 1
         self._queue.append(_Request(rid, ids, feats, n, temp, k_top, p_top, float(repetition_penalty or 1.0), u, session,
-                                    prefix, logprobs=None if logprobs is None else int(logprobs), lookup=lookup))
+                                    prefix, logprobs=None if logprobs is None else int(logprobs), lookup=lookup,
+                                    constraints=cons))
         if sess is not None:
             sess.busy = True
         return rid
@@ -599,6 +628,8 @@ class SlotScheduler:
                 kw["logprobs"] = r.logprobs
             if r.lookup is not None:
                 kw["lookup"] = r.lookup
+            if r.constraints is not None:
+                kw["constraints"] = r.constraints
             eng.admit(j, r.input_ids, r.max_new, r.temperature, r.top_k, r.top_p, r.penalty, r.u, **kw, **feats)
             r.features, r.u = {}, None
             if long:
