@@ -370,7 +370,9 @@ int uvx_kv_write(const void* qkv, int64_t row_stride, int64_t k_col, int64_t v_c
  *                         scratch: [B, seq_stride] fp32.
  * uvx_sample              out[b] ~ softmax(logits[b] / temperature) restricted to the top_k largest logits (top_k <= 0: all),
  *                         by inverse CDF on the uniform u[step_idx[0] * u_stride + b] (step_idx NULL = 0): the do_sample branch of
- *                         ref:ultravox/inference/infer.py:319-328.  Deterministic given u.
+ *                         ref:ultravox/inference/infer.py:319-328.  Deterministic given u.  The pick always has positive
+ *                         mass (never a -inf logit); a row with no mass (all -inf) gives 0, as uvx_argmax does.  -0.0 and
+ *                         +0.0 are one value for the top-k cut and the tie groups below.
  * uvx_sample_top_p        uvx_sample with nucleus filtering after the top-k cut, in HF's order (hf:generation/logits_process.py
  *                         TemperatureLogitsWarper -> TopKLogitsWarper -> TopPLogitsWarper): with P = softmax(logits[b] / temperature)
  *                         over the top-k survivors, token i stays iff sum_{j: x_j <= x_i} P_j > 1 - top_p, and the largest logit
@@ -427,8 +429,8 @@ int uvx_slot_finish(const int64_t* tok, int32_t* done, const int64_t* eos_ids, i
  *                     processed scores (`output_scores`, hf:generation/utils.py _sample) of the penalised logits: for
  *                     temperature <= 0 (greedy: HF adds no warper) the row itself, otherwise TemperatureLogitsWarper ->
  *                     TopKLogitsWarper -> TopPLogitsWarper: x / temperature (IEEE division) on the entries uvx_sample /
- *                     uvx_sample_top_p draw from with the same temperature, top_k and top_p, -inf elsewhere, so a sampled
- *                     token always has a finite score.  scores / raw are [steps, B, V] fp32; either may be NULL.  V <= 2^24. */
+ *                     uvx_sample_top_p draw from with the same temperature, top_k and top_p (a tie group, -0.0 == +0.0,
+ *                     kept or dropped whole), -inf elsewhere, so a sampled token always has a finite score.  scores / raw are [steps, B, V] fp32; either may be NULL.  V <= 2^24. */
 int uvx_token_logprobs(const float* logits, int64_t B, int64_t V, const int64_t* tok, const int32_t* n_top, const int32_t* dst,
                        int64_t cap, int32_t n_max, float* out_lp, int64_t* out_ids, float* out_top, uvx_stream_t stream);
 int uvx_record_scores(const float* logits, int64_t B, int64_t V, float temperature, int32_t top_k, float top_p,

@@ -70,9 +70,12 @@ __global__ void __launch_bounds__(1024) rep_penalty_kernel(float* __restrict__ l
   }
 }
 
-__device__ __forceinline__ uint32_t f2key(float f) {  // order-preserving float -> uint map
+// Order-preserving float -> uint map.  A negative float maps to -bits (mod 2^32) rather than ~bits, which puts -0.0 on the key
+// of +0.0 (0x80000000): the two compare equal, so a top-k cut, a top-p tie group and the (value desc, index asc) order of
+// uvx_token_logprobs treat them as one value.  The same instruction count as ~bits.
+__device__ __forceinline__ uint32_t f2key(float f) {
   const uint32_t u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+  return (u & 0x80000000u) ? 0u - u : (u | 0x80000000u);
 }
 
 // One CTA (1024 threads) per row: max, optional exact k-th-largest threshold by 4-pass radix select on the float keys,
@@ -295,13 +298,17 @@ __device__ __forceinline__ void sample_row(const float* __restrict__ row, int64_
     wt = win_thread;
   }
   if (tid == (wt < 0 ? 0 : wt)) {
+    // The walk re-adds the chunk's masses onto excl, which rounds differently from excl + local: a target in the top ulps
+    // of the chunk (or past it, wt < 0) can outrun it.  The pick is then the chunk's last entry with positive mass - never a
+    // kept entry of mass 0 (a -inf logit, or one __expf flushes to 0).  A row without mass (all -inf: NaN masses) gives 0.
     float acc = excl;
     int64_t pick = -1, last = -1;
     for (int64_t i = lo; i < hi; ++i) {
       const float x = row[i];
       if (f2key(x) < thr_key) continue;
-      last = i;
-      acc += __expf((x - mx) * inv_temp);
+      const float m = __expf((x - mx) * inv_temp);
+      if (m > 0.f) last = i;
+      acc += m;
       if (acc > target) { pick = i; break; }
     }
     if (pick < 0) pick = last >= 0 ? last : 0;
