@@ -465,6 +465,47 @@ int uvx_repetition_penalty_rows(float* logits, int64_t B, int64_t V, const int64
 int uvx_record_scores_rows(const float* logits, int64_t B, int64_t V, float temperature, int32_t top_k, float top_p,
                            const int32_t* idx, int64_t steps, float* scores, float* raw, uvx_stream_t stream);
 
+/* Sampling cut-offs after top-k / top-p, in HF's order (hf:generation/logits_process.py, transformers 5.5, min_tokens_to_keep = 1):
+ * TemperatureLogitsWarper -> TopKLogitsWarper -> TopPLogitsWarper -> MinPLogitsWarper -> TypicalLogitsWarper ->
+ * EpsilonLogitsWarper -> EtaLogitsWarper, each on the survivors of the one before.  With P = softmax(x / temperature) over the
+ * current survivors and H = -sum P log P:
+ *   min_p      keep P_i >= min_p * max P (the maximum always stays).  0 <= min_p <= 1; 0 is off.
+ *   typical_p  d_i = |-log P_i - H|; with the survivors sorted by d ascending, keep d_i <= the d of the first one whose cumulative
+ *              P reaches typical_p.  This may drop the row maximum.  0 < typical_p; >= 1 is off.
+ *   epsilon    keep P_i >= epsilon, and the largest survivor's tie group.  0 <= epsilon < 1; 0 is off.
+ *   eta        keep P_i >= min(eta, sqrt(eta) * exp(-H)), and the largest survivor's tie group.  0 <= eta < 1; 0 is off.
+ * Arguments outside those ranges (NaN included) give UVX_ERR_ARG.  Ties: a tie group (equal logits, -0.0 == +0.0) is kept or
+ * dropped whole at every cut, which HF's per-element comparisons also do.  The kept set is a band lo <= key <= hi of the
+ * sampler's order-preserving float keys; the masses are 64-bit fixed point (2^-40) and the entropy a fixed-order float64 sum,
+ * so the band, and the pick given u, depend on the row and its settings alone.  V <= 2^24.  Each cut-off that is on costs
+ * one to six more passes over the row; with every cut-off off each entry below is its plain form bit for bit.
+ * uvx_sample_cutoffs              uvx_sample_top_p, then the cut-offs; the draw is the inverse CDF over the kept band on u.
+ * uvx_record_scores_cutoffs       uvx_record_scores with the cut-offs: x / temperature exactly where uvx_sample_cutoffs can
+ *                                 pick, -inf elsewhere (greedy, temperature <= 0, ignores them as HF does).
+ * uvx_record_scores_rows_cutoffs  uvx_record_scores_rows with the cut-offs.
+ * uvx_sample_slots_cutoffs        uvx_sample_slots with slot b's cut-offs at cutoffs[4 b .. 4 b + 4) = (min_p, typical_p, epsilon,
+ *                                 eta) fp32 on the device, off encoded as (0, 1, 0, 0); a row with every cut-off off makes the
+ *                                 pick uvx_sample_slots makes, bit for bit.  Values are not checked on the device: the caller
+ *                                 writes them in range.
+ * uvx_sample_rows_cutoffs         uvx_sample_rows with slot row_slot[r]'s cut-offs, as above.                                   */
+typedef struct uvx_cutoffs {
+  float min_p, typical_p, epsilon, eta;
+} uvx_cutoffs;
+int uvx_sample_cutoffs(const float* logits, int64_t B, int64_t V, float temperature, int32_t top_k, float top_p, uvx_cutoffs cutoffs,
+                       const float* u, const int32_t* step_idx, int64_t u_stride, int64_t* out_idx, uvx_stream_t stream);
+int uvx_record_scores_cutoffs(const float* logits, int64_t B, int64_t V, float temperature, int32_t top_k, float top_p,
+                              uvx_cutoffs cutoffs, const int32_t* step_idx, int64_t steps, float* scores, float* raw,
+                              uvx_stream_t stream);
+int uvx_record_scores_rows_cutoffs(const float* logits, int64_t B, int64_t V, float temperature, int32_t top_k, float top_p,
+                                   uvx_cutoffs cutoffs, const int32_t* idx, int64_t steps, float* scores, float* raw,
+                                   uvx_stream_t stream);
+int uvx_sample_slots_cutoffs(const float* logits, int64_t B, int64_t V, const float* temperature, const int32_t* top_k,
+                             const float* top_p, const float* cutoffs, const float* u, int64_t u_stride, const int32_t* n_new,
+                             const int32_t* active, int64_t* out_idx, uvx_stream_t stream);
+int uvx_sample_rows_cutoffs(const float* logits, int64_t R, int64_t V, const float* temperature, const int32_t* top_k,
+                            const float* top_p, const float* cutoffs, const float* u, int64_t u_stride, const int32_t* active,
+                            const int32_t* row_slot, const int32_t* row_idx, int64_t* out_idx, uvx_stream_t stream);
+
 /* Prompt lookup inside the slot step (ultravox_b200/engine.py SlotDecodeEngine with prompt_lookup_num_tokens = K): slot s owns
  * the R = slots * (K + 1) step rows r = s * (K + 1) + i, i <= K.  Per-slot arrays are [slots]; per-row arrays are [R]; seq is
  * [slots, seq_stride] int64.

@@ -27,6 +27,11 @@ class GemmArgs(C.Structure):
                 ("rope_pos_offset", c_i64), ("flags", c_i32), ("w_perm", c_i32)]
 
 
+class Cutoffs(C.Structure):
+    """``struct uvx_cutoffs`` (include/uvx.h), passed by value."""
+    _fields_ = [("min_p", c_f32), ("typical_p", c_f32), ("epsilon", c_f32), ("eta", c_f32)]
+
+
 class AttnArgs(C.Structure):
     """``struct uvx_attn_args`` (include/uvx.h)."""
     _fields_ = [("q", c_vp), ("k", c_vp), ("v", c_vp), ("o", c_vp), ("B", c_i64), ("Hq", c_i64), ("Hkv", c_i64),
@@ -110,6 +115,11 @@ SIGNATURES = {
     "uvx_lookup_accept": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp, c_vp]),
     "uvx_repetition_penalty_rows": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_f32, c_vp, c_i64, c_vp]),
     "uvx_record_scores_rows": (C.c_int, [c_vp, c_i64, c_i64, c_f32, c_i32, c_f32, c_vp, c_i64, c_vp, c_vp, c_vp]),
+    "uvx_sample_cutoffs": (C.c_int, [c_vp, c_i64, c_i64, c_f32, c_i32, c_f32, Cutoffs, c_vp, c_vp, c_i64, c_vp, c_vp]),
+    "uvx_record_scores_cutoffs": (C.c_int, [c_vp, c_i64, c_i64, c_f32, c_i32, c_f32, Cutoffs, c_vp, c_i64, c_vp, c_vp, c_vp]),
+    "uvx_record_scores_rows_cutoffs": (C.c_int, [c_vp, c_i64, c_i64, c_f32, c_i32, c_f32, Cutoffs, c_vp, c_i64, c_vp, c_vp, c_vp]),
+    "uvx_sample_slots_cutoffs": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp]),
+    "uvx_sample_rows_cutoffs": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "uvx_lookup_draft_slots": (C.c_int, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64,
                                          c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "uvx_lookup_accept_slots": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_i32, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp,

@@ -5,6 +5,8 @@
 //   uvx_sample              temperature / top-k multinomial sampling (ref:ultravox/inference/infer.py:319-328: do_sample when
 //                           temperature > 0; hf:generation/utils.py _sample: softmax(logits / T) -> multinomial)
 //   uvx_sample_top_p        the same with nucleus (top-p) filtering after top-k (hf:generation/logits_process.py TopPLogitsWarper)
+//   uvx_sample_cutoffs      the same with min_p / typical_p / epsilon / eta cut-offs after top-p (MinP, Typical, Epsilon, Eta
+//                           LogitsWarper); _slots_cutoffs / _rows_cutoffs with each slot's own cut-offs
 //   uvx_token_finish        EOS / pad bookkeeping of the finished rows, append to `sequences`, advance positions
 //   uvx_sample_slots        continuous batching: per-row greedy / sampled pick with each row's own settings and uniform
 //   uvx_repetition_penalty_slots   the repetition penalty with each row's own penalty and length
@@ -129,6 +131,95 @@ struct ThresholdSmem {  // keep_threshold's shared memory, declared by the calle
   uint32_t* p_prefix;
 };
 
+// Mass-weighted radix select over the entries in_set(x, key_of(x)) accepts, keyed by key_of(x): the smallest key v such that the mass of the
+// entries with key <= v exceeds target_of(total mass), total > 0 (0 when no entry has mass: the caller then makes no cut).  From
+// the top byte down: a 256-bin mass histogram of the keys that match the prefix, scanned upward from the mass carried below the
+// prefix.  Masses m = exp((x - max) / T) are 64-bit fixed point (kMassOne = 1), so the atomics are order-free and the result
+// deterministic; equal keys share a bin and are counted or passed over whole.  Entries whose mass rounds to 0 never cross the
+// threshold and are skipped.  The typical cut (keys = deviation from the mean log-mass).  It is keep_threshold's top-p pass
+// with the key, the set and the target as parameters; keep_threshold keeps its own copy because routing it through this one
+// changes the SASS of uvx_sample_top_p and uvx_record_scores (+32 instructions of scheduling) for no change in what they do.
+template <class KeyOf, class InSet, class TargetOf>
+__device__ __forceinline__ uint32_t mass_select(const float* __restrict__ row, int64_t V, float mx, float inv_temp, KeyOf key_of,
+                                                InSet in_set, TargetOf target_of, const ThresholdSmem& sm) {
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  unsigned long long* mhist = sm.mhist;
+  unsigned long long& p_below = *sm.p_below;
+  unsigned long long& p_target = *sm.p_target;
+  uint32_t& p_prefix = *sm.p_prefix;
+  if (tid == 0) { p_prefix = 0u; p_below = 0ull; p_target = 0ull; }
+  for (int pass = 3; pass >= 0; --pass) {
+    if (tid < 256) mhist[tid] = 0ull;
+    __syncthreads();
+    const uint32_t prefix = p_prefix;
+    const uint32_t hi_mask = pass == 3 ? 0u : (0xFFFFFFFFu << ((pass + 1) * 8));
+    // a per-thread cache of 4 (bin, mass) slots in registers: without top-k most of the row carries mass, and the first pass
+    // puts it in the few top-byte bins its exponents span, where shared atomics would serialise on a handful of addresses
+    uint32_t cb[4] = {~0u, ~0u, ~0u, ~0u};
+    unsigned long long cs[4] = {0ull, 0ull, 0ull, 0ull};
+    constexpr int kLoads = 8;  // independent loads in flight per thread: one at a time, a pass is bound by L2 latency
+    for (int64_t base = tid; base < V; base += 1024 * kLoads) {
+      float xs[kLoads];
+#pragma unroll
+      for (int j = 0; j < kLoads; ++j) {
+        const int64_t i = base + (int64_t)j * 1024;
+        xs[j] = i < V ? row[i] : -INFINITY;
+      }
+#pragma unroll
+      for (int j = 0; j < kLoads; ++j) {
+        const float x = xs[j];
+        const uint32_t k = key_of(x);
+        if (base + (int64_t)j * 1024 >= V || !in_set(x, k) || (k & hi_mask) != (prefix & hi_mask)) continue;
+        const unsigned long long m = __float2ull_rn(__expf((x - mx) * inv_temp) * kMassOne);
+        if (m == 0ull) continue;
+        const uint32_t bin = (k >> (pass * 8)) & 255u;
+        bool held = false;
+#pragma unroll
+        for (int s = 0; s < 4; ++s)
+          if (!held && cb[s] == bin) { cs[s] += m; held = true; }
+#pragma unroll
+        for (int s = 0; s < 4; ++s)
+          if (!held && cs[s] == 0ull) { cb[s] = bin; cs[s] = m; held = true; }
+        if (!held) atomicAdd(&mhist[bin], m);
+      }
+    }
+#pragma unroll
+    for (int s = 0; s < 4; ++s)
+      if (cs[s] != 0ull) atomicAdd(&mhist[cb[s]], cs[s]);
+    __syncthreads();
+    if (w == 0) {  // lane l scans bins [8l, 8l + 8)
+      unsigned long long s = 0ull;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) s += mhist[lane * 8 + j];
+      unsigned long long incl = s;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+      }
+      if (pass == 3) {  // the first pass sees every entry of the set: its histogram total is the whole mass
+        const unsigned long long total = __shfl_sync(0xffffffffu, incl, 31);
+        if (lane == 0 && total > 0ull) p_target = target_of(total);
+        __syncwarp();
+      }
+      const unsigned long long below = p_below, target = p_target;
+      const unsigned hit = __ballot_sync(0xffffffffu, below + incl > target);
+      if (hit != 0u && lane == __ffs(hit) - 1) {  // no hit only for a set without mass (all -inf)
+        unsigned long long acc = below + incl - s;
+        int d = lane * 8;
+        for (; d < lane * 8 + 7; ++d) {
+          if (acc + mhist[d] > target) break;
+          acc += mhist[d];
+        }
+        p_prefix = prefix | ((uint32_t)d << (pass * 8));
+        p_below = acc;
+      }
+    }
+    __syncthreads();
+  }
+  return p_prefix;
+}
+
 template <int TOP_P>
 __device__ __forceinline__ uint32_t keep_threshold(const float* __restrict__ row, int64_t V, float inv_temp, int top_k, float top_p,
                                                    ThresholdSmem sm, float& mx_out) {
@@ -238,11 +329,181 @@ __device__ __forceinline__ uint32_t keep_threshold(const float* __restrict__ row
   return thr_key;
 }
 
-// The body of sample_kernel, shared with uvx_sample_slots (TOP_P as in keep_threshold).  The caller's CTA handles one row.
-template <int TOP_P>
+// ---------------------------------------------------------------------------------------------------------------------------
+// Sampling cut-offs after top-k / top-p (hf:generation/logits_process.py MinPLogitsWarper, TypicalLogitsWarper,
+// EpsilonLogitsWarper, EtaLogitsWarper, in that order, min_tokens_to_keep = 1).  Each acts on the survivors of the one before;
+// every one is on only when its value is (the host encodes off as min_p 0, typical 1, epsilon 0, eta 0).  The kept set is a band
+// lo <= f2key(x) <= hi: min_p, epsilon and eta raise lo, typical can also lower hi (it may drop the row maximum).
+struct Cutoffs {
+  float min_p, typical_p, epsilon, eta;
+};
+
+__device__ __forceinline__ bool cutoffs_on(const Cutoffs& cf) {
+  return cf.min_p > 0.f || cf.typical_p < 1.f || cf.epsilon > 0.f || cf.eta > 0.f;
+}
+
+struct CutoffSmem {  // the cut-off stage's shared memory, besides ThresholdSmem's
+  double* dred;      // [32]
+  unsigned long long* zsum;
+  uint32_t *klo, *khi;
+};
+
+// Z = sum of the fixed-point masses over the band (integer atomics: order-free) and, when S is wanted, S = sum m * a with
+// a = (x - max) / T in float64, reduced in a fixed order (per-thread stride, warp butterfly, warp 0 over the 32 partials), so the
+// value depends on the row alone.  Entries of mass 0 add nothing (HF's 0 * log 0 = 0).
+template <bool kWithS>
+__device__ __forceinline__ void band_moments(const float* __restrict__ row, int64_t V, float mx, float inv_temp, uint32_t lo,
+                                             uint32_t hi, const CutoffSmem& cs, unsigned long long& Z, double& S) {
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  if (tid == 0) *cs.zsum = 0ull;
+  __syncthreads();
+  unsigned long long z = 0ull;
+  double s = 0.0;
+  for (int64_t i = tid; i < V; i += 1024) {
+    const float x = row[i];
+    const uint32_t k = f2key(x);
+    if (k < lo || k > hi) continue;
+    const float a = (x - mx) * inv_temp;
+    const float m = __expf(a);
+    if (!(m > 0.f)) continue;
+    z += __float2ull_rn(m * kMassOne);
+    if (kWithS) s += (double)m * (double)a;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) z += __shfl_xor_sync(0xffffffffu, z, o);
+  if (lane == 0 && z) atomicAdd(cs.zsum, z);
+  if (kWithS) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) cs.dred[w] = s;
+  }
+  __syncthreads();
+  Z = *cs.zsum;
+  if (kWithS) {
+    s = cs.dred[lane];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    S = s;
+  }
+  __syncthreads();
+}
+
+// The smallest key in the band whose fp32 mass __expf((x - max) / T) is >= mt (~0u when none is): a lower cut that keeps tie
+// groups whole, as equal keys have equal masses.  Integer atomicMin: order-free.
+__device__ __forceinline__ uint32_t band_min_key(const float* __restrict__ row, int64_t V, float mx, float inv_temp, uint32_t lo,
+                                                 uint32_t hi, float mt, const CutoffSmem& cs) {
+  if (threadIdx.x == 0) *cs.klo = ~0u;
+  __syncthreads();
+  uint32_t best = ~0u;
+  for (int64_t i = threadIdx.x; i < V; i += 1024) {
+    const float x = row[i];
+    const uint32_t k = f2key(x);
+    if (k >= lo && k <= hi && k < best && __expf((x - mx) * inv_temp) >= mt) best = k;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) best = min(best, __shfl_xor_sync(0xffffffffu, best, o));
+  if ((threadIdx.x & 31) == 0 && best != ~0u) atomicMin(cs.klo, best);
+  __syncthreads();
+  const uint32_t r = *cs.klo;
+  __syncthreads();
+  return r;
+}
+
+// The cut-offs over the band [lo, hi] left by top-k / top-p (hi = ~0u).  With p = m / Z over the current survivors:
+//  min_p:     keep m >= min_p (m_max = 1: p >= min_p * max p).
+//  typical:   d = |-log p - H| = |a - S / Z|; the smallest deviation key D whose cumulative mass (by d ascending) reaches
+//             typical_p * Z (HF's last_ind), by mass_select over deviation keys; keep d <= D, converted to the key band it spans
+//             (d is V-shaped in x, so {d <= D} is an interval of keys).
+//  epsilon:   keep m >= epsilon * Z, and the band's top key (the largest survivor's tie group).
+//  eta:       keep m >= min(epsilon, sqrt(eta) exp(-H)) * Z, H = log Z - S / Z, and the band's top key.
+// A band without mass (an all -inf row) is left as it is.  Every value that decides a cut is a fixed-point sum, a fixed-order
+// float64 sum or an integer atomic: the band depends on the row and its settings alone.
+__device__ __forceinline__ void cutoff_band(const float* __restrict__ row, int64_t V, float mx, float inv_temp, const Cutoffs& cf,
+                                            const ThresholdSmem& sm, const CutoffSmem& cs, uint32_t& lo, uint32_t& hi) {
+  const int tid = threadIdx.x;
+  if (!(mx > -INFINITY)) return;
+  if (cf.min_p > 0.f) {
+    const uint32_t k = band_min_key(row, V, mx, inv_temp, lo, hi, cf.min_p, cs);
+    if (k != ~0u) lo = max(lo, k);
+  }
+  if (cf.typical_p < 1.f) {
+    unsigned long long Z;
+    double S;
+    band_moments<true>(row, V, mx, inv_temp, lo, hi, cs, Z, S);
+    if (Z > 0ull) {
+      const float c = (float)(S / ((double)Z / (double)kMassOne));
+      const uint32_t blo = lo, bhi = hi;
+      const auto dkey = [mx, inv_temp, c](float x) { return __float_as_uint(fabsf((x - mx) * inv_temp - c)); };
+      const float tp = cf.typical_p;
+      const uint32_t D = mass_select(
+          row, V, mx, inv_temp, dkey,
+          [blo, bhi](float x, uint32_t) {
+            const uint32_t k = f2key(x);
+            return k >= blo && k <= bhi;
+          },
+          [tp](unsigned long long total) {  // mass(d <= D) >= typical_p * Z: the first sorted cumulative mass not < typical_p
+            const double want = ceil((double)tp * (double)total);
+            const unsigned long long t = want >= 1.0 ? (unsigned long long)want - 1ull : 0ull;
+            return t < total - 1ull ? t : total - 1ull;
+          },
+          sm);
+      if (tid == 0) { *cs.klo = ~0u; *cs.khi = 0u; }
+      __syncthreads();
+      uint32_t kl = ~0u, kh = 0u;
+      for (int64_t i = tid; i < V; i += 1024) {
+        const float x = row[i];
+        const uint32_t k = f2key(x);
+        if (k >= blo && k <= bhi && __expf((x - mx) * inv_temp) > 0.f && dkey(x) <= D) { kl = min(kl, k); kh = max(kh, k); }
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        kl = min(kl, __shfl_xor_sync(0xffffffffu, kl, o));
+        kh = max(kh, __shfl_xor_sync(0xffffffffu, kh, o));
+      }
+      if ((tid & 31) == 0 && kl != ~0u) { atomicMin(cs.klo, kl); atomicMax(cs.khi, kh); }
+      __syncthreads();
+      if (*cs.klo != ~0u) { lo = *cs.klo; hi = *cs.khi; }
+      __syncthreads();
+    }
+  }
+  // the band's top key: the row maximum's while typical has not lowered hi
+  const uint32_t top = hi == ~0u ? f2key(mx) : hi;
+  if (cf.epsilon > 0.f) {
+    unsigned long long Z;
+    double S;
+    band_moments<false>(row, V, mx, inv_temp, lo, hi, cs, Z, S);
+    const uint32_t k = band_min_key(row, V, mx, inv_temp, lo, hi, (float)((double)cf.epsilon * ((double)Z / (double)kMassOne)), cs);
+    lo = max(lo, min(k, top));
+  }
+  if (cf.eta > 0.f) {
+    unsigned long long Z;
+    double S;
+    band_moments<true>(row, V, mx, inv_temp, lo, hi, cs, Z, S);
+    const double z = (double)Z / (double)kMassOne;
+    const double H = log(z) - S / z;
+    const double e = (double)cf.eta;
+    const uint32_t k = band_min_key(row, V, mx, inv_temp, lo, hi, (float)(fmin(e, sqrt(e) * exp(-H)) * z), cs);
+    lo = max(lo, min(k, top));
+  }
+}
+
+// keep_threshold, then (CUT = 1 always, 2 when the row has a cut-off on, 0 never) cutoff_band: the kept set is lo <= key <= hi.
+// CUT = 0 is keep_threshold itself with hi = ~0u.
+template <int TOP_P, int CUT>
+__device__ __forceinline__ uint32_t keep_band(const float* __restrict__ row, int64_t V, float inv_temp, int top_k, float top_p,
+                                              const Cutoffs& cf, ThresholdSmem sm, const CutoffSmem& cs, float& mx, uint32_t& hi) {
+  uint32_t lo = keep_threshold<TOP_P>(row, V, inv_temp, top_k, top_p, sm, mx);
+  hi = ~0u;
+  if (CUT == 1 || (CUT == 2 && cutoffs_on(cf))) cutoff_band(row, V, mx, inv_temp, cf, sm, cs, lo, hi);
+  return lo;
+}
+
+// The body of sample_kernel, shared with uvx_sample_slots (TOP_P as in keep_threshold, CUT as in keep_band).  The caller's CTA
+// handles one row.
+template <int TOP_P, int CUT>
 __device__ __forceinline__ void sample_row(const float* __restrict__ row, int64_t V, float inv_temp, int top_k, float top_p,
-                                           const float* __restrict__ u_all, const int32_t* __restrict__ step_idx, int64_t u_stride,
-                                           int64_t col, int64_t* __restrict__ out_ptr) {
+                                           const Cutoffs& cf, const float* __restrict__ u_all, const int32_t* __restrict__ step_idx,
+                                           int64_t u_stride, int64_t col, int64_t* __restrict__ out_ptr) {
   __shared__ float red[32];
   __shared__ uint32_t hist[256];
   __shared__ uint32_t sel_prefix, sel_remaining;
@@ -251,17 +512,27 @@ __device__ __forceinline__ void sample_row(const float* __restrict__ row, int64_
   __shared__ unsigned long long mhist[256];
   __shared__ unsigned long long p_below, p_target;
   __shared__ uint32_t p_prefix;
+  CutoffSmem cs{};
+  if constexpr (CUT != 0) {
+    __shared__ double dred[32];
+    __shared__ unsigned long long zsum;
+    __shared__ uint32_t klo, khi;
+    cs = {dred, &zsum, &klo, &khi};
+  }
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   float mx;
-  const uint32_t thr_key = keep_threshold<TOP_P>(row, V, inv_temp, top_k, top_p,
-                                                 {red, hist, &sel_prefix, &sel_remaining, mhist, &p_below, &p_target, &p_prefix}, mx);
+  uint32_t thr_hi;
+  const uint32_t thr_key = keep_band<TOP_P, CUT>(row, V, inv_temp, top_k, top_p, cf,
+                                                 {red, hist, &sel_prefix, &sel_remaining, mhist, &p_below, &p_target, &p_prefix}, cs,
+                                                 mx, thr_hi);
   // ---- chunk sums
   const int64_t c = (V + 1023) / 1024;
   const int64_t lo = (int64_t)tid * c, hi = lo + c < V ? lo + c : V;
   float local = 0.f;
   for (int64_t i = lo; i < hi; ++i) {
     const float x = row[i];
-    if (f2key(x) >= thr_key) local += __expf((x - mx) * inv_temp);
+    const uint32_t k = f2key(x);
+    if (k >= thr_key && k <= thr_hi) local += __expf((x - mx) * inv_temp);
   }
   // inclusive scan over the 1024 chunk sums
   float incl = local;
@@ -305,7 +576,8 @@ __device__ __forceinline__ void sample_row(const float* __restrict__ row, int64_
     int64_t pick = -1, last = -1;
     for (int64_t i = lo; i < hi; ++i) {
       const float x = row[i];
-      if (f2key(x) < thr_key) continue;
+      const uint32_t k = f2key(x);
+      if (k < thr_key || k > thr_hi) continue;
       const float m = __expf((x - mx) * inv_temp);
       if (m > 0.f) last = i;
       acc += m;
@@ -316,15 +588,17 @@ __device__ __forceinline__ void sample_row(const float* __restrict__ row, int64_
   }
 }
 
-template <bool TOP_P>  // (1024, 1): lets ptxas use the 64 registers a lone 1024-thread CTA may have (the top-p form uses 56)
+// (1024, 1): lets ptxas use the 64 registers a lone 1024-thread CTA may have (the top-p form uses 56).  CUT: uvx_sample_cutoffs
+// (cf read only then; appended last so the other forms keep their parameter layout).
+template <bool TOP_P, bool CUT>
 __global__ void __launch_bounds__(1024, 1) sample_kernel(const float* __restrict__ logits, int64_t V, float inv_temp, int top_k,
                                                      float top_p, const float* __restrict__ u_all,
                                                      const int32_t* __restrict__ step_idx, int64_t u_stride,
-                                                     int64_t* __restrict__ out) {
+                                                     int64_t* __restrict__ out, Cutoffs cf) {
   pdl_trigger();
   pdl_wait();
   const int64_t b = blockIdx.x;
-  sample_row<TOP_P ? 1 : 0>(logits + b * V, V, inv_temp, top_k, top_p, u_all, step_idx, u_stride, b, out + b);
+  sample_row<TOP_P ? 1 : 0, CUT ? 1 : 0>(logits + b * V, V, inv_temp, top_k, top_p, cf, u_all, step_idx, u_stride, b, out + b);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -367,10 +641,14 @@ __device__ __forceinline__ void argmax_row(const float* row, int64_t V, int64_t*
 // settings and the uniform u[row * u_stride + n_new[row]].
 // Row-mapped form (row_slot != NULL, uvx_sample_rows): row b takes slot s = row_slot[b]'s settings and the uniform
 // u[s * u_stride + row_idx[b]]; rows with row_idx[b] < 0 are left alone.
+// CUT (uvx_sample_slots_cutoffs / uvx_sample_rows_cutoffs): slot s's cut-offs are cut[4 s .. 4 s + 4) = (min_p, typical_p,
+// epsilon, eta); a row whose cut-offs are all off takes the path of CUT = false.
+template <bool CUT>
 __global__ void __launch_bounds__(1024, 1) sample_slots_kernel(const float* logits, int64_t V, const float* temperature,
                                                                const int32_t* top_k, const float* top_p, const float* u,
                                                                int64_t u_stride, const int32_t* n_new, const int32_t* active,
-                                                               int64_t* out, const int32_t* row_slot, const int32_t* row_idx) {
+                                                               int64_t* out, const int32_t* row_slot, const int32_t* row_idx,
+                                                               const float* cut) {
   pdl_trigger();
   pdl_wait();
   const int64_t b = blockIdx.x;
@@ -383,7 +661,9 @@ __global__ void __launch_bounds__(1024, 1) sample_slots_kernel(const float* logi
     argmax_row(row, V, out + b);
     return;
   }
-  sample_row<2>(row, V, __frcp_rn(t), top_k[s], top_p[s], u + s * u_stride, step, 1, 0, out + b);
+  Cutoffs cf{0.f, 1.f, 0.f, 0.f};
+  if (CUT) cf = {cut[4 * s], cut[4 * s + 1], cut[4 * s + 2], cut[4 * s + 3]};
+  sample_row<2, CUT ? 2 : 0>(row, V, __frcp_rn(t), top_k[s], top_p[s], cf, u + s * u_stride, step, 1, 0, out + b);
 }
 
 // uvx_repetition_penalty's rule on one row (the caller's CTA) with penalty pen over sq[0:n], staging the original scores in
@@ -674,10 +954,12 @@ __global__ void __launch_bounds__(1024, 1) token_logprobs_kernel(const float* lo
 // division, TemperatureLogitsWarper) on the entries keep_threshold keeps (TopKLogitsWarper, TopPLogitsWarper) and -inf on the
 // rest.  Either output may be NULL.
 // kRows (uvx_record_scores_rows): per-row destinations instead, row b at index s = step_idx[b] of [steps, V] buffers.
-template <bool kRows>
+// CUT (the _cutoffs forms): the band of keep_band<2, 1> with cf instead (MinP / Typical / Epsilon / EtaLogitsWarper after TopP).
+template <bool kRows, bool CUT>
 __global__ void __launch_bounds__(1024, 1) record_scores_kernel(const float* logits, int64_t V, float temperature, float inv_temp,
                                                                 int top_k, float top_p, const int32_t* step_idx, int64_t steps,
-                                                                int64_t B, float* __restrict__ scores, float* __restrict__ raw) {
+                                                                int64_t B, float* __restrict__ scores, float* __restrict__ raw,
+                                                                Cutoffs cf) {
   pdl_trigger();
   pdl_wait();
   __shared__ float red[32];
@@ -698,12 +980,22 @@ __global__ void __launch_bounds__(1024, 1) record_scores_kernel(const float* log
     for (int64_t i = threadIdx.x; i < V; i += 1024) scores[o + i] = row[i];
     return;
   }
+  CutoffSmem cs{};
+  if constexpr (CUT) {
+    __shared__ double dred[32];
+    __shared__ unsigned long long zsum;
+    __shared__ uint32_t klo, khi;
+    cs = {dred, &zsum, &klo, &khi};
+  }
   float mx;
-  const uint32_t thr = keep_threshold<2>(row, V, inv_temp, top_k, top_p,
-                                         {red, hist, &sel_prefix, &sel_remaining, mhist, &p_below, &p_target, &p_prefix}, mx);
+  uint32_t hi;
+  const uint32_t thr = keep_band<2, CUT ? 1 : 0>(row, V, inv_temp, top_k, top_p, cf,
+                                                 {red, hist, &sel_prefix, &sel_remaining, mhist, &p_below, &p_target, &p_prefix}, cs,
+                                                 mx, hi);
   for (int64_t i = threadIdx.x; i < V; i += 1024) {
     const float x = row[i];
-    scores[o + i] = f2key(x) >= thr ? x / temperature : -INFINITY;
+    const uint32_t k = f2key(x);
+    scores[o + i] = k >= thr && k <= hi ? x / temperature : -INFINITY;
   }
 }
 
@@ -1401,8 +1693,8 @@ extern "C" int uvx_sample(const float* logits, int64_t B, int64_t V, float tempe
                           const int32_t* step_idx, int64_t u_stride, int64_t* out_idx, uvx_stream_t stream) {
   using namespace uvx;
   UVX_REQUIRE(logits && u && out_idx && B >= 1 && V >= 1 && temperature > 0.f, "uvx_sample: bad arguments");
-  launch_k(sample_kernel<false>, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, 1.0f / temperature, (int)top_k,
-           1.0f, u, step_idx, u_stride, out_idx);
+  launch_k(sample_kernel<false, false>, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, 1.0f / temperature,
+           (int)top_k, 1.0f, u, step_idx, u_stride, out_idx, Cutoffs{0.f, 1.f, 0.f, 0.f});
   return check_launch("sample_kernel");
 }
 
@@ -1413,9 +1705,38 @@ extern "C" int uvx_sample_top_p(const float* logits, int64_t B, int64_t V, float
                   top_p <= 1.f,
               "uvx_sample_top_p: bad arguments");
   if (top_p >= 1.f) return uvx_sample(logits, B, V, temperature, top_k, u, step_idx, u_stride, out_idx, stream);
-  launch_k(sample_kernel<true>, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, 1.0f / temperature, (int)top_k,
-           top_p, u, step_idx, u_stride, out_idx);
+  launch_k(sample_kernel<true, false>, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, 1.0f / temperature,
+           (int)top_k, top_p, u, step_idx, u_stride, out_idx, Cutoffs{0.f, 1.f, 0.f, 0.f});
   return check_launch("sample_kernel_top_p");
+}
+
+namespace uvx {
+// The host's encoding of the four cut-offs (include/uvx.h uvx_cutoffs): min_p in [0, 1], typical_p in (0, 1] (>= 1 off),
+// epsilon / eta in [0, 1) (0 off; HF also gates values outside (0, 1) off).  NaN fails every check.
+static bool cutoffs_valid(const uvx_cutoffs& c) {
+  return c.min_p >= 0.f && c.min_p <= 1.f && c.typical_p > 0.f && c.epsilon >= 0.f && c.epsilon < 1.f && c.eta >= 0.f &&
+         c.eta < 1.f;
+}
+static Cutoffs cutoffs_of(const uvx_cutoffs& c) { return {c.min_p, c.typical_p < 1.f ? c.typical_p : 1.f, c.epsilon, c.eta}; }
+static bool cutoffs_on_host(const uvx_cutoffs& c) { return c.min_p > 0.f || c.typical_p < 1.f || c.epsilon > 0.f || c.eta > 0.f; }
+}  // namespace uvx
+
+extern "C" int uvx_sample_cutoffs(const float* logits, int64_t B, int64_t V, float temperature, int32_t top_k, float top_p,
+                                  uvx_cutoffs cutoffs, const float* u, const int32_t* step_idx, int64_t u_stride, int64_t* out_idx,
+                                  uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(logits && u && out_idx && B >= 1 && V >= 1 && V <= (int64_t)1 << 24 && temperature > 0.f && top_p >= 0.f &&
+                  top_p <= 1.f && cutoffs_valid(cutoffs),
+              "uvx_sample_cutoffs: bad arguments");
+  if (!cutoffs_on_host(cutoffs))
+    return uvx_sample_top_p(logits, B, V, temperature, top_k, top_p, u, step_idx, u_stride, out_idx, stream);
+  if (top_p < 1.f)
+    launch_k(sample_kernel<true, true>, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, 1.0f / temperature,
+             (int)top_k, top_p, u, step_idx, u_stride, out_idx, cutoffs_of(cutoffs));
+  else
+    launch_k(sample_kernel<false, true>, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, 1.0f / temperature,
+             (int)top_k, 1.0f, u, step_idx, u_stride, out_idx, cutoffs_of(cutoffs));
+  return check_launch("sample_kernel_cutoffs");
 }
 
 extern "C" int uvx_sample_slots(const float* logits, int64_t B, int64_t V, const float* temperature, const int32_t* top_k,
@@ -1425,9 +1746,21 @@ extern "C" int uvx_sample_slots(const float* logits, int64_t B, int64_t V, const
   UVX_REQUIRE(logits && temperature && top_k && top_p && u && n_new && active && out_idx && B >= 1 && V >= 1 &&
                   V <= (int64_t)1 << 24 && u_stride >= 0,
               "uvx_sample_slots: bad arguments");
-  launch_k(sample_slots_kernel, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, temperature, top_k, top_p, u,
-           u_stride, n_new, active, out_idx, (const int32_t*)nullptr, (const int32_t*)nullptr);
+  launch_k(sample_slots_kernel<false>, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, temperature, top_k, top_p,
+           u, u_stride, n_new, active, out_idx, (const int32_t*)nullptr, (const int32_t*)nullptr, (const float*)nullptr);
   return check_launch("sample_slots_kernel");
+}
+
+extern "C" int uvx_sample_slots_cutoffs(const float* logits, int64_t B, int64_t V, const float* temperature, const int32_t* top_k,
+                                        const float* top_p, const float* cutoffs, const float* u, int64_t u_stride,
+                                        const int32_t* n_new, const int32_t* active, int64_t* out_idx, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(logits && temperature && top_k && top_p && cutoffs && u && n_new && active && out_idx && B >= 1 && V >= 1 &&
+                  V <= (int64_t)1 << 24 && u_stride >= 0,
+              "uvx_sample_slots_cutoffs: bad arguments");
+  launch_k(sample_slots_kernel<true>, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, temperature, top_k, top_p,
+           u, u_stride, n_new, active, out_idx, (const int32_t*)nullptr, (const int32_t*)nullptr, cutoffs);
+  return check_launch("sample_slots_kernel (cutoffs)");
 }
 
 extern "C" int uvx_repetition_penalty_slots(float* logits, int64_t B, int64_t V, const int64_t* seq, int64_t seq_stride,
@@ -1518,9 +1851,22 @@ extern "C" int uvx_sample_rows(const float* logits, int64_t R, int64_t V, const 
   UVX_REQUIRE(logits && temperature && top_k && top_p && u && active && row_slot && row_idx && out_idx && R >= 1 && R < 65536 &&
                   V >= 1 && V <= (int64_t)1 << 24 && u_stride >= 0,
               "uvx_sample_rows: bad arguments");
-  launch_k(sample_slots_kernel, dim3((unsigned)R), dim3(1024), 0, (cudaStream_t)stream, logits, V, temperature, top_k, top_p, u,
-           u_stride, (const int32_t*)nullptr, active, out_idx, row_slot, row_idx);
+  launch_k(sample_slots_kernel<false>, dim3((unsigned)R), dim3(1024), 0, (cudaStream_t)stream, logits, V, temperature, top_k, top_p,
+           u, u_stride, (const int32_t*)nullptr, active, out_idx, row_slot, row_idx, (const float*)nullptr);
   return check_launch("sample_slots_kernel (rows)");
+}
+
+extern "C" int uvx_sample_rows_cutoffs(const float* logits, int64_t R, int64_t V, const float* temperature, const int32_t* top_k,
+                                       const float* top_p, const float* cutoffs, const float* u, int64_t u_stride,
+                                       const int32_t* active, const int32_t* row_slot, const int32_t* row_idx, int64_t* out_idx,
+                                       uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(logits && temperature && top_k && top_p && cutoffs && u && active && row_slot && row_idx && out_idx && R >= 1 &&
+                  R < 65536 && V >= 1 && V <= (int64_t)1 << 24 && u_stride >= 0,
+              "uvx_sample_rows_cutoffs: bad arguments");
+  launch_k(sample_slots_kernel<true>, dim3((unsigned)R), dim3(1024), 0, (cudaStream_t)stream, logits, V, temperature, top_k, top_p,
+           u, u_stride, (const int32_t*)nullptr, active, out_idx, row_slot, row_idx, cutoffs);
+  return check_launch("sample_slots_kernel (rows, cutoffs)");
 }
 
 extern "C" int uvx_repetition_penalty_rows_map(float* logits, int64_t R, int64_t V, const int64_t* seq, int64_t seq_stride,
@@ -1785,8 +2131,8 @@ extern "C" int uvx_record_scores(const float* logits, int64_t B, int64_t V, floa
                   top_p <= 1.f,
               "uvx_record_scores: bad arguments");
   const float t = temperature > 0.f ? temperature : 0.f;
-  launch_k(record_scores_kernel<false>, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, t, t > 0.f ? 1.0f / t : 0.f,
-           (int)top_k, top_p, step_idx, steps, B, scores, raw);
+  launch_k(record_scores_kernel<false, false>, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, t,
+           t > 0.f ? 1.0f / t : 0.f, (int)top_k, top_p, step_idx, steps, B, scores, raw, Cutoffs{0.f, 1.f, 0.f, 0.f});
   return check_launch("record_scores_kernel");
 }
 
@@ -1797,7 +2143,36 @@ extern "C" int uvx_record_scores_rows(const float* logits, int64_t B, int64_t V,
                   top_p <= 1.f,
               "uvx_record_scores_rows: bad arguments");
   const float t = temperature > 0.f ? temperature : 0.f;
-  launch_k(record_scores_kernel<true>, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, t, t > 0.f ? 1.0f / t : 0.f,
-           (int)top_k, top_p, idx, steps, B, scores, raw);
+  launch_k(record_scores_kernel<true, false>, dim3((unsigned)B), dim3(1024), 0, (cudaStream_t)stream, logits, V, t,
+           t > 0.f ? 1.0f / t : 0.f, (int)top_k, top_p, idx, steps, B, scores, raw, Cutoffs{0.f, 1.f, 0.f, 0.f});
   return check_launch("record_scores_rows_kernel");
+}
+
+// The two scalar record forms with cut-offs (kRows as in record_scores_kernel); no cut-off on is the plain form.
+static int record_scores_cutoffs(bool rows, const float* logits, int64_t B, int64_t V, float temperature, int32_t top_k, float top_p,
+                                 uvx_cutoffs cutoffs, const int32_t* idx, int64_t steps, float* scores, float* raw,
+                                 uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(logits && idx && (scores || raw) && B >= 1 && V >= 1 && V <= (int64_t)1 << 24 && steps >= 1 && top_p >= 0.f &&
+                  top_p <= 1.f && cutoffs_valid(cutoffs),
+              rows ? "uvx_record_scores_rows_cutoffs: bad arguments" : "uvx_record_scores_cutoffs: bad arguments");
+  const float t = temperature > 0.f ? temperature : 0.f;
+  if (!cutoffs_on_host(cutoffs) || !(t > 0.f))
+    return rows ? uvx_record_scores_rows(logits, B, V, temperature, top_k, top_p, idx, steps, scores, raw, stream)
+                : uvx_record_scores(logits, B, V, temperature, top_k, top_p, idx, steps, scores, raw, stream);
+  launch_k(rows ? record_scores_kernel<true, true> : record_scores_kernel<false, true>, dim3((unsigned)B), dim3(1024), 0,
+           (cudaStream_t)stream, logits, V, t, 1.0f / t, (int)top_k, top_p, idx, steps, B, scores, raw, cutoffs_of(cutoffs));
+  return check_launch(rows ? "record_scores_rows_kernel (cutoffs)" : "record_scores_kernel (cutoffs)");
+}
+
+extern "C" int uvx_record_scores_cutoffs(const float* logits, int64_t B, int64_t V, float temperature, int32_t top_k, float top_p,
+                                         uvx_cutoffs cutoffs, const int32_t* step_idx, int64_t steps, float* scores, float* raw,
+                                         uvx_stream_t stream) {
+  return record_scores_cutoffs(false, logits, B, V, temperature, top_k, top_p, cutoffs, step_idx, steps, scores, raw, stream);
+}
+
+extern "C" int uvx_record_scores_rows_cutoffs(const float* logits, int64_t B, int64_t V, float temperature, int32_t top_k,
+                                              float top_p, uvx_cutoffs cutoffs, const int32_t* idx, int64_t steps, float* scores,
+                                              float* raw, uvx_stream_t stream) {
+  return record_scores_cutoffs(true, logits, B, V, temperature, top_k, top_p, cutoffs, idx, steps, scores, raw, stream);
 }

@@ -486,7 +486,7 @@ class DecodeEngine(_Decoder):
                  eos_token_ids=None, pad_token_id: int = 0, temperature: float = 0.0, top_k: int = 0,
                  repetition_penalty: float = 1.0, generator: Optional[torch.Generator] = None, top_p: Optional[float] = None,
                  output_scores: bool = False, output_logits: bool = False, max_new_tokens: Optional[int] = None,
-                 constraints=None):
+                 constraints=None, cutoffs=None):
         """``output_scores`` / ``output_logits``: every pick (the first one, in ``begin``, is step 0) also records HF's processed
         scores / the raw logits of its rows into ``scores`` / ``raw_logits`` [max_new_tokens, batch, V] fp32, at the device
         step counter (``uvx_record_scores``).  That is one [batch, V] fp32 tensor per generated token, which is what HF's
@@ -494,7 +494,10 @@ class DecodeEngine(_Decoder):
         unchanged.
 
         ``constraints`` (``constraints.LogitsConstraints``): every pick first runs ``uvx_logits_constraints`` over the rows'
-        sequences, before the repetition penalty.  None (the default): nothing is allocated and the step is unchanged."""
+        sequences, before the repetition penalty.  None (the default): nothing is allocated and the step is unchanged.
+
+        ``cutoffs``: (min_p, typical_p, epsilon, eta) after top-p (``uvx_sample_cutoffs`` / ``uvx_record_scores_cutoffs``), off
+        encoded as (0, 1, 0, 0).  With none on (or None) the step launches exactly the kernels it launches without them."""
         super().__init__(model, batch, _RowKV(cache if cache is not None else model.new_cache(batch, max_len)), eos_token_ids,
                          pad_token_id, use_graph)
         dev = model.device
@@ -520,6 +523,7 @@ class DecodeEngine(_Decoder):
             self.scores = torch.empty(shape, dtype=torch.float32, device=dev) if output_scores else None
             self.raw_logits = torch.empty(shape, dtype=torch.float32, device=dev) if output_logits else None
         self.constraints = None if constraints is None else constraints.device_tables(dev)
+        self.cutoffs = tuple(float(v) for v in cutoffs) if ops.cutoffs_on(cutoffs) else None
 
     # -- state ---------------------------------------------------------------------------------------------
     def begin(self, input_ids: torch.Tensor, first_logits: torch.Tensor, kv_start: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -560,10 +564,10 @@ class DecodeEngine(_Decoder):
         if self.penalty != 1.0:
             ops.repetition_penalty_(logits, self.seq, self.cur_len, self.penalty, self.scratch)
         if self.scores is not None or (self.raw_logits is not None and not raw_first):
-            ops.record_scores(logits, *rec, scores=self.scores, raw=None if raw_first else self.raw_logits)
+            ops.record_scores(logits, *rec, scores=self.scores, raw=None if raw_first else self.raw_logits, cutoffs=self.cutoffs)
         tok = self.token.view(-1)
         if self.temperature > 0:
-            ops.sample(logits, self.temperature, self.top_k, self.u, self.step_idx, out=tok, top_p=self.top_p)
+            ops.sample(logits, self.temperature, self.top_k, self.u, self.step_idx, out=tok, top_p=self.top_p, cutoffs=self.cutoffs)
         else:
             ops.argmax(logits, out=tok)
         ops.token_finish(tok, self.done, self.eos, self.pad_id, self.seq, self.cur_len, self.step_idx,
@@ -610,10 +614,11 @@ class LookupDecodeEngine(_Decoder):
                  use_graph: bool = True, cache=None, eos_token_ids=None, pad_token_id: int = 0, temperature: float = 0.0,
                  top_k: int = 0, top_p: Optional[float] = None, repetition_penalty: float = 1.0,
                  generator: Optional[torch.Generator] = None, output_scores: bool = False, output_logits: bool = False,
-                 uniforms: Optional[int] = None, constraints=None):
+                 uniforms: Optional[int] = None, constraints=None, cutoffs=None):
         """``uniforms``: how many uniforms to draw when sampling, default S + max_new_tokens + 1 - the count ``DecodeEngine``
         draws (its cache capacity + 1) for the same call, so that a seeded ``generator`` gives the same tokens.
-        ``constraints``: as ``DecodeEngine``'s, row i over the sequence up to its position (``uvx_logits_constraints_rows``)."""
+        ``constraints``: as ``DecodeEngine``'s, row i over the sequence up to its position (``uvx_logits_constraints_rows``).
+        ``cutoffs``: as ``DecodeEngine``'s, on every row."""
         k, n, S, N = int(num_tokens), int(ngram), int(prompt_len), int(max_new_tokens)
         if not 1 <= k <= ops.LOOKUP_MAX_K:
             raise ValueError(f"prompt_lookup_num_tokens must be in [1, {ops.LOOKUP_MAX_K}], got {num_tokens}")
@@ -656,6 +661,7 @@ class LookupDecodeEngine(_Decoder):
         self.scores = torch.empty(N, 1, V, dtype=torch.float32, device=dev) if output_scores else None
         self.raw_logits = torch.empty(N, 1, V, dtype=torch.float32, device=dev) if output_logits else None
         self.constraints = None if constraints is None else constraints.device_tables(dev)
+        self.cutoffs = tuple(float(v) for v in cutoffs) if ops.cutoffs_on(cutoffs) else None
 
     def begin(self, input_ids: torch.Tensor, first_logits: torch.Tensor) -> None:
         """After the prompt input_ids [1, S] has been prefilled into the cache: seeds the sequence and the counters and picks the
@@ -687,10 +693,10 @@ class LookupDecodeEngine(_Decoder):
             ops.repetition_penalty_rows_(logits, self.seq.view(1, -1).expand(R, -1), self.pen_len[:R], self.penalty,
                                          self.scratch[:R])
         if scores is not None or (raw is not None and not raw_first):
-            ops.record_scores_rows(logits, *rec, scores=scores, raw=None if raw_first else raw)
+            ops.record_scores_rows(logits, *rec, scores=scores, raw=None if raw_first else raw, cutoffs=self.cutoffs)
         pick = self.pick[:R]
         if self.temperature > 0:
-            ops.sample(logits, self.temperature, self.top_k, self.u, self.n_new, out=pick, top_p=self.top_p)
+            ops.sample(logits, self.temperature, self.top_k, self.u, self.n_new, out=pick, top_p=self.top_p, cutoffs=self.cutoffs)
         else:
             ops.argmax(logits, out=pick)
         ops.lookup_accept(pick, self.token.view(-1)[:R], self.n_draft, self.eos, self.seq, self.cur_len, self.n_new, self.max_new,
@@ -832,7 +838,7 @@ class BeamDecodeEngine(DecodeEngine):
 
 class SlotDecodeEngine(_Decoder):
     """Continuous batching: ``slots`` decode rows that each carry their own request.  The step is the shared step loop over
-    all rows followed by three per-row kernels (``uvx_repetition_penalty_slots``, ``uvx_sample_slots``, ``uvx_slot_finish``);
+    all rows followed by three per-row kernels (``uvx_repetition_penalty_slots``, ``uvx_sample_slots_cutoffs``, ``uvx_slot_finish``);
     every per-request value - positions, lengths, budget, active / done flags, sampling settings, the uniforms - lives in a
     device array [slots], so the step is captured once per engine and admission and retirement only write into those arrays
     between replays.
@@ -909,6 +915,7 @@ class SlotDecodeEngine(_Decoder):
         self.temps = torch.zeros(slots, **f32)
         self.top_ks = torch.zeros(slots, **i32)
         self.top_ps = torch.ones(slots, **f32)
+        self.cutoffs = torch.tensor([ops.CUTOFFS_OFF] * slots, **f32)   # per slot (min_p, typical_p, epsilon, eta), off = (0, 1, 0, 0)
         self.penalties = torch.ones(slots, **f32)
         self.u = torch.zeros(slots, self.max_len + 1, **f32)
         self.scratch = torch.empty(slots, self.max_len + 1, **f32)
@@ -1004,7 +1011,7 @@ class SlotDecodeEngine(_Decoder):
             ops.logits_constraints_rows_map_(logits, self.seq, self.active, self._lk_slot, self._lk_pen, self._lk_idx, self.ck)
         ops.repetition_penalty_rows_map_(logits, self.seq, self.penalties, self.active, self._lk_slot, self._lk_pen, self._lk_idx,
                                          self._lk_scratch[:R])
-        ops.sample_rows(logits, self.temps, self.top_ks, self.top_ps, self.u, self.active, *rows, self._lk_pick)
+        ops.sample_rows_cutoffs(logits, self.temps, self.top_ks, self.top_ps, self.cutoffs, self.u, self.active, *rows, self._lk_pick)
         if self.max_logprobs:       # at n_new + i, before the accept advances n_new; rows past the drafts (idx -1) record nothing
             ops.token_logprobs_rows(self._lk_raw, self._lk_pick, self.n_top, *rows, self.lp_token, self.lp_ids, self.lp_top)
         ops.lookup_accept_slots(self._lk_pick, self._lk_tok.view(-1), self.n_draft, self.K, self.eos, self.seq, self.token.view(-1),
@@ -1019,7 +1026,8 @@ class SlotDecodeEngine(_Decoder):
         if self.ck is not None:
             ops.logits_constraints_slots_(logits, self.seq[r], self.cur_len[r], self.active[r], tuple(t[r] for t in self.ck))
         ops.repetition_penalty_slots_(logits, self.seq[r], self.cur_len[r], self.penalties[r], self.active[r], self.scratch[r])
-        ops.sample_slots(logits, self.temps[r], self.top_ks[r], self.top_ps[r], self.u[r], self.n_new[r], self.active[r], tok)
+        ops.sample_slots_cutoffs(logits, self.temps[r], self.top_ks[r], self.top_ps[r], self.cutoffs[r], self.u[r], self.n_new[r],
+                                 self.active[r], tok)
         if self.max_logprobs:       # at n_new, before the finish kernel advances it
             ops.token_logprobs(raw, tok, self.n_top[r], self.n_new[r], self.lp_token[r], self.lp_ids[r], self.lp_top[r])
         ops.slot_finish(tok, self.done[r], self.eos, self.seq[r], self.cur_len[r], self.n_new[r], self.max_new[r], self.active[r],
@@ -1085,7 +1093,7 @@ class SlotDecodeEngine(_Decoder):
 
     def admit(self, slot: int, input_ids: torch.Tensor, max_new_tokens: int, temperature: float = 0.0, top_k: int = 0,
               top_p: float = 1.0, repetition_penalty: float = 1.0, u: Optional[torch.Tensor] = None, past: int = 0,
-              pages=None, logprobs: Optional[int] = None, lookup: Optional[tuple] = None, constraints=None,
+              pages=None, logprobs: Optional[int] = None, lookup: Optional[tuple] = None, constraints=None, cutoffs=None,
               **features) -> torch.Tensor:
         """Prefills one request (``input_ids`` [1, S] plus the processor's audio features, passed to ``model.forward``) at B = 1
         into cache row ``slot``, sets the slot's state and picks its first token from the prefill logits with the slot kernels.
@@ -1109,7 +1117,10 @@ class SlotDecodeEngine(_Decoder):
         to n >= 1 tokens; None or k = 0 drafts nothing.
 
         ``constraints`` (engines with ``max_constraint_tokens`` = N): the request's ``constraints.LogitsConstraints`` (built
-        with its whole prompt's length), at most N ids; None: no constraints."""
+        with its whole prompt's length), at most N ids; None: no constraints.
+
+        ``cutoffs``: the request's (min_p, typical_p, epsilon, eta), as ``generate()`` checks them, off = (0, 1, 0, 0) (None:
+        all off).  Every pick reads them from ``cutoffs`` [slots, 4] (``uvx_sample_slots_cutoffs`` / ``_rows_cutoffs``)."""
         n_top = self.check_logprobs(logprobs)
         ck_rows = self.check_constraints(constraints)
         lk, ln = (0, 2) if lookup is None else (int(lookup[0]), int(lookup[1]))
@@ -1163,6 +1174,7 @@ class SlotDecodeEngine(_Decoder):
         self.temps[j] = float(temperature) if temperature > 0 else 0.0
         self.top_ks[j] = int(top_k or 0)
         self.top_ps[j] = float(top_p)
+        self.cutoffs[j] = torch.tensor(ops.CUTOFFS_OFF if cutoffs is None else [float(v) for v in cutoffs])
         self.penalties[j] = float(repetition_penalty or 1.0)
         if u is not None:
             w = min(u.numel(), self.max_len + 1)

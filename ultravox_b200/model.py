@@ -899,7 +899,9 @@ class UltravoxModel(nn.Module):
                  output_logits: bool = False, prompt_lookup_num_tokens: Optional[int] = None,
                  max_matching_ngram_size: Optional[int] = None, no_repeat_ngram_size: Optional[int] = None,
                  bad_words_ids=None, sequence_bias=None, min_length: Optional[int] = None, min_new_tokens: Optional[int] = None,
-                 suppress_tokens=None, begin_suppress_tokens=None, **kwargs):
+                 suppress_tokens=None, begin_suppress_tokens=None, min_p: Optional[float] = None,
+                 typical_p: Optional[float] = None, epsilon_cutoff: Optional[float] = None, eta_cutoff: Optional[float] = None,
+                 **kwargs):
         """``GenerationMixin.generate`` for this model (ref :398-426; arguments as ``LocalInference._generate`` passes them, ref
         infer.py:309-342).  Returns prompt ids followed by the new tokens.
 
@@ -910,6 +912,14 @@ class UltravoxModel(nn.Module):
         set of largest logits whose probability exceeds ``top_p`` (always the largest one, so ``top_p=0`` is greedy; a tie
         group at the cut is kept whole).  ``top_p`` must lie in [0, 1] (``ValueError`` otherwise); it is ignored when not
         sampling, and ``None`` or 1.0 means no nucleus filter.
+        Sampling cut-offs after top-p, in HF's order (``MinPLogitsWarper``, ``TypicalLogitsWarper``, ``EpsilonLogitsWarper``,
+        ``EtaLogitsWarper``), each on the survivors of the one before, with p = softmax(logits / temperature) over them and H
+        their entropy.  ``min_p``: keep p >= min_p * max p (``ValueError`` unless in [0, 1]).  ``typical_p``: keep the tokens
+        whose |-log p - H| is smallest until their probability reaches ``typical_p`` (``ValueError`` for <= 0; >= 1 is off);
+        this cut can drop the most likely token.  ``epsilon_cutoff``: keep p >= epsilon.  ``eta_cutoff``: keep p >=
+        min(eta, sqrt(eta) exp(-H)).  The last two keep the most likely survivor and are off outside (0, 1), as in HF.  A tie
+        group (equal logits) is kept or dropped whole at every cut.  They are ignored when not sampling; ``None`` is off.  The
+        sampler kernel runs them (``uvx_sample_cutoffs``), one to six extra passes over the row per cut-off that is on.
         ``past_key_values``: conversation KV reuse (ref infer.py:126-148): the cache already holds the first
         ``past_key_values.length`` positions of ``input_ids`` (earlier turns incl. the reply), so only the new suffix is
         embedded, spliced and prefilled; ``return_dict_in_generate=True`` hands the cache back for the next turn.
@@ -924,7 +934,7 @@ class UltravoxModel(nn.Module):
         ``logits`` of the result are tuples with one [B, V] fp32 tensor per new token, as HF's ``_sample`` returns them:
         ``logits[t]`` the raw LM-head output of step t, ``scores[t]`` the distribution the token was picked from - the repetition
         penalty, then (when sampling) ``TemperatureLogitsWarper`` (x / temperature), ``TopKLogitsWarper`` and
-        ``TopPLogitsWarper`` (-inf outside the kept set).  The step records them on the device into [max_new_tokens, B, V]
+        ``TopPLogitsWarper`` and the cut-offs above (-inf outside the kept set).  The step records them on the device into [max_new_tokens, B, V]
         buffers (``uvx_record_scores``), the memory HF holds for them as well; rows that have finished keep getting entries.
         ``compute_transition_scores`` turns them into per-token scores.
 
@@ -993,7 +1003,10 @@ class UltravoxModel(nn.Module):
                 raise ValueError(f"early_stopping must be True, False or 'never', got {early_stopping!r}")
         if top_p is not None and not 0.0 <= float(top_p) <= 1.0:       # NaN fails too
             raise ValueError(f"`top_p` has to be a float in [0, 1], but is {top_p}")
+        cutoffs = ops.sampling_cutoffs(min_p, typical_p, epsilon_cutoff, eta_cutoff)
         sampling = bool(do_sample) and (temperature is None or float(temperature) > 0)
+        if not sampling:
+            cutoffs = None
         temp = (1.0 if temperature is None else float(temperature)) if sampling else 0.0
         k_top = (50 if top_k is None else int(top_k)) if sampling else 0
         p_top = float(top_p) if sampling and top_p is not None else 1.0
@@ -1058,11 +1071,12 @@ class UltravoxModel(nn.Module):
             return self._lookup_decode(input_ids, out.logits.view(1, -1), cache, k_look, n_look, max_new_tokens, eos, pad_id,
                                        temp, k_top, p_top, repetition_penalty or 1.0, generator, want_scores, want_logits, streamer,
                                        use_graph, (S + max_new_tokens if past_key_values is None else plain_cap) + 1,
-                                       return_dict_in_generate, cons)
+                                       return_dict_in_generate, cons, cutoffs)
         eng = DecodeEngine(self, B, cache.capacity, use_graph=use_graph, cache=cache, eos_token_ids=eos, pad_token_id=pad_id,
                            temperature=temp, top_k=k_top, top_p=p_top, repetition_penalty=repetition_penalty or 1.0,
                            generator=generator, output_scores=want_scores, output_logits=want_logits,
-                           max_new_tokens=max_new_tokens if want_scores or want_logits else None, constraints=cons)
+                           max_new_tokens=max_new_tokens if want_scores or want_logits else None, constraints=cons,
+                           cutoffs=cutoffs)
         if streamer is not None:
             streamer.put(input_ids)
         tok = eng.begin(input_ids, out.logits.view(B, -1), kv_start)
@@ -1115,14 +1129,14 @@ class UltravoxModel(nn.Module):
     def _lookup_decode(self, input_ids: torch.Tensor, first_logits: torch.Tensor, cache: KVCache, k: int, n: int,
                        max_new_tokens: int, eos, pad_id: int, temp: float, k_top: int, p_top: float, penalty: float, generator,
                        want_scores: bool, want_logits: bool, streamer, use_graph: bool, uniforms: int, return_dict: bool,
-                       constraints=None):
+                       constraints=None, cutoffs=None):
         """``generate``'s prompt-lookup loop after the prefill of ``input_ids`` [1, S] into ``cache``."""
         from .engine import LookupDecodeEngine
         S = int(input_ids.shape[1])
         eng = LookupDecodeEngine(self, S, max_new_tokens, k, n, use_graph=use_graph, cache=cache, eos_token_ids=eos,
                                  pad_token_id=pad_id, temperature=temp, top_k=k_top, top_p=p_top, repetition_penalty=penalty,
                                  generator=generator, output_scores=want_scores, output_logits=want_logits, uniforms=uniforms,
-                                 constraints=constraints)
+                                 constraints=constraints, cutoffs=cutoffs)
         if streamer is not None:
             streamer.put(input_ids)
         eng.begin(input_ids, first_logits)

@@ -961,16 +961,54 @@ def repetition_penalty_(logits: torch.Tensor, seq: torch.Tensor, cur_len: torch.
     return logits
 
 
+CUTOFFS_OFF = (0.0, 1.0, 0.0, 0.0)   # (min_p, typical_p, epsilon, eta) with every cut-off off: uvx_cutoffs' encoding
+
+
+def sampling_cutoffs(min_p=None, typical_p=None, epsilon_cutoff=None, eta_cutoff=None) -> tuple:
+    """``generate()``'s four cut-off arguments -> the (min_p, typical_p, epsilon, eta) tuple the kernels read, off = (0, 1, 0, 0).
+    The checks of transformers' warper constructors: ``min_p`` outside [0, 1] and ``typical_p`` <= 0 raise ValueError (NaN
+    too); ``typical_p`` >= 1 is off, and ``epsilon_cutoff`` / ``eta_cutoff`` outside (0, 1) are off, as HF only adds those
+    warpers for such values."""
+    mp, tp, eps, eta = CUTOFFS_OFF
+    if min_p is not None:
+        mp = float(min_p)
+        if not 0.0 <= mp <= 1.0:                                   # NaN fails too
+            raise ValueError(f"`min_p` has to be a float in the [0, 1] interval, but is {min_p}")
+    if typical_p is not None:
+        tp = float(typical_p)
+        if not tp > 0.0:
+            raise ValueError(f"`typical_p` has to be a float > 0, but is {typical_p}")
+        tp = min(tp, 1.0)
+    if epsilon_cutoff is not None and 0.0 < float(epsilon_cutoff) < 1.0:
+        eps = float(epsilon_cutoff)
+    if eta_cutoff is not None and 0.0 < float(eta_cutoff) < 1.0:
+        eta = float(eta_cutoff)
+    return (mp, tp, eps, eta)
+
+
+def cutoffs_on(cutoffs) -> bool:
+    """Whether a (min_p, typical_p, epsilon, eta) tuple has a cut-off on (None: off)."""
+    if cutoffs is None:
+        return False
+    mp, tp, eps, eta = (float(v) for v in cutoffs)
+    return mp > 0.0 or tp < 1.0 or eps > 0.0 or eta > 0.0
+
+
 def sample(logits: torch.Tensor, temperature: float, top_k: int, u: torch.Tensor, step_idx: Optional[torch.Tensor] = None,
-           out: Optional[torch.Tensor] = None, top_p: float = 1.0) -> torch.Tensor:
+           out: Optional[torch.Tensor] = None, top_p: float = 1.0, cutoffs=None) -> torch.Tensor:
     """logits [B, V] fp32, u [steps, B] (or [B]) uniforms in [0, 1) -> sampled ids [B] int64.  ``top_p < 1`` adds nucleus
-    filtering after the top-k cut (``uvx_sample_top_p``); ``top_p >= 1`` is plain ``uvx_sample``."""
+    filtering after the top-k cut (``uvx_sample_top_p``); ``top_p >= 1`` is plain ``uvx_sample``.  ``cutoffs`` =
+    (min_p, typical_p, epsilon, eta) with one of them on adds those cuts after top-p (``uvx_sample_cutoffs``)."""
     _cuda(logits, torch.float32, "logits"), _cuda(u, torch.float32, "u")
     B, V = logits.shape
     if out is None:
         out = torch.empty(B, dtype=torch.int64, device=logits.device)
     u_stride = u.stride(0) if u.dim() == 2 else 0
-    if top_p >= 1.0:
+    if cutoffs_on(cutoffs):
+        check(lib().uvx_sample_cutoffs(logits.data_ptr(), B, V, float(temperature), int(top_k or 0), float(top_p),
+                                       _lib.Cutoffs(*(float(v) for v in cutoffs)), u.data_ptr(), _p(step_idx), u_stride,
+                                       out.data_ptr(), _stream()), "uvx_sample_cutoffs")
+    elif top_p >= 1.0:
         check(lib().uvx_sample(logits.data_ptr(), B, V, float(temperature), int(top_k or 0), u.data_ptr(), _p(step_idx), u_stride,
                                out.data_ptr(), _stream()), "uvx_sample")
     else:
@@ -1019,6 +1057,31 @@ def sample_slots(logits: torch.Tensor, temperature: torch.Tensor, top_k: torch.T
     _seq_rows(u, torch.float32, B, "u")
     check(lib().uvx_sample_slots(logits.data_ptr(), B, V, temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), u.data_ptr(),
                                  u.stride(0), n_new.data_ptr(), active.data_ptr(), out.data_ptr(), _stream()), "uvx_sample_slots")
+    return out
+
+
+def _cutoff_rows(cutoffs: torch.Tensor, S: int) -> torch.Tensor:
+    """A contiguous per-slot cut-off array [S, 4] fp32 on the device: (min_p, typical_p, epsilon, eta), off = (0, 1, 0, 0)."""
+    _cuda(cutoffs, torch.float32, "cutoffs")
+    if cutoffs.shape != (S, 4) or not cutoffs.is_contiguous():
+        raise ValueError(f"cutoffs must be a contiguous [{S}, 4] tensor, got {tuple(cutoffs.shape)}")
+    return cutoffs
+
+
+def sample_slots_cutoffs(logits: torch.Tensor, temperature: torch.Tensor, top_k: torch.Tensor, top_p: torch.Tensor,
+                         cutoffs: torch.Tensor, u: torch.Tensor, n_new: torch.Tensor, active: torch.Tensor,
+                         out: torch.Tensor) -> torch.Tensor:
+    """``uvx_sample_slots_cutoffs``: ``sample_slots`` with row b's cut-offs cutoffs[b] ([B, 4] fp32, off = (0, 1, 0, 0))."""
+    _cuda(logits, torch.float32, "logits")
+    if logits.dim() != 2 or not logits.is_contiguous():
+        raise ValueError("logits must be a contiguous [B, V] tensor")
+    B, V = logits.shape
+    _rows(temperature, torch.float32, B, "temperature"), _rows(top_k, torch.int32, B, "top_k"), _rows(top_p, torch.float32, B, "top_p")
+    _rows(n_new, torch.int32, B, "n_new"), _rows(active, torch.int32, B, "active"), _rows(out, torch.int64, B, "out")
+    _seq_rows(u, torch.float32, B, "u"), _cutoff_rows(cutoffs, B)
+    check(lib().uvx_sample_slots_cutoffs(logits.data_ptr(), B, V, temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(),
+                                         cutoffs.data_ptr(), u.data_ptr(), u.stride(0), n_new.data_ptr(), active.data_ptr(),
+                                         out.data_ptr(), _stream()), "uvx_sample_slots_cutoffs")
     return out
 
 
@@ -1090,10 +1153,10 @@ def token_logprobs(logits: torch.Tensor, tok: torch.Tensor, n_top: torch.Tensor,
 
 
 def record_scores(logits: torch.Tensor, temperature: float, top_k: int, top_p: float, step_idx: torch.Tensor,
-                  scores: Optional[torch.Tensor] = None, raw: Optional[torch.Tensor] = None) -> None:
+                  scores: Optional[torch.Tensor] = None, raw: Optional[torch.Tensor] = None, cutoffs=None) -> None:
     """``uvx_record_scores``: logits [B, V] fp32 -> at step s = step_idx[0] of the [steps, B, V] fp32 buffers, raw[s] = the
     logits as given and scores[s] = HF's processed scores (temperature <= 0: the logits; else x / temperature on the entries the
-    sampler keeps with top_k / top_p, -inf elsewhere)."""
+    sampler keeps with top_k / top_p and, when on, the (min_p, typical_p, epsilon, eta) ``cutoffs``; -inf elsewhere)."""
     _cuda(logits, torch.float32, "logits"), _cuda(step_idx, torch.int32, "step_idx")
     if logits.dim() != 2 or not logits.is_contiguous():
         raise ValueError("logits must be a contiguous [B, V] tensor")
@@ -1107,14 +1170,20 @@ def record_scores(logits: torch.Tensor, temperature: float, top_k: int, top_p: f
             steps = t.shape[0]
     if steps is None:
         raise ValueError("record_scores needs scores, raw or both")
+    if cutoffs_on(cutoffs):
+        check(lib().uvx_record_scores_cutoffs(logits.data_ptr(), B, V, float(temperature), int(top_k or 0), float(top_p),
+                                              _lib.Cutoffs(*(float(v) for v in cutoffs)), step_idx.data_ptr(), steps, _p(scores),
+                                              _p(raw), _stream()), "uvx_record_scores_cutoffs")
+        return
     check(lib().uvx_record_scores(logits.data_ptr(), B, V, float(temperature), int(top_k or 0), float(top_p), step_idx.data_ptr(),
                                   steps, _p(scores), _p(raw), _stream()), "uvx_record_scores")
 
 
 def record_scores_rows(logits: torch.Tensor, temperature: float, top_k: int, top_p: float, idx: torch.Tensor,
-                       scores: Optional[torch.Tensor] = None, raw: Optional[torch.Tensor] = None) -> None:
+                       scores: Optional[torch.Tensor] = None, raw: Optional[torch.Tensor] = None, cutoffs=None) -> None:
     """``uvx_record_scores_rows``: ``record_scores`` with per-row destinations - row b of logits [B, V] fp32 goes to index
-    s = idx[b] ([B] int32) of the [steps, V] fp32 buffers (nothing when s is outside [0, steps))."""
+    s = idx[b] ([B] int32) of the [steps, V] fp32 buffers (nothing when s is outside [0, steps)).  ``cutoffs`` as in
+    ``record_scores`` (``uvx_record_scores_rows_cutoffs``)."""
     _cuda(logits, torch.float32, "logits")
     if logits.dim() != 2 or not logits.is_contiguous():
         raise ValueError("logits must be a contiguous [B, V] tensor")
@@ -1129,6 +1198,11 @@ def record_scores_rows(logits: torch.Tensor, temperature: float, top_k: int, top
             steps = t.shape[0]
     if steps is None:
         raise ValueError("record_scores_rows needs scores, raw or both")
+    if cutoffs_on(cutoffs):
+        check(lib().uvx_record_scores_rows_cutoffs(logits.data_ptr(), B, V, float(temperature), int(top_k or 0), float(top_p),
+                                                   _lib.Cutoffs(*(float(v) for v in cutoffs)), idx.data_ptr(), steps, _p(scores),
+                                                   _p(raw), _stream()), "uvx_record_scores_rows_cutoffs")
+        return
     check(lib().uvx_record_scores_rows(logits.data_ptr(), B, V, float(temperature), int(top_k or 0), float(top_p), idx.data_ptr(),
                                        steps, _p(scores), _p(raw), _stream()), "uvx_record_scores_rows")
 
@@ -1363,6 +1437,24 @@ def sample_rows(logits: torch.Tensor, temperature: torch.Tensor, top_k: torch.Te
     check(lib().uvx_sample_rows(logits.data_ptr(), R, V, temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), u.data_ptr(),
                                 u.stride(0), active.data_ptr(), row_slot.data_ptr(), row_idx.data_ptr(), out.data_ptr(), _stream()),
           "uvx_sample_rows")
+    return out
+
+
+def sample_rows_cutoffs(logits: torch.Tensor, temperature: torch.Tensor, top_k: torch.Tensor, top_p: torch.Tensor,
+                        cutoffs: torch.Tensor, u: torch.Tensor, active: torch.Tensor, row_slot: torch.Tensor, row_idx: torch.Tensor,
+                        out: torch.Tensor) -> torch.Tensor:
+    """``uvx_sample_rows_cutoffs``: ``sample_rows`` with slot row_slot[r]'s cut-offs (cutoffs [slots, 4] fp32)."""
+    _cuda(logits, torch.float32, "logits")
+    if logits.dim() != 2 or not logits.is_contiguous():
+        raise ValueError("logits must be a contiguous [R, V] tensor")
+    R, V = logits.shape
+    S = temperature.shape[0]
+    _rows(temperature, torch.float32, S, "temperature"), _rows(top_k, torch.int32, S, "top_k"), _rows(top_p, torch.float32, S, "top_p")
+    _rows(active, torch.int32, S, "active"), _seq_rows(u, torch.float32, S, "u"), _cutoff_rows(cutoffs, S)
+    _rows(row_slot, torch.int32, R, "row_slot"), _rows(row_idx, torch.int32, R, "row_idx"), _rows(out, torch.int64, R, "out")
+    check(lib().uvx_sample_rows_cutoffs(logits.data_ptr(), R, V, temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(),
+                                        cutoffs.data_ptr(), u.data_ptr(), u.stride(0), active.data_ptr(), row_slot.data_ptr(),
+                                        row_idx.data_ptr(), out.data_ptr(), _stream()), "uvx_sample_rows_cutoffs")
     return out
 
 

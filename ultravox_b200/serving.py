@@ -291,6 +291,7 @@ class _Request:
     logprobs: Optional[int] = None     # alternatives per token asked for (None: no log-probs)
     lookup: Optional[tuple] = None     # (k, n) of prompt lookup (None: the engine has none)
     constraints: Optional[LogitsConstraints] = None
+    cutoffs: Optional[tuple] = None    # (min_p, typical_p, epsilon, eta) when sampled with one on
 
 
 class SlotScheduler:
@@ -488,7 +489,9 @@ class SlotScheduler:
                logprobs: Optional[int] = None, prompt_lookup_num_tokens: Optional[int] = None,
                max_matching_ngram_size: Optional[int] = None, no_repeat_ngram_size: Optional[int] = None,
                min_new_tokens: Optional[int] = None, min_length: Optional[int] = None, bad_words_ids=None, sequence_bias=None,
-               suppress_tokens=None, begin_suppress_tokens=None) -> int:
+               suppress_tokens=None, begin_suppress_tokens=None, min_p: Optional[float] = None,
+               typical_p: Optional[float] = None, epsilon_cutoff: Optional[float] = None,
+               eta_cutoff: Optional[float] = None) -> int:
         """Queues one request: ``features`` is the processor's output for it (``input_ids`` [1, S] and, for audio, its mel or
         waveform fields).  Arguments and defaults are ``generate()``'s: greedy unless ``do_sample``; sampling defaults to
         temperature 1 and top_k 50; ``top_p`` must lie in [0, 1].  A sampled request draws its uniforms here, as ``generate()``
@@ -507,7 +510,10 @@ class SlotScheduler:
         ``no_repeat_ngram_size``, ``min_new_tokens``, ``min_length``, ``bad_words_ids``, ``sequence_bias``, ``suppress_tokens``,
         ``begin_suppress_tokens`` (a scheduler built with ``max_constraint_tokens``): ``generate()``'s token constraints and
         checks.  ValueError when the scheduler has no constraints or the request's table needs more than
-        ``max_constraint_tokens`` ids."""
+        ``max_constraint_tokens`` ids.
+
+        ``min_p``, ``typical_p``, ``epsilon_cutoff``, ``eta_cutoff``: ``generate()``'s sampling cut-offs and checks, held per
+        slot and read by the captured step; ignored when not sampling."""
         if logprobs is not None:
             self.engine.check_logprobs(logprobs)
         lookup = self._check_lookup(prompt_lookup_num_tokens, max_matching_ngram_size)
@@ -515,6 +521,7 @@ class SlotScheduler:
             raise NotImplementedError("beam search is not built into the slot engine; use generate(num_beams=...)")
         if top_p is not None and not 0.0 <= float(top_p) <= 1.0:       # NaN fails too
             raise ValueError(f"`top_p` has to be a float in [0, 1], but is {top_p}")
+        cutoffs = ops.sampling_cutoffs(min_p, typical_p, epsilon_cutoff, eta_cutoff)
         ids = features.get("input_ids")
         if ids is None or ids.dim() != 2 or ids.shape[0] != 1:
             raise ValueError("submit() takes one request: features['input_ids'] must be [1, S]")
@@ -563,7 +570,7 @@ class SlotScheduler:
         self._next_id += 1
         self._queue.append(_Request(rid, ids, feats, n, temp, k_top, p_top, float(repetition_penalty or 1.0), u, session,
                                     prefix, logprobs=None if logprobs is None else int(logprobs), lookup=lookup,
-                                    constraints=cons))
+                                    constraints=cons, cutoffs=cutoffs if sampling and ops.cutoffs_on(cutoffs) else None))
         if sess is not None:
             sess.busy = True
         return rid
@@ -630,6 +637,8 @@ class SlotScheduler:
                 kw["lookup"] = r.lookup
             if r.constraints is not None:
                 kw["constraints"] = r.constraints
+            if r.cutoffs is not None:
+                kw["cutoffs"] = r.cutoffs
             eng.admit(j, r.input_ids, r.max_new, r.temperature, r.top_k, r.top_p, r.penalty, r.u, **kw, **feats)
             r.features, r.u = {}, None
             if long:
