@@ -193,9 +193,12 @@ def _inputs(A, seed):
 
 @pytest.mark.parametrize("case", list(ATTN_CASES))
 def test_attention_bwd_vs_fp32(case):
+    bwd_vs_fp32_case(Attn(**ATTN_CASES[case]), case)
+
+
+def bwd_vs_fp32_case(A, case):
     """Forward out / lse, then dQ, dK, dV per batch element against fp32 autograd (rel < 1e-2) and against the rounding-matched
     fp32 reference (rel < 1e-3)."""
-    A = Attn(**ATTN_CASES[case])
     qkv, dout = _inputs(A, 11)
     out, lse, dqkv = A.run(qkv, dout)
     ref_o, ref_lse, ref_g = A.autograd_ref(qkv, dout)
@@ -215,8 +218,11 @@ def test_attention_bwd_vs_fp32(case):
 
 @pytest.mark.parametrize("case", list(ATTN_CASES))
 def test_attention_bwd_masks_exact(case):
+    bwd_masks_case(Attn(**ATTN_CASES[case]), case)
+
+
+def bwd_masks_case(A, case):
     """Bit-level mask checks: what the mask hides cannot move a single bit, what it shows must move something."""
-    A = Attn(**ATTN_CASES[case])
     B, S, sec = A.B, A.S, A.sections()
     kv = slice(sec["dK"].start, sec["dV"].stop)                 # the k | v columns of the fused layout (and of dqkv)
     qkv, dout = _inputs(A, 21)
@@ -298,6 +304,10 @@ def test_rmsnorm_bwd_stack_mode_dx(T2):
 
 @pytest.mark.parametrize("rows,cols,eps", [(402, 4096, 1e-5), (201, 8192, 1e-5), (376, 2048, 1e-6)])
 def test_rmsnorm_bwd_plain_width(rows, cols, eps):
+    rmsnorm_bwd_case(rows, cols, eps)
+
+
+def rmsnorm_bwd_case(rows, cols, eps):
     """The LLM's norms (4096 at B*S = 402, 8192 for 70B widths) and the v0_5_8b projector's ln_mid (2048 over N*rows_a = 376,
     eps 1e-6), with the residual gradient, and dw accumulated (+=) into a pre-filled buffer."""
     from ultravox_b200 import ops
@@ -349,6 +359,10 @@ def test_gelu_bwd_every_bf16_in_range():
 
 @pytest.mark.parametrize("rows,H,gate_first", [(201, 14336, True), (376, 2048, False)])
 def test_swiglu_bwd_width(rows, H, gate_first):
+    swiglu_bwd_case(rows, H, gate_first)
+
+
+def swiglu_bwd_case(rows, H, gate_first):
     """LLM MLP (H = 14336, gate | up) and projector (H = 2048, up | gate), gates in [-40, 40] so the sigmoid saturates."""
     from ultravox_b200 import ops
     g = torch.Generator().manual_seed(1)
@@ -367,12 +381,16 @@ def test_swiglu_bwd_width(rows, H, gate_first):
 
 @pytest.mark.parametrize("pos_offset", [0, 37])
 def test_rope_bwd_llama3_d128(pos_offset):
-    """Llama-3.1-8B rope (theta 5e5, llama3 scaling), head_dim 128, 32 / 8 heads, B = 2 sequences of 201 rows: the explicit
+    rope_bwd_case(pos_offset, 32, 8, 128, "v0_5_8b")
+
+
+def rope_bwd_case(pos_offset, Hq, Hkv, D, name):
+    """The rope of preset ``name`` (theta, llama3 scaling) at head_dim D, Hq / Hkv heads, B = 2 sequences of 201 rows: the explicit
     transposed rotation per (position, frequency); the v section is not touched."""
     from ultravox_b200 import ops
     from ultravox_b200.config import PRESETS
-    tc = PRESETS["v0_5_8b"]["text_config"]
-    Hq, Hkv, D, S, B = 32, 8, 128, 201, 2
+    tc = PRESETS[name]["text_config"]
+    S, B = 201, 2
     inv = ops.llama3_inv_freq(D, tc["rope_theta"], tc["rope_scaling"])
     cos, sin = ops.rope_tables(inv, 256, "cuda")
     x = rnd(B * S, (Hq + 2 * Hkv) * D, seed=1)

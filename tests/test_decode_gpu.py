@@ -183,11 +183,14 @@ PAD_STARTS = (0, 5, 64, 130)
 @pytest.mark.parametrize("B", [1, 3, 8, 32])
 @pytest.mark.parametrize("width", ["8b", "70b"])
 def test_decode_attention_over_cache(width, B, smax, left_pad):
+    Wd = W8B if width == "8b" else W70B
+    decode_attention_case(Wd["Hq"], Wd["Hkv"], HD, B, smax, left_pad, width)
+
+
+def decode_attention_case(Hq, Hkv, D, B, smax, left_pad, width):
     """One query per stream (Sq = 1, non-causal, kv_len = lens) over the whole static cache on ``attn_fwd_kernel``; B = 32 is
     8 prompts x 4 beams.  Then bit-exact: a row whose one visible key is kv_len - 1 returns that key's V row, kv_start = kv_len
     returns zeros, and another row's cache changes no output of this row."""
-    Wd = W8B if width == "8b" else W70B
-    Hq, Hkv, D = Wd["Hq"], Wd["Hkv"], HD
     off = {1: 5, 3: 2, 8: 0, 32: 3}[B] + (smax == 4160)
     L = [smax + x if x <= 0 else x for x in DECODE_LENS]
     lens = [L[(b + off) % len(L)] for b in range(B)]
@@ -220,12 +223,15 @@ def test_decode_attention_over_cache(width, B, smax, left_pad):
 @pytest.mark.parametrize("Sq", [2, 7, 15, 16, 33])
 @pytest.mark.parametrize("width", ["8b", "70b"])
 def test_prefill_attention_on_cache(width, Sq, left_pad):
+    Wd = W8B if width == "8b" else W70B
+    prefill_on_cache_case(Wd["Hq"], Wd["Hkv"], HD, Sq, left_pad, width)
+
+
+def prefill_on_cache_case(Hq, Hkv, D, Sq, left_pad, width):
     """A short prompt or conversation turn prefilled on top of a cache (model.py ``llama_hidden``): causal with past = 137 keys
     before the Sq queries (shift = Skv - Sq > 0), kv_start in {0, 5, 64, 130}.  Sq < 16 runs on the mma.sync kernel, Sq >= 16 on
     the wgmma kernel and once more on the mma.sync kernel."""
     from ultravox_b200 import _lib
-    Wd = W8B if width == "8b" else W70B
-    Hq, Hkv, D = Wd["Hq"], Wd["Hkv"], HD
     B, past, smax = 4, 137, 210
     Skv = past + Sq
     start_t = torch.tensor(PAD_STARTS, dtype=torch.int32, device="cuda") if left_pad else None
@@ -271,13 +277,16 @@ def strided(t, pad_front, pad_back):
 
 @pytest.mark.parametrize("shape", list(GEMV_SHAPES))
 def test_gemv_and_decode_gemm_at_width(shape):
+    gemv_case(*GEMV_SHAPES[shape], shape)
+
+
+def gemv_case(N, K, shape):
     """``ops.gemv`` at B in {1, 2, 5, 8} with a residual, x / residual / out as strided views: fp32 output within
     gamma(8 ceil(K/256) + 6) sum|x w| of fp64 (8 FMAs per lane per 256 columns, a 5-level shuffle tree, the residual add), bf16
     output within that plus one ulp and rel < 1e-3; the same bits as dense operands.  K = 28672 at B = 8 takes the slab loop (3
     slabs).  Then, for the eight 8B / 70B projections, the decode form of the tensor-core GEMM (``ops.linear``, 2+ streams) at
     B in {2, 3, 8}, plain and with a residual: rel < 1e-3 against fp32 math and the same bits from run to run."""
     from ultravox_b200 import ops
-    N, K = GEMV_SHAPES[shape]
     w = rnd(N, K, scale=0.02, seed=N + K)
     x8, r8 = rnd(8, K, seed=1), rnd(8, N, scale=0.5, seed=2)
     ref8, mag8 = matvec_f64(x8, w, r8)
@@ -331,6 +340,10 @@ def swiglu_hf(gu):
     # SwiGLU prologue: down_proj; each side of ops.gemv's shared-memory switch (B * 2K * 2 bytes > 200 KiB -> unfused)
     ("swiglu", 4096, 14336, (1, 7, 8)), ("swiglu", 8192, 28672, (1, 3, 4, 8))])
 def test_gemv_fused_prologues_at_width(case):
+    gemv_prologue_case(case)
+
+
+def gemv_prologue_case(case):
     """``gemv(norm=)`` / ``gemv(swiglu=True)`` against fp64 LlamaRMSNorm / act(gate) * up in HF's rounding order followed by
     the matmul (rel < 1e-3), and bit-identical to the separate kernels they replace."""
     from ultravox_b200 import ops
@@ -427,15 +440,19 @@ def test_argmax_ties_and_edges(V):
 # ================================================================================================ 5. RoPE + cache append
 @pytest.mark.parametrize("width", ["8b", "70b"])
 def test_rope_kv_append_long_positions(width):
+    Wd = W8B if width == "8b" else W70B
+    rope_kv_append_case(Wd["Hq"], Wd["Hkv"], HD, "v0_5_8b", width)
+
+
+def rope_kv_append_case(Hq, Hkv, D, name, width):
     """B = 8 streams at RoPE positions up to 131071 (llama3 scaling) written to cache slots that differ from them (left
     padding): q and k within one ulp of the fp64 rotation with the same fp32 tables (+ 2^-23 (|x1 c| + |x2 s|), the fp32
     rounding of the two products when they cancel); the cache row is the rotated k and the raw v bit for bit; every other
     slot keeps its sentinel; ``rope_`` with ``positions=`` + ``kv_append`` give the same bits."""
     from ultravox_b200 import ops
     from ultravox_b200.config import PRESETS
-    tc = PRESETS["v0_5_8b"]["text_config"]
-    Wd = W8B if width == "8b" else W70B
-    Hq, Hkv, D, B, smax = Wd["Hq"], Wd["Hkv"], HD, 8, 210
+    tc = PRESETS[name]["text_config"]
+    B, smax = 8, 210
     inv = ops.llama3_inv_freq(D, tc["rope_theta"], tc["rope_scaling"])
     cos, sin = ops.rope_tables(inv, 131072, "cuda")
     rope_pos = torch.tensor([0, 1, 8191, 8192, 65535, 100003, 131070, 131071], dtype=torch.int32, device="cuda")

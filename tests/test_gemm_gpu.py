@@ -300,9 +300,13 @@ def short(name: str) -> str:
 
 def run(ops, fn, expect, twice=True):
     """fn() -> tuple of fresh output tensors.  The split-K workspace is filled with NaN before each call; the first call runs under
-    the profiler and exactly the kernels in ``expect`` must have run; the second must give the same bits."""
+    the profiler and exactly the kernels in ``expect`` must have run; the second must give the same bits.  ``expect=None``: the
+    first call is not profiled (for callers that assert the dispatch of the same call in a process of its own)."""
     from torch.profiler import ProfilerActivity, profile
-    for _ in range(3):
+    if expect is None:
+        ops.gemm_workspace(torch.device("cuda")).fill_(255)
+        out = fn()
+    for _ in range(8 if expect is not None else 0):
         ops.gemm_workspace(torch.device("cuda")).fill_(255)
         torch.cuda.synchronize()
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
@@ -310,9 +314,10 @@ def run(ops, fn, expect, twice=True):
             torch.cuda.synchronize()
         ran = sorted({short(e.name) for e in prof.events()
                       if e.device_type == torch.autograd.DeviceType.CUDA and "uvx::" in e.name})
-        if ran:                    # now and then the profiler delivers no activity records for a window: profile the call again
+        if set(expect) <= set(ran):    # now and then the profiler drops some or all records of a window: profile the call again
             break
-    assert ran == sorted(set(expect)), f"dispatch: ran {ran}, expected {sorted(set(expect))}"
+    if expect is not None:
+        assert ran == sorted(set(expect)), f"dispatch: ran {ran}, expected {sorted(set(expect))}"
     if twice:
         ops.gemm_workspace(torch.device("cuda")).fill_(255)
         again = fn()

@@ -129,21 +129,21 @@ def flat(*shape, seed, device, scale=1.0):
     return (torch.randn(*shape, generator=g, device=device) * scale).to(BF)
 
 
-def needle_q(rows, Hq, D, device):
-    """Needle queries [rows, Hq * D]: every element NEEDLE_Q."""
-    return torch.full((rows, Hq * D), NEEDLE_Q, dtype=BF, device=device)
+def needle_q(rows, Hq, D, device, val=NEEDLE_Q):
+    """Needle queries [rows, Hq * D]: every element ``val``."""
+    return torch.full((rows, Hq * D), val, dtype=BF, device=device)
 
 
-def plant_needle(k, p):
+def plant_needle(k, p, val=NEEDLE_Q):
     """Key p of k [..., S, Hkv, D] (every head) becomes the needle query's own vector: score NEEDLE_Q^2 D = 2048 at D = 128,
     against 4 sum(k_j) ~ N(0, 2048) for randn keys, a scaled log2 gap of ~ (2048 - 5.2 * 45) / sqrt(128) * log2 e ~ 230."""
-    k[..., p, :, :] = NEEDLE_Q
+    k[..., p, :, :] = val
 
 
-def needle_gap(k, p, begin, end, D=HD):
+def needle_gap(k, p, begin, end, D=HD, val=NEEDLE_Q):
     """min over KV heads and visible keys j != p of (s_p - s_j) * D^-0.5 * log2 e for the needle query (fp64): the kernels'
     exp2 of minus this underflows to 0 in fp32 when it is > 150."""
-    s = NEEDLE_Q * k[begin:end].float().sum(-1).double()          # [n, Hkv]
+    s = val * k[begin:end].float().sum(-1).double()               # [n, Hkv]
     sp = s[p - begin].clone()
     s[p - begin] = float("-inf")
     return float(((sp - s.amax(0)) * D ** -0.5 * LOG2E).min())
@@ -222,13 +222,13 @@ def assert_kernel(fn, want):
 class Stats:
     """Largest errors seen in one test, printed at its end."""
 
-    def __init__(self, what):
-        self.what, self.r32, self.rm = what, 0.0, 0.0
+    def __init__(self, what, D=HD):
+        self.what, self.D, self.r32, self.rm = what, D, 0.0, 0.0
 
     def check(self, got, q, k, v, begin, end, shift=None, what=""):
         """got [Sq, Hq * D] against both references of one batch row; returns the rounding-matched reference."""
         Sq = got.shape[0]
-        ref, matched = attention_refs(q.view(Sq, -1, HD), k, v, begin, end, shift)
+        ref, matched = attention_refs(q.view(Sq, -1, self.D), k, v, begin, end, shift)
         r32, rm = rel(got, ref.to(BF)), rel(got, matched)
         self.r32, self.rm = max(self.r32, r32), max(self.rm, rm)
         assert torch.isfinite(got.float()).all(), (self.what, what, "non-finite output")
@@ -276,16 +276,23 @@ DECODE_CASES = [("8b", 8193, 1), ("8b", 8193, 3), ("8b", 32768, 3), ("8b", SMAX,
 
 @pytest.mark.parametrize("width,smax,B", DECODE_CASES)
 def test_decode_long_cache(width, smax, B):
-    Hq = HQ8 if width == "8b" else HQ70
+    decode_long_case(HQ8 if width == "8b" else HQ70, smax, B, width)
+
+
+def decode_long_case(Hq, smax, B, width, D=HD, needle=NEEDLE_Q, check_dispatch=True):
+    """``ops.attention`` with one query per row over a contiguous cache of S_max keys at head_dim D; ``needle`` is the needle's
+    q / k element value (large enough for NEEDLE_GAP at that D); ``check_dispatch=False`` for callers that assert the kernel of
+    the same call in a process of their own."""
     lens, starts = decode_rows(smax, B)
     lens_t, start_t = i32(lens), i32(starts)
     what = f"decode {width} S_max={smax} B={B} lens={lens} starts={starts}"
-    st = Stats(what)
+    st = Stats(what, D)
     seed = smax + B + Hq
-    kc, vc = flat(B, smax, HKV, HD, seed=seed, device="cuda"), flat(B, smax, HKV, HD, seed=seed + 1, device="cuda")
-    q = flat(B, Hq * HD, seed=seed + 2, device="cuda")
+    kc, vc = flat(B, smax, HKV, D, seed=seed, device="cuda"), flat(B, smax, HKV, D, seed=seed + 1, device="cuda")
+    q = flat(B, Hq * D, seed=seed + 2, device="cuda")
     run = lambda: decode(q, kc, vc, Hq, lens_t, start_t)          # noqa: E731
-    assert_kernel(run, "attn_fwd_kernel<128, false, false>")
+    if check_dispatch:
+        assert_kernel(run, f"attn_fwd_kernel<{D}, false, false>")
     # flat: both references per row, the same bits twice, masked positions never read, row isolation
     out = twice(run)
     for b in range(B):
@@ -295,20 +302,20 @@ def test_decode_long_cache(width, smax, B):
     del kp, vp
     if B > 1:
         k2, v2 = kc.clone(), vc.clone()
-        k2[0], v2[0] = flat(smax, HKV, HD, seed=seed + 3, device="cuda"), flat(smax, HKV, HD, seed=seed + 4, device="cuda")
+        k2[0], v2[0] = flat(smax, HKV, D, seed=seed + 3, device="cuda"), flat(smax, HKV, D, seed=seed + 4, device="cuda")
         o2 = decode(q, k2, v2, Hq, lens_t, start_t)
         assert torch.equal(o2[1:], out[1:]) and not torch.equal(o2[0], out[0]), (what, "row isolation")
         del k2, v2
     # needle: bit for bit the needle's V row in every q head of its group
-    qn = needle_q(B, Hq, HD, "cuda")
+    qn = needle_q(B, Hq, D, "cuda", needle)
     G = Hq // HKV
     for b in range(B):
         e = lens[b]
         spots = sorted({0, 63, 64, starts[b], PAGE * ((starts[b] + e) // 128) + 17, PAGE * ((e - 1) // PAGE), e - 1})
         for p in (p for p in spots if starts[b] <= p < e):
             k0 = kc[b, p].clone()
-            plant_needle(kc[b], p)
-            assert needle_gap(kc[b], p, starts[b], e) > NEEDLE_GAP
+            plant_needle(kc[b], p, needle)
+            assert needle_gap(kc[b], p, starts[b], e, D, needle) > NEEDLE_GAP
             got = decode(qn, kc, vc, Hq, lens_t, start_t)[b]
             want = vc[b, p].repeat_interleave(G, 0).reshape(-1)
             assert torch.equal(got, want), (what, f"needle row {b} at {p}", int((got != want).sum()))
@@ -317,7 +324,7 @@ def test_decode_long_cache(width, smax, B):
     qs = q.clone()
     k3 = kc.clone()
     for b in range(B):
-        sink_recency(qs[b:b + 1], k3[b], starts[b], lens[b], Hq, HD)
+        sink_recency(qs[b:b + 1], k3[b], starts[b], lens[b], Hq, D)
     out = twice(lambda: decode(qs, k3, vc, Hq, lens_t, start_t))
     for b in range(B):
         st.check(out[b:b + 1], qs[b], k3[b], vc[b], starts[b], lens[b], what=f"sink row {b}")
@@ -325,7 +332,7 @@ def test_decode_long_cache(width, smax, B):
     k3.copy_(kc)
     for b in range(B):
         for p in tie_positions(starts[b], lens[b]):
-            plant_needle(k3[b], p)
+            plant_needle(k3[b], p, needle)
     out = twice(lambda: decode(qn, k3, vc, Hq, lens_t, start_t))
     for b in range(B):
         st.check(out[b:b + 1], qn[b], k3[b], vc[b], starts[b], lens[b], what=f"ties row {b}")
@@ -401,9 +408,9 @@ def paged_table(lens, n_pages, hot, seed):
     return table
 
 
-def rows_with_nan_tail(B, lens, seed, scale=1.0):
+def rows_with_nan_tail(B, lens, seed, scale=1.0, D=HD):
     """k, v [B, 131072, Hkv, D] randn rows, NaN at positions >= lens[b]."""
-    k, v = flat(B, SMAX, HKV, HD, seed=seed, device="cuda", scale=scale), flat(B, SMAX, HKV, HD, seed=seed + 1, device="cuda")
+    k, v = flat(B, SMAX, HKV, D, seed=seed, device="cuda", scale=scale), flat(B, SMAX, HKV, D, seed=seed + 1, device="cuda")
     for b, e in enumerate(lens):
         k[b, e:], v[b, e:] = NAN, NAN
     return k, v
@@ -445,6 +452,10 @@ def paged_needles(e):
 
 @pytest.mark.parametrize("kind", ["bf16", "fp8-0", "fp8-1", "fp8-2"])
 def test_paged_decode_long_table(kind):
+    paged_long_case(kind)
+
+
+def paged_long_case(kind, D=HD, needle=NEEDLE_Q, check_dispatch=True):
     """``attention_paged`` (and its ``kv_row`` form) through 2048-entry tables into a pool of > 16384 bf16 pages (page byte
     offsets >= 2^31) or > 32768 e4m3 pages (element and byte offsets >= 2^31), every page outside the tables NaN; the needle's
     tiles sit in the pages with the largest pool indices.  e4m3: also bit for bit the bf16 kernel on the dequantized pool."""
@@ -458,34 +469,35 @@ def test_paged_decode_long_table(kind):
     assert int(table.max()) >= (32768 if fp8 else 16384)
     lens_t = i32(lens)
     what = f"paged decode {kind} n_pages={n_pages}"
-    st = Stats(what)
-    k, v = rows_with_nan_tail(B, lens, seed=11)
+    st = Stats(what, D)
+    k, v = rows_with_nan_tail(B, lens, seed=11, D=D)
     if fp8:
         kq, vq = quant(k, sk), quant(v, sv)
         k, v = dequant(kq, sk), dequant(vq, sv)                      # what the kernel sees; also the bf16 twin's pool
-        pk = torch.full((n_pages, PAGE, HKV, HD), NAN_BYTE, dtype=torch.uint8, device="cuda").view(E4M3)
+        pk = torch.full((n_pages, PAGE, HKV, D), NAN_BYTE, dtype=torch.uint8, device="cuda").view(E4M3)
         pv = pk.clone()
         fill_pool(pk, kq, table), fill_pool(pv, vq, table)
         del kq, vq
         scale = torch.tensor([sk, sv], dtype=torch.float32, device="cuda")
         twin_table = torch.arange(B * W, dtype=torch.int32, device="cuda").view(B, W).masked_fill(table < 0, -1)
     else:
-        pk = torch.full((n_pages, PAGE, HKV, HD), NAN, dtype=BF, device="cuda")
+        pk = torch.full((n_pages, PAGE, HKV, D), NAN, dtype=BF, device="cuda")
         pv = pk.clone()
         fill_pool(pk, k, table), fill_pool(pv, v, table)
         scale = None
-    q = flat(B, Hq * HD, seed=12, device="cuda")
+    q = flat(B, Hq * D, seed=12, device="cuda")
 
     def run(qq=q, rows=None, lt=lens_t):
-        out = torch.zeros(B, Hq * HD, dtype=BF, device="cuda")
-        return ops.attention_paged(qq, pk, pv, out, Hq, HD ** -0.5, table, lt, kv_scale=scale, kv_row=rows)
+        out = torch.zeros(B, Hq * D, dtype=BF, device="cuda")
+        return ops.attention_paged(qq, pk, pv, out, Hq, D ** -0.5, table, lt, kv_scale=scale, kv_row=rows)
 
     def twin(qq):
-        out = torch.zeros(B, Hq * HD, dtype=BF, device="cuda")
-        return ops.attention_paged(qq, k.view(B * W, PAGE, HKV, HD), v.view(B * W, PAGE, HKV, HD), out, Hq, HD ** -0.5, twin_table,
+        out = torch.zeros(B, Hq * D, dtype=BF, device="cuda")
+        return ops.attention_paged(qq, k.view(B * W, PAGE, HKV, D), v.view(B * W, PAGE, HKV, D), out, Hq, D ** -0.5, twin_table,
                                    lens_t)
 
-    assert_kernel(run, f"attn_fwd_kernel<128, true, {'true' if fp8 else 'false'}>")
+    if check_dispatch:
+        assert_kernel(run, f"attn_fwd_kernel<{D}, true, {'true' if fp8 else 'false'}>")
     out = twice(run)
     for b in range(B):
         st.check(out[b:b + 1], q[b], k[b], v[b], 0, lens[b], what=f"flat row {b}")
@@ -496,15 +508,15 @@ def test_paged_decode_long_table(kind):
     # row isolation: new values in row 1's pages change no bit of row 0
     pages1 = table[1][table[1] >= 0].long()
     keep = pk[pages1].clone(), pv[pages1].clone()
-    pk[pages1] = (flat(len(pages1), PAGE, HKV, HD, seed=13, device="cuda").float() / sk).to(pk.dtype)
+    pk[pages1] = (flat(len(pages1), PAGE, HKV, D, seed=13, device="cuda").float() / sk).to(pk.dtype)
     o2 = run()
     assert torch.equal(o2[0], out[0]) and not torch.equal(o2[1], out[1]), (what, "row isolation")
     pk[pages1], pv[pages1] = keep
     del keep
     # needle in the pages with the largest pool indices
-    qn = needle_q(B, Hq, HD, "cuda")
+    qn = needle_q(B, Hq, D, "cuda", needle)
     G = Hq // HKV
-    needle_byte = quant(torch.tensor(NEEDLE_Q, device="cuda"), sk) if fp8 else None
+    needle_byte = quant(torch.tensor(needle, device="cuda"), sk) if fp8 else None
     for b in range(B):
         for p in paged_needles(lens[b]):
             pg, off = page_of(table, b, p)
@@ -513,9 +525,9 @@ def test_paged_decode_long_table(kind):
                 pk[pg, off] = needle_byte
                 k[b, p] = dequant(needle_byte, sk)
             else:
-                pk[pg, off] = NEEDLE_Q
-                k[b, p] = NEEDLE_Q
-            assert needle_gap(k[b], p, 0, lens[b]) > NEEDLE_GAP
+                pk[pg, off] = needle
+                k[b, p] = needle
+            assert needle_gap(k[b], p, 0, lens[b], D, needle) > NEEDLE_GAP
             got = run(qq=qn)
             assert torch.equal(got[b], v[b, p].repeat_interleave(G, 0).reshape(-1)), (what, f"needle row {b} at {p} page {pg}")
             if fp8:
@@ -524,7 +536,7 @@ def test_paged_decode_long_table(kind):
     # sink + recency
     qs = q.clone()
     for b in range(B):
-        sink_recency(qs[b:b + 1], k[b], 0, lens[b], Hq, HD)
+        sink_recency(qs[b:b + 1], k[b], 0, lens[b], Hq, D)
         pos = [0] + list(range(lens[b] - 256, lens[b]))
         if fp8:
             k[b, pos] = dequant(quant(k[b, pos], sk), sk)            # the sink / band values as the pool holds them

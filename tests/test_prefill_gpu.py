@@ -395,19 +395,22 @@ def test_attention_prefill(case):
 @pytest.mark.parametrize("past", [1, 63, 300, 4000])
 @pytest.mark.parametrize("Sq", [64, 70, 201])
 def test_attention_prefill_on_cache(Sq, past, B):
+    prefill_on_cache_case(Sq, past, B, 128, *((64, 8) if (Sq, past) == (70, 300) else (32, 8)))
+
+
+def prefill_on_cache_case(Sq, past, B, D, Hq, Hkv):
     """A conversation turn prefilled on a KV cache (model.py ``llama_hidden`` with a cache): Sq new queries over past + Sq keys
     read from caches [B, S_max, Hkv, D] with S_max = Skv + 37, causal with shift = past > 0; at B = 3 each row has its own
     ``kv_start`` (up to past) and ``kv_len`` (up to Skv).  The cache tail [Skv, S_max) holds NaN / Inf in the poisoned runs."""
     Skv = past + Sq
-    Hq, Hkv = (64, 8) if (Sq, past) == (70, 300) else (32, 8)
     starts = None if B == 1 else [0, min(past, 64), min(past, 130)]
     lens = None if B == 1 else [Skv, Skv - 1, Skv - Sq // 2]
-    c = AttnCase("cache", B, Sq, Hq, Hkv, 128, causal=True, past=past, lens=lens, starts=starts, seed=Sq + past + B)
-    out = check_attention(c, f"cache prefill Sq={Sq} past={past} B={B} heads={Hq}/{Hkv} starts={starts} lens={lens}")
+    c = AttnCase("cache", B, Sq, Hq, Hkv, D, causal=True, past=past, lens=lens, starts=starts, seed=Sq + past + B)
+    out = check_attention(c, f"cache prefill D={D} Sq={Sq} past={past} B={B} heads={Hq}/{Hkv} starts={starts} lens={lens}")
     # causality, bit-exact: key past + i0 reaches no query before i0 and does reach query i0
     i0 = Sq // 3
     st = c.clone()
-    st["kc"][:, past + i0], st["vc"][:, past + i0] = rnd(B, Hkv, 128, seed=3), rnd(B, Hkv, 128, seed=4)
+    st["kc"][:, past + i0], st["vc"][:, past + i0] = rnd(B, Hkv, D, seed=3), rnd(B, Hkv, D, seed=4)
     o2 = c.run(st)
     assert torch.equal(o2[:, :i0], out[:, :i0]), "a query sees a later key"
     assert not torch.equal(o2[0, i0], out[0, i0])
@@ -415,10 +418,12 @@ def test_attention_prefill_on_cache(Sq, past, B):
 
 @pytest.mark.parametrize("form", ["cache", "fused"])
 def test_attention_eligibility_edge(form):
-    """The two sides of ``attn_wg_eligible``: Sq = 16 runs on the wgmma kernel, Sq = 15 on the mma.sync kernel.  With the same
-    data (the first 15 queries, the same keys: causal, so query i sees the same keys in both calls) the two agree per row, and
-    the Sq = 15 side passes the same reference, mask and edge-key checks."""
-    B, Hq, Hkv, D = 3, 32, 8, 128
+    eligibility_edge_case(form, 128)
+
+
+def eligibility_cases(form, D):
+    """(Sq = 16 case, Sq = 15 case) over the same data: the first 15 queries of the Sq = 16 case and the same keys."""
+    B, Hq, Hkv = 3, 32, 8
     past = 137 if form == "cache" else 0
     c16 = AttnCase(form, B, 16, Hq, Hkv, D, causal=True, past=past, starts=[0, 5, 2 if form == "fused" else 64],
                    lens=[past + 16, past + 15, past + 9], seed=16)
@@ -426,22 +431,34 @@ def test_attention_eligibility_edge(form):
     c15.st["qkv"] = c16.st["qkv"].view(B, 16, -1)[:, :15].reshape(B * 15, -1).contiguous()
     if form == "cache":
         c15.st["kc"], c15.st["vc"] = c16.st["kc"][:, :c15.rows].contiguous(), c16.st["vc"][:, :c15.rows].contiguous()
-    o16 = check_attention(c16, f"eligibility {form} Sq=16")
-    o15 = check_attention(c15, f"eligibility {form} Sq=15", both_kernels=False)
+    return c16, c15
+
+
+def eligibility_edge_case(form, D):
+    """The two sides of ``attn_wg_eligible``: Sq = 16 runs on the wgmma kernel, Sq = 15 on the mma.sync kernel.  With the same
+    data (causal, so query i sees the same keys in both calls) the two agree per row, and the Sq = 15 side passes the same
+    reference, mask and edge-key checks."""
+    c16, c15 = eligibility_cases(form, D)
+    B = c16.B
+    o16 = check_attention(c16, f"eligibility {form} D={D} Sq=16")
+    o15 = check_attention(c15, f"eligibility {form} D={D} Sq=15", both_kernels=False)
     worst = 0.0
     for b in range(B):
         seen = c15.mask(b).any(-1)
         assert torch.equal(seen, c16.mask(b).any(-1)[:15])
         worst = max(worst, float(row_rel(o15[b][seen], o16[b, :15][seen].float()).max()))
-    print(f"eligibility {form}: Sq=15 (mma.sync) vs Sq=16 (wgmma) row rel {worst:.3e}")
+    print(f"eligibility {form} D={D}: Sq=15 (mma.sync) vs Sq=16 (wgmma) row rel {worst:.3e}")
     assert worst < ROW_REL, worst
 
 
 @pytest.mark.parametrize("form,Hq,Hkv", [("enc", 20, 20), ("fused", 32, 8), ("fused", 64, 8), ("cache", 32, 8)])
 def test_attention_batch_and_head_isolation(form, Hq, Hkv):
+    isolation_case(form, Hq, Hkv, 64 if form == "enc" else 128)
+
+
+def isolation_case(form, Hq, Hkv, D):
     """New q / k / v for batch element b change only element b's output bits; new k / v for KV head g change the query heads of
     group g, every one of them, and no other head."""
-    D = 64 if form == "enc" else 128
     B, Sq = 3, 140
     past = 75 if form == "cache" else 0
     c = AttnCase(form, B, Sq, Hq, Hkv, D, causal=form != "enc", past=past, lens=[past + 140, past + 101, past + 90],
@@ -466,11 +483,15 @@ def test_attention_batch_and_head_isolation(form, Hq, Hkv):
 
 @pytest.mark.parametrize("kernel", ["wgmma", "mma.sync"])
 def test_attention_empty_rows_and_lse(kernel):
+    empty_rows_case(kernel, 128)
+
+
+def empty_rows_case(kernel, D):
     """Rows that see no key - queries inside the left padding (causal) and every query of a sequence with kv_len == 0 - write an
     output of exactly 0 and lse = -inf (log of an empty sum), on both kernels; every other row's lse is the log-sum-exp of its
     scaled visible scores."""
     from ultravox_b200 import _lib
-    c = AttnCase("fused", 4, 130, 32, 8, 128, causal=True, starts=[0, 64, 129, 17], lens=[130, 130, 130, 0], seed=9)
+    c = AttnCase("fused", 4, 130, 32, 8, D, causal=True, starts=[0, 64, 129, 17], lens=[130, 130, 130, 0], seed=9)
     _lib.lib().uvx_debug_attn_tc(0 if kernel == "mma.sync" else -1)
     try:
         out, lse = c.run(lse=True)
@@ -489,11 +510,11 @@ def test_attention_empty_rows_and_lse(kernel):
 
 
 # ================================================================================================ 2. RoPE and the prefill cache fill
-def _llama3_tables():
+def _llama3_tables(D=128, name="v0_5_8b"):
     from ultravox_b200 import ops
     from ultravox_b200.config import PRESETS
-    tc = PRESETS["v0_5_8b"]["text_config"]
-    inv = ops.llama3_inv_freq(128, tc["rope_theta"], tc["rope_scaling"])
+    tc = PRESETS[name]["text_config"]
+    inv = ops.llama3_inv_freq(D, tc["rope_theta"], tc["rope_scaling"])
     return ops.rope_tables(inv, 131072, "cuda")
 
 
@@ -512,16 +533,19 @@ def rope_ref(qkv0, Hq, Hkv, D, cos, sin, pos):
 @pytest.mark.parametrize("B", [1, 3])
 @pytest.mark.parametrize("heads", ["8b", "70b"])
 def test_rope_offsets_and_positions(heads, B):
-    """``ops.rope_`` (the yardstick of the fused-RoPE GEMM epilogues) at head_dim 128 with the llama3-scaled tables, S = 201, on
+    rope_case(*((32, 8) if heads == "8b" else (64, 8)), 128, B, _llama3_tables(), heads)
+
+
+def rope_case(Hq, Hkv, D, B, tables, heads):
+    """``ops.rope_`` (the yardstick of the fused-RoPE GEMM epilogues) at head_dim D with the llama3-scaled ``tables``, S = 201, on
     rows that are a column view of a wider buffer: ``pos_offset`` in {0, 37, 8191, 131071 - S} (row r of every sequence is at
     pos_offset + r % S), and the explicit ``positions`` of a left-padded batch as ``generate`` derives them from the attention
     mask, (cumsum(mask) - 1).clamp_min(0): a pad row is at position 0, where cos = 1 and sin = 0, so it comes back bit for bit.
     The V section and the buffer outside the view keep their bits; one sequence's rows do not depend on another's."""
     from ultravox_b200 import ops
-    Hq, Hkv = (32, 8) if heads == "8b" else (64, 8)
-    D, S = 128, 201
+    S = 201
     W, nr = (Hq + 2 * Hkv) * D, (Hq + Hkv) * D
-    cos, sin = _llama3_tables()
+    cos, sin = tables
     buf0 = rnd(B * S, W + 16, scale=2.0, seed=B + Hq)
     worst = 0.0
     for off in (0, 37, 8191, 131071 - S):
@@ -559,14 +583,17 @@ def test_rope_offsets_and_positions(heads, B):
 @pytest.mark.parametrize("past", [0, 300])
 @pytest.mark.parametrize("heads", ["8b", "70b"])
 def test_kv_write_fills_the_cache(heads, past, B):
-    """``ops.rope_`` then ``ops.kv_write`` in model.py's order, S = 201 rows per sequence into caches [B, S_max, Hkv, 128] with
+    kv_write_case(*((32, 8) if heads == "8b" else (64, 8)), 128, past, B, _llama3_tables())
+
+
+def kv_write_case(Hq, Hkv, D, past, B, tables):
+    """``ops.rope_`` then ``ops.kv_write`` in model.py's order, S = 201 rows per sequence into caches [B, S_max, Hkv, D] with
     S_max = past + S + 11 filled with a position-dependent sentinel: cache rows [past, past + S) are the rotated K section and
     the raw V section bit for bit, and every other cache element keeps its sentinel."""
     from ultravox_b200 import ops
-    Hq, Hkv = (32, 8) if heads == "8b" else (64, 8)
-    D, S = 128, 201
+    S = 201
     smax = past + S + 11
-    cos, sin = _llama3_tables()
+    cos, sin = tables
     qkv0 = rnd(B * S, (Hq + 2 * Hkv) * D, seed=past + B)
     qkv = qkv0.clone()
     ops.rope_(qkv, Hq, Hkv, D, cos, sin, rows_per_seq=S, pos_offset=past)
@@ -587,13 +614,17 @@ def test_kv_write_fills_the_cache(heads, past, B):
 @pytest.mark.parametrize("B", [1, 2])
 @pytest.mark.parametrize("layer", ["conv1_T3000", "conv2_T3000", "conv2_T2999"])
 def test_conv_stem_per_element(layer, B, with_pos):
+    conv_case(*{"conv1_T3000": (128, 1280, 1, 3000), "conv2_T3000": (1280, 1280, 2, 3000), "conv2_T2999": (1280, 1280, 2, 2999)}[layer],
+              B, with_pos, layer)
+
+
+def conv_case(Cin, Cout, stride, T, B, with_pos, layer):
     """Whisper-large's conv stem through ``ops.conv1d_k3``: conv1 (128 -> 1280, stride 1, into a guard-padded buffer as
     ``encode_audio`` calls it) and conv2 (1280 -> 1280, stride 2, T = 3000 and the odd T = 2999 whose last output frame reads
     the trailing guard row), per element against fp64 conv1d + exact-erf GELU (+ pos).  The frames where the padding enters
     (0, 1, Tout - 2, Tout - 1) are asserted on their own; guard rows of the output are not written; clip b does not depend on
     clip b'."""
     from ultravox_b200 import ops
-    Cin, Cout, stride, T = {"conv1_T3000": (128, 1280, 1, 3000), "conv2_T3000": (1280, 1280, 2, 3000), "conv2_T2999": (1280, 1280, 2, 2999)}[layer]
     Tout = (T + stride - 1) // stride
     guard = stride == 1
     x = rnd(B, T, Cin, seed=1)
@@ -706,6 +737,10 @@ def _layernorm_rows(rows, cols, seed):
 
 @pytest.mark.parametrize("rows,cols", [(1500, 1280), (3000, 1280), (201, 4096)])
 def test_layernorm_per_element(rows, cols):
+    layernorm_case(rows, cols)
+
+
+def layernorm_case(rows, cols):
     """Whisper-large's LayerNorms (1 and 2 clips of 1500 frames x 1280: the warp-per-row kernel) and the block kernel
     (cols > 2048), on a dense input, on a strided view (row stride cols + 64) and with ``out=`` a separate buffer: per element
     within half an ulp + the fp32 term of the module docstring of fp64.  A constant row (variance 0) gives the bias exactly."""
