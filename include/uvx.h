@@ -587,6 +587,65 @@ int uvx_logits_constraints_rows_map(float* logits, int64_t R, int64_t V, const i
                                     const int32_t* cfg, const int64_t* ids, const int32_t* end, const float* bias, const int32_t* kind,
                                     int64_t tab_stride, uvx_stream_t stream);
 
+/* Stop strings (hf:generation/stopping_criteria.py StopStringCriteria, transformers 5.5), checked on the device after the pick,
+ * so a row that completes a stop string finishes inside the captured step.  The table is HF's precompute in sparse form, int32:
+ *   [0] n_ent  [1] n_stop  [2] mvp (max_valid_positions)  [3] mvel (max_valid_end_lens)  [4] W_max (longest string, characters)
+ *   [5, 5 + n_stop)  the target lengths;  then ids [n_ent], ascending: the tokens with an entry other than -1 outside HF's
+ *   length column;  then their HF rows [n_ent][rw], rw = n_stop * (mvp + mvel) + 1: the valid positions of string s at
+ *   s * mvp, its end overlaps at n_stop * mvp + s * mvel, the token's length last.  n_ent = 0: no stop strings (hit 0).
+ * Rule for one row with x = (the L preceding tokens, the candidate): W = min(W_max, L + 1); for each string s and each end
+ * overlap e > 0 of the candidate, c = e, hit if c >= |s|; then for j = 1 .. W - 1 with y = x[L - j]: stop this chain unless c
+ * is one of y's valid positions for s, else c += len(y), hit if c >= |s|.  Ids outside the table have no entries.  hit[r] is
+ * 1 or 0.  seq is never read at or past L.  One warp per row (32 threads): the lanes walk the chains, the window is looked up
+ * 32 tokens at a time (binary search over ids).
+ * uvx_stop_strings           B rows, row b's candidate tok[b] after seq[b * seq_stride, 0:cur_len[0]], one table.
+ * uvx_stop_strings_slots     active rows b after seq[b, 0:cur_len[b]] with table b (tab + b * tab_stride); inactive rows untouched.
+ * uvx_stop_strings_rows      row r after seq[r * seq_stride, 0:len[r]] (seq_stride 0: one shared sequence), one table.
+ * uvx_stop_strings_rows_map  row r of slot s = row_slot[r] (active[s], row_idx[r] >= 0; others untouched) after
+ *                            seq[s, 0:row_len[r]] with table s.
+ * uvx_stop_strings_beam      beam search: row r = b * K + c is candidate c of prompt b (cand_i [B, K] of uvx_beam_select),
+ *                            token cand_i[r] % V after run_seq[b * nb + cand_i[r] / V, 0:cur_len[0]] (its parent's running
+ *                            sequence, read before uvx_beam_update rewrites it), one table; hit [B * K].
+ * Finishing forms that honour hit (each one the entry without _stop when hit is all zero, same bits):
+ * uvx_token_finish_stop         uvx_token_finish; a row not yet done with hit[b] finishes too (its token kept, later ones pad), and a
+ *                               row that finishes in this step (EOS or hit) gets fin_len[b] = cur_len[0] + 1 (its length then).
+ * uvx_slot_finish_stop          uvx_slot_finish; hit[b] finishes the row as an EOS id would.
+ * uvx_lookup_accept_stop        uvx_lookup_accept with m cut at the first i <= m with hit[i]; a hit at the last kept pick finishes.
+ * uvx_lookup_accept_slots_stop  uvx_lookup_accept_slots with the same cut over the slot's rows hit[s * (K + 1) + i].
+ * uvx_beam_update_stop          uvx_beam_update where candidate c of prompt b also hits the stopping criteria when
+ *                               hit[b * K + c] (HF _beam_search's next_token_hits_stopping_criteria with StopStringCriteria).          */
+int uvx_stop_strings(const int64_t* tok, int64_t B, const int64_t* seq, int64_t seq_stride, const int32_t* cur_len, const int32_t* tab,
+                     int32_t* hit, uvx_stream_t stream);
+int uvx_stop_strings_slots(const int64_t* tok, int64_t B, const int64_t* seq, int64_t seq_stride, const int32_t* cur_len,
+                           const int32_t* active, const int32_t* tab, int64_t tab_stride, int32_t* hit, uvx_stream_t stream);
+int uvx_stop_strings_rows(const int64_t* tok, int64_t R, const int64_t* seq, int64_t seq_stride, const int32_t* len, const int32_t* tab,
+                          int32_t* hit, uvx_stream_t stream);
+int uvx_stop_strings_rows_map(const int64_t* tok, int64_t R, const int64_t* seq, int64_t seq_stride, const int32_t* active,
+                              const int32_t* row_slot, const int32_t* row_len, const int32_t* row_idx, const int32_t* tab,
+                              int64_t tab_stride, int32_t* hit, uvx_stream_t stream);
+int uvx_stop_strings_beam(const int64_t* cand_i, int64_t B, int32_t nb, int32_t K, int64_t V, const int64_t* run_seq,
+                          int64_t seq_stride, const int32_t* cur_len, const int32_t* tab, int32_t* hit, uvx_stream_t stream);
+int uvx_beam_update_stop(const float* cand_s, const int64_t* cand_i, int64_t B, int32_t nb, int32_t K, int64_t V, const int64_t* eos_ids,
+                         int32_t n_eos, int32_t max_new, const float* len_div, int32_t early_stopping, int32_t lp_positive,
+                         float* run_score, int64_t* run_seq, int64_t* pool_seq, int64_t seq_stride, float* pool_score,
+                         int32_t* pool_len, int32_t* pool_fin, int32_t* parent, int64_t* tok, int32_t* heur, int32_t* flags,
+                         uint32_t* ticket, int32_t* cur_len, int32_t* step_idx, int32_t* bump0, int32_t* bump1, int32_t* bump2,
+                         int32_t* done, const int32_t* hit, uvx_stream_t stream);
+int uvx_token_finish_stop(int64_t* tok, int32_t* done, const int64_t* eos_ids, int32_t n_eos, int64_t pad_id, int64_t* seq,
+                          int64_t seq_stride, int32_t* cur_len, int32_t* step_idx, int32_t* bump0, int32_t* bump1, int32_t* bump2,
+                          int32_t* all_done, int64_t B, const int32_t* hit, int32_t* fin_len, uvx_stream_t stream);
+int uvx_slot_finish_stop(const int64_t* tok, int32_t* done, const int64_t* eos_ids, int32_t n_eos, int64_t* seq, int64_t seq_stride,
+                         int32_t* cur_len, int32_t* n_new, const int32_t* max_new, const int32_t* active, int32_t* pos, int32_t* lens,
+                         int32_t* rope_pos, int32_t* n_open, int64_t B, const int32_t* hit, uvx_stream_t stream);
+int uvx_lookup_accept_stop(const int64_t* pick, const int64_t* tok, const int32_t* n_draft, const int64_t* eos_ids, int32_t n_eos,
+                           int64_t* seq, int32_t* cur_len, int32_t* n_new, int32_t max_new, int32_t* step, int32_t* accepted,
+                           int32_t steps, int32_t* done, const int32_t* hit, uvx_stream_t stream);
+int uvx_lookup_accept_slots_stop(const int64_t* pick, const int64_t* tok, const int32_t* n_draft, int64_t slots, int32_t K,
+                                 const int64_t* eos_ids, int32_t n_eos, int64_t* seq, int64_t seq_stride, int64_t* token, int32_t* done,
+                                 int32_t* cur_len, int32_t* n_new, const int32_t* max_new, const int32_t* active, int32_t* pos,
+                                 int32_t* lens, int32_t* rope_pos, int32_t* accepted, int32_t* n_open, const int32_t* hit,
+                                 uvx_stream_t stream);
+
 /* Beam search (hf:generation/utils.py _beam_search, transformers 5.5, and the helpers above it), one decode step as four
  * launches that read every per-step scalar from device memory.  B prompts, nb <= 8 beams each: row r = b * nb + j.
  * uvx_log_softmax   out[r] = log_softmax(in[r]) in fp32 (in == out allowed).  Beam search scores log-probs; the repetition

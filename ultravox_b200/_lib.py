@@ -133,6 +133,21 @@ SIGNATURES = {
     "uvx_logits_constraints_rows": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "uvx_logits_constraints_rows_map": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
                                                   c_vp, c_i64, c_vp]),
+    "uvx_stop_strings": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp]),
+    "uvx_stop_strings_slots": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp]),
+    "uvx_stop_strings_rows": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp]),
+    "uvx_stop_strings_rows_map": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp]),
+    "uvx_stop_strings_beam": (C.c_int, [c_vp, c_i64, c_i32, c_i32, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp]),
+    "uvx_beam_update_stop": (C.c_int, [c_vp, c_vp, c_i64, c_i32, c_i32, c_i64, c_vp, c_i32, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp,
+                                       c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                       c_vp, c_vp, c_vp]),
+    "uvx_token_finish_stop": (C.c_int, [c_vp, c_vp, c_vp, c_i32, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp,
+                                        c_vp, c_vp]),
+    "uvx_slot_finish_stop": (C.c_int, [c_vp, c_vp, c_vp, c_i32, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64,
+                                       c_vp, c_vp]),
+    "uvx_lookup_accept_stop": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp]),
+    "uvx_lookup_accept_slots_stop": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_i32, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp,
+                                               c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "uvx_attention_rows": (C.c_int, [C.POINTER(AttnArgs), c_vp, c_vp]),
     "uvx_attention_paged_rows": (C.c_int, [C.POINTER(AttnArgs), c_vp, c_i64, c_vp, c_vp]),
     "uvx_attention_paged_fp8_rows": (C.c_int, [C.POINTER(AttnArgs), c_vp, c_i64, c_vp, c_vp, c_vp]),

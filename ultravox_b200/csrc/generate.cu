@@ -772,11 +772,104 @@ __global__ void __launch_bounds__(1024) logits_constraints_kernel(float* logits,
   constrain_row(logits + b * V, V, seq + s * seq_stride, len[b * len_stride], cfg + 4 * c, ids + o, end + o, bias + o, kind + o);
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// Stop strings (hf:generation/stopping_criteria.py StopStringCriteria).  The packed table (include/uvx.h): header n_ent,
+// n_stop, mvp, mvel, W_max, then the n_stop target lengths, the n_ent sorted token ids and their HF rows of
+// rw = n_stop * (mvp + mvel) + 1 int32 (positions of string s at s * mvp, end overlaps at n_stop * mvp + s * mvel, length last).
+constexpr int kStopHdr = 5;
+
+// Index of token t among the sorted ids[0:n], -1 when absent (ids outside the table have no entries, as HF's clamped row).
+__device__ __forceinline__ int stop_find(const int32_t* ids, int n, int64_t t) {
+  if (t < 0 || t > INT32_MAX) return -1;
+  int lo = 0, hi = n;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (ids[mid] < t) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo < n && ids[lo] == t ? lo : -1;
+}
+
+// One warp per row r.  Slot s = row_slot ? row_slot[r] : r; the row's candidate is tok[r], preceded by
+// seq[s * seq_stride, 0:L), L = len[r * len_stride]; the table is tab + (per_slot ? s * tab_stride : 0).  Beam form (beam_V > 0):
+// row r is candidate r % K of prompt r / K, tok[r] = parent beam * beam_V + token, s = (r / K) * nb + tok[r] / beam_V and the
+// candidate token tok[r] % beam_V.  Rows of an inactive
+// slot (active given) or with row_idx[r] < 0 (row_idx given) are not written.  Lane c walks chain c = (string c / mvel, end
+// overlap slot c % mvel) of the candidate, 32 chains per round; the window tokens x[L - j], j = 1 .. W - 1 (W = min(W_max,
+// L + 1)), are looked up 32 at a time by the 32 lanes into shared memory, so seq is read only inside [L - W + 1, L).
+__global__ void __launch_bounds__(32) stop_strings_kernel(const int64_t* tok, const int64_t* seq, int64_t seq_stride,
+                                                          const int32_t* len, int64_t len_stride, const int32_t* active,
+                                                          const int32_t* row_slot, const int32_t* row_idx, const int32_t* tab,
+                                                          int64_t tab_stride, int per_slot, int32_t* hit, int64_t beam_V, int nb,
+                                                          int K) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ int win[32];
+  const int lane = threadIdx.x;
+  const int64_t r = blockIdx.x;
+  int64_t t0 = tok[r];
+  int64_t s = row_slot ? row_slot[r] : r;
+  if (beam_V > 0) {
+    s = (r / K) * nb + t0 / beam_V;
+    t0 %= beam_V;
+  }
+  if ((active && !active[s]) || (row_idx && row_idx[r] < 0)) return;
+  const int32_t* T = tab + (per_slot ? s * tab_stride : 0);
+  const int n_ent = T[0], n_stop = T[1], mvp = T[2], mvel = T[3], wmax = T[4];
+  const int32_t* tgt = T + kStopHdr;
+  const int32_t* ids = tgt + n_stop;
+  const int32_t* rows = ids + n_ent;
+  const int rw = n_stop * (mvp + mvel) + 1;
+  const int64_t* sq = seq + s * seq_stride;
+  const int L = len[r * len_stride];
+  const int W = min(wmax, L + 1);
+  const int first = n_ent > 0 ? stop_find(ids, n_ent, t0) : -1;
+  int found = 0;
+  if (first >= 0) {
+    const int n_chain = n_stop * mvel;
+    for (int c0 = 0; c0 < n_chain && !found; c0 += 32) {
+      const int c = c0 + lane;
+      int st = -1, cv = 0;  // the chain's string (-1: dead) and the characters matched so far
+      if (c < n_chain) {
+        cv = rows[(int64_t)first * rw + n_stop * mvp + c];
+        st = cv > 0 ? c / mvel : -1;
+        found = st >= 0 && cv >= tgt[st];
+      }
+      for (int j0 = 1; j0 < W; j0 += 32) {
+        if (__any_sync(0xffffffffu, found) || !__any_sync(0xffffffffu, st >= 0)) break;
+        const int j = j0 + lane;
+        win[lane] = j < W ? stop_find(ids, n_ent, sq[L - j]) : -1;
+        __syncwarp();
+        const int jn = min(32, W - j0);
+        for (int q = 0; q < jn && st >= 0 && !found; ++q) {
+          const int y = win[q];
+          bool ok = false;
+          if (y >= 0) {
+            const int32_t* yr = rows + (int64_t)y * rw + st * mvp;
+            for (int p = 0; p < mvp; ++p) ok |= yr[p] == cv;
+          }
+          if (!ok) {
+            st = -1;
+            break;
+          }
+          cv += rows[(int64_t)y * rw + rw - 1];
+          found = cv >= tgt[st];
+        }
+        __syncwarp();
+      }
+      found = __any_sync(0xffffffffu, found);
+    }
+  }
+  if (lane == 0) hit[r] = found;
+}
+
 // One CTA: for each active, unfinished row append tok at seq[b, cur_len[b]], advance cur_len / n_new, finish on an EOS id or
-// at the budget, and advance pos / lens / rope_pos only while the row stays open.  n_open[0] = active rows still open.
+// at the budget (kStop: or on hit[b]), and advance pos / lens / rope_pos only while the row stays open.  n_open[0] = active rows
+// still open.
+template <bool kStop>
 __global__ void slot_finish_kernel(const int64_t* tok, int32_t* done, const int64_t* __restrict__ eos, int n_eos, int64_t* seq,
                                    int64_t seq_stride, int32_t* cur_len, int32_t* n_new, const int32_t* max_new, const int32_t* active,
-                                   int32_t* pos, int32_t* lens, int32_t* rope_pos, int32_t* n_open, int64_t B) {
+                                   int32_t* pos, int32_t* lens, int32_t* rope_pos, int32_t* n_open, int64_t B, const int32_t* hit) {
   pdl_trigger();
   pdl_wait();
   __shared__ int open;
@@ -792,6 +885,7 @@ __global__ void slot_finish_kernel(const int64_t* tok, int32_t* done, const int6
     n_new[b] = k;
     int d = k >= max_new[b];
     for (int e = 0; e < n_eos; ++e) d |= (t == eos[e]);
+    if (kStop) d |= hit[b] != 0;
     done[b] = d;
     if (!d) {
       pos[b] += 1;
@@ -805,12 +899,14 @@ __global__ void slot_finish_kernel(const int64_t* tok, int32_t* done, const int6
 }
 
 // One CTA: rows that already produced an EOS emit pad_id (HF semantics), the token is appended to `sequences`, rows whose token
-// is an EOS become finished, every counter in `bump` advances by one, all_done[0] = (every row finished).
+// is an EOS become finished, every counter in `bump` advances by one, all_done[0] = (every row finished).  kStop: an open row
+// with hit[b] finishes too (its token kept), and a row that finishes in this step gets fin_len[b] = cur_len + 1.
+template <bool kStop>
 __global__ void token_finish_kernel(int64_t* __restrict__ tok, int32_t* __restrict__ done, const int64_t* __restrict__ eos,
                                     int n_eos, int64_t pad_id, int64_t* __restrict__ seq, int64_t seq_stride,
                                     int32_t* __restrict__ cur_len, int32_t* __restrict__ step_idx, int32_t* __restrict__ bump0,
                                     int32_t* __restrict__ bump1, int32_t* __restrict__ bump2, int32_t* __restrict__ all_done,
-                                    int64_t B) {
+                                    int64_t B, const int32_t* hit, int32_t* fin_len) {
   pdl_trigger();
   pdl_wait();
   __shared__ int any_open;
@@ -820,10 +916,15 @@ __global__ void token_finish_kernel(int64_t* __restrict__ tok, int32_t* __restri
   for (int64_t b = threadIdx.x; b < B; b += blockDim.x) {
     int64_t t = tok[b];
     int d = done[b];
+    const int was = d;
     if (d) t = pad_id;
     tok[b] = t;
     if (seq) seq[b * seq_stride + n] = t;
     for (int e = 0; e < n_eos; ++e) d |= (t == eos[e]);
+    if (kStop) {
+      if (!was) d |= hit[b] != 0;
+      if (d && !was) fin_len[b] = n + 1;
+    }
     done[b] = d;
     if (!d) atomicOr(&any_open, 1);
     if (bump0) bump0[b] += 1;
@@ -1096,34 +1197,39 @@ __global__ void __launch_bounds__(1024) lookup_draft_kernel(int64_t* seq, const 
 
 // One warp: the count m of leading picks that equal the drafts; pick[0 : m + 1] are appended at seq[L] (lanes <= m), and
 // whether the last of them finishes the sequence (an EOS id or the budget) is returned.  Shared by lookup_accept_kernel and
-// lookup_accept_slots_kernel.
+// lookup_accept_slots_kernel.  kStop: m is cut at the first row i <= m with hit[i] (a stop string ends at pick[i]), which then
+// finishes the sequence.
+template <bool kStop>
 __device__ __forceinline__ int lookup_match(const int64_t* pick, const int64_t* tok, int d, const int64_t* __restrict__ eos, int n_eos,
-                                            int64_t* seq, int L, int nn, int max_new, int& fin) {
+                                            int64_t* seq, int L, int nn, int max_new, int& fin, const int32_t* hit) {
   const int lane = threadIdx.x & 31;
-  const bool miss = lane >= d || pick[lane] != tok[lane + 1];
+  bool miss = lane >= d || pick[lane] != tok[lane + 1];
+  if (kStop) miss = miss || (lane <= d && hit[lane] != 0);
   const int m = __ffs(__ballot_sync(0xffffffffu, miss)) - 1;  // d <= 31: lane d always misses
   if (lane <= m) seq[L + lane] = pick[lane];
   const int64_t t = pick[m];
   fin = nn + m + 1 >= max_new;
   for (int i = 0; i < n_eos; ++i) fin |= t == eos[i];
+  if (kStop) fin |= hit[m] != 0;
   return m;
 }
 
 // One warp.  n_matches = the leading picks that equal the drafts (pick[i] == tok[i + 1], i < d), the valid tokens are
 // pick[0 : n_matches + 1] (HF _assisted_decoding): appended at seq[cur_len], cur_len and n_new advance by their count, done when
 // the last is an EOS (drafts hold none, so only the last can be) or n_new reaches max_new.  accepted[step] = n_matches and step
-// advances (when accepted is given).  Nothing happens once done.
+// advances (when accepted is given).  Nothing happens once done.  kStop: lookup_match's cut at the first hit.
+template <bool kStop>
 __global__ void __launch_bounds__(32) lookup_accept_kernel(const int64_t* pick, const int64_t* tok, const int32_t* n_draft,
                                                            const int64_t* __restrict__ eos, int n_eos, int64_t* seq, int32_t* cur_len,
                                                            int32_t* n_new, int max_new, int32_t* step, int32_t* accepted, int steps,
-                                                           int32_t* done) {
+                                                           int32_t* done, const int32_t* hit) {
   pdl_trigger();
   pdl_wait();
   if (*done) return;
   const int lane = threadIdx.x;
   const int L = *cur_len, nn = *n_new;
   int fin;
-  const int m = lookup_match(pick, tok, *n_draft, eos, n_eos, seq, L, nn, max_new, fin);
+  const int m = lookup_match<kStop>(pick, tok, *n_draft, eos, n_eos, seq, L, nn, max_new, fin, hit);
   if (lane == 0) {
     *cur_len = L + m + 1;
     *n_new = nn + m + 1;
@@ -1185,12 +1291,14 @@ __global__ void __launch_bounds__(1024) lookup_draft_slots_kernel(int64_t* seq, 
 // Warp w of one CTA takes slots w, w + warps, ...: for each active slot that is not done, lookup_match over its rows, then
 // uvx_slot_finish's bookkeeping for the m + 1 tokens - cur_len / n_new += m + 1, done = the last is an EOS id or the budget is
 // reached, pos / lens / rope_pos += m + 1 while the slot stays open (m when it finishes: only the last token can finish it) -
-// token[s] = the last pick (fed next), accepted[s] += m.  n_open[0] = active slots still open.
+// token[s] = the last pick (fed next), accepted[s] += m.  n_open[0] = active slots still open.  kStop: the slot's rows' hits
+// cut m as in lookup_accept_kernel.
+template <bool kStop>
 __global__ void lookup_accept_slots_kernel(const int64_t* pick, const int64_t* tok, const int32_t* n_draft, int K,
                                            const int64_t* __restrict__ eos, int n_eos, int64_t* seq, int64_t seq_stride,
                                            int64_t* token, int32_t* done, int32_t* cur_len, int32_t* n_new, const int32_t* max_new,
                                            const int32_t* active, int32_t* pos, int32_t* lens, int32_t* rope_pos,
-                                           int32_t* accepted, int32_t* n_open, int slots) {
+                                           int32_t* accepted, int32_t* n_open, int slots, const int32_t* hit) {
   pdl_trigger();
   pdl_wait();
   __shared__ int open;
@@ -1202,7 +1310,8 @@ __global__ void lookup_accept_slots_kernel(const int64_t* pick, const int64_t* t
     const int64_t r0 = (int64_t)s * (K + 1);
     const int L = cur_len[s], nn = n_new[s];
     int fin;
-    const int m = lookup_match(pick + r0, tok + r0, n_draft[s], eos, n_eos, seq + s * seq_stride, L, nn, max_new[s], fin);
+    const int m = lookup_match<kStop>(pick + r0, tok + r0, n_draft[s], eos, n_eos, seq + s * seq_stride, L, nn, max_new[s], fin,
+                                      kStop ? hit + r0 : hit);
     if (lane == 0) {
       cur_len[s] = L + m + 1;
       n_new[s] = nn + m + 1;
@@ -1378,6 +1487,7 @@ __global__ void __launch_bounds__(kBeamMax * kBeamMaxK) beam_merge_kernel(const 
 // operation is HF's, in HF's order; top-k ties are broken towards the lower index.  The last CTA to finish (ticket) folds the
 // per-prompt flags into the loop condition and advances the step counters.  With done[0] set nothing changes except parent,
 // which becomes the identity (so the uvx_kv_reorder that follows is a no-op).
+template <bool kStop>
 __global__ void __launch_bounds__(256) beam_update_kernel(
     const float* cand_s, const int64_t* cand_i, int64_t V, int nb, int K, const int64_t* __restrict__ eos,
     int n_eos, int max_new, const float* __restrict__ len_div, int early_stopping, int lp_positive, float* __restrict__ run_score,
@@ -1385,7 +1495,7 @@ __global__ void __launch_bounds__(256) beam_update_kernel(
     int32_t* __restrict__ pool_len, int32_t* __restrict__ pool_fin, int32_t* __restrict__ parent, int64_t* __restrict__ tok,
     int32_t* __restrict__ heur, int32_t* __restrict__ flags, uint32_t* __restrict__ ticket, int32_t* __restrict__ cur_len,
     int32_t* __restrict__ step_idx, int32_t* __restrict__ bump0, int32_t* __restrict__ bump1, int32_t* __restrict__ bump2,
-    int32_t* __restrict__ done, int64_t B) {
+    int32_t* __restrict__ done, int64_t B, const int32_t* stop_hit) {
   pdl_trigger();
   pdl_wait();
   __shared__ float rsc[kBeamMaxK], psc[kBeamMaxK];  // running-selection / pool-merge scores of the candidates
@@ -1417,6 +1527,7 @@ __global__ void __launch_bounds__(256) beam_update_kernel(
     const int64_t t = idx % V;
     int hit = gen >= max_new;  // MaxLengthCriteria: cur_len + 1 >= prompt + max_new_tokens
     for (int e = 0; e < n_eos; ++e) hit |= t == eos[e];
+    if (kStop) hit |= stop_hit[b * K + tid] != 0;  // StopStringCriteria on the candidate's sequence
     cj[tid] = (int)(idx / V);
     ct[tid] = t;
     chit[tid] = hit;
@@ -1805,8 +1916,8 @@ extern "C" int uvx_lookup_accept(const int64_t* pick, const int64_t* tok, const 
   UVX_REQUIRE(pick && tok && n_draft && seq && cur_len && n_new && done && (n_eos == 0 || eos_ids) && n_eos >= 0 && max_new >= 1 &&
                   (!accepted || (step && steps >= 0)),
               "uvx_lookup_accept: bad arguments");
-  launch_k(lookup_accept_kernel, dim3(1), dim3(32), 0, (cudaStream_t)stream, pick, tok, n_draft, eos_ids, (int)n_eos, seq, cur_len,
-           n_new, (int)max_new, step, accepted, (int)steps, done);
+  launch_k(lookup_accept_kernel<false>, dim3(1), dim3(32), 0, (cudaStream_t)stream, pick, tok, n_draft, eos_ids, (int)n_eos, seq,
+           cur_len, n_new, (int)max_new, step, accepted, (int)steps, done, (const int32_t*)nullptr);
   return check_launch("lookup_accept_kernel");
 }
 
@@ -1839,8 +1950,9 @@ extern "C" int uvx_lookup_accept_slots(const int64_t* pick, const int64_t* tok, 
                   K <= kLookupMaxK,
               "uvx_lookup_accept_slots: bad arguments (1 <= K <= %d)", kLookupMaxK);
   const int warps = slots < 32 ? (int)slots : 32;
-  launch_k(lookup_accept_slots_kernel, dim3(1), dim3(32 * warps), 0, (cudaStream_t)stream, pick, tok, n_draft, (int)K, eos_ids,
-           (int)n_eos, seq, seq_stride, token, done, cur_len, n_new, max_new, active, pos, lens, rope_pos, accepted, n_open, (int)slots);
+  launch_k(lookup_accept_slots_kernel<false>, dim3(1), dim3(32 * warps), 0, (cudaStream_t)stream, pick, tok, n_draft, (int)K,
+           eos_ids, (int)n_eos, seq, seq_stride, token, done, cur_len, n_new, max_new, active, pos, lens, rope_pos, accepted, n_open,
+           (int)slots, (const int32_t*)nullptr);
   return check_launch("lookup_accept_slots_kernel");
 }
 
@@ -1938,8 +2050,8 @@ extern "C" int uvx_slot_finish(const int64_t* tok, int32_t* done, const int64_t*
   UVX_REQUIRE(tok && done && seq && cur_len && n_new && max_new && active && pos && lens && rope_pos && n_open && B >= 1 &&
                   n_eos >= 0 && (n_eos == 0 || eos_ids),
               "uvx_slot_finish: bad arguments");
-  launch_k(slot_finish_kernel, dim3(1), dim3(128), 0, (cudaStream_t)stream, tok, done, eos_ids, (int)n_eos, seq, seq_stride, cur_len,
-           n_new, max_new, active, pos, lens, rope_pos, n_open, B);
+  launch_k(slot_finish_kernel<false>, dim3(1), dim3(128), 0, (cudaStream_t)stream, tok, done, eos_ids, (int)n_eos, seq, seq_stride,
+           cur_len, n_new, max_new, active, pos, lens, rope_pos, n_open, B, (const int32_t*)nullptr);
   return check_launch("slot_finish_kernel");
 }
 
@@ -1948,9 +2060,116 @@ extern "C" int uvx_token_finish(int64_t* tok, int32_t* done, const int64_t* eos_
                                 int32_t* bump2, int32_t* all_done, int64_t B, uvx_stream_t stream) {
   using namespace uvx;
   UVX_REQUIRE(tok && done && cur_len && B >= 1 && (n_eos == 0 || eos_ids), "uvx_token_finish: bad arguments");
-  launch_k(token_finish_kernel, dim3(1), dim3(128), 0, (cudaStream_t)stream, tok, done, eos_ids, (int)n_eos, pad_id, seq, seq_stride,
-           cur_len, step_idx, bump0, bump1, bump2, all_done, B);
+  launch_k(token_finish_kernel<false>, dim3(1), dim3(128), 0, (cudaStream_t)stream, tok, done, eos_ids, (int)n_eos, pad_id, seq,
+           seq_stride, cur_len, step_idx, bump0, bump1, bump2, all_done, B, (const int32_t*)nullptr, (int32_t*)nullptr);
   return check_launch("token_finish_kernel");
+}
+
+namespace uvx {
+static int stop_strings_launch(const char* name, int64_t R, const int64_t* tok, const int64_t* seq, int64_t seq_stride,
+                               const int32_t* len, int64_t len_stride, const int32_t* active, const int32_t* row_slot,
+                               const int32_t* row_idx, const int32_t* tab, int64_t tab_stride, int per_slot, int32_t* hit,
+                               uvx_stream_t stream) {
+  UVX_REQUIRE(tok && seq && len && tab && hit && R >= 1 && R < 65536 && seq_stride >= 0 && tab_stride >= 0 &&
+                  (!per_slot || tab_stride >= kStopHdr),
+              "%s: bad arguments", name);
+  launch_k(stop_strings_kernel, dim3((unsigned)R), dim3(32), 0, (cudaStream_t)stream, tok, seq, seq_stride, len, len_stride, active,
+           row_slot, row_idx, tab, tab_stride, per_slot, hit, (int64_t)0, 0, 0);
+  return check_launch(name);
+}
+}  // namespace uvx
+
+extern "C" int uvx_stop_strings(const int64_t* tok, int64_t B, const int64_t* seq, int64_t seq_stride, const int32_t* cur_len,
+                                const int32_t* tab, int32_t* hit, uvx_stream_t stream) {
+  return uvx::stop_strings_launch("uvx_stop_strings", B, tok, seq, seq_stride, cur_len, 0, nullptr, nullptr, nullptr, tab, 0, 0,
+                                  hit, stream);
+}
+
+extern "C" int uvx_stop_strings_slots(const int64_t* tok, int64_t B, const int64_t* seq, int64_t seq_stride, const int32_t* cur_len,
+                                      const int32_t* active, const int32_t* tab, int64_t tab_stride, int32_t* hit, uvx_stream_t stream) {
+  UVX_REQUIRE(active, "uvx_stop_strings_slots: bad arguments");
+  return uvx::stop_strings_launch("uvx_stop_strings_slots", B, tok, seq, seq_stride, cur_len, 1, active, nullptr, nullptr, tab,
+                                  tab_stride, 1, hit, stream);
+}
+
+extern "C" int uvx_stop_strings_rows(const int64_t* tok, int64_t R, const int64_t* seq, int64_t seq_stride, const int32_t* len,
+                                     const int32_t* tab, int32_t* hit, uvx_stream_t stream) {
+  return uvx::stop_strings_launch("uvx_stop_strings_rows", R, tok, seq, seq_stride, len, 1, nullptr, nullptr, nullptr, tab, 0, 0,
+                                  hit, stream);
+}
+
+extern "C" int uvx_stop_strings_rows_map(const int64_t* tok, int64_t R, const int64_t* seq, int64_t seq_stride, const int32_t* active,
+                                         const int32_t* row_slot, const int32_t* row_len, const int32_t* row_idx, const int32_t* tab,
+                                         int64_t tab_stride, int32_t* hit, uvx_stream_t stream) {
+  UVX_REQUIRE(active && row_slot && row_idx, "uvx_stop_strings_rows_map: bad arguments");
+  return uvx::stop_strings_launch("uvx_stop_strings_rows_map", R, tok, seq, seq_stride, row_len, 1, active, row_slot, row_idx, tab,
+                                  tab_stride, 1, hit, stream);
+}
+
+extern "C" int uvx_stop_strings_beam(const int64_t* cand_i, int64_t B, int32_t nb, int32_t K, int64_t V, const int64_t* run_seq,
+                                     int64_t seq_stride, const int32_t* cur_len, const int32_t* tab, int32_t* hit,
+                                     uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(cand_i && run_seq && cur_len && tab && hit && B >= 1 && nb >= 1 && nb <= kBeamMax && K >= 1 && K <= kBeamMaxK &&
+                  V >= 1 && B * K < 65536 && seq_stride >= 1,
+              "uvx_stop_strings_beam: bad arguments");
+  launch_k(stop_strings_kernel, dim3((unsigned)(B * K)), dim3(32), 0, (cudaStream_t)stream, cand_i, run_seq, seq_stride, cur_len,
+           (int64_t)0, (const int32_t*)nullptr, (const int32_t*)nullptr, (const int32_t*)nullptr, tab, (int64_t)0, 0, hit, V,
+           (int)nb, (int)K);
+  return check_launch("uvx_stop_strings_beam");
+}
+
+extern "C" int uvx_token_finish_stop(int64_t* tok, int32_t* done, const int64_t* eos_ids, int32_t n_eos, int64_t pad_id, int64_t* seq,
+                                     int64_t seq_stride, int32_t* cur_len, int32_t* step_idx, int32_t* bump0, int32_t* bump1,
+                                     int32_t* bump2, int32_t* all_done, int64_t B, const int32_t* hit, int32_t* fin_len,
+                                     uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(tok && done && cur_len && hit && fin_len && B >= 1 && (n_eos == 0 || eos_ids), "uvx_token_finish_stop: bad arguments");
+  launch_k(token_finish_kernel<true>, dim3(1), dim3(128), 0, (cudaStream_t)stream, tok, done, eos_ids, (int)n_eos, pad_id, seq,
+           seq_stride, cur_len, step_idx, bump0, bump1, bump2, all_done, B, hit, fin_len);
+  return check_launch("token_finish_kernel (stop)");
+}
+
+extern "C" int uvx_slot_finish_stop(const int64_t* tok, int32_t* done, const int64_t* eos_ids, int32_t n_eos, int64_t* seq,
+                                    int64_t seq_stride, int32_t* cur_len, int32_t* n_new, const int32_t* max_new, const int32_t* active,
+                                    int32_t* pos, int32_t* lens, int32_t* rope_pos, int32_t* n_open, int64_t B, const int32_t* hit,
+                                    uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(tok && done && seq && cur_len && n_new && max_new && active && pos && lens && rope_pos && n_open && hit && B >= 1 &&
+                  n_eos >= 0 && (n_eos == 0 || eos_ids),
+              "uvx_slot_finish_stop: bad arguments");
+  launch_k(slot_finish_kernel<true>, dim3(1), dim3(128), 0, (cudaStream_t)stream, tok, done, eos_ids, (int)n_eos, seq, seq_stride,
+           cur_len, n_new, max_new, active, pos, lens, rope_pos, n_open, B, hit);
+  return check_launch("slot_finish_kernel (stop)");
+}
+
+extern "C" int uvx_lookup_accept_stop(const int64_t* pick, const int64_t* tok, const int32_t* n_draft, const int64_t* eos_ids,
+                                      int32_t n_eos, int64_t* seq, int32_t* cur_len, int32_t* n_new, int32_t max_new, int32_t* step,
+                                      int32_t* accepted, int32_t steps, int32_t* done, const int32_t* hit, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(pick && tok && n_draft && seq && cur_len && n_new && done && hit && (n_eos == 0 || eos_ids) && n_eos >= 0 &&
+                  max_new >= 1 && (!accepted || (step && steps >= 0)),
+              "uvx_lookup_accept_stop: bad arguments");
+  launch_k(lookup_accept_kernel<true>, dim3(1), dim3(32), 0, (cudaStream_t)stream, pick, tok, n_draft, eos_ids, (int)n_eos, seq,
+           cur_len, n_new, (int)max_new, step, accepted, (int)steps, done, hit);
+  return check_launch("lookup_accept_kernel (stop)");
+}
+
+extern "C" int uvx_lookup_accept_slots_stop(const int64_t* pick, const int64_t* tok, const int32_t* n_draft, int64_t slots, int32_t K,
+                                            const int64_t* eos_ids, int32_t n_eos, int64_t* seq, int64_t seq_stride, int64_t* token,
+                                            int32_t* done, int32_t* cur_len, int32_t* n_new, const int32_t* max_new,
+                                            const int32_t* active, int32_t* pos, int32_t* lens, int32_t* rope_pos, int32_t* accepted,
+                                            int32_t* n_open, const int32_t* hit, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(pick && tok && n_draft && seq && token && done && cur_len && n_new && max_new && active && pos && lens && rope_pos &&
+                  accepted && n_open && hit && (n_eos == 0 || eos_ids) && n_eos >= 0 && slots >= 1 && slots < 65536 && K >= 1 &&
+                  K <= kLookupMaxK,
+              "uvx_lookup_accept_slots_stop: bad arguments (1 <= K <= %d)", kLookupMaxK);
+  const int warps = slots < 32 ? (int)slots : 32;
+  launch_k(lookup_accept_slots_kernel<true>, dim3(1), dim3(32 * warps), 0, (cudaStream_t)stream, pick, tok, n_draft, (int)K,
+           eos_ids, (int)n_eos, seq, seq_stride, token, done, cur_len, n_new, max_new, active, pos, lens, rope_pos, accepted, n_open,
+           (int)slots, hit);
+  return check_launch("lookup_accept_slots_kernel (stop)");
 }
 
 extern "C" int uvx_log_softmax(const float* in, float* out, int64_t rows, int64_t V, uvx_stream_t stream) {
@@ -1986,10 +2205,31 @@ extern "C" int uvx_beam_update(const float* cand_s, const int64_t* cand_i, int64
                   K <= kBeamMaxK && V >= 1 && (n_eos == 0 || eos_ids) && n_eos >= 0 && max_new >= 1 && early_stopping >= 0 &&
                   early_stopping <= 2,
               "uvx_beam_update: bad arguments");
-  launch_k(beam_update_kernel, dim3((unsigned)B), dim3(256), 0, (cudaStream_t)stream, cand_s, cand_i, V, (int)nb, (int)K, eos_ids,
-           (int)n_eos, (int)max_new, len_div, (int)early_stopping, (int)lp_positive, run_score, run_seq, pool_seq, seq_stride,
-           pool_score, pool_len, pool_fin, parent, tok, heur, flags, ticket, cur_len, step_idx, bump0, bump1, bump2, done, B);
+  launch_k(beam_update_kernel<false>, dim3((unsigned)B), dim3(256), 0, (cudaStream_t)stream, cand_s, cand_i, V, (int)nb, (int)K,
+           eos_ids, (int)n_eos, (int)max_new, len_div, (int)early_stopping, (int)lp_positive, run_score, run_seq, pool_seq,
+           seq_stride, pool_score, pool_len, pool_fin, parent, tok, heur, flags, ticket, cur_len, step_idx, bump0, bump1, bump2,
+           done, B, (const int32_t*)nullptr);
   return check_launch("beam_update_kernel");
+}
+
+extern "C" int uvx_beam_update_stop(const float* cand_s, const int64_t* cand_i, int64_t B, int32_t nb, int32_t K, int64_t V,
+                                    const int64_t* eos_ids, int32_t n_eos, int32_t max_new, const float* len_div,
+                                    int32_t early_stopping, int32_t lp_positive, float* run_score, int64_t* run_seq,
+                                    int64_t* pool_seq, int64_t seq_stride, float* pool_score, int32_t* pool_len, int32_t* pool_fin,
+                                    int32_t* parent, int64_t* tok, int32_t* heur, int32_t* flags, uint32_t* ticket,
+                                    int32_t* cur_len, int32_t* step_idx, int32_t* bump0, int32_t* bump1, int32_t* bump2,
+                                    int32_t* done, const int32_t* hit, uvx_stream_t stream) {
+  using namespace uvx;
+  UVX_REQUIRE(cand_s && cand_i && len_div && run_score && run_seq && pool_seq && pool_score && pool_len && pool_fin && parent && tok &&
+                  heur && flags && ticket && cur_len && step_idx && done && hit && B >= 1 && nb >= 1 && nb <= kBeamMax && K >= nb &&
+                  K <= kBeamMaxK && V >= 1 && (n_eos == 0 || eos_ids) && n_eos >= 0 && max_new >= 1 && early_stopping >= 0 &&
+                  early_stopping <= 2,
+              "uvx_beam_update_stop: bad arguments");
+  launch_k(beam_update_kernel<true>, dim3((unsigned)B), dim3(256), 0, (cudaStream_t)stream, cand_s, cand_i, V, (int)nb, (int)K,
+           eos_ids, (int)n_eos, (int)max_new, len_div, (int)early_stopping, (int)lp_positive, run_score, run_seq, pool_seq,
+           seq_stride, pool_score, pool_len, pool_fin, parent, tok, heur, flags, ticket, cur_len, step_idx, bump0, bump1, bump2,
+           done, B, hit);
+  return check_launch("beam_update_kernel (stop)");
 }
 
 extern "C" int uvx_kv_reorder(void* k_cache, void* v_cache, int64_t L, int64_t B, int32_t nb, int64_t S_max, int64_t row_elems,

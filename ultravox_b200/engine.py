@@ -202,6 +202,15 @@ def check_lookup_k(slots: int, k) -> int:
     return int(k)
 
 
+def check_stop_table(n) -> Optional[int]:
+    """The slot engines' ``max_stop_table`` (None: off); ValueError unless None or an integer >= the table header."""
+    if n is None:
+        return None
+    if isinstance(n, bool) or not isinstance(n, numbers.Integral) or n < ops.STOP_HEADER:
+        raise ValueError(f"max_stop_table must be None or an integer >= {ops.STOP_HEADER} (int32 words per slot), got {n!r}")
+    return int(n)
+
+
 def check_constraint_tokens(n) -> Optional[int]:
     """The slot engines' ``max_constraint_tokens`` (None: off); ValueError unless None or an integer >= 0."""
     if n is None:
@@ -486,7 +495,7 @@ class DecodeEngine(_Decoder):
                  eos_token_ids=None, pad_token_id: int = 0, temperature: float = 0.0, top_k: int = 0,
                  repetition_penalty: float = 1.0, generator: Optional[torch.Generator] = None, top_p: Optional[float] = None,
                  output_scores: bool = False, output_logits: bool = False, max_new_tokens: Optional[int] = None,
-                 constraints=None, cutoffs=None):
+                 constraints=None, cutoffs=None, stop=None):
         """``output_scores`` / ``output_logits``: every pick (the first one, in ``begin``, is step 0) also records HF's processed
         scores / the raw logits of its rows into ``scores`` / ``raw_logits`` [max_new_tokens, batch, V] fp32, at the device
         step counter (``uvx_record_scores``).  That is one [batch, V] fp32 tensor per generated token, which is what HF's
@@ -497,7 +506,11 @@ class DecodeEngine(_Decoder):
         sequences, before the repetition penalty.  None (the default): nothing is allocated and the step is unchanged.
 
         ``cutoffs``: (min_p, typical_p, epsilon, eta) after top-p (``uvx_sample_cutoffs`` / ``uvx_record_scores_cutoffs``), off
-        encoded as (0, 1, 0, 0).  With none on (or None) the step launches exactly the kernels it launches without them."""
+        encoded as (0, 1, 0, 0).  With none on (or None) the step launches exactly the kernels it launches without them.
+
+        ``stop`` (``stop_strings.StopStrings``): every pick runs ``uvx_stop_strings`` on the picked tokens and finishes with
+        ``uvx_token_finish_stop``, so a row whose token ends a stop string finishes as on an EOS id; ``fin_len`` [batch] holds
+        each finished row's length at the step it finished.  None (the default): nothing is allocated and the step is unchanged."""
         super().__init__(model, batch, _RowKV(cache if cache is not None else model.new_cache(batch, max_len)), eos_token_ids,
                          pad_token_id, use_graph)
         dev = model.device
@@ -524,6 +537,11 @@ class DecodeEngine(_Decoder):
             self.raw_logits = torch.empty(shape, dtype=torch.float32, device=dev) if output_logits else None
         self.constraints = None if constraints is None else constraints.device_tables(dev)
         self.cutoffs = tuple(float(v) for v in cutoffs) if ops.cutoffs_on(cutoffs) else None
+        self.stop = None
+        if stop is not None:
+            self.stop = stop.device_table(dev)
+            self.stop_hit = torch.zeros(batch, dtype=torch.int32, device=dev)
+            self.fin_len = torch.zeros(batch, dtype=torch.int32, device=dev)
 
     # -- state ---------------------------------------------------------------------------------------------
     def begin(self, input_ids: torch.Tensor, first_logits: torch.Tensor, kv_start: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -537,6 +555,8 @@ class DecodeEngine(_Decoder):
         self.step_idx.zero_()
         self.done.zero_()
         self.all_done.zero_()
+        if self.stop is not None:
+            self.fin_len.zero_()
         self.kv_start = kv_start
         self._seed(slice(None), S, 0 if kv_start is None else kv_start.to(torch.int32))
         self._pick(first_logits.contiguous())
@@ -570,11 +590,16 @@ class DecodeEngine(_Decoder):
             ops.sample(logits, self.temperature, self.top_k, self.u, self.step_idx, out=tok, top_p=self.top_p, cutoffs=self.cutoffs)
         else:
             ops.argmax(logits, out=tok)
+        stop = None
+        if self.stop is not None:
+            ops.stop_strings(tok, self.seq, self.cur_len, self.stop, self.stop_hit)
+            stop = (self.stop_hit, self.fin_len)
         ops.token_finish(tok, self.done, self.eos, self.pad_id, self.seq, self.cur_len, self.step_idx,
-                         (self.pos, self.lens, self.rope_pos), self.all_done)
+                         (self.pos, self.lens, self.rope_pos), self.all_done, stop=stop)
 
     def _state(self):
-        return [self.pos, self.lens, self.rope_pos, self.token, self.cur_len, self.step_idx, self.done, self.all_done]
+        fin = [self.fin_len] if self.stop is not None else []
+        return [self.pos, self.lens, self.rope_pos, self.token, self.cur_len, self.step_idx, self.done, self.all_done] + fin
 
 
 class _SeqKV(_RowKV):
@@ -614,11 +639,13 @@ class LookupDecodeEngine(_Decoder):
                  use_graph: bool = True, cache=None, eos_token_ids=None, pad_token_id: int = 0, temperature: float = 0.0,
                  top_k: int = 0, top_p: Optional[float] = None, repetition_penalty: float = 1.0,
                  generator: Optional[torch.Generator] = None, output_scores: bool = False, output_logits: bool = False,
-                 uniforms: Optional[int] = None, constraints=None, cutoffs=None):
+                 uniforms: Optional[int] = None, constraints=None, cutoffs=None, stop=None):
         """``uniforms``: how many uniforms to draw when sampling, default S + max_new_tokens + 1 - the count ``DecodeEngine``
         draws (its cache capacity + 1) for the same call, so that a seeded ``generator`` gives the same tokens.
         ``constraints``: as ``DecodeEngine``'s, row i over the sequence up to its position (``uvx_logits_constraints_rows``).
-        ``cutoffs``: as ``DecodeEngine``'s, on every row."""
+        ``cutoffs``: as ``DecodeEngine``'s, on every row.
+        ``stop``: as ``DecodeEngine``'s; row i is checked after the sequence up to its position (``uvx_stop_strings_rows``) and
+        the accept is cut at the first row that ends a stop string (``uvx_lookup_accept_stop``), which finishes the sequence."""
         k, n, S, N = int(num_tokens), int(ngram), int(prompt_len), int(max_new_tokens)
         if not 1 <= k <= ops.LOOKUP_MAX_K:
             raise ValueError(f"prompt_lookup_num_tokens must be in [1, {ops.LOOKUP_MAX_K}], got {num_tokens}")
@@ -662,6 +689,8 @@ class LookupDecodeEngine(_Decoder):
         self.raw_logits = torch.empty(N, 1, V, dtype=torch.float32, device=dev) if output_logits else None
         self.constraints = None if constraints is None else constraints.device_tables(dev)
         self.cutoffs = tuple(float(v) for v in cutoffs) if ops.cutoffs_on(cutoffs) else None
+        self.stop = None if stop is None else stop.device_table(dev)
+        self.stop_hit = torch.zeros(k + 1, **i32) if stop is not None else None
 
     def begin(self, input_ids: torch.Tensor, first_logits: torch.Tensor) -> None:
         """After the prompt input_ids [1, S] has been prefilled into the cache: seeds the sequence and the counters and picks the
@@ -699,8 +728,11 @@ class LookupDecodeEngine(_Decoder):
             ops.sample(logits, self.temperature, self.top_k, self.u, self.n_new, out=pick, top_p=self.top_p, cutoffs=self.cutoffs)
         else:
             ops.argmax(logits, out=pick)
+        hit = None
+        if self.stop is not None:
+            hit = ops.stop_strings_rows(pick, self.seq.view(1, -1).expand(R, -1), self.pen_len[:R], self.stop, self.stop_hit[:R])
         ops.lookup_accept(pick, self.token.view(-1)[:R], self.n_draft, self.eos, self.seq, self.cur_len, self.n_new, self.max_new,
-                          self.done, self.step_idx if log else None, self.accepted if log else None)
+                          self.done, self.step_idx if log else None, self.accepted if log else None, hit=hit)
 
     def _step(self):
         ops.lookup_draft(self.seq, self.cur_len, self.n_new, self.max_new, self.k, self.ngram, self.eos, self.done,
@@ -724,7 +756,10 @@ class BeamDecodeEngine(DecodeEngine):
 
     def __init__(self, model: UltravoxModel, batch: int, num_beams: int, max_len: int, max_new_tokens: int, use_graph: bool = True,
                  cache=None, eos_token_ids=None, length_penalty: float = 1.0, early_stopping=False, repetition_penalty: float = 1.0,
-                 constraints=None):
+                 constraints=None, stop=None):
+        """``stop`` (``stop_strings.StopStrings``): every step checks each candidate's sequence (its parent's running sequence
+        plus its token, ``uvx_stop_strings_beam``) and a hit finishes the candidate as an EOS id does (``uvx_beam_update_stop``),
+        as HF's ``_beam_search`` does with ``StopStringCriteria``.  None: the step is unchanged."""
         nb = int(num_beams)
         if not 1 <= nb <= ops.BEAM_MAX:
             raise ValueError(f"num_beams must be in [1, {ops.BEAM_MAX}], got {num_beams}")
@@ -767,6 +802,8 @@ class BeamDecodeEngine(DecodeEngine):
                           pool_len=self.pool_len, pool_fin=self.pool_fin, parent=self.parent, tok=self.token.view(-1),
                           heur=self.heur, flags=self.flags, ticket=self.ticket)
         self._counters = dict(cur_len=self.cur_len, step_idx=self.step_idx, done=self.all_done)
+        self.beam_stop = None if stop is None else stop.device_table(dev)
+        self.beam_hit = torch.zeros(batch * self.K, **i32) if stop is not None else None
 
     def begin(self, input_ids: torch.Tensor, first_logits: torch.Tensor, kv_start: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``input_ids`` [batch, S] prompts prefilled into cache rows b * num_beams, ``first_logits`` [batch, V] their last
@@ -810,8 +847,11 @@ class BeamDecodeEngine(DecodeEngine):
         if self.penalty != 1.0:
             ops.repetition_penalty_(lp, self.seq, self.cur_len, self.penalty, self.scratch)
         s, i = ops.beam_select(lp, self.run_score, self.nb, self.K, scratch=self.row_buf, out=self.cand)
+        hit = None
+        if self.beam_stop is not None:      # before the update rewrites the running sequences
+            hit = ops.stop_strings_beam(i, self.V, self.nb, self.seq, self.cur_len, self.beam_stop, self.beam_hit)
         ops.beam_update(s, i, self.V, self.nb, self.eos, self.max_new, self.len_div, self.es, self.length_penalty > 0.0, self._beam,
-                        self._counters, (self.pos, self.lens, self.rope_pos))
+                        self._counters, (self.pos, self.lens, self.rope_pos), hit=hit)
         # the update advanced pos to the slot of the token fed next: the cache holds positions [0, pos)
         ops.kv_reorder_(self.cache.k, self.cache.v, self.parent, self.pos, self.nb)
 
@@ -882,22 +922,29 @@ class SlotDecodeEngine(_Decoder):
     ``ck_end``, ``ck_bias``, ``ck_kind`` [slots, max(N, 1)]), written by ``admit(..., constraints=...)`` between replays and
     cleared when the slot goes idle.  Every pick (the plain, mixed and lookup steps' and the admission pick) then runs
     ``uvx_logits_constraints_slots`` (``_rows_map`` in the lookup step) after the raw copy for log-probs and before the penalty.
-    None allocates nothing and launches nothing: the steps are unchanged."""
+    None allocates nothing and launches nothing: the steps are unchanged.
+
+    ``max_stop_table`` = N (None, the default: off) adds ``generate()``'s stop strings per slot: ``stop_tab`` [slots, N] int32
+    holds each slot's packed table (``stop_strings.StopStrings``, written by ``admit(..., stop=...)``; a slot without stop
+    strings has an all-zero header).  Every pick then runs ``uvx_stop_strings_slots`` after the sampler and finishes with
+    ``uvx_slot_finish_stop`` (the lookup step: ``uvx_stop_strings_rows_map`` and ``uvx_lookup_accept_slots_stop``), so a slot
+    whose token ends a stop string finishes as on an EOS id.  None allocates and launches nothing."""
 
     def __init__(self, model: UltravoxModel, slots: int, max_len: int, eos_token_ids=None, pad_token_id: int = 0,
                  use_graph: bool = True, cache=None, max_logprobs: int = 0, prompt_lookup_num_tokens: Optional[int] = None,
-                 max_constraint_tokens: Optional[int] = None):
+                 max_constraint_tokens: Optional[int] = None, max_stop_table: Optional[int] = None):
         check_lookup_k(int(slots), prompt_lookup_num_tokens)      # before the cache is allocated
         kv = _RowKV(cache if cache is not None else model.new_cache(slots, max_len))
         self._setup(model, int(slots), kv, eos_token_ids, pad_token_id, use_graph, max_logprobs, prompt_lookup_num_tokens,
-                    max_constraint_tokens)
+                    max_constraint_tokens, max_stop_table)
 
     def _setup(self, model: UltravoxModel, slots: int, kv, eos_token_ids, pad_token_id: int, use_graph: bool, max_logprobs: int = 0,
-               lookup_k: Optional[int] = None, max_constraint_tokens: Optional[int] = None):
+               lookup_k: Optional[int] = None, max_constraint_tokens: Optional[int] = None, max_stop_table: Optional[int] = None):
         if isinstance(max_logprobs, bool) or not isinstance(max_logprobs, numbers.Integral) or \
                 not 0 <= max_logprobs <= ops.LOGPROBS_MAX:
             raise ValueError(f"max_logprobs must be an integer in [0, {ops.LOGPROBS_MAX}], got {max_logprobs!r}")
         self.max_constraint_tokens = check_constraint_tokens(max_constraint_tokens)
+        self.max_stop_table = check_stop_table(max_stop_table)
         self.K = check_lookup_k(slots, lookup_k)
         self.max_logprobs = int(max_logprobs)
         self.slots = slots
@@ -966,6 +1013,12 @@ class SlotDecodeEngine(_Decoder):
             self.ck_end, self.ck_kind = torch.zeros(slots, T, **i32), torch.zeros(slots, T, **i32)
             self.ck_bias = torch.zeros(slots, T, **f32)
             self.ck = (self.ck_cfg, self.ck_ids, self.ck_end, self.ck_bias, self.ck_kind)
+        self.stop_tab = None
+        if self.max_stop_table is not None:
+            self.stop_tab = torch.zeros(slots, self.max_stop_table, **i32)
+            self.stop_hit = torch.zeros(slots, **i32)
+            if self.K:
+                self._lk_hit = torch.zeros(slots * (self.K + 1), **i32)
         self.busy = [False] * slots
         for j in range(slots):
             self._idle(j)
@@ -989,6 +1042,8 @@ class SlotDecodeEngine(_Decoder):
             self._slot_k[j] = 0
         if self.ck is not None:
             self.ck_cfg[j] = 0          # no n-gram size and no entries: the kernel leaves the row alone
+        if self.stop_tab is not None:
+            self.stop_tab[j, :ops.STOP_HEADER] = 0      # no stop strings: no hit
         self.kv.release(j)
 
     def _state(self):
@@ -1014,9 +1069,13 @@ class SlotDecodeEngine(_Decoder):
         ops.sample_rows_cutoffs(logits, self.temps, self.top_ks, self.top_ps, self.cutoffs, self.u, self.active, *rows, self._lk_pick)
         if self.max_logprobs:       # at n_new + i, before the accept advances n_new; rows past the drafts (idx -1) record nothing
             ops.token_logprobs_rows(self._lk_raw, self._lk_pick, self.n_top, *rows, self.lp_token, self.lp_ids, self.lp_top)
+        hit = None
+        if self.stop_tab is not None:
+            hit = ops.stop_strings_rows_map(self._lk_pick, self.seq, self.active, self._lk_slot, self._lk_pen, self._lk_idx,
+                                            self.stop_tab, self._lk_hit)
         ops.lookup_accept_slots(self._lk_pick, self._lk_tok.view(-1), self.n_draft, self.K, self.eos, self.seq, self.token.view(-1),
                                 self.done, self.cur_len, self.n_new, self.max_new, self.active, self.pos, self.lens, self.rope_pos,
-                                self.accepted, self.n_open)
+                                self.accepted, self.n_open, hit=hit)
 
     def _pick_rows(self, logits: torch.Tensor, r: slice, n_open: torch.Tensor) -> None:
         tok = self.token.view(-1)[r]
@@ -1030,8 +1089,11 @@ class SlotDecodeEngine(_Decoder):
                                  self.active[r], tok)
         if self.max_logprobs:       # at n_new, before the finish kernel advances it
             ops.token_logprobs(raw, tok, self.n_top[r], self.n_new[r], self.lp_token[r], self.lp_ids[r], self.lp_top[r])
+        hit = None
+        if self.stop_tab is not None:
+            hit = ops.stop_strings_slots(tok, self.seq[r], self.cur_len[r], self.active[r], self.stop_tab[r], self.stop_hit[r])
         ops.slot_finish(tok, self.done[r], self.eos, self.seq[r], self.cur_len[r], self.n_new[r], self.max_new[r], self.active[r],
-                        self.pos[r], self.lens[r], self.rope_pos[r], n_open)
+                        self.pos[r], self.lens[r], self.rope_pos[r], n_open, hit=hit)
 
     def _pick(self, logits: torch.Tensor):
         self.logits = logits
@@ -1094,7 +1156,7 @@ class SlotDecodeEngine(_Decoder):
     def admit(self, slot: int, input_ids: torch.Tensor, max_new_tokens: int, temperature: float = 0.0, top_k: int = 0,
               top_p: float = 1.0, repetition_penalty: float = 1.0, u: Optional[torch.Tensor] = None, past: int = 0,
               pages=None, logprobs: Optional[int] = None, lookup: Optional[tuple] = None, constraints=None, cutoffs=None,
-              **features) -> torch.Tensor:
+              stop=None, **features) -> torch.Tensor:
         """Prefills one request (``input_ids`` [1, S] plus the processor's audio features, passed to ``model.forward``) at B = 1
         into cache row ``slot``, sets the slot's state and picks its first token from the prefill logits with the slot kernels.
         ``temperature <= 0`` is greedy; a sampled request reads ``u`` (its uniforms, one per step, as ``generate()`` draws them
@@ -1120,9 +1182,13 @@ class SlotDecodeEngine(_Decoder):
         with its whole prompt's length), at most N ids; None: no constraints.
 
         ``cutoffs``: the request's (min_p, typical_p, epsilon, eta), as ``generate()`` checks them, off = (0, 1, 0, 0) (None:
-        all off).  Every pick reads them from ``cutoffs`` [slots, 4] (``uvx_sample_slots_cutoffs`` / ``_rows_cutoffs``)."""
+        all off).  Every pick reads them from ``cutoffs`` [slots, 4] (``uvx_sample_slots_cutoffs`` / ``_rows_cutoffs``).
+
+        ``stop`` (engines with ``max_stop_table`` = N): the request's ``stop_strings.StopStrings``, a table of at most N words;
+        None: no stop strings."""
         n_top = self.check_logprobs(logprobs)
         ck_rows = self.check_constraints(constraints)
+        self.check_stop(stop)
         lk, ln = (0, 2) if lookup is None else (int(lookup[0]), int(lookup[1]))
         if lookup is not None and not self.K:
             raise ValueError("this engine has no prompt lookup: create it with prompt_lookup_num_tokens = K")
@@ -1189,6 +1255,11 @@ class SlotDecodeEngine(_Decoder):
             else:
                 for t, a in zip(self.ck, ck_rows):
                     t[j].copy_(torch.from_numpy(a))
+        if self.stop_tab is not None:
+            if stop is None:
+                self.stop_tab[j, :ops.STOP_HEADER] = 0
+            else:
+                self.stop_tab[j, :stop.n_words].copy_(stop.device_table(self.stop_tab.device))     # device to device
         if not chunked:
             if self.max_logprobs:
                 self.n_top[j] = n_top
@@ -1206,6 +1277,17 @@ class SlotDecodeEngine(_Decoder):
             raise ValueError(f"the request's constraints need a table of {constraints.n_ids} ids; max_constraint_tokens = "
                              f"{self.max_constraint_tokens}")
         return constraints.tables(self.ck_ids.shape[1])
+
+    def check_stop(self, stop) -> None:
+        """ValueError when a request has stop strings (``stop_strings.StopStrings``) and the engine has no stop tables or the
+        request's table is longer than ``max_stop_table`` words."""
+        if stop is None:
+            return
+        if self.stop_tab is None:
+            raise ValueError("this engine has no stop strings: create it with max_stop_table = N")
+        if stop.n_words > self.max_stop_table:
+            raise ValueError(f"the request's stop strings need a table of {stop.n_words} int32 words; max_stop_table = "
+                             f"{self.max_stop_table}")
 
     def check_logprobs(self, logprobs) -> int:
         """The slot kernels' n_top of a request's ``logprobs`` argument (None -> -1); ValueError unless it is None or an integer
@@ -1256,11 +1338,12 @@ class PagedSlotDecodeEngine(SlotDecodeEngine):
 
     def __init__(self, model: UltravoxModel, slots: int, max_len: int, kv_pages: int, eos_token_ids=None, pad_token_id: int = 0,
                  use_graph: bool = True, max_logprobs: int = 0, kv_cache_dtype: str = "bf16", kv_scales=None, host_kv_pages: int = 0,
-                 prompt_lookup_num_tokens: Optional[int] = None, max_constraint_tokens: Optional[int] = None):
+                 prompt_lookup_num_tokens: Optional[int] = None, max_constraint_tokens: Optional[int] = None,
+                 max_stop_table: Optional[int] = None):
         check_lookup_k(int(slots), prompt_lookup_num_tokens)      # before the pool is allocated
         kv = _PagedKV(model, int(slots), max_len, kv_pages, kv_cache_dtype, kv_scales, host_kv_pages)
         self.kv_pages, self.pool_k, self.pool_v, self.kv_scales = kv.kv_pages, kv.pool_k, kv.pool_v, kv.kv_scales
         self.host_kv_pages, self.host_k, self.host_v = kv.host_kv_pages, kv.host_k, kv.host_v
         self.swap_out, self.swap_in = kv.swap_out, kv.swap_in
         self._setup(model, int(slots), kv, eos_token_ids, pad_token_id, use_graph, max_logprobs, prompt_lookup_num_tokens,
-                    max_constraint_tokens)
+                    max_constraint_tokens, max_stop_table)

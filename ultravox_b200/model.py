@@ -901,7 +901,7 @@ class UltravoxModel(nn.Module):
                  bad_words_ids=None, sequence_bias=None, min_length: Optional[int] = None, min_new_tokens: Optional[int] = None,
                  suppress_tokens=None, begin_suppress_tokens=None, min_p: Optional[float] = None,
                  typical_p: Optional[float] = None, epsilon_cutoff: Optional[float] = None, eta_cutoff: Optional[float] = None,
-                 **kwargs):
+                 stop_strings=None, tokenizer=None, **kwargs):
         """``GenerationMixin.generate`` for this model (ref :398-426; arguments as ``LocalInference._generate`` passes them, ref
         infer.py:309-342).  Returns prompt ids followed by the new tokens.
 
@@ -976,9 +976,22 @@ class UltravoxModel(nn.Module):
         (``uvx_logits_constraints``) applies them inside the captured step before the penalty, which gives HF's scores (up to the
         sign of a zero score: HF's bias processors turn -0.0 into +0.0 in every column).
         They work with greedy and sampled decoding, padded batches, conversation turns, the streamer, prompt lookup and beams
-        (on the log-probs, as HF); ``output_scores`` then holds the constrained scores and ``output_logits`` the raw ones."""
+        (on the log-probs, as HF); ``output_scores`` then holds the constrained scores and ``output_logits`` the raw ones.
+
+        ``stop_strings`` (a str or a list of str) with ``tokenizer``: a row finishes when its text ends with one of the strings,
+        by transformers 5.5's ``StopStringCriteria`` rule (built here from ``tokenizer``; a string may start or end inside a
+        token, and may begin in the prompt).  The finishing token is kept, later tokens of that row are ``pad_token_id`` and
+        the output ends at the step the last row finished, as for an EOS id; the stop text is not trimmed.  ``ValueError``
+        without a tokenizer, for an empty string or list, and when no vocabulary token can end a string; ``tokenizer`` alone is
+        ignored.  The check runs on the device after every pick (``uvx_stop_strings``), so the step stays one graph replay.
+        Two differences from HF: in a batch without EOS ids, HF's stopped rows keep sampling where these emit pad (B = 1, or
+        any EOS id, gives HF's output); with prompt lookup every accepted position is checked and the accept is cut at the
+        first hit, so the tokens stay those of plain decoding, where HF checks only the last accepted token.  With beam search
+        each step's candidates are checked (``uvx_stop_strings_beam``) and a hit finishes a hypothesis, as HF's ``_beam_search``
+        does."""
         from .constraints import LogitsConstraints
         from .engine import DecodeEngine
+        from .stop_strings import StopStrings
         unknown = [k for k, v in kwargs.items() if isinstance(v, torch.Tensor)]
         if unknown:
             raise TypeError(f"generate() got unexpected tensor arguments {unknown}")
@@ -988,6 +1001,7 @@ class UltravoxModel(nn.Module):
                                                 max_matching_ngram_size)
         if not isinstance(num_beams, int) or not 1 <= num_beams <= ops.BEAM_MAX:
             raise ValueError(f"num_beams must be an integer in [1, {ops.BEAM_MAX}], got {num_beams!r}")
+        stops = StopStrings.build(tokenizer, stop_strings)
         if not isinstance(num_return_sequences, int) or not 1 <= num_return_sequences <= num_beams:
             raise ValueError(f"num_return_sequences ({num_return_sequences!r}) must be in [1, num_beams = {num_beams}]")
         if num_beams > 1:
@@ -1035,7 +1049,7 @@ class UltravoxModel(nn.Module):
                                 audio_batch_size=audio_batch_size, position_ids=position_ids, audio_waveforms=audio_waveforms,
                                 audio_num_frames=audio_num_frames, audio_pad_frames=audio_pad_frames),
                 kv_start, max_new_tokens, eos_token_id, pad_token_id, num_beams, length_penalty, early_stopping,
-                num_return_sequences, repetition_penalty or 1.0, use_graph, constraints=cons)
+                num_return_sequences, repetition_penalty or 1.0, use_graph, constraints=cons, stop=stops)
             if return_dict_in_generate:
                 return GenerateOutput(seqs, None, scores if output_scores else None)
             return seqs
@@ -1071,12 +1085,12 @@ class UltravoxModel(nn.Module):
             return self._lookup_decode(input_ids, out.logits.view(1, -1), cache, k_look, n_look, max_new_tokens, eos, pad_id,
                                        temp, k_top, p_top, repetition_penalty or 1.0, generator, want_scores, want_logits, streamer,
                                        use_graph, (S + max_new_tokens if past_key_values is None else plain_cap) + 1,
-                                       return_dict_in_generate, cons, cutoffs)
+                                       return_dict_in_generate, cons, cutoffs, stops)
         eng = DecodeEngine(self, B, cache.capacity, use_graph=use_graph, cache=cache, eos_token_ids=eos, pad_token_id=pad_id,
                            temperature=temp, top_k=k_top, top_p=p_top, repetition_penalty=repetition_penalty or 1.0,
                            generator=generator, output_scores=want_scores, output_logits=want_logits,
                            max_new_tokens=max_new_tokens if want_scores or want_logits else None, constraints=cons,
-                           cutoffs=cutoffs)
+                           cutoffs=cutoffs, stop=stops)
         if streamer is not None:
             streamer.put(input_ids)
         tok = eng.begin(input_ids, out.logits.view(B, -1), kv_start)
@@ -1086,7 +1100,7 @@ class UltravoxModel(nn.Module):
             if streamer is not None:
                 streamer.put(tok.clone())
             stop = n_new >= max_new_tokens
-            if not stop and eos and (streamer is not None or n_new % sync_every == 0):
+            if not stop and (eos or eng.stop is not None) and (streamer is not None or n_new % sync_every == 0):
                 stop = bool(int(eng.all_done))
             if stop:
                 break
@@ -1095,7 +1109,12 @@ class UltravoxModel(nn.Module):
         if streamer is not None:
             streamer.end()
         new = eng.seq[:, S:S + n_new]
-        if eos and streamer is None and n_new > 1:
+        if eng.stop is not None:
+            # every row has finished: HF stops at the step the last one did (each row's length then is on the device)
+            if n_new > 1 and bool(int(eng.all_done)):
+                n_new = min(n_new, int(eng.fin_len.max()) - S)
+                new = new[:, :n_new]
+        elif eos and streamer is None and n_new > 1:
             # the loop may have run a few tokens past the step at which every row had finished: HF stops right there
             hit = torch.isin(new, eng.eos)
             first = torch.where(hit.any(-1), hit.to(torch.int32).argmax(-1), torch.full((B,), n_new, device=dev))
@@ -1129,14 +1148,14 @@ class UltravoxModel(nn.Module):
     def _lookup_decode(self, input_ids: torch.Tensor, first_logits: torch.Tensor, cache: KVCache, k: int, n: int,
                        max_new_tokens: int, eos, pad_id: int, temp: float, k_top: int, p_top: float, penalty: float, generator,
                        want_scores: bool, want_logits: bool, streamer, use_graph: bool, uniforms: int, return_dict: bool,
-                       constraints=None, cutoffs=None):
+                       constraints=None, cutoffs=None, stop=None):
         """``generate``'s prompt-lookup loop after the prefill of ``input_ids`` [1, S] into ``cache``."""
         from .engine import LookupDecodeEngine
         S = int(input_ids.shape[1])
         eng = LookupDecodeEngine(self, S, max_new_tokens, k, n, use_graph=use_graph, cache=cache, eos_token_ids=eos,
                                  pad_token_id=pad_id, temperature=temp, top_k=k_top, top_p=p_top, repetition_penalty=penalty,
                                  generator=generator, output_scores=want_scores, output_logits=want_logits, uniforms=uniforms,
-                                 constraints=constraints, cutoffs=cutoffs)
+                                 constraints=constraints, cutoffs=cutoffs, stop=stop)
         if streamer is not None:
             streamer.put(input_ids)
         eng.begin(input_ids, first_logits)
@@ -1183,7 +1202,8 @@ class UltravoxModel(nn.Module):
 
     def _beam_search(self, input_ids: torch.Tensor, forward_kw: dict, kv_start: Optional[torch.Tensor], max_new_tokens: int,
                      eos_token_id, pad_token_id: Optional[int], num_beams: int, length_penalty: float, early_stopping,
-                     num_return_sequences: int, repetition_penalty: float, use_graph: bool, step_hook=None, constraints=None):
+                     num_return_sequences: int, repetition_penalty: float, use_graph: bool, step_hook=None, constraints=None,
+                     stop=None):
         """``generate``'s beam branch -> (sequences [B * num_return_sequences, S + longest], their scores).  The B prompts are
         prefilled once into cache rows b * num_beams (a view of the [L, B * num_beams, S_max, ...] cache as B rows of
         num_beams * S_max positions).  ``step_hook(engine)``, if given, runs after every beam step (the host then checks
@@ -1202,7 +1222,7 @@ class UltravoxModel(nn.Module):
                            fk.pop("audio_batch_size"), prompt_rows, logits_to_keep=1, **fk)
         eng = BeamDecodeEngine(self, B, num_beams, cache.capacity, max_new_tokens, use_graph=use_graph, cache=cache,
                                eos_token_ids=eos_list, length_penalty=length_penalty, early_stopping=early_stopping,
-                               repetition_penalty=repetition_penalty, constraints=constraints)
+                               repetition_penalty=repetition_penalty, constraints=constraints, stop=stop)
         eng.begin(input_ids, out.logits.view(B, -1), kv_start)
         n_new = 1
         sync_every = 8          # the host looks at the device's done flag every few steps only

@@ -1019,12 +1019,20 @@ def sample(logits: torch.Tensor, temperature: float, top_k: int, u: torch.Tensor
 
 def token_finish(tok: torch.Tensor, done: torch.Tensor, eos_ids: Optional[torch.Tensor], pad_id: int, seq: Optional[torch.Tensor],
                  cur_len: torch.Tensor, step_idx: Optional[torch.Tensor] = None, bumps: tuple = (),
-                 all_done: Optional[torch.Tensor] = None) -> None:
+                 all_done: Optional[torch.Tensor] = None, stop: Optional[tuple] = None) -> None:
+    """``uvx_token_finish``; ``stop`` = (hit [B] int32, fin_len [B] int32): ``uvx_token_finish_stop``, where a row with hit[b]
+    finishes too and a row finishing in this step gets fin_len[b] = its length."""
     _cuda(tok, torch.int64, "tok"), _cuda(done, torch.int32, "done")
     b = list(bumps) + [None] * (3 - len(bumps))
-    check(lib().uvx_token_finish(tok.data_ptr(), done.data_ptr(), _p(eos_ids), 0 if eos_ids is None else eos_ids.numel(), int(pad_id),
-                                 _p(seq), seq.stride(0) if seq is not None else 0, cur_len.data_ptr(), _p(step_idx), _p(b[0]), _p(b[1]),
-                                 _p(b[2]), _p(all_done), tok.numel(), _stream()), "uvx_token_finish")
+    args = (tok.data_ptr(), done.data_ptr(), _p(eos_ids), 0 if eos_ids is None else eos_ids.numel(), int(pad_id), _p(seq),
+            seq.stride(0) if seq is not None else 0, cur_len.data_ptr(), _p(step_idx), _p(b[0]), _p(b[1]), _p(b[2]), _p(all_done),
+            tok.numel())
+    if stop is None:
+        check(lib().uvx_token_finish(*args, _stream()), "uvx_token_finish")
+        return
+    B = tok.numel()
+    hit, fin_len = _rows(stop[0], torch.int32, B, "hit"), _rows(stop[1], torch.int32, B, "fin_len")
+    check(lib().uvx_token_finish_stop(*args, hit.data_ptr(), fin_len.data_ptr(), _stream()), "uvx_token_finish_stop")
 
 
 # ------------------------------------------------------------------------------------------ continuous batching (slots)
@@ -1107,9 +1115,10 @@ def repetition_penalty_slots_(logits: torch.Tensor, seq: torch.Tensor, cur_len: 
 
 def slot_finish(tok: torch.Tensor, done: torch.Tensor, eos_ids: Optional[torch.Tensor], seq: torch.Tensor, cur_len: torch.Tensor,
                 n_new: torch.Tensor, max_new: torch.Tensor, active: torch.Tensor, pos: torch.Tensor, lens: torch.Tensor,
-                rope_pos: torch.Tensor, n_open: torch.Tensor) -> None:
+                rope_pos: torch.Tensor, n_open: torch.Tensor, hit: Optional[torch.Tensor] = None) -> None:
     """``uvx_slot_finish``: tok [B] int64, seq [B, W] int64, every other per-row array [B] int32, eos_ids int64 or None,
-    n_open [1] int32 (the count of active rows still open)."""
+    n_open [1] int32 (the count of active rows still open).  ``hit`` [B] int32: ``uvx_slot_finish_stop`` (a hit finishes the
+    row as an EOS id does)."""
     B = tok.numel()
     _rows(tok, torch.int64, B, "tok"), _seq_rows(seq, torch.int64, B, "seq")
     for t, name in ((done, "done"), (cur_len, "cur_len"), (n_new, "n_new"), (max_new, "max_new"), (active, "active"), (pos, "pos"),
@@ -1118,9 +1127,13 @@ def slot_finish(tok: torch.Tensor, done: torch.Tensor, eos_ids: Optional[torch.T
     _rows(n_open, torch.int32, 1, "n_open")
     if eos_ids is not None:
         _cuda(eos_ids, torch.int64, "eos_ids")
-    check(lib().uvx_slot_finish(tok.data_ptr(), done.data_ptr(), _p(eos_ids), 0 if eos_ids is None else eos_ids.numel(), seq.data_ptr(),
-                                seq.stride(0), cur_len.data_ptr(), n_new.data_ptr(), max_new.data_ptr(), active.data_ptr(), pos.data_ptr(),
-                                lens.data_ptr(), rope_pos.data_ptr(), n_open.data_ptr(), B, _stream()), "uvx_slot_finish")
+    args = (tok.data_ptr(), done.data_ptr(), _p(eos_ids), 0 if eos_ids is None else eos_ids.numel(), seq.data_ptr(), seq.stride(0),
+            cur_len.data_ptr(), n_new.data_ptr(), max_new.data_ptr(), active.data_ptr(), pos.data_ptr(), lens.data_ptr(),
+            rope_pos.data_ptr(), n_open.data_ptr(), B)
+    if hit is None:
+        check(lib().uvx_slot_finish(*args, _stream()), "uvx_slot_finish")
+    else:
+        check(lib().uvx_slot_finish_stop(*args, _rows(hit, torch.int32, B, "hit").data_ptr(), _stream()), "uvx_slot_finish_stop")
 
 
 # ------------------------------------------------------------------------------------------ log-probabilities
@@ -1304,6 +1317,85 @@ def logits_constraints_rows_map_(logits: torch.Tensor, seq: torch.Tensor, active
     return logits
 
 
+# ------------------------------------------------------------------------------------------ stop strings
+from .stop_strings import HEADER as STOP_HEADER     # noqa: E402  (the table header's words, kStopHdr in generate.cu)
+
+
+def _stop_table(tab: torch.Tensor, rows: Optional[int] = None) -> torch.Tensor:
+    """A packed stop-string table (``stop_strings.StopStrings``): int32 [W] (one) or [rows, W] (one per slot), contiguous."""
+    _cuda(tab, torch.int32, "stop table")
+    if not tab.is_contiguous() or (rows is None and tab.dim() != 1) or (rows is not None and (tab.dim() != 2 or tab.shape[0] != rows)):
+        raise ValueError(f"the stop table must be a contiguous int32 {'[W]' if rows is None else f'[{rows}, W]'} tensor, got "
+                         f"{tuple(tab.shape)}")
+    if tab.shape[-1] < STOP_HEADER:
+        raise ValueError(f"a stop table holds at least its {STOP_HEADER}-word header")
+    return tab
+
+
+def stop_strings(tok: torch.Tensor, seq: torch.Tensor, cur_len: torch.Tensor, table: torch.Tensor, hit: torch.Tensor) -> torch.Tensor:
+    """``uvx_stop_strings``: hit[b] = whether candidate tok[b] after seq[b, :cur_len[0]] ends a stop string of ``table``."""
+    B = tok.numel()
+    _rows(tok, torch.int64, B, "tok"), _seq_rows(seq, torch.int64, B, "seq"), _rows(hit, torch.int32, B, "hit")
+    _rows(cur_len, torch.int32, 1, "cur_len"), _stop_table(table)
+    check(lib().uvx_stop_strings(tok.data_ptr(), B, seq.data_ptr(), seq.stride(0), cur_len.data_ptr(), table.data_ptr(), hit.data_ptr(),
+                                 _stream()), "uvx_stop_strings")
+    return hit
+
+
+def stop_strings_beam(cand_i: torch.Tensor, V: int, num_beams: int, run_seq: torch.Tensor, cur_len: torch.Tensor,
+                      table: torch.Tensor, hit: torch.Tensor) -> torch.Tensor:
+    """``uvx_stop_strings_beam``: candidate c of prompt b (cand_i [B, K] int64 = parent beam * V + token) after its parent's
+    running sequence run_seq[b * num_beams + parent, :cur_len[0]] -> hit [B * K] int32."""
+    _cuda(cand_i, torch.int64, "cand_i")
+    if cand_i.dim() != 2 or not cand_i.is_contiguous():
+        raise ValueError("cand_i must be a contiguous [B, K] tensor")
+    B, K = cand_i.shape
+    _seq_rows(run_seq, torch.int64, B * int(num_beams), "run_seq"), _rows(cur_len, torch.int32, 1, "cur_len")
+    _rows(hit, torch.int32, B * K, "hit"), _stop_table(table)
+    check(lib().uvx_stop_strings_beam(cand_i.data_ptr(), B, int(num_beams), K, int(V), run_seq.data_ptr(), run_seq.stride(0),
+                                      cur_len.data_ptr(), table.data_ptr(), hit.data_ptr(), _stream()), "uvx_stop_strings_beam")
+    return hit
+
+
+def stop_strings_slots(tok: torch.Tensor, seq: torch.Tensor, cur_len: torch.Tensor, active: torch.Tensor, table: torch.Tensor,
+                       hit: torch.Tensor) -> torch.Tensor:
+    """``uvx_stop_strings_slots``: active row b after seq[b, :cur_len[b]] with its own table[b] ([B, W] int32); inactive rows'
+    hit untouched."""
+    B = tok.numel()
+    _rows(tok, torch.int64, B, "tok"), _seq_rows(seq, torch.int64, B, "seq"), _rows(hit, torch.int32, B, "hit")
+    _rows(cur_len, torch.int32, B, "cur_len"), _rows(active, torch.int32, B, "active"), _stop_table(table, B)
+    check(lib().uvx_stop_strings_slots(tok.data_ptr(), B, seq.data_ptr(), seq.stride(0), cur_len.data_ptr(), active.data_ptr(),
+                                       table.data_ptr(), table.stride(0), hit.data_ptr(), _stream()), "uvx_stop_strings_slots")
+    return hit
+
+
+def stop_strings_rows(tok: torch.Tensor, seq: torch.Tensor, lens: torch.Tensor, table: torch.Tensor, hit: torch.Tensor) -> torch.Tensor:
+    """``uvx_stop_strings_rows``: row r after seq[r, :lens[r]] (seq's row stride may be 0: one shared sequence), one table."""
+    R = tok.numel()
+    _rows(tok, torch.int64, R, "tok"), _rows(lens, torch.int32, R, "lens"), _rows(hit, torch.int32, R, "hit"), _stop_table(table)
+    _cuda(seq, torch.int64, "seq")
+    if seq.dim() != 2 or seq.shape[0] != R or seq.stride(1) != 1:
+        raise ValueError(f"seq must be [{R}, W] with unit column stride (row stride 0 allowed), got {tuple(seq.shape)}")
+    check(lib().uvx_stop_strings_rows(tok.data_ptr(), R, seq.data_ptr(), seq.stride(0), lens.data_ptr(), table.data_ptr(), hit.data_ptr(),
+                                      _stream()), "uvx_stop_strings_rows")
+    return hit
+
+
+def stop_strings_rows_map(tok: torch.Tensor, seq: torch.Tensor, active: torch.Tensor, row_slot: torch.Tensor, row_len: torch.Tensor,
+                          row_idx: torch.Tensor, table: torch.Tensor, hit: torch.Tensor) -> torch.Tensor:
+    """``uvx_stop_strings_rows_map``: row r of slot s = row_slot[r] after seq[s, :row_len[r]] with table[s]; rows of inactive
+    slots or with row_idx[r] < 0 untouched."""
+    R, S = tok.numel(), active.numel()
+    _rows(tok, torch.int64, R, "tok"), _seq_rows(seq, torch.int64, S, "seq"), _rows(active, torch.int32, S, "active")
+    for t, name in ((row_slot, "row_slot"), (row_len, "row_len"), (row_idx, "row_idx"), (hit, "hit")):
+        _rows(t, torch.int32, R, name)
+    _stop_table(table, S)
+    check(lib().uvx_stop_strings_rows_map(tok.data_ptr(), R, seq.data_ptr(), seq.stride(0), active.data_ptr(), row_slot.data_ptr(),
+                                          row_len.data_ptr(), row_idx.data_ptr(), table.data_ptr(), table.stride(0), hit.data_ptr(),
+                                          _stream()), "uvx_stop_strings_rows_map")
+    return hit
+
+
 def lookup_draft(seq: torch.Tensor, cur_len: torch.Tensor, n_new: torch.Tensor, max_new: int, k: int, n: int,
                  eos_ids: Optional[torch.Tensor], done: torch.Tensor, tok: torch.Tensor, n_draft: torch.Tensor, pos: torch.Tensor,
                  lens: torch.Tensor, rope_pos: torch.Tensor, pen_len: torch.Tensor, idx: torch.Tensor) -> None:
@@ -1335,10 +1427,11 @@ def lookup_draft(seq: torch.Tensor, cur_len: torch.Tensor, n_new: torch.Tensor, 
 
 def lookup_accept(pick: torch.Tensor, tok: torch.Tensor, n_draft: torch.Tensor, eos_ids: Optional[torch.Tensor], seq: torch.Tensor,
                   cur_len: torch.Tensor, n_new: torch.Tensor, max_new: int, done: torch.Tensor, step: Optional[torch.Tensor] = None,
-                  accepted: Optional[torch.Tensor] = None) -> None:
+                  accepted: Optional[torch.Tensor] = None, hit: Optional[torch.Tensor] = None) -> None:
     """``uvx_lookup_accept`` (include/uvx.h): picks [R] int64 of the rows that fed tok [R] int64 (R >= n_draft[0] + 1) -> the
     agreeing prefix plus one token appended to seq [W] int64 at cur_len[0]; cur_len / n_new / done [1] int32 advance.  With
-    ``accepted`` ([steps] int32) and ``step`` ([1] int32) the step's accepted draft count is logged at step[0]."""
+    ``accepted`` ([steps] int32) and ``step`` ([1] int32) the step's accepted draft count is logged at step[0].  ``hit`` [R]
+    int32: ``uvx_lookup_accept_stop``, the accept cut at the first row with a stop-string hit."""
     R = pick.numel()
     if not 1 <= R <= LOOKUP_MAX_K + 1:
         raise ValueError(f"pick must hold 1..{LOOKUP_MAX_K + 1} rows, got {R}")
@@ -1359,10 +1452,13 @@ def lookup_accept(pick: torch.Tensor, tok: torch.Tensor, n_draft: torch.Tensor, 
         raise ValueError(f"max_new must be >= 1, got {max_new}")
     if eos_ids is not None:
         _cuda(eos_ids, torch.int64, "eos_ids")
-    check(lib().uvx_lookup_accept(pick.data_ptr(), tok.data_ptr(), n_draft.data_ptr(), _p(eos_ids),
-                                  0 if eos_ids is None else eos_ids.numel(), seq.data_ptr(), cur_len.data_ptr(), n_new.data_ptr(),
-                                  int(max_new), _p(step), _p(accepted), 0 if accepted is None else accepted.numel(), done.data_ptr(),
-                                  _stream()), "uvx_lookup_accept")
+    args = (pick.data_ptr(), tok.data_ptr(), n_draft.data_ptr(), _p(eos_ids), 0 if eos_ids is None else eos_ids.numel(),
+            seq.data_ptr(), cur_len.data_ptr(), n_new.data_ptr(), int(max_new), _p(step), _p(accepted),
+            0 if accepted is None else accepted.numel(), done.data_ptr())
+    if hit is None:
+        check(lib().uvx_lookup_accept(*args, _stream()), "uvx_lookup_accept")
+    else:
+        check(lib().uvx_lookup_accept_stop(*args, _rows(hit, torch.int32, R, "hit").data_ptr(), _stream()), "uvx_lookup_accept_stop")
 
 
 # ------------------------------------------------------------------------------------------ prompt lookup in slots
@@ -1400,9 +1496,10 @@ def lookup_draft_slots(seq: torch.Tensor, token: torch.Tensor, cur_len: torch.Te
 def lookup_accept_slots(pick: torch.Tensor, tok: torch.Tensor, n_draft: torch.Tensor, K: int, eos_ids: Optional[torch.Tensor],
                         seq: torch.Tensor, token: torch.Tensor, done: torch.Tensor, cur_len: torch.Tensor, n_new: torch.Tensor,
                         max_new: torch.Tensor, active: torch.Tensor, pos: torch.Tensor, lens: torch.Tensor, rope_pos: torch.Tensor,
-                        accepted: torch.Tensor, n_open: torch.Tensor) -> None:
+                        accepted: torch.Tensor, n_open: torch.Tensor, hit: Optional[torch.Tensor] = None) -> None:
     """``uvx_lookup_accept_slots`` (include/uvx.h): picks [R] int64 of the rows that fed tok [R] -> each open slot's agreeing
-    drafts plus one token appended to seq [slots, W] int64 with ``uvx_slot_finish``'s bookkeeping; accepted [slots] += m."""
+    drafts plus one token appended to seq [slots, W] int64 with ``uvx_slot_finish``'s bookkeeping; accepted [slots] += m.
+    ``hit`` [R] int32: ``uvx_lookup_accept_slots_stop``, each slot's accept cut at its first row with a stop-string hit."""
     S = cur_len.shape[0]
     if not 1 <= int(K) <= LOOKUP_MAX_K:
         raise ValueError(f"K must be in [1, {LOOKUP_MAX_K}], got {K}")
@@ -1415,11 +1512,15 @@ def lookup_accept_slots(pick: torch.Tensor, tok: torch.Tensor, n_draft: torch.Te
     _rows(n_open, torch.int32, 1, "n_open")
     if eos_ids is not None:
         _cuda(eos_ids, torch.int64, "eos_ids")
-    check(lib().uvx_lookup_accept_slots(pick.data_ptr(), tok.data_ptr(), n_draft.data_ptr(), S, int(K), _p(eos_ids),
-                                        0 if eos_ids is None else eos_ids.numel(), seq.data_ptr(), seq.stride(0), token.data_ptr(),
-                                        done.data_ptr(), cur_len.data_ptr(), n_new.data_ptr(), max_new.data_ptr(), active.data_ptr(),
-                                        pos.data_ptr(), lens.data_ptr(), rope_pos.data_ptr(), accepted.data_ptr(), n_open.data_ptr(),
-                                        _stream()), "uvx_lookup_accept_slots")
+    args = (pick.data_ptr(), tok.data_ptr(), n_draft.data_ptr(), S, int(K), _p(eos_ids), 0 if eos_ids is None else eos_ids.numel(),
+            seq.data_ptr(), seq.stride(0), token.data_ptr(), done.data_ptr(), cur_len.data_ptr(), n_new.data_ptr(),
+            max_new.data_ptr(), active.data_ptr(), pos.data_ptr(), lens.data_ptr(), rope_pos.data_ptr(), accepted.data_ptr(),
+            n_open.data_ptr())
+    if hit is None:
+        check(lib().uvx_lookup_accept_slots(*args, _stream()), "uvx_lookup_accept_slots")
+    else:
+        check(lib().uvx_lookup_accept_slots_stop(*args, _rows(hit, torch.int32, R, "hit").data_ptr(), _stream()),
+              "uvx_lookup_accept_slots_stop")
 
 
 def sample_rows(logits: torch.Tensor, temperature: torch.Tensor, top_k: torch.Tensor, top_p: torch.Tensor, u: torch.Tensor,
@@ -1538,19 +1639,24 @@ def beam_select(logprobs: torch.Tensor, run_score: torch.Tensor, num_beams: int,
 
 
 def beam_update(cand_s: torch.Tensor, cand_i: torch.Tensor, V: int, num_beams: int, eos_ids: Optional[torch.Tensor], max_new: int,
-                len_div: torch.Tensor, early_stopping: int, lp_positive: bool, state: dict, counters: dict, bumps: tuple = ()) -> None:
+                len_div: torch.Tensor, early_stopping: int, lp_positive: bool, state: dict, counters: dict, bumps: tuple = (),
+                hit: Optional[torch.Tensor] = None) -> None:
     """``uvx_beam_update`` on the candidates of ``beam_select``.  ``state`` holds the device tensors run_score, run_seq,
-    pool_seq, pool_score, pool_len, pool_fin, parent, tok, heur, flags, ticket; ``counters`` cur_len, step_idx, done."""
+    pool_seq, pool_score, pool_len, pool_fin, parent, tok, heur, flags, ticket; ``counters`` cur_len, step_idx, done.
+    ``hit`` [B * K] int32 (``stop_strings_beam``): ``uvx_beam_update_stop``, a candidate with a hit finishes."""
     B, K = cand_s.shape
     s, c = state, counters
     b = list(bumps) + [None] * (3 - len(bumps))
-    check(lib().uvx_beam_update(cand_s.data_ptr(), cand_i.data_ptr(), B, num_beams, K, V, _p(eos_ids),
-                                0 if eos_ids is None else eos_ids.numel(), int(max_new), len_div.data_ptr(), int(early_stopping),
-                                int(bool(lp_positive)), s["run_score"].data_ptr(), s["run_seq"].data_ptr(), s["pool_seq"].data_ptr(),
-                                s["run_seq"].stride(0), s["pool_score"].data_ptr(), s["pool_len"].data_ptr(), s["pool_fin"].data_ptr(),
-                                s["parent"].data_ptr(), s["tok"].data_ptr(), s["heur"].data_ptr(), s["flags"].data_ptr(),
-                                s["ticket"].data_ptr(), c["cur_len"].data_ptr(), c["step_idx"].data_ptr(), _p(b[0]), _p(b[1]), _p(b[2]),
-                                c["done"].data_ptr(), _stream()), "uvx_beam_update")
+    args = (cand_s.data_ptr(), cand_i.data_ptr(), B, num_beams, K, V, _p(eos_ids), 0 if eos_ids is None else eos_ids.numel(),
+            int(max_new), len_div.data_ptr(), int(early_stopping), int(bool(lp_positive)), s["run_score"].data_ptr(),
+            s["run_seq"].data_ptr(), s["pool_seq"].data_ptr(), s["run_seq"].stride(0), s["pool_score"].data_ptr(),
+            s["pool_len"].data_ptr(), s["pool_fin"].data_ptr(), s["parent"].data_ptr(), s["tok"].data_ptr(), s["heur"].data_ptr(),
+            s["flags"].data_ptr(), s["ticket"].data_ptr(), c["cur_len"].data_ptr(), c["step_idx"].data_ptr(), _p(b[0]), _p(b[1]),
+            _p(b[2]), c["done"].data_ptr())
+    if hit is None:
+        check(lib().uvx_beam_update(*args, _stream()), "uvx_beam_update")
+    else:
+        check(lib().uvx_beam_update_stop(*args, _rows(hit, torch.int32, B * K, "hit").data_ptr(), _stream()), "uvx_beam_update_stop")
 
 
 def kv_reorder_(k_cache: torch.Tensor, v_cache: torch.Tensor, parent: torch.Tensor, n_pos: torch.Tensor, num_beams: int) -> None:

@@ -29,6 +29,7 @@ import torch
 
 from . import ops
 from .constraints import LogitsConstraints
+from .stop_strings import StopStrings
 from .engine import (PREFILL_ROWS, PagedSlotDecodeEngine, SlotDecodeEngine, TokenLogprobs, check_kv_scales,
                      check_lookup_k)
 
@@ -292,6 +293,7 @@ class _Request:
     lookup: Optional[tuple] = None     # (k, n) of prompt lookup (None: the engine has none)
     constraints: Optional[LogitsConstraints] = None
     cutoffs: Optional[tuple] = None    # (min_p, typical_p, epsilon, eta) when sampled with one on
+    stop: Optional[StopStrings] = None
 
 
 class SlotScheduler:
@@ -358,12 +360,19 @@ class SlotScheduler:
     the conversation so far).  A request's packed table may hold up to N token ids (each entry's ids; EOS ids count once per
     entry under ``min_*``).  Each slot's settings live in device arrays, so the steps stay captured once; the constraints run
     inside every pick, before the penalty, and a request's tokens are those ``generate()`` gives it alone with the same
-    options.  With None the engine allocates nothing for them and its steps are unchanged."""
+    options.  With None the engine allocates nothing for them and its steps are unchanged.
+
+    ``max_stop_table`` = N (None, the default: off): requests may take ``generate()``'s stop strings, ``submit(...,
+    stop_strings=, tokenizer=)``, with its meaning and checks.  Each slot holds a packed table of up to N int32 words on the
+    device (``StopStrings.n_words`` reports a request's size), written at admission; the check runs inside every pick (the
+    plain, mixed, admission and lookup steps), and a slot whose text ends with a stop string finishes as on an EOS id.  With
+    None nothing is allocated and the steps are unchanged."""
 
     def __init__(self, model, slots: int = 8, max_len: int = 2048, eos_token_ids=None, pad_token_id: Optional[int] = None,
                  sync_every: int = 8, use_graph: bool = True, kv_pages: Optional[int] = None, prefix_cache: bool = False,
                  max_logprobs: int = 0, kv_cache_dtype: str = "bf16", kv_scales=None, host_kv_pages: int = 0,
-                 prompt_lookup_num_tokens: Optional[int] = None, max_constraint_tokens: Optional[int] = None):
+                 prompt_lookup_num_tokens: Optional[int] = None, max_constraint_tokens: Optional[int] = None,
+                 max_stop_table: Optional[int] = None):
         eos = sorted(set([eos_token_ids] if isinstance(eos_token_ids, int) else (eos_token_ids or [])))
         pad = pad_token_id if pad_token_id is not None else (min(eos) if eos else 0)     # generate()'s default
         if int(sync_every) < 1:
@@ -395,6 +404,8 @@ class SlotScheduler:
             lp["prompt_lookup_num_tokens"] = self.lookup_k
         if max_constraint_tokens is not None:
             lp["max_constraint_tokens"] = max_constraint_tokens       # the engine validates it
+        if max_stop_table is not None:
+            lp["max_stop_table"] = max_stop_table                     # the engine validates it
         self._eos = eos
         self.accepted_drafts: Dict[int, int] = {}
         if host_kv_pages:
@@ -491,7 +502,7 @@ class SlotScheduler:
                min_new_tokens: Optional[int] = None, min_length: Optional[int] = None, bad_words_ids=None, sequence_bias=None,
                suppress_tokens=None, begin_suppress_tokens=None, min_p: Optional[float] = None,
                typical_p: Optional[float] = None, epsilon_cutoff: Optional[float] = None,
-               eta_cutoff: Optional[float] = None) -> int:
+               eta_cutoff: Optional[float] = None, stop_strings=None, tokenizer=None) -> int:
         """Queues one request: ``features`` is the processor's output for it (``input_ids`` [1, S] and, for audio, its mel or
         waveform fields).  Arguments and defaults are ``generate()``'s: greedy unless ``do_sample``; sampling defaults to
         temperature 1 and top_k 50; ``top_p`` must lie in [0, 1].  A sampled request draws its uniforms here, as ``generate()``
@@ -513,7 +524,10 @@ class SlotScheduler:
         ``max_constraint_tokens`` ids.
 
         ``min_p``, ``typical_p``, ``epsilon_cutoff``, ``eta_cutoff``: ``generate()``'s sampling cut-offs and checks, held per
-        slot and read by the captured step; ignored when not sampling."""
+        slot and read by the captured step; ignored when not sampling.
+
+        ``stop_strings`` with ``tokenizer`` (a scheduler built with ``max_stop_table``): ``generate()``'s stop strings and checks.
+        ValueError when the scheduler has no stop tables or the request's table needs more than ``max_stop_table`` words."""
         if logprobs is not None:
             self.engine.check_logprobs(logprobs)
         lookup = self._check_lookup(prompt_lookup_num_tokens, max_matching_ngram_size)
@@ -537,6 +551,11 @@ class SlotScheduler:
                 raise ValueError("token constraints need a table per slot: SlotScheduler(..., max_constraint_tokens=N)")
             cons = LogitsConstraints.build(self.model.language_model.lm_head.weight.shape[0], self._eos, S, *ck_args)
             self.engine.check_constraints(cons)
+        stop = StopStrings.build(tokenizer, stop_strings)
+        if stop is not None:
+            if self.engine.max_stop_table is None:
+                raise ValueError("stop strings need a table per slot: SlotScheduler(..., max_stop_table=N)")
+            self.engine.check_stop(stop)
         if n < 1:
             raise ValueError(f"max_new_tokens must be >= 1, got {max_new_tokens}")
         if S + n > self.capacity:
@@ -570,7 +589,8 @@ class SlotScheduler:
         self._next_id += 1
         self._queue.append(_Request(rid, ids, feats, n, temp, k_top, p_top, float(repetition_penalty or 1.0), u, session,
                                     prefix, logprobs=None if logprobs is None else int(logprobs), lookup=lookup,
-                                    constraints=cons, cutoffs=cutoffs if sampling and ops.cutoffs_on(cutoffs) else None))
+                                    constraints=cons, cutoffs=cutoffs if sampling and ops.cutoffs_on(cutoffs) else None,
+                                    stop=stop))
         if sess is not None:
             sess.busy = True
         return rid
@@ -639,6 +659,8 @@ class SlotScheduler:
                 kw["constraints"] = r.constraints
             if r.cutoffs is not None:
                 kw["cutoffs"] = r.cutoffs
+            if r.stop is not None:
+                kw["stop"] = r.stop
             eng.admit(j, r.input_ids, r.max_new, r.temperature, r.top_k, r.top_p, r.penalty, r.u, **kw, **feats)
             r.features, r.u = {}, None
             if long:
